@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the denoising hot path (BASELINE.json metric: denoising-steps/sec).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--no-secondary]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--no-secondary] [--dump-outputs DIR]
 
 One "step" = one DDIM step of the workload's whole per-GPU batch: Beff U-Net evaluations (2B with
 classifier-free guidance) + the CFG/DDIM update.  Default workload = BASELINE.json configs[1]:
@@ -14,6 +14,10 @@ The ONE JSON line (rank 0) carries, besides the contract keys,
   secondary.workloads                      the same measurements for BASELINE configs 3 (L512_B32) and 5 (L992_B8) at N=1,
                                            and for config 4's per-GPU batch (32 charts / GPU) at every N.
 --impl reference times the CPU oracle port of the reference path (oracle/mug_oracle.py: torch CPU fp32) on the same workload.
+--dump-outputs DIR writes what the timed loop computed in its last step (rank 0, headline workload) as float32 .npy files:
+  z.npy    [B, 16, L]     the latent after the K timed DDIM steps (what DDIMSampler.sample returns as z)
+  eps.npy  [Beff, 16, L]  the U-Net output of the last timed step (unconditional half first under CFG)
+The timed steps always start from the workload's seeded x_T at schedule step 0, so the same arguments give the same inputs.
 """
 import argparse
 import json
@@ -52,27 +56,13 @@ def config_of(name, wl, world=1, **extra):
     return d
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(tflops=float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))), hbm=float(d.get("hbm_gbs", 6650.0)),
-                    src="measured (MEASURED_PEAKS.json bf16_tflops_sustained)")
-    return dict(tflops=1400.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
-
-
-def ncu_step_traffic(name):
-    """Whole-step DRAM traffic from the committed ncu capture of ONE graphed-plan evaluation of this workload
-    (profiles/r02_step_traffic.json, written by tools/summarize_step_ncu.py): every launch of the eval, --cache-control none."""
-    p = os.path.join(ROOT, "profiles", "r02_step_traffic.json")
-    try:
-        return json.load(open(p)).get(name)
-    except Exception:
-        return None
+def data_sheet_peaks():
+    """H100 SXM data sheet (dense BF16 tensor rate, HBM3 bandwidth) at a 700 W power limit: a ceiling, never a measured figure."""
+    return dict(tflops=989.0, hbm=3350.0, src="H100 SXM data sheet, dense BF16 at 700 W (not a measured figure)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons while the step loop runs (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons while the step loop runs (read-only queries every 50 ms)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -216,7 +206,7 @@ def run_reference(args, wl, name):
     line = dict(metric=METRIC, value=v, unit=UNIT, n_gpus=args.gpus, steps=args.steps, warmup=args.warmup,
                 ms_per_step=1000.0 / v, higher_is_better=True, scaling="weak", vs_baseline=None, dtype="f32", data="synthetic",
                 impl="reference",
-                config=config_of(name, wl, args.gpus),        # identical keys and values to the B200 arm's `config`
+                config=config_of(name, wl, args.gpus),        # identical keys and values to the GPU arm's `config`
                 info=dict(note="CPU oracle port of the reference PyTorch path (oracle/mug_oracle.py, bit-identical to the reference on "
                                "tests/golden); S4 kernels regenerated every eval like the reference.  One host runs ONE per-GPU batch: at "
                                "--gpus N > 1 only rank 0 measures one per-GPU batch, so the driver's ratio compares N GPUs with one CPU host"),
@@ -226,7 +216,7 @@ def run_reference(args, wl, name):
 
 
 # ---------------------------------------------------------------------------------------------------
-# the B200 arm
+# the GPU arm
 # ---------------------------------------------------------------------------------------------------
 class _NoBar:
     def __init__(self, it, **kw):
@@ -253,8 +243,9 @@ def build_model(L, world, rank, dev, gemm):
     return MugDiffusionB200(sd, cfg, z_length=L, device=dev, gemm_impl=gemm, fold_ln={"0": False, "1": True}.get(os.environ.get("MUGD_FOLD_LN", ""))), sd
 
 
-def measure(model, name, wl, steps, warmup, world, rank, dev, with_roofline=True, sustain=True):
-    """value (device-resident loop, CUDA events, max over ranks), roofline of the GEMM family, e2e through the public API."""
+def measure(model, name, wl, steps, warmup, world, rank, dev, with_roofline=True, sustain=True, dump_dir=None):
+    """value (device-resident loop, CUDA events, max over ranks), roofline of the GEMM family, e2e through the public API.
+    dump_dir: write the last timed step's latent and U-Net output there (see --dump-outputs)."""
     import torch.distributed as dist
 
     from mug_diffusion_b200 import lib as L_
@@ -323,8 +314,7 @@ def measure(model, name, wl, steps, warmup, world, rank, dev, with_roofline=True
             for _ in range(10):
                 step()
             torch.cuda.synchronize()
-    if budget[0] < steps:
-        restart()
+    restart()                                   # the timed steps start from x_T at schedule step 0: their outputs are reproducible
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     torch.cuda.synchronize()
     if world > 1:
@@ -343,7 +333,12 @@ def measure(model, name, wl, steps, warmup, world, rank, dev, with_roofline=True
     clock_info = clocks.stop() if rank == 0 else None
     launches_per_step = sess.plan.launches + 2
     value = world * steps / (ms / 1000.0)
-    finite = bool(torch.isfinite(sess.read_rows(sess.eps, Beff, 16, L)).all())
+    eps_last = sess.read_rows(sess.eps, Beff, 16, L)
+    finite = bool(torch.isfinite(eps_last).all())
+    if dump_dir is not None and rank == 0:
+        os.makedirs(dump_dir, exist_ok=True)
+        np.save(os.path.join(dump_dir, "z.npy"), sess.read_rows(sess.xin, B, 16, L).cpu().numpy().astype(np.float32))
+        np.save(os.path.join(dump_dir, "eps.npy"), eps_last.cpu().numpy().astype(np.float32))
 
     # ---- roofline of the dominant kernel family (GEMM) -----------------------------------------------------
     # Device time per kernel family, measured live with CUDA events: the ops of one family are put in their own
@@ -375,17 +370,12 @@ def measure(model, name, wl, steps, warmup, world, rank, dev, with_roofline=True
             torch.cuda.synchronize()
             fam_ms[kind] = a0.elapsed_time(a1) / 5
             fam_n[kind] = pl.launches
-        pk = measured_peaks()
+        pk = data_sheet_peaks()
         gemm_ms, gemm_n = fam_ms[L_.OP_GEMM], fam_n[L_.OP_GEMM]
         ach = gemm_flops / (gemm_ms * 1e-3) / 1e12
-        tr = ncu_step_traffic(name)
-        roof = dict(bound="tensor", kernel=f"gemm_tc_kernel (tcgen05 3xTF32; impl={eng.gemm_impl})", achieved=ach, peak=pk["tflops"],
+        roof = dict(bound="tensor", kernel=f"gemm_tc_kernel (wgmma 3xTF32; impl={eng.gemm_impl})", achieved=ach, peak=pk["tflops"],
                     unit="TFLOP/s", frac=ach / pk["tflops"], frac_of_3xtf32_ceiling=ach / (pk["tflops"] / 6.0),
-                    traffic=(tr or {}).get("gemm_bytes_per_launch"), peak_source=pk["src"], launches=gemm_n,
-                    traffic_note=("profiles/r02_step_traffic.json: dram__bytes_read+write summed over EVERY gemm_tc launch of one whole eval "
-                                  "of this workload (ncu --cache-control none), divided by the launches; whole-step sum and the ratio to the "
-                                  "algorithmic bytes are in `step_traffic`") if tr else "no committed whole-step ncu capture for this workload",
-                    step_traffic=tr,
+                    peak_source=pk["src"], launches=gemm_n,
                     avg_launch_us=1000.0 * gemm_ms / max(gemm_n, 1), algorithmic_gflop_per_step=gemm_flops / 1e9,
                     note="3xTF32 issues 3 tensor-core products per fp32 product and TF32 runs at half the bf16 rate: "
                          "the fp32-exact ceiling is peak/6",
@@ -458,6 +448,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the secondary workloads (configs 3/4/5)")
     ap.add_argument("--cpu-steps", type=int, default=10)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (z.npy, eps.npy; float32) to DIR")
     args = ap.parse_args()
     name = args.workload
     wl = WORKLOADS[name]
@@ -478,7 +470,7 @@ def main():
 
     model, sd = build_model(L, world, rank, dev, args.gemm)
     eng = model.engine
-    m = measure(model, name, wl, args.steps, args.warmup, world, rank, dev)
+    m = measure(model, name, wl, args.steps, args.warmup, world, rank, dev, dump_dir=args.dump_outputs)
 
     # ---- secondary numbers: the same loop without guidance, the decode, and the other BASELINE configs -----------------------
     secondary = None

@@ -1,5 +1,5 @@
 /*
- * mugd.h -- C ABI of libmugd.so, the sm_100a (B200) denoising engine for Mug-Diffusion.
+ * mugd.h -- C ABI of libmugd.so, the sm_90a (H100) denoising engine for Mug-Diffusion.
  *
  * The reference (Keytoyze/Mug-Diffusion) has no FFI: its hot path is Python calling ATen.  The boundary
  * this library replaces is therefore the set of Python call sites
@@ -37,7 +37,7 @@ enum mugd_status {
     MUGD_OK = 0,
     MUGD_ERR_INVALID = 1,      /* bad argument / unsupported shape            */
     MUGD_ERR_CUDA = 2,         /* CUDA runtime error (see mugd_last_error)    */
-    MUGD_ERR_NO_DEVICE = 3,    /* not an sm_100 device; there is no fallback  */
+    MUGD_ERR_NO_DEVICE = 3,    /* not an sm_90 device; there is no fallback   */
     MUGD_ERR_OOM = 4
 };
 
@@ -71,7 +71,7 @@ enum mugd_act { MUGD_ACT_NONE = 0, MUGD_ACT_SILU = 1, MUGD_ACT_GELU = 2 };
 enum mugd_gate { MUGD_GATE_NONE = 0, MUGD_GATE_GEGLU = 1 /* a*gelu(g), attention.py:38-45 */,
                  MUGD_GATE_GLU = 2 /* a*sigmoid(g), s4.py:191-192,1536 */ };
 enum mugd_gemm_impl { MUGD_GEMM_AUTO = 0, MUGD_GEMM_SIMT = 1 /* exact fp32 FMA */,
-                      MUGD_GEMM_TC = 2 /* tcgen05 3xTF32 split, fp32 accumulate in TMEM */ };
+                      MUGD_GEMM_TC = 2 /* wgmma 3xTF32 split, fp32 accumulate in registers */ };
 
 typedef struct mugd_gemm {
     const float* A;  int64_t lda;          /* [B*Lin, K] activations                                       */
@@ -102,8 +102,8 @@ typedef struct mugd_gemm {
     int32_t K2; int32_t reserved_;
     /* Row moments of the OUTPUT for a LayerNorm that follows (tensor-core path, act == gate == NONE only): while the tile is stored,
      * row_moments[m*2 + {0,1}] += {sum, sum of squares} of the columns of output row m (fp64 atomics; the plan zeroes the buffer at
-     * the start of every evaluation).  Round 2 also built GroupNorm-moment sinks + a single-pass apply kernel; they lost at every batch
-     * size (profiles/r02_norm_fusion_ab.md) and were removed. */
+     * the start of every evaluation).  GroupNorm-moment sinks + a single-pass apply kernel were also built;
+     * they lost at every batch size and were removed. */
     double* row_moments;
     /* LayerNorm folded into this GEMM (attention.py:147-151: norm_i followed by a Linear): with W' = W diag(gamma) packed as the
      * weight, colsum[n] = sum_k W'[n][k] and bias' = W beta + b,   C = rstd_m * (A W'^T - mean_m * colsum) + bias'   where mean_m,
@@ -203,7 +203,7 @@ typedef struct mugd_op {
 /* ---- lifecycle -------------------------------------------------------------------------------- */
 int  mugd_abi_version(void);
 const char* mugd_last_error(void);                         /* thread-local message of the last failure */
-int  mugd_create(int device, mugd_handle** out);           /* MUGD_ERR_NO_DEVICE unless sm_100          */
+int  mugd_create(int device, mugd_handle** out);           /* MUGD_ERR_NO_DEVICE unless sm_90           */
 void mugd_destroy(mugd_handle* h);
 int  mugd_device_info(mugd_handle* h, int32_t* sm_count, int32_t* cc_major, int32_t* cc_minor);
 int  mugd_set_gemm_impl(mugd_handle* h, int impl);         /* default for ops with impl == AUTO         */
@@ -253,12 +253,12 @@ int  mugd_s4_kernel_gen(mugd_handle* h,
                         void* workspace, int64_t workspace_bytes, /* >= 16*H*(L_internal/2+1) bytes */
                         void* stream);
 
-/* ---- tensor-core GEMM planning: is this GEMM taken by the tcgen05 kernel, with which K split, and how much
+/* ---- tensor-core GEMM planning: is this GEMM taken by the wgmma kernel, with which K split, and how much
  * split-K workspace / how many tile counters does it need (the host allocates them once per plan) ------ */
 int  mugd_gemm_tc_query(mugd_handle* h, const mugd_gemm* g, int32_t sm_count, int32_t* supported, int32_t* splits,
                         int64_t* workspace_bytes, int32_t* n_tiles);
-/* which kernel variant the planner picks for this GEMM on a machine with sm_count SMs: tile width (64 / 128 / 256; 0 = not taken by the
- * tensor-core kernel), CTAs per SM it is built for (1, or 2 = the 128-wide variant whose CTAs walk a tile list), CTAs launched */
+/* which kernel variant the planner picks for this GEMM on a machine with sm_count SMs: tile width (64 / 128; 0 = not taken by the
+ * tensor-core kernel), CTAs per SM it is built for (always 1), CTAs launched */
 int  mugd_gemm_tc_variant(const mugd_gemm* g, int32_t sm_count, int32_t* tile_n, int32_t* ctas_per_sm, int32_t* grid_ctas);
 
 /* ---- per-handle switches -------------------------------------------------------------------------
@@ -267,20 +267,20 @@ int  mugd_gemm_tc_variant(const mugd_gemm* g, int32_t sm_count, int32_t* tile_n,
  * bench.py use 0.  Plans created (and graphs captured) earlier keep the mode they were created with. */
 int  mugd_set_tc_single_pass_tf32(mugd_handle* h, int enabled);
 
-/* attention kernel: 1 (default) = QK^T and PV on the tcgen05 tensor cores (3xTF32, fp32 accuracy); 0 = exact-fp32 FFMA kernel
+/* attention kernel: 1 (default) = QK^T and PV on the wgmma tensor cores (3xTF32, fp32 accuracy); 0 = exact-fp32 FFMA kernel
  * (the referee of the parity tests).  Replaces the einsum/softmax body of CrossAttention.forward, attention.py:99-121 */
 int  mugd_set_attention_impl(mugd_handle* h, int impl);
 
 /* ---- measurement aids (process-wide, not needed in production) -------------------------------------
- * planner cost constants of the tensor-core GEMM (us per 32-deep k-step of a 128- and a 256-column tile, us per split-K
- * round trip, fixed us of the two-CTAs-per-SM variant); values <= 0 keep the current one.  For tuning sweeps (tools/). */
+ * planner cost constants of the tensor-core GEMM (relative cost of a 32-deep k-step of a 128-column tile, unused, of a
+ * split-K round trip, unused); values <= 0 keep the current one.  For tuning sweeps (tools/). */
 int  mugd_debug_set_tc_cost(float kstep128_us, float kstep256_us, float split_us, float two_cta_fixed_us);
 
-/* force the tensor-core tile variant (64, 128, 256 columns, or 130 = 128 columns built for two CTAs per SM) where legal; 0 = cost model */
+/* force the tensor-core tile width (64 or 128 columns) where legal; 0 = cost model */
 int  mugd_debug_set_tc_tile_n(int bn);
 
-/* CTA (0,0,0) of the tensor-core attention kernel dumps 40 floats per query row of its first key tile
- * (raw logits, O tile, running max / sum, first operand words) into buf[128*40]; NULL switches it off */
+/* CTA (0,0,0) of the tensor-core attention kernel dumps the first 16 raw logits of every query row of its
+ * first key tile into buf[128*40] (floats 0..15 of each 40-float row); NULL switches it off */
 int  mugd_debug_set_attention_dump(float* buf);
 
 /* builds with -DMUGD_TC_TIMELINE only (tools/build_variant.py): CTA (0,0,0) of every tensor-core GEMM launch writes

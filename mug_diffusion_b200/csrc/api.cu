@@ -9,7 +9,7 @@
 namespace mugd {
 
 static thread_local char g_err[1024] = "";
-// Programmatic launch edges with the implicit (grid-completion) trigger: graph edge 0.57 vs 0.69 us, 3.97 vs 4.02 ms/step.  This is a
+// Programmatic launch edges with the implicit (grid-completion) trigger: a shorter edge between dependent kernels.  This is a
 // launch attribute without numerical effect; it is process-wide because launch_k() has no handle (mugd_set_pdl is an A/B switch).
 bool g_use_pdl = true;
 
@@ -82,8 +82,8 @@ int mugd_create(int device, mugd_handle** out) {
     }
     cudaDeviceProp prop;
     MUGD_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        set_error("mugd_create: device %d is sm_%d%d; libmugd is built for sm_100a (B200) only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("mugd_create: device %d is sm_%d%d; libmugd is built for sm_90a (H100) only", device, prop.major, prop.minor);
         return MUGD_ERR_NO_DEVICE;
     }
     MUGD_CHECK_CUDA(cudaSetDevice(device));

@@ -182,7 +182,7 @@ static int attention_launch(const mugd_attention& a, cudaStream_t st) {
 
 // =====================================================================================================
 // Few keys (Lk <= 32): the cross attention to the 21 prompt tokens, 16 of the 32 attention launches of an evaluation.
-// A 128-key tensor-core tile would be 5/6 zero fill behind ~5 us of fixed cost (tensor-memory allocation, TMA, operand splits);
+// A 128-key tensor-core tile would be 5/6 zero fill behind a fixed cost (barriers, TMA, operand splits);
 // here ONE LANE OWNS ONE KEY: lane j keeps k_j in registers, a warp takes four query rows at a time (four independent dependency
 // chains) -- the rows are read back from shared memory as broadcast float4s for the D-long dot products, max / sum are warp shuffles, and for O = (P*gain) V lane d owns output
 // channels d, d+32 and receives p_j from lane j by shuffle.  Exact fp32, same formula order as the FFMA referee above.
@@ -309,7 +309,7 @@ static int attention_smallk_launch(const mugd_attention& a, cudaStream_t st) {
 }
 
 int launch_attention_tc(const DeviceInfo& dev, const mugd_attention& a, cudaStream_t st);   // attention_tc.cu
-// 1 (default): both contractions on the tcgen05 tensor cores (attention_tc.cu), a lane-per-key kernel when there are at most 32 keys;
+// 1 (default): both contractions on the wgmma tensor cores (attention_tc.cu), a lane-per-key kernel when there are at most 32 keys;
 // 0: the tiled FFMA kernel above for everything (referee)
 int launch_attention(const DeviceInfo& dev, const mugd_attention& a, cudaStream_t st, int* launches) {
     MUGD_REQUIRE(a.B > 0 && a.H > 0 && a.Lq > 0 && a.Lk > 0, "attention: empty shape");
@@ -320,9 +320,8 @@ int launch_attention(const DeviceInfo& dev, const mugd_attention& a, cudaStream_
     MUGD_REQUIRE(a.ldq >= a.H * a.D && a.ldk >= a.H * a.D && a.ldv >= a.H * a.D && a.ldo >= a.H * a.D, "attention: ld < H*D");
     MUGD_REQUIRE(a.relpos && a.cgain, "attention: tables missing");
     int rc;
-    // measured per shape (tools/profile_ops.py --only attention): with head dim 32 (Lq = 256 at the default length) the rows are many
-    // and short and the FFMA lanes saturate (6.9 vs 5.8 us at Beff = 8); with head dim 48 / 64 the lane-per-key kernel wins
-    // (5.7 vs 7.6, 4.2 vs 6.5 us at Beff = 8; 26.8 vs 28.0, 17.3 vs 23.9 us at Beff = 64)
+    // per shape (tools/profile_ops.py --only attention): with head dim 32 (Lq = 256 at the default length) the rows are many
+    // and short and the FFMA lanes saturate; with head dim 48 / 64 the lane-per-key kernel wins
     if (dev.attention_impl == 1 && a.Lk <= 32 && a.D >= 48)
         rc = (a.D == 48) ? attention_smallk_launch<48>(a, st) : attention_smallk_launch<64>(a, st);
     else if (dev.attention_impl == 1) rc = launch_attention_tc(dev, a, st);

@@ -1,28 +1,29 @@
-// Attention of mug/model/attention.py:91-126 (CrossAttention.forward) with both contractions on the tcgen05 tensor
-// cores, fp32 in / fp32 out through the same 3xTF32 split as gemm_tc.cu:
+// Attention of mug/model/attention.py:91-126 (CrossAttention.forward) with both contractions on the Hopper warpgroup tensor
+// cores (wgmma), fp32 in / fp32 out through the same 3xTF32 split as gemm_tc.cu:
 //
 //     idx_ij = clamp(j - i, -P, P) + P
-//     s_ij   = (q_i . k_j + relpos[idx_ij, h]) * scale                 S = Q K^T   : tcgen05.mma, A = Q from TMEM
-//     o_i    = sum_j softmax_j(s_i)_j * cgain[idx_ij, h] * v_j         O = P V     : tcgen05.mma, A = P from TMEM
+//     s_ij   = (q_i . k_j + relpos[idx_ij, h]) * scale                 S = Q K^T   : wgmma, A = Q from registers
+//     o_i    = sum_j softmax_j(s_i)_j * cgain[idx_ij, h] * v_j         O = P V     : wgmma, A = P from registers
 //
-// One CTA owns 128 queries of one (sample, head) and streams 128-key tiles (flash style: no [Lq, Lk] matrix in
-// memory, running max / sum per query row).  Thread t and thread t+128 share query row (t & 127) = TMEM lane:
-//   * Q is split into q_hi / q_lo once and lives in tensor memory for the whole CTA (A operand, "TS" form);
-//   * the raw K and V head slices of a key tile arrive by TMA (3-D tensor maps (channel, key, sample), 128B swizzle,
-//     keys past Lk zero-filled by the TMA bounds check), one tile ahead of the math when two stages fit (head dim 32);
-//     the key tile is split in place into k_hi / k_lo (row = key, 128 bytes of channels: the K-major B operand of
-//     S = Q K^T); the value tile is split and transposed shared -> shared into V^T hi / lo (row = channel, keys
-//     contiguous: the K-major B operand of O = P V) -- tcgen05 takes MN-major TF32 operands only in a different
-//     swizzle, so the transpose is done by hand, one conflict-free 32-key x 4-channel block per warp step;
-//   * S lands in TMEM columns [0,128); each thread pulls its half of the row into registers, applies the
-//     relative-position bias, scale and key mask, and the two halves combine max / sum through shared memory;
-//   * P * gain is split into hi / lo and written back to tensor memory (hi over the S columns it came from, lo next
-//     to it): the second MMA consumes it from there, so P never touches shared or global memory;
-//   * the per-tile O lands in TMEM and is folded into the register accumulator with the usual exp(m_old - m_new).
+// One CTA owns 128 queries of one (sample, head) and streams 128-key tiles (flash style: no [Lq, Lk] matrix in memory, running
+// max / sum per query row).  Warpgroup w owns query rows 64w..64w+63; a thread holds two rows (g, g+8 of its warp's 16):
+//   * Q is split into q_hi / q_lo once and stays in registers for the whole CTA, in the wgmma A-fragment layout;
+//   * the raw K and V head slices of a key tile arrive by TMA (3-D tensor maps (channel, key, sample), 128B swizzle, keys past Lk
+//     zero-filled by the TMA bounds check), one tile ahead of the math when two stages fit (head dim 32 / 48);
+//     the key tile is split in place into k_hi / k_lo (row = key, 128 bytes of channels: the K-major B operand of S = Q K^T);
+//     the value tile is split and transposed shared -> shared into V^T hi / lo (row = channel, keys contiguous: the K-major B
+//     operand of O = P V) while the tensor cores compute S, one conflict-free 32-key x 4-channel block per warp step;
+//   * S lands in registers; bias, scale, key mask and the online softmax run there (a row is spread over the 4 threads of a
+//     quad: two shuffles for its max, its sum is kept per thread and reduced once at the end);
+//   * P * gain is split into hi / lo and fed straight back as the A fragments of P V.  The accumulator holds keys 2t, 2t+1 of
+//     each 8-key group where the A fragment expects keys t, t+4, so V^T stores the keys of every 8-group in the order
+//     0 2 4 6 1 3 5 7: the contraction runs over the same pairs and P never leaves the registers;
+//   * O accumulates in registers, rescaled by exp(m_old - m_new) before each tile's P V.
 // The FFMA kernel in attention.cu stays as the exact-fp32 referee (mugd_set_attention_impl(0)).
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 #include <math.h>
 
@@ -63,15 +64,7 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
         ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// one lane of a converged warp (see gemm_tc.cu: uniform-datapath instructions must not sit in a lane-divergent branch)
+// one lane of a converged warp (see gemm_tc.cuh: uniform-datapath instructions must not sit in a lane-divergent branch)
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred = 0;
     asm volatile(
@@ -81,39 +74,11 @@ __device__ __forceinline__ bool elect_one() {
         : "=r"(pred));
     return pred != 0;
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout, version 1, same encoding as
-// gemm_tc.cu): rows of 128 bytes, 8-row groups 1024 B apart (SBO), LBO unused.
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
 __device__ __forceinline__ float to_tf32(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
     return __uint_as_float(r);
 }
-// 8 consecutive 32-bit TMEM columns of this thread's lane
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-                   "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-                   "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-                 : "memory");
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
     float4 v;
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
@@ -135,7 +100,7 @@ struct Smem {
     static constexpr uint32_t VT_SLAB = D * 128;           // V^T: D channel rows x (32 keys = 128 B)
     static constexpr uint32_t VT_BYTES = (BKV / 32) * VT_SLAB;
     static constexpr uint32_t TILE_BYTES = STAGES * STAGE_BYTES + OPER + 2 * VT_BYTES;   // + k_lo + V^T hi + V^T lo
-    static constexpr uint32_t AUX_BYTES = 64 + 4 * BQ * 4; // mbarriers + tmem slot | mx[2][128] rs[2][128]
+    static constexpr uint32_t AUX_BYTES = 64;              // mbarriers
     static size_t total(int pos_max) { return TILE_BYTES + AUX_BYTES + 2 * (2 * pos_max + 1) * 4 + 1024; }
 };
 
@@ -143,9 +108,9 @@ template <int D>
 __global__ void __launch_bounds__(THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const mugd_attention a, float* dbg) {
     using S = Smem<D>;
-    constexpr int HC = D / 2;                               // Q / O columns owned by one thread of a row pair
     constexpr int STAGES = S::STAGES;
-    constexpr uint32_t TM_S = 0, TM_PLO = 128, TM_O = 256, TM_QHI = 320, TM_QLO = 384, TM_COLS = 512;
+    constexpr int KD = D / 8;                               // k8 steps of S = Q K^T
+    constexpr int NO = D / 2;                               // O accumulator registers per thread
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;           // SWIZZLE_128B operands need 1024-byte alignment
@@ -154,34 +119,23 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     const uint32_t k_lo = base + STAGES * S::STAGE_BYTES, vt_hi = k_lo + S::OPER, vt_lo = vt_hi + S::VT_BYTES;
     const uint32_t aux = base + S::TILE_BYTES;
     auto bar_full = [&](int s) { return aux + 8u * s; };
-    const uint32_t bar_s = aux + 16, bar_o = aux + 24, tmem_slot = aux + 32;
-    float* red = reinterpret_cast<float*>(smem_raw + (aux - raw) + 64);   // mx[2][128], rs[2][128]
-    float* rel = red + 4 * BQ;
+    float* rel = reinterpret_cast<float*>(smem_raw + (aux - raw) + 64);
     const int P = a.pos_max, NT = 2 * P + 1;
     float* cg = rel + NT;
 
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const int g = tid >> 7, r = tid & 127;                  // thread group (column half), query row = TMEM lane
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int g8 = lane >> 2, t4 = lane & 3;
     const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * BQ;
+    const int rq = (warp >> 2) * 64 + (warp & 3) * 16 + g8;  // this thread's query rows: rq, rq + 8 (tile-relative)
+    const int qa = q0 + rq, qb = qa + 8;
     const int ntiles = (a.Lk + BKV - 1) / BKV;
 
     pdl_trigger();
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) mbar_init(bar_full(s), 1);
-        mbar_init(bar_s, 1);
-        mbar_init(bar_o, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fence_before();
     __syncthreads();
-    fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-    const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
     pdl_wait();
 
     // raw K / V head slices of key tile t -> stage t % STAGES (keys >= Lk and channels >= H*D arrive as zeros)
@@ -205,40 +159,37 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
         rel[t] = a.relpos[t * a.H + h] * a.scale;      // (s + rel) * scale == fma(s, scale, rel * scale) up to one rounding
         cg[t] = a.cgain[t * a.H + h];
     }
-    // ---- Q row half -> q_hi / q_lo in tensor memory --------------------------------------------------------
-    const int qi = q0 + r;
+    // ---- Q rows -> q_hi / q_lo A fragments (a[0] row g col t, a[1] row g+8 col t, a[2] row g col t+4, a[3] row g+8 col t+4) ----
+    uint32_t qhi[KD][4], qlo[KD][4];
     {
-        const float* qp = a.q + ((int64_t)b * a.Lq + qi) * a.ldq + h * D + g * HC;
+        const float* qpa = a.q + ((int64_t)b * a.Lq + qa) * a.ldq + h * D;
+        const float* qpb = a.q + ((int64_t)b * a.Lq + qb) * a.ldq + h * D;
 #pragma unroll
-        for (int c = 0; c < HC / 8; ++c) {
-            float hi[8], lo[8];
-            float4 x0 = make_float4(0.f, 0.f, 0.f, 0.f), x1 = x0;
-            if (qi < a.Lq) { x0 = ld_f4(qp + c * 8); x1 = ld_f4(qp + c * 8 + 4); }
-            const float x[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+        for (int kk = 0; kk < KD; ++kk) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) { hi[j] = to_tf32(x[j]); lo[j] = to_tf32(x[j] - hi[j]); }
-            tmem_st8(lane_addr + TM_QHI + g * HC + c * 8, hi);
-            tmem_st8(lane_addr + TM_QLO + g * HC + c * 8, lo);
+            for (int e = 0; e < 4; ++e) {
+                const int c = kk * 8 + t4 + (e >> 1) * 4;
+                const bool rb = e & 1;
+                float x = 0.f;
+                if ((rb ? qb : qa) < a.Lq) x = (rb ? qpb : qpa)[c];
+                const float hi = to_tf32(x);
+                qhi[kk][e] = __float_as_uint(hi);
+                qlo[kk][e] = __float_as_uint(to_tf32(x - hi));
+            }
         }
-        tmem_wait_st();
     }
-    float m_i = -INFINITY, l_i = 0.f, o[HC];
+    float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f, o[NO];
 #pragma unroll
-    for (int c = 0; c < HC; ++c) o[c] = 0.f;
-    // instruction descriptor: D=F32 [4,6)=1, A=TF32 [7,10)=2, B=TF32 [10,13)=2, K-major A/B, N>>3 at [17,23), M>>4 at [24,29)
-    const uint32_t idesc0 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BQ >> 4) << 24);
-    uint32_t ph = 0;
+    for (int c = 0; c < NO; ++c) o[c] = 0.f;
 
     for (int t = 0; t < ntiles; ++t) {
         const int s = t % STAGES;
         const int j0 = t * BKV;
         const int nk = min(BKV, a.Lk - j0);
-        const int NK = (nk + 15) & ~15;                     // MMA N (S) and K extent (PV): padded keys are zero / masked
         mbar_wait(bar_full(s), (uint32_t)(t / STAGES) & 1u);
-        // ---- key tile: raw -> k_hi in place, k_lo beside it (elementwise, so swizzle-agnostic) -------------------
+        // ---- key tile: raw -> k_hi in place, k_lo beside it (elementwise, so swizzle-agnostic); keys past Lk -> 0 -------------
         for (int f = tid; f < S::KSLABS * 1024; f += THREADS) {
             const int row = (f & 1023) >> 3;                // key within the tile
-            if (row >= NK) continue;
             float4 x = lds_f4(k_hi(s) + (uint32_t)f * 16u);
             if (row >= nk) x = make_float4(0.f, 0.f, 0.f, 0.f);
             float4 hi, lo;
@@ -247,40 +198,35 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
             sts_f4(k_hi(s) + (uint32_t)f * 16u, hi);
             sts_f4(k_lo + (uint32_t)f * 16u, lo);
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to the MMA / TMA
-        fence_before();
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to the tensor cores
         __syncthreads();
-        // ---- S = Q K^T ----------------------------------------------------------------------------------------
-        if (warp == 0) {
-            fence_after();
-            if (elect_one()) {
-            const uint32_t idesc = idesc0 | ((uint32_t)(NK >> 3) << 17);
+        // ---- S = Q K^T (asynchronous: the value tile is prepared meanwhile) ---------------------------------------------------
+        float sacc[BKV / 2];
 #pragma unroll
-            for (int kk = 0; kk < D / 8; ++kk) {
-                const uint32_t so = (uint32_t)(kk >> 2) * SLAB;
-                const uint64_t ko = (uint64_t)((kk & 3) * 2);          // 8 channels = 32 bytes = 2 x 16-byte units
-                const uint64_t dh = umma_desc_kmajor(k_hi(s) + so) + ko, dl = umma_desc_kmajor(k_lo + so) + ko;
-                umma_tf32_ts(tmem_base + TM_S, tmem_base + TM_QLO + kk * 8, dh, idesc, kk > 0 ? 1u : 0u);
-                umma_tf32_ts(tmem_base + TM_S, tmem_base + TM_QHI + kk * 8, dl, idesc, 1u);
-                umma_tf32_ts(tmem_base + TM_S, tmem_base + TM_QHI + kk * 8, dh, idesc, 1u);
-            }
-            umma_commit(bar_s);
-            }
-            __syncwarp();
+        for (int j = 0; j < BKV / 2; ++j) sacc[j] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < KD; ++kk) {
+            const uint32_t so = (uint32_t)(kk >> 2) * SLAB;
+            const uint64_t ko = (uint64_t)((kk & 3) * 2);          // 8 channels = 32 bytes = 2 x 16-byte units
+            const uint64_t dh = wgmma_desc(k_hi(s) + so) + ko, dl = wgmma_desc(k_lo + so) + ko;
+            Wgmma<BKV>::mma(sacc, qlo[kk], dh);
+            Wgmma<BKV>::mma(sacc, qhi[kk], dl);
+            Wgmma<BKV>::mma(sacc, qhi[kk], dh);
         }
-        // ---- value tile (needed by the SECOND contraction only, so it is prepared while the tensor cores work on S): split + transpose
-        // into V^T (row = channel, 32-key slabs).  One warp step = 32 keys x one 16-byte channel chunk: the reads hit 8 distinct
-        // swizzled chunks per quarter warp and the 32 lanes of each scalar store fill one 128-byte row, so both sides are
-        // bank-conflict free.
-        for (int it = warp; it < D; it += THREADS / 32) {
+        wgmma_commit();
+        // ---- value tile: split + transpose into V^T (row = channel, 32-key slabs; keys of each 8-group stored 0 2 4 6 1 3 5 7).
+        // One warp step = 32 keys x one 16-byte channel chunk: the reads hit 8 distinct swizzled chunks per quarter warp and the
+        // 32 lanes of each scalar store fill one 128-byte row, so both sides are bank-conflict free.
+        for (int it = warp; it < (BKV / 32) * (D / 4); it += THREADS / 32) {
             const int kg = it / (D / 4), c = it - kg * (D / 4);
-            const int key = kg * 32 + (tid & 31);
-            if (key >= NK) continue;
+            const int key = kg * 32 + lane;
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
             if (key < nk) x = lds_f4(v_raw(s) + (uint32_t)(c >> 3) * SLAB + (uint32_t)key * 128u + (uint32_t)(((c & 7) ^ (key & 7)) << 4));
             const float xs[4] = {x.x, x.y, x.z, x.w};
-            const uint32_t col = (uint32_t)kg * S::VT_SLAB + (uint32_t)((key & 3) << 2);
-            const int kc = (key & 31) >> 2;                 // 16-byte chunk of this key inside its 32-key slab row
+            const int kp = (lane & 24) | ((lane & 1) << 2) | ((lane & 7) >> 1);   // position of the key inside its 32-key slab row
+            const uint32_t col = (uint32_t)kg * S::VT_SLAB + (uint32_t)((kp & 3) << 2);
+            const int kc = kp >> 2;                         // 16-byte chunk of this key inside its 32-key slab row
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const int d = c * 4 + j;
@@ -290,121 +236,89 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
                 sts_f1(vt_lo + off, lo);
             }
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // V^T writes -> visible to the PV MMAs (issued behind the next barriers)
-        mbar_wait(bar_s, ph);
-        fence_after();
-        // ---- bias, scale, mask, online softmax on this thread's half of the row (logits stay in registers) -------
-        const int split = min(NK, ((NK >> 4) + 1) / 2 * 16);
-        const int c_lo = g == 0 ? 0 : split, c_hi = g == 0 ? split : NK;
-        float sv[64];
-        float mx = -INFINITY;
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // V^T writes -> visible to the P V MMAs (behind the barrier below)
+        wgmma_wait<0>();
+        if (dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && t == 0) {       // logits 0..15 of row rq
+            for (int j = 0; j < 4; ++j) dbg[rq * 40 + (j >> 1) * 8 + 2 * t4 + (j & 1)] = sacc[(j >> 1) * 4 + (j & 1)];
+        }
+        // ---- bias, scale, mask, online softmax (row rq: even/odd sacc of each quad, row rq + 8: the other two) ----------------
+        float mxa = -INFINITY, mxb = -INFINITY;
 #pragma unroll
-        for (int ci = 0; ci < 4; ++ci) {
-            const int c0 = c_lo + ci * 16;
-            if (c0 < c_hi) {                                // uniform over the warp (g, NK are)
-                float v[16];
-                tmem_ld8(lane_addr + TM_S + c0, v);
-                tmem_ld8(lane_addr + TM_S + c0 + 8, v + 8);
-                tmem_wait_ld();
-                if (dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && t == 0 && g == 0 && ci == 0) {
-                    for (int j = 0; j < 16; ++j) dbg[r * 40 + j] = v[j];
-                    const float4 vv = lds_f4(vt_hi + (r & 63) * 128), kv = lds_f4(k_hi(s) + r * 128);
-                    dbg[r * 40 + 26] = vv.x; dbg[r * 40 + 27] = vv.y; dbg[r * 40 + 28] = vv.z; dbg[r * 40 + 29] = vv.w;
-                    dbg[r * 40 + 30] = kv.x; dbg[r * 40 + 31] = kv.y; dbg[r * 40 + 32] = kv.z; dbg[r * 40 + 33] = kv.w;
-                }
+        for (int j = 0; j < BKV / 8; ++j) {
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int kj = j0 + c0 + j;
+            for (int e = 0; e < 4; ++e) {
+                const int kj = j0 + j * 8 + 2 * t4 + (e & 1);
+                const int qi = (e & 2) ? qb : qa;
+                const int idx = max(-P, min(P, kj - qi)) + P;
+                const float sc = (kj < a.Lk) ? fmaf(sacc[4 * j + e], a.scale, rel[idx]) : -INFINITY;
+                sacc[4 * j + e] = sc;
+                if (e & 2) mxb = fmaxf(mxb, sc); else mxa = fmaxf(mxa, sc);
+            }
+        }
+        mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, 1)); mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, 2));
+        mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, 1)); mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, 2));
+        const float mna = fmaxf(m_a, mxa), mnb = fmaxf(m_b, mxb);      // finite: key j0 is always valid
+        const float ca = expf(m_a - mna), cb = expf(m_b - mnb);
+        m_a = mna; m_b = mnb;
+        l_a *= ca; l_b *= cb;
+#pragma unroll
+        for (int j = 0; j < NO / 4; ++j) { o[4 * j] *= ca; o[4 * j + 1] *= ca; o[4 * j + 2] *= cb; o[4 * j + 3] *= cb; }
+        __syncthreads();                                    // V^T of this tile complete
+        // ---- O += P V, in two halves of the key tile (half the P fragments live at a time) ---------------------------------------
+        // P * gain as hi / lo A fragments of k8 chunk j: a[0] = (row g, key 2t) = sacc[4j], a[1] = (g+8, 2t) = sacc[4j+2],
+        // a[2] = (g, 2t+1) = sacc[4j+1], a[3] = (g+8, 2t+1) = sacc[4j+3] -- V^T holds its keys in the matching order
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            if (half * (BKV / 2) >= nk) break;              // uniform: keys past the last one contribute zeros
+            uint32_t phi[BKV / 16][4], plo[BKV / 16][4];
+#pragma unroll
+            for (int jj = 0; jj < BKV / 16; ++jj) {
+                const int j = half * (BKV / 16) + jj;
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int src = 4 * j + ((e & 1) << 1) + (e >> 1);
+                    const bool rb = e & 1;
+                    const int kj = j0 + j * 8 + 2 * t4 + (e >> 1);
+                    const int qi = rb ? qb : qa;
                     const int idx = max(-P, min(P, kj - qi)) + P;
-                    const float sc = (kj < a.Lk) ? fmaf(v[j], a.scale, rel[idx]) : -INFINITY;
-                    sv[ci * 16 + j] = sc;
-                    mx = fmaxf(mx, sc);
-                }
-            }
-        }
-        red[g * BQ + r] = mx;
-        __syncthreads();
-        const float mnew = fmaxf(m_i, fmaxf(red[r], red[BQ + r]));     // finite: key j0 is always valid
-        const float corr = expf(m_i - mnew);
-        float rs = 0.f;
-#pragma unroll
-        for (int ci = 0; ci < 4; ++ci) {
-            const int c0 = c_lo + ci * 16;
-            if (c0 < c_hi) {
-                float phi[16], plo[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int idx = max(-P, min(P, j0 + c0 + j - qi)) + P;
-                    const float pe = expf(sv[ci * 16 + j] - mnew);      // 0 for masked keys
-                    rs += pe;
+                    const float pe = expf(sacc[src] - (rb ? mnb : mna));       // 0 for masked keys
+                    if (rb) l_b += pe; else l_a += pe;
                     const float pg = pe * cg[idx];
-                    phi[j] = to_tf32(pg);
-                    plo[j] = to_tf32(pg - phi[j]);
+                    const float hi = to_tf32(pg);
+                    phi[jj][e] = __float_as_uint(hi);
+                    plo[jj][e] = __float_as_uint(to_tf32(pg - hi));
                 }
-                tmem_st8(lane_addr + TM_S + c0, phi);                   // p_hi overwrites the logits it was made from
-                tmem_st8(lane_addr + TM_S + c0 + 8, phi + 8);
-                tmem_st8(lane_addr + TM_PLO + c0, plo);
-                tmem_st8(lane_addr + TM_PLO + c0 + 8, plo + 8);
             }
+            wgmma_fence();
+#pragma unroll
+            for (int jj = 0; jj < BKV / 16; ++jj) {
+                const int j = half * (BKV / 16) + jj;
+                const uint32_t so = (uint32_t)(j >> 2) * S::VT_SLAB;
+                const uint64_t ko = (uint64_t)((j & 3) * 2);       // 8 keys = 32 bytes = 2 x 16-byte units
+                const uint64_t dh = wgmma_desc(vt_hi + so) + ko, dl = wgmma_desc(vt_lo + so) + ko;
+                Wgmma<D>::mma(o, plo[jj], dh);
+                Wgmma<D>::mma(o, phi[jj], dl);
+                Wgmma<D>::mma(o, phi[jj], dh);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
         }
-        tmem_wait_st();
-        red[2 * BQ + g * BQ + r] = rs;
-        fence_before();
-        __syncthreads();
-        l_i = l_i * corr + (red[2 * BQ + r] + red[3 * BQ + r]);
-        m_i = mnew;
-        // ---- O_tile = P V ----------------------------------------------------------------------------------------
-        if (warp == 0) {
-            fence_after();
-            if (elect_one()) {
-            const uint32_t idesc = idesc0 | ((uint32_t)(D >> 3) << 17);
-            for (int kk = 0; kk < NK / 8; ++kk) {
-                const uint32_t so = (uint32_t)(kk >> 2) * S::VT_SLAB;
-                const uint64_t ko = (uint64_t)((kk & 3) * 2);           // 8 keys = 32 bytes = 2 x 16-byte units
-                const uint64_t dh = umma_desc_kmajor(vt_hi + so) + ko, dl = umma_desc_kmajor(vt_lo + so) + ko;
-                umma_tf32_ts(tmem_base + TM_O, tmem_base + TM_PLO + kk * 8, dh, idesc, kk > 0 ? 1u : 0u);
-                umma_tf32_ts(tmem_base + TM_O, tmem_base + TM_S + kk * 8, dl, idesc, 1u);
-                umma_tf32_ts(tmem_base + TM_O, tmem_base + TM_S + kk * 8, dh, idesc, 1u);
-            }
-            umma_commit(bar_o);
-            }
-            __syncwarp();
-        }
-        mbar_wait(bar_o, ph);
-        fence_after();
-        // every MMA that read stage s has retired: refill it (the split's generic writes were fenced above)
+        __syncthreads();                                    // every MMA that read stage s, k_lo and V^T has retired
         if (warp == 0 && t + STAGES < ntiles) {
-            __syncwarp();
             if (elect_one()) issue_tile(t + STAGES);
             __syncwarp();
         }
-#pragma unroll
-        for (int c = 0; c < HC / 8; ++c) {
-            float ot[8];
-            tmem_ld8(lane_addr + TM_O + g * HC + c * 8, ot);
-            tmem_wait_ld();
-            if (dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && t == 0 && g == 0 && c == 0) {
-                for (int j = 0; j < 8; ++j) dbg[r * 40 + 16 + j] = ot[j];
-                dbg[r * 40 + 24] = m_i; dbg[r * 40 + 25] = l_i;
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[c * 8 + j] = fmaf(o[c * 8 + j], corr, ot[j]);
-        }
-        ph ^= 1u;
-        fence_before();                                     // orders these TMEM reads before the next tile's MMAs
     }
-    if (qi < a.Lq) {
-        const float inv = 1.0f / l_i;
-        float* op = a.o + ((int64_t)b * a.Lq + qi) * a.ldo + h * D + g * HC;
+    l_a += __shfl_xor_sync(0xffffffffu, l_a, 1); l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
+    l_b += __shfl_xor_sync(0xffffffffu, l_b, 1); l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
+    const float ia = 1.0f / l_a, ib = 1.0f / l_b;
+    float* opa = a.o + ((int64_t)b * a.Lq + qa) * a.ldo + h * D;
+    float* opb = a.o + ((int64_t)b * a.Lq + qb) * a.ldo + h * D;
 #pragma unroll
-        for (int c = 0; c < HC / 4; ++c)
-            st_f4(op + c * 4, make_float4(o[c * 4] * inv, o[c * 4 + 1] * inv, o[c * 4 + 2] * inv, o[c * 4 + 3] * inv));
-    }
-    fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TM_COLS) : "memory");
+    for (int j = 0; j < NO / 4; ++j) {
+        const int c = j * 8 + 2 * t4;
+        if (qa < a.Lq) *reinterpret_cast<float2*>(opa + c) = make_float2(o[4 * j] * ia, o[4 * j + 1] * ia);
+        if (qb < a.Lq) *reinterpret_cast<float2*>(opb + c) = make_float2(o[4 * j + 2] * ib, o[4 * j + 3] * ib);
     }
 }
 
@@ -436,7 +350,7 @@ static int encode_kv(EncodeTiledFn enc, CUtensorMap* tm, const float* p, int64_t
     return MUGD_OK;
 }
 
-static float* g_dbg = nullptr;      // debugging aid: CTA (0,0,0) dumps 40 floats per query row of its first key tile
+static float* g_dbg = nullptr;      // debugging aid: CTA (0,0,0) dumps the raw logits of its first key tile (16 of each row's 40 floats)
 
 template <int D>
 static int launch(const mugd_attention& a, cudaStream_t st) {

@@ -1,4 +1,4 @@
-// Shared host/device helpers of libmugd (sm_100a only).
+// Shared host/device helpers of libmugd (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,8 +9,8 @@
 
 #include "../../include/mugd.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libmugd is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libmugd is written for sm_90a (H100) only"
 #endif
 
 namespace mugd {
@@ -37,12 +37,12 @@ void set_error(const char* fmt, ...);
 
 struct DeviceInfo {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int cc_major = 0, cc_minor = 0;
     int max_smem_optin = 0;
-    // per-handle switches (round 1 kept these as process globals)
+    // per-handle switches
     int tc_single_pass = 0;     // opt-in plain-TF32 tensor-core products (NOT fp32-accurate; never used by parity tests / bench)
-    int attention_impl = 1;     // 1 = tcgen05 attention, 0 = exact-fp32 FFMA referee
+    int attention_impl = 1;     // 1 = wgmma attention, 0 = exact-fp32 FFMA referee
 };
 
 // per-family launchers (each validates its descriptor and enqueues kernels on `st`);
@@ -64,7 +64,7 @@ bool gemm_tc_supported(const mugd_gemm& g);
 
 // Programmatic dependent launch (PDL): every hot-path kernel is launched with the programmatic-stream-serialization
 // attribute, signals `launch_dependents` at entry and executes `griddepcontrol.wait` before its first global-memory
-// access.  The next kernel's launch latency and prologue (block scheduling, barrier init, TMEM allocation,
+// access.  The next kernel's launch latency and prologue (block scheduling, barrier init,
 // tensor-map fetch) then overlap the tail of the current one; data hazards are unchanged because the wait
 // only returns when the prerequisite grid has completed and flushed.
 extern bool g_use_pdl;
@@ -85,8 +85,8 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 // No kernel signals launch_dependents explicitly: the trigger is implicit at grid completion, so PDL only overlaps the dependent's
-// launch with this grid's memory flush (graph edge 0.57 us instead of 0.69 us, tools/experiments/sync_probe.cu).  Explicit triggers
-// (at entry, in the short kernels only, after the GEMM main loop) were measured slower in round 1 (DESIGN.md 4) and removed.
+// launch with this grid's memory flush.  Explicit triggers
+// (at entry, in the short kernels only, after the GEMM main loop) were tried and not kept.
 __device__ __forceinline__ void pdl_trigger() {}
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 

@@ -5,7 +5,7 @@
 //
 //   C[m, n] = epi( sum_{t < taps} sum_{k < K} A[row(m, t), k] * W[n, t*K + k] )
 //
-// This is the bit-faithful fp32 path (also the numerical referee for the tcgen05 3xTF32 kernel in
+// This is the bit-faithful fp32 path (also the numerical referee for the wgmma 3xTF32 kernel in
 // gemm_tc.cu).  Tiles 64x64 or 128x128, BK = 16, 256 threads, register-prefetch double buffering.
 //
 // Reference call sites: unet.py:153-157,174-181,187-193 (ResBlock convs/skip), attention.py:38-65,

@@ -1,4 +1,4 @@
-// tcgen05 implicit GEMM: stand-alone kernels + host side (geometry planner, tensor-map encoding, launch).
+// wgmma implicit GEMM: stand-alone kernels + host side (geometry planner, tensor-map encoding, launch).
 // The device code lives in gemm_tc.cuh (shared with other kernels that embed GEMM tiles).
 //
 // Reference call sites are the same as gemm_simt.cu (which remains the exact-fp32 referee and the fallback for
@@ -7,79 +7,28 @@
 
 namespace mugd {
 
-template <int BN, int EPI, int OCC = 1>
-__global__ void __launch_bounds__(TC_THREADS, OCC)
+template <int BN, int EPI>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA1,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmWhi,
                const __grid_constant__ CUtensorMap tmWlo, const __grid_constant__ TcParams p) {
-    using S = TcSmem<BN, OCC>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;       // SWIZZLE_128B needs 1024-B alignment
-    const TcBars<BN, OCC> B(base);
-    const int warp = threadIdx.x >> 5;
+    const TcBars<BN> B(base);
 #ifdef MUGD_TC_TIMELINE
     if (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0) p.dbg[0] = gtimer();
 #endif
-    // ---- one-time setup: barriers, tensor memory; nothing here touches memory written by the previous kernel ----
-    // The producer warp arms the barriers itself and starts fetching operands at once: it only ARRIVES at the setup rendezvous
-    // (named barrier 1), the other seven warps wait there for it and for the tensor-memory allocation.  The first TMA leaves
-    // ~0.8 us earlier than behind a CTA-wide __syncthreads (tools/gemm_timeline.py: setup took 0.86 us, first TMA at 1.4 us).
-    uint32_t tmem_base = 0;
-    if (warp == 0) {
+    // ---- one-time setup: barriers; nothing here touches memory written by the previous kernel ----
+    if (threadIdx.x < 32) {
         B.init_parallel((int)threadIdx.x);
-        __syncwarp();
-        asm volatile("bar.arrive 1, %0;" ::"n"(TC_THREADS) : "memory");
-    } else {
-        if (threadIdx.x >= 32 && threadIdx.x < 38) {
-            // warm the TMA descriptor cache while the barriers / tensor memory are set up
-            const CUtensorMap* m = threadIdx.x == 32 ? &tmA : threadIdx.x == 33 ? &tmA1 : threadIdx.x == 34 ? &tmA2
-                                 : threadIdx.x == 35 ? &tmB : threadIdx.x == 36 ? &tmWhi : &tmWlo;
-            asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
-        }
-        if (warp == 2) {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(B.tmem_slot()), "r"((uint32_t)S::TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-            // Kernel parameters live in constant memory and a fresh launch misses on every 64-byte line it touches; the epilogue reads
-            // fields from five of them one after the other (tools/gemm_timeline.py: a bias-free 128x128 tile took 3.2 us to store
-            // against 1.0 us for a split-K partial, which reads two).  This otherwise idle warp touches every line of the block now, so
-            // that the misses overlap the main loop instead of stretching the epilogue.
-            constexpr int LINES = (int)((sizeof(TcParams) + 63) / 64);
-            const int* pw = reinterpret_cast<const int*>(&p);
-#pragma unroll
-            for (int k = 0; k < LINES; ++k) {
-                const int v = pw[k * 16];
-                asm volatile("" ::"r"(v));
-            }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        asm volatile("bar.sync 1, %0;" ::"n"(TC_THREADS) : "memory");
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(B.tmem_slot()));
-        // the producer warp waits for the previous kernel (griddepcontrol.wait) before its first activation load; every other
-        // global access of this kernel (epilogue) is ordered behind data that went through that load
-        pdl_wait();
+    } else if (threadIdx.x < 38) {
+        // warm the TMA descriptor cache while the barriers are set up
+        const CUtensorMap* m = threadIdx.x == 32 ? &tmA : threadIdx.x == 33 ? &tmA1 : threadIdx.x == 34 ? &tmA2
+                             : threadIdx.x == 35 ? &tmB : threadIdx.x == 36 ? &tmWhi : &tmWlo;
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
     }
-    if constexpr (OCC == 2) {
-        // Two residents per SM, launched as at most 2 x SMs CTAs: a CTA walks the tile list with stride gridDim.x (consecutive CTAs
-        // take neighbouring column tiles of one row band: the band's activations are fetched once into L2) and keeps its tensor
-        // memory, its tensor-map cache lines and its warm instruction cache from tile to tile; the barrier rings keep turning
-        // (it0 / acc_phase of gemm_tc_tile), nothing is re-armed.
-        const int n_tiles = p.gx * p.gy;
-        int done = 0;
-        for (int tile = (int)blockIdx.x; tile < n_tiles; tile += (int)gridDim.x, ++done) {
-            gemm_tc_tile<BN, true, EPI, OCC>(&tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p, tile % p.gx, tile / p.gx, 0, base, tmem_base,
-                                             done * p.hot.total_it, (uint32_t)done & 1u);
-            __syncthreads();         // the staged tile has been read: the next tile's TMA may overwrite the pipeline buffers
-        }
-    } else {
-        gemm_tc_tile<BN, true, EPI, OCC>(&tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p, blockIdx.x, blockIdx.y, blockIdx.z, base, tmem_base);
-    }
-    // ---- teardown (all tcgen05.ld completed before the phase-2 barrier inside the tile function) ----
     __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)S::TMEM_COLS) : "memory");
-    }
+    gemm_tc_tile<BN, true, EPI>(&tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p, blockIdx.x, blockIdx.y, blockIdx.z, base);
 }
 
 // split-K second pass: fully parallel over the GPU and L2-resident (see tc_reduce_rows).
@@ -92,17 +41,10 @@ gemm_tc_reduce_kernel(const __grid_constant__ TcParams p) {
 #ifdef MUGD_TC_TIMELINE
 static long long* g_tc_dbg = nullptr;
 #endif
-// planner constants: us per k-step of a 128- / 256-wide tile (tools/bench_gemm.py), us per split-K round trip (workspace + reduce
-// launch).  The split cost was 4.0 in round 1; with the slimmer kernels of round 2 the sweep (tools/experiments/sweep_cost.sh:
-// 299 / 303 / 312 / 312 steps/s at 5.0 / 4.0 / 3.0 / 2.0) favours splitting a little more.  mugd_debug_set_tc_cost for sweeps
-// The two-CTAs-per-SM variant (TcSmem<128, 2>) is taken when its estimate -- tiles per SM x k-steps x the 128-wide k-step, two residents
-// sharing one tensor pipe -- beats the best single-resident estimate by more than g_tc_cost[3].  That constant is a CREDIT (negative):
-// the single-resident estimates carry 1.0 us of fill per wave because only their differences matter to the split decision, while a
-// wave really exposes ~7 us of prologue + accumulator drain that two residents hide behind each other's main loop.  Fitted on the
-// per-op tables of Beff = 64 / L = 512 and Beff = 16 / L = 992 (tools/compare_ops.py): every GEMM it picks was measured faster
-// (0.71-0.98x), the ones it leaves alone (fewer tiles than SMs, or long K with < 2 tiles per SM) were slower or even.
-static float g_tc_cost[4] = {0.55f, 0.9f, 3.0f, -6.5f};
-static int g_tc_force_bn = 0;        // experiments: 0 = cost model, 64 / 128 / 256 = force the tile width where legal
+// planner constants: us per k-step of a 128-wide tile, (unused) second tile-width slot, us per split-K round trip (workspace + reduce
+// launch), (unused) fourth slot.  They are relative weights of the tile-width / K-split decision; mugd_debug_set_tc_cost for sweeps.
+static float g_tc_cost[4] = {0.55f, 0.9f, 3.0f, 0.f};
+static int g_tc_force_bn = 0;        // experiments: 0 = cost model, 64 / 128 = force the tile width where legal
 
 // =====================================================================================================
 // host side
@@ -154,7 +96,6 @@ static int tc_validate_fusions(const mugd_gemm& g) {
 TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split) {
     TcGeometry t;
     t.BN = (g.N >= 128) ? 128 : 64;
-    t.occ = 1;
     if (g.conv_mode == MUGD_CONV_NONE) { t.Lrows = g.M; t.Bs = 1; }
     else { t.Lrows = g.Lout; t.Bs = g.M / g.Lout; }
     if (t.Lrows >= TC_BM) {
@@ -169,40 +110,28 @@ TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split) {
         t.gy = (t.Bs + t.box_b - 1) / t.box_b;
     }
     t.total_it = g.taps * (g.K / TC_BK) + g.K2 / TC_BK;
-    // Cost model from the B200 micro-benchmark (tools/bench_gemm.py): a CTA needs ~1 us to fill its pipeline and
-    // ~0.55 us per k-step with 128-wide tiles (~0.9 us with 256-wide tiles, which do twice the math per step);
-    // splitting K adds the workspace round trip and a second (reduce) launch, ~4 us.
-    // Candidates: tile width 64 for narrow N, 128, 256 when N allows it, each with its best K split.
+    // Cost model: a CTA needs ~1 unit to fill its pipeline and g_tc_cost[0] per k-step of a 128-wide tile (0.4 with 64-wide tiles);
+    // splitting K adds the workspace round trip and a second (reduce) launch, g_tc_cost[2].
+    // Candidates: tile width 64 (narrow N, or forced), 128 when N allows it, each with its best K split.
     int splits = 1;
     float best = 1e30f;
-    static const int cands[4] = {64, 128, 256, 130 /* 128 wide, two CTAs per SM */};
-    for (int cand = 0; cand < 4; ++cand) {
-        const int code = cands[cand];
-        const int bn = code == 130 ? 128 : code;
-        const int occ = code == 130 ? 2 : 1;
+    static const int cands[2] = {64, 128};
+    for (int cand = 0; cand < 2; ++cand) {
+        const int bn = cands[cand];
         if (bn > 64 && g.N < bn) continue;
         if (bn == 64 && g.N >= 128 && g_tc_force_bn != 64) continue;
-        if (g_tc_force_bn && code != g_tc_force_bn && !((g_tc_force_bn == 256 ? 256 : 128) > g.N && code == (g.N >= 128 ? 128 : 64))) continue;
+        if (g_tc_force_bn && bn != g_tc_force_bn && !(g_tc_force_bn > g.N && bn == 64)) continue;
         const int gx = (g.N + bn - 1) / bn;
         const int tiles = gx * t.gy;
-        if (occ == 2) {
-            // two residents per SM share one tensor pipe: n tiles per SM back to back, one exposed prologue + epilogue
-            if (forced_split > 1 || (tiles <= sm_count && g_tc_force_bn != 130)) continue;
-            const int n = (tiles + sm_count - 1) / sm_count;
-            const float est = g_tc_cost[3] + n * g_tc_cost[0] * t.total_it;
-            if (est < best - 0.25f || g_tc_force_bn == 130) { best = est; splits = 1; t.BN = 128; t.occ = 2; }
-            continue;
-        }
-        const float kstep = bn == 256 ? g_tc_cost[1] : (bn == 128 ? g_tc_cost[0] : 0.4f);
-        // 256-wide tiles only pay off unsplit (measured: l1/l2 FF1 and the B=64 convs gain 15-25 %, split cases lose)
-        const int sp_max = forced_split > 0 ? forced_split : ((tiles < sm_count && bn != 256) ? 16 : 1);
+        const float kstep = bn == 128 ? g_tc_cost[0] : 0.4f;
+        const int sp_max = forced_split > 0 ? forced_split : (tiles < sm_count ? 16 : 1);
         for (int sp = forced_split > 0 ? forced_split : 1; sp <= sp_max && sp <= t.total_it; ++sp) {
             const int per = (t.total_it + sp - 1) / sp;
             if (forced_split <= 0 && sp > 1 && per < 2) break;
             if (forced_split <= 0 && sp > 1 && tiles * sp > 2 * sm_count) break;   // bounds the workspace: < 2*SMs partial tiles
             const int waves = (tiles * sp + sm_count - 1) / sm_count;
             const float est = waves * (1.0f + kstep * per) + (sp > 1 ? g_tc_cost[2] : 0.0f);
-            if (est < best - 0.25f) { best = est; splits = sp; t.BN = bn; t.occ = 1; }
+            if (est < best - 0.25f) { best = est; splits = sp; t.BN = bn; }
         }
     }
     t.gx = (g.N + t.BN - 1) / t.BN;
@@ -284,7 +213,6 @@ int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, TcPlanned* out) {
     p.tiles_per_sample = t.tiles_per_sample;
     p.single_pass = dev.tc_single_pass ? 1 : 0;
     p.BN = t.BN;
-    p.occ = t.occ;
     p.sm_count = dev.sm_count;
     p.gx = t.gx;
     p.gy = t.gy;
@@ -314,21 +242,6 @@ static int tc_launch(const TcPlanned& pl, cudaStream_t st) {
         MUGD_CHECK_CUDA(launch_k(gemm_tc_reduce_kernel<BN, EPI>, dim3((unsigned)(p.gx * p.gy * TcReduceGeom<BN>::BPT)), dim3(TC_THREADS), 0, st, p));
         return MUGD_OK;
     }
-    if constexpr (BN == 128) {
-        if (p.occ == 2) {
-            static bool configured2 = false;
-            if (!configured2) {
-                MUGD_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcSmem<BN, 2>::TOTAL));
-                MUGD_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, 2>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-                configured2 = true;
-            }
-            const int n_tiles = p.gx * p.gy;
-            const int ctas = n_tiles < 2 * p.sm_count ? n_tiles : 2 * p.sm_count;
-            MUGD_CHECK_CUDA(launch_k(gemm_tc_kernel<BN, EPI, 2>, dim3(ctas, 1, 1), dim3(TC_THREADS), TcSmem<BN, 2>::TOTAL, st, pl.maps[0], pl.maps[1],
-                                     pl.maps[2], pl.maps[3], pl.maps[4], pl.maps[5], p));
-            return MUGD_OK;
-        }
-    }
     static bool configured = false;
     if (!configured) {
         MUGD_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcSmem<BN>::TOTAL));
@@ -357,8 +270,7 @@ int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, cudaStream_t st, i
     TcPlanned pl;
     int rc = tc_plan(dev, g, &pl);
     if (rc != MUGD_OK) return rc;
-    if (pl.p.BN == 256) rc = tc_launch_bn<256>(pl, st);
-    else if (pl.p.BN == 128) rc = tc_launch_bn<128>(pl, st);
+    if (pl.p.BN == 128) rc = tc_launch_bn<128>(pl, st);
     else rc = tc_launch_bn<64>(pl, st);
     if (rc != MUGD_OK) return rc;
     if (launches) *launches += pl.p.splits > 1 ? 2 : 1;
@@ -368,7 +280,7 @@ int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, cudaStream_t st, i
 }  // namespace mugd
 
 extern "C" int mugd_debug_set_tc_cost(float kstep128_us, float kstep256_us, float split_us, float two_cta_fixed_us) {
-    if (two_cta_fixed_us != 0.f) mugd::g_tc_cost[3] = two_cta_fixed_us;      // may be negative (a credit); 1e9 = never
+    if (two_cta_fixed_us != 0.f) mugd::g_tc_cost[3] = two_cta_fixed_us;
     if (kstep128_us > 0.f) mugd::g_tc_cost[0] = kstep128_us;
     if (kstep256_us > 0.f) mugd::g_tc_cost[1] = kstep256_us;
     if (split_us > 0.f) mugd::g_tc_cost[2] = split_us;
@@ -376,7 +288,7 @@ extern "C" int mugd_debug_set_tc_cost(float kstep128_us, float kstep256_us, floa
 }
 
 extern "C" int mugd_debug_set_tc_tile_n(int bn) {
-    mugd::g_tc_force_bn = (bn == 64 || bn == 128 || bn == 256 || bn == 130 /* 128 wide, two CTAs per SM */) ? bn : 0;
+    mugd::g_tc_force_bn = (bn == 64 || bn == 128) ? bn : 0;
     return MUGD_OK;
 }
 
@@ -400,12 +312,12 @@ extern "C" int mugd_gemm_tc_variant(const mugd_gemm* g, int32_t sm_count, int32_
         if (grid_ctas) *grid_ctas = 0;
         return MUGD_OK;
     }
-    const int sms = sm_count > 0 ? sm_count : 148;
+    const int sms = sm_count > 0 ? sm_count : 132;
     const TcGeometry t = tc_geometry(*g, sms, g->split_k);
     const int tiles = t.gx * t.gy;
     if (tile_n) *tile_n = t.BN;
-    if (ctas_per_sm) *ctas_per_sm = t.occ;
-    if (grid_ctas) *grid_ctas = t.occ == 2 ? (tiles < 2 * sms ? tiles : 2 * sms) : tiles * t.splits;
+    if (ctas_per_sm) *ctas_per_sm = 1;
+    if (grid_ctas) *grid_ctas = tiles * t.splits;
     return MUGD_OK;
 }
 
@@ -421,7 +333,7 @@ extern "C" int mugd_gemm_tc_query(mugd_handle*, const mugd_gemm* g, int32_t sm_c
         if (n_tiles) *n_tiles = 0;
         return MUGD_OK;
     }
-    const TcGeometry t = tc_geometry(*g, sm_count > 0 ? sm_count : 148, g->split_k);
+    const TcGeometry t = tc_geometry(*g, sm_count > 0 ? sm_count : 132, g->split_k);
     if (splits) *splits = t.splits;
     if (workspace_bytes) *workspace_bytes = t.ws_floats * 4;
     if (n_tiles) *n_tiles = t.gx * t.gy;

@@ -24,7 +24,7 @@ __device__ __forceinline__ void gn_block_stats(double s, double ss, double inv_n
     if (lane == 0) { red[0][warp] = s; red[1][warp] = ss; }
     __syncthreads();
     // every thread adds the eight warp partials itself (broadcast reads, same order everywhere): one barrier instead of
-    // barrier -> thread 0 -> barrier on the critical path of a 3 us kernel
+    // barrier -> thread 0 -> barrier on the critical path of a short kernel
     double ts = 0.0, tss = 0.0;
 #pragma unroll
     for (int w = 0; w < GN_THREADS / 32; ++w) { ts += red[0][w]; tss += red[1][w]; }
@@ -144,8 +144,7 @@ groupnorm_silu_kernel(const float* __restrict__ x, int64_t ldx, float* __restric
 }
 
 // A second form -- one thread-block CLUSTER per sample, CTAs owning bands of whole rows (fully coalesced, gamma / beta per thread,
-// band moments exchanged through distributed shared memory) -- was built and measured in round 2 and lost almost everywhere
-// (profiles/r02_groupnorm_ab.md: 0.30 -> 0.49 ms per step at Beff = 8, 1.29 -> 1.36 at Beff = 64, 0.77 -> 1.03 at L = 992): inside the
+// band moments exchanged through distributed shared memory) -- was built, measured and lost almost everywhere: inside the
 // graph the slabs come out of L2, where the 16..48-byte pieces of this kernel cost little, while two cluster barriers + the DSMEM
 // exchange sit on every launch's critical path.  Removed.
 int launch_groupnorm(const DeviceInfo&, const mugd_groupnorm& g, cudaStream_t st, int* launches) {

@@ -140,8 +140,7 @@ int launch_s4conv(const DeviceInfo& dev, const mugd_s4conv& s, cudaStream_t st, 
     int nsplit = 1;
     // A pair of super blocks is the unit of work (constant cost).  Output blocks are split over more CTAs while every worker (warp) still
     // gets two pairs -- and, as long as there are fewer CTAs than SMs, even when the doubled CTAs leave half of their warps without
-    // a pair: the busy warps then share a scheduler with fewer others (Beff = 8, L = 512, H = 128: 64 -> 128 CTAs, 20.3 -> 13.6 us;
-    // with the machine already full the same step costs time: Beff = 16, L = 496: 37.2 -> 39.8 us).
+    // a pair: the busy warps then share a scheduler with fewer others; with the machine already full the same step costs time.
     while (nsplit < 16 && ((base * nsplit < 2 * dev.sm_count && nsplit * 2 * S4_WARPS <= npairs) ||
                            (base * nsplit < dev.sm_count && nsplit * S4_WARPS <= npairs)))
         nsplit *= 2;

@@ -1,4 +1,4 @@
-"""Launch-plan compiler and runtime of the B200 sampler.
+"""Launch-plan compiler and runtime of the H100 sampler.
 
 ``MugEngine`` owns a libmugd handle and the packed weight blob on one GPU.  ``Session`` is the compiled
 state for one (effective batch, z_length): an activation arena, the S4 convolution kernels for that
@@ -227,8 +227,8 @@ class UNetCompiler:
 
     def compile(self, arena: Arena, Beff: int, Lz: int, ext: Dict[str, int], per_sample_t: bool, fold_ln: Optional[bool] = None) -> dict:
         """fold_ln: every LayerNorm of the transformer blocks is folded into the Linear behind it (the producer of its input delivers
-        the row moments, the Linear corrects in its epilogue; no LayerNorm kernel, the normalised tensor is never written).  Worth
-        1.2 % at Beff = 8 and -0.8 % at Beff = 64 (profiles/r02_norm_fusion_ab.md), so None = fold below 8192 token rows.
+        the row moments, the Linear corrects in its epilogue; no LayerNorm kernel, the normalised tensor is never written).  It gains
+        at small batches and loses slightly at large ones, so None = fold below 8192 token rows.
         False = stand-alone LayerNorm kernels (the referee path, and what the exact-fp32 FFMA GEMM uses)."""
         cfg = self.cfg
         ops = OpList(tc_weight_map(self.blob, self.wbase))

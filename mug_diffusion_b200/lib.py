@@ -1,7 +1,7 @@
 """ctypes binding of libmugd.so (the C ABI in include/mugd.h).
 
 There is no CPU fallback: importing this module without the built library, or creating an engine on a
-machine without an sm_100 GPU, raises.
+machine without an sm_90 GPU, raises.
 """
 from __future__ import annotations
 
@@ -176,7 +176,7 @@ def load() -> C.CDLL:
     # measurement switches for tuning sweeps (tools/); none of them changes results
     if os.environ.get("MUGD_TC_COST"):
         lib.mugd_debug_set_tc_cost(*([float(v) for v in os.environ["MUGD_TC_COST"].split(",")] + [0.0] * 4)[:4])
-    if os.environ.get("MUGD_TC_TILE"):                       # experiments: force the tile variant (64 / 128 / 256 / 130 = 128 x two CTAs per SM)
+    if os.environ.get("MUGD_TC_TILE"):                       # experiments: force the tile width (64 / 128)
         lib.mugd_debug_set_tc_tile_n(int(os.environ["MUGD_TC_TILE"]))
     if os.environ.get("MUGD_TC_BN"):
         lib.mugd_debug_set_tc_tile_n(int(os.environ["MUGD_TC_BN"]))

@@ -247,7 +247,7 @@ def pack_model(sd: Dict[str, torch.Tensor], ucfg: UNetConfig, dcfg: DecoderConfi
         pack_wave(blob, sd, wave_cfg or WaveConfig())
     # Tensor-core weights (K per tap % 32 == 0, N >= 16) get their TF32 hi / lo operands ON THE DEVICE, after the blob has been
     # uploaded or broadcast (MUGD_OP_TF32_SPLIT: hi over the plain weight, lo in a second buffer).  The host blob -- what is packed,
-    # stored and broadcast -- holds every weight once (0.56 GB; round 1 shipped W + W_hi + W_lo = 1.66 GB).
+    # stored and broadcast -- holds every weight once (0.56 GB, instead of W + W_hi + W_lo = 1.66 GB).
     blob.tc = []
     lo = 0
     for name in list(blob.entries):

@@ -67,7 +67,7 @@ class MugEngine:
                  device: Optional[torch.device] = None, gemm_impl: str = "auto", blob: Optional[WeightBlob] = None,
                  max_sessions: int = 4, fold_ln: Optional[bool] = None):
         if not torch.cuda.is_available():
-            raise L_.MugdError("mug_diffusion_b200 needs an sm_100 (B200) GPU; there is no CPU fallback")
+            raise L_.MugdError("mug_diffusion_b200 needs an sm_90 (H100) GPU; there is no CPU fallback")
         self.cfg = cfg or ModelConfig()
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         torch.cuda.set_device(self.device)

@@ -5,7 +5,7 @@ Reference: ``MelspectrogramScaleEncoder1D`` (mug/cond/wave.py:398-473, shipped c
 no time embedding) ; ContextualTransformer without context at the 3 coarsest levels]; returns the 10 level outputs, of which
 the U-Net consumes the last four (unet.py:527-543).  49.8 GFLOP per sample at T = 32768 frames, run once per request.
 
-Everything here reuses the hot-path kernels (tcgen05 GEMM with dilated-tap TMA addressing, GroupNorm+SiLU, LayerNorm,
+Everything here reuses the hot-path kernels (wgmma GEMM with dilated-tap TMA addressing, GroupNorm+SiLU, LayerNorm,
 attention) through launch plans; no new kernel was needed except the tap dilation in the GEMM addressing.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""End-to-end parity on the B200 through the reference-shaped surface (DDIMSampler.sample,
+"""End-to-end parity on the GPU through the reference-shaped surface (DDIMSampler.sample,
 model.model.forward, model.model.decode), against (a) the committed outputs of the UNMODIFIED reference
 (tests/golden/, made by tools/make_goldens.py) and (b) the CPU oracle on the same seeded inputs.
 

@@ -1,4 +1,4 @@
-"""tcgen05 3xTF32 GEMM (gemm_tc.cu) through the C ABI against an fp64 torch statement of the same contraction.
+"""wgmma 3xTF32 GEMM (gemm_tc.cu) through the C ABI against an fp64 torch statement of the same contraction.
 Tolerance 1e-5 of the output's max magnitude (the exact-fp32 FFMA kernel sits at ~1e-6; a single-pass TF32
 GEMM would be ~5e-4 and fails this test by construction)."""
 import math
@@ -45,7 +45,7 @@ def test_tf32_split_is_exact_enough():
 
 
 @pytest.mark.parametrize("M,K,N", [(256, 128, 128), (100, 256, 192), (300, 64, 64), (1024, 512, 1536), (4096, 128, 384), (37, 32, 64),
-                                   (4096, 128, 16), (700, 256, 40), (16384, 384, 3072)])     # narrow N (zero-filled weight rows), two-CTA variant
+                                   (4096, 128, 16), (700, 256, 40), (16384, 384, 3072)])     # narrow N (zero-filled weight rows), many waves
 def test_tc_linear(R, M, K, N):
     x, w, b = g("x", (M, K)), g("w", (N, K)) / math.sqrt(K), 0.1 * g("b", (N,))
     ref = F.linear(x.double(), w.double(), b.double())
@@ -167,8 +167,7 @@ def test_upsample_as_two_parity_gemms(R, impl, B, L, C):
 
 @pytest.mark.parametrize("kind", ["linear", "conv3"])
 def test_tc_oversubscribed_grid(R, kind):
-    """grids of several waves (more tiles than the 148 SMs, 256-wide tiles with the decoupled weight ring where N allows):
-    same numbers as the fp64 reference"""
+    """grids of several waves (more tiles than the 132 SMs): same numbers as the fp64 reference"""
     if kind == "linear":
         M, K, N = 296 * 128, 128, 256
         x, w, b = g("mcx", (M, K)), g("mcw", (N, K)) / math.sqrt(K), 0.1 * g("mcb", (N,))
@@ -229,55 +228,3 @@ def test_gemm_ff_out_composed(R, impl):
     ops.gemm(view(fc), ptr(wc), C, 4 * C, view(out), W_hi=ptr(hc), W_lo=ptr(lc), bias=ptr(bc), residual=view(xc), A2=view(hcc), impl=impl)
     R.run(ops)
     assert rel_err(out, ref) < TOL
-
-
-@pytest.mark.parametrize("case", ["linear_bias", "conv3_rowvec_residual", "geglu", "ragged"])
-def test_two_ctas_per_sm_variant_walks_its_tile_list(R, case):
-    """the 128-wide variant built for two CTAs per SM (TcSmem<128, 2>): at most 2 x SMs CTAs walk the tile list with running barrier
-    rings -- forced here so that every CTA runs several tiles (the planner picks it by itself for GEMMs with more tiles than SMs)"""
-    import ctypes as C
-    R.lib.mugd_debug_set_tc_tile_n(130)
-    try:
-        if case == "linear_bias":
-            M, K, N = 12288, 256, 1024                                     # 96 x 8 = 768 tiles over 296 CTAs
-            x, w, b = g("ox", (M, K)), g("ow", (N, K)) / math.sqrt(K), 0.1 * g("ob", (N,))
-            ref = F.linear(x.double(), w.double(), b.double())
-            xc, bc, out = x.cuda(), b.cuda(), torch.zeros(M, N).cuda()
-            ops = run_tc(R, view(xc), w, N, K, view(out), bias=ptr(bc))
-            got = out
-        elif case == "conv3_rowvec_residual":
-            B, L, Cin, Cout = 48, 512, 128, 256                            # 192 x 2 = 384 tiles
-            x, w, b = g("px", (B, Cin, L)), g("pw", (Cout, Cin, 3)) / math.sqrt(3 * Cin), 0.1 * g("pb", (Cout,))
-            emb, res = g("pe", (B, Cout)), g("pr", (B, Cout, L))
-            ref = F.conv1d(x.double(), w.double(), b.double(), padding=1) + emb.double()[:, :, None] + res.double()
-            wp = w.permute(0, 2, 1).contiguous().reshape(Cout, 3 * Cin)
-            xc, bc, ec, rc = nlc(x).cuda(), b.cuda(), emb.cuda(), nlc(res).cuda()
-            out = torch.zeros(B * L, Cout).cuda()
-            ops = run_tc(R, view(xc), wp, Cout, Cin, view(out), bias=ptr(bc), taps=3, mode=L_.CONV_SAME, Lin=L, Lout=L, rowvec=ptr(ec),
-                         rowvec_b_stride=Cout, residual=view(rc))
-            got, ref = ncl(out.cpu(), B), ref
-        elif case == "geglu":
-            M, K, Hh = 8192, 128, 512                                      # N = 1024: 64 x 8 = 512 tiles
-            x, w, b = g("qx", (M, K)), g("qw", (2 * Hh, K)) / math.sqrt(K), 0.1 * g("qb", (2 * Hh,))
-            a, gt = F.linear(x.double(), w.double(), b.double()).chunk(2, dim=-1)
-            ref = a * F.gelu(gt)
-            xc, bi, out = x.cuda(), _interleave_halves(b).cuda(), torch.zeros(M, Hh).cuda()
-            ops = run_tc(R, view(xc), _interleave_halves(w), 2 * Hh, K, view(out), bias=ptr(bi), gate=L_.GATE_GEGLU)
-            got = out
-        else:
-            M, K, N = 20000, 96, 328                                       # 157 x 3 tiles; last row tile and last column tile are partial
-            x, w = g("rx", (M, K)), g("rw", (N, K)) / math.sqrt(K)
-            ref = F.linear(x.double(), w.double())
-            xc, out = x.cuda(), torch.zeros(M, N).cuda()
-            ops = run_tc(R, view(xc), w, N, K, view(out))
-            got = out
-        gm = ops.ops[0].u.gemm
-        ok, sp, nt, ws = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int64()
-        R.lib.mugd_gemm_tc_query(None, C.byref(gm), 148, C.byref(ok), C.byref(sp), C.byref(ws), C.byref(nt))
-        assert ok.value and sp.value == 1 and nt.value > 2 * 148            # more tiles than resident CTAs: the walk is exercised
-        assert rel_err(got.cpu() if got.is_cuda else got, ref) < TOL
-        first = out.clone()
-        R.run(ops)
-        assert torch.equal(first, out)
-    finally:
-        R.lib.mugd_debug_set_tc_tile_n(0)

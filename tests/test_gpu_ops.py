@@ -1,5 +1,5 @@
 """Per-kernel parity: every libmugd op, called through the C ABI (mugd_op_run), against the CPU oracle /
-a plain torch fp32 statement of the same op on the same seeded inputs.  Run on the B200: pytest -m gpu.
+a plain torch fp32 statement of the same op on the same seeded inputs.  Run on the GPU: pytest -m gpu.
 
 Tolerances (fp32 path): 2e-5 relative to the output's max magnitude for contractions (different
 summation order only), 1e-5 for norms, bit-exact for the DDIM update and the copies.

@@ -157,7 +157,7 @@ def test_synthetic_streams_are_stable():
 
 @pytest.mark.parametrize("Beff,Lz", [(2, 96), (8, 512), (64, 512), (16, 992)])
 def test_tensor_core_planner_invariants(packed, Beff, Lz):
-    """tile / split-K planning of the tcgen05 GEMM (pure host code in libmugd, no GPU needed) over every GEMM of real plans:
+    """tile / split-K planning of the wgmma GEMM (pure host code in libmugd, no GPU needed) over every GEMM of real plans:
     what it takes it must be able to run with the engine's fixed 32 MB workspace and 4096 tile counters."""
     import ctypes as C
     cfg, sd, blob = packed
@@ -170,7 +170,7 @@ def test_tensor_core_planner_invariants(packed, Beff, Lz):
             continue
         g = o.u.gemm
         ok, sp, nt, ws = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int64()
-        assert lib.mugd_gemm_tc_query(None, C.byref(g), 148, C.byref(ok), C.byref(sp), C.byref(ws), C.byref(nt)) == 0
+        assert lib.mugd_gemm_tc_query(None, C.byref(g), 132, C.byref(ok), C.byref(sp), C.byref(ws), C.byref(nt)) == 0
         small = g.K % 32 != 0 or g.N < 16                       # conv_in (K = 16 per tap) stays on the FFMA kernel
         assert bool(ok.value) == (not small), (g.M, g.N, g.K)
         if not ok.value:
@@ -183,7 +183,7 @@ def test_tensor_core_planner_invariants(packed, Beff, Lz):
         assert 1 <= sp.value <= ksteps and 1 <= nt.value <= 4096
         if sp.value > 1:
             n_split += 1
-            assert nt.value * sp.value <= 2 * 148               # bounds the workspace: fewer than 2 partial tiles per SM
+            assert nt.value * sp.value <= 2 * 132               # bounds the workspace: fewer than 2 partial tiles per SM
             assert ksteps // sp.value >= 2                       # a split never leaves a CTA with a single k-step
             assert 0 < ws.value <= 32 << 20
             assert ws.value % (128 * 64 * 4) == 0                # whole 128-row partial tiles
@@ -195,41 +195,34 @@ def test_tensor_core_planner_invariants(packed, Beff, Lz):
         assert sp2.value == 1 or nt2.value * sp2.value <= 2 * 64
     assert n_tc >= 190          # 228 - 32 (fused second-source GEMMs) + 1
     if Beff <= 8:
-        assert n_split > 100                                     # small batches underfill 148 SMs: most GEMMs are split
+        assert n_split > 100                                     # small batches underfill 132 SMs: most GEMMs are split
     if Beff == 64:
         assert n_split < n_tc // 2
 
 
 @pytest.mark.parametrize("Beff,Lz", [(8, 512), (64, 512), (16, 992)])
 def test_tensor_core_variant_rule(packed, Beff, Lz):
-    """which GEMM kernel variant the planner picks (pure host code): the two-CTAs-per-SM variant only for unsplit GEMMs with more
-    128-wide tiles than SMs, never more than 2 x SMs CTAs; small batches never see it except for their widest GEMMs"""
+    """which GEMM kernel variant the planner picks (pure host code): 64- or 128-wide tiles, one CTA per SM, a grid of exactly
+    tiles x K splits CTAs; every GEMM with a K that is a multiple of 32 is taken by the tensor-core kernel"""
     import ctypes as C
     cfg, sd, blob = packed
     lib = L_.load()
     comp = UNetCompiler(cfg.unet, blob, 1 << 30)
     res = comp.compile(Arena(1 << 32), Beff, Lz, _fake_ext(comp, Beff, Lz), False)
-    n_two = n_tc = 0
+    n_tc = 0
     for o in res["ops"].ops:
         if o.kind != L_.OP_GEMM:
             continue
         g = o.u.gemm
         bn, occ, ctas = C.c_int32(), C.c_int32(), C.c_int32()
-        assert lib.mugd_gemm_tc_variant(C.byref(g), 148, C.byref(bn), C.byref(occ), C.byref(ctas)) == 0
+        assert lib.mugd_gemm_tc_variant(C.byref(g), 132, C.byref(bn), C.byref(occ), C.byref(ctas)) == 0
         if bn.value == 0:
             assert g.K % 32 != 0                                  # only conv_in stays on the FFMA kernel
             continue
         n_tc += 1
         sp, nt = C.c_int32(), C.c_int32()
-        lib.mugd_gemm_tc_query(None, C.byref(g), 148, None, C.byref(sp), None, C.byref(nt))
-        assert bn.value in (64, 128, 256) and occ.value in (1, 2)
-        if occ.value == 2:
-            n_two += 1
-            assert bn.value == 128 and sp.value == 1 and nt.value > 148 and ctas.value == min(nt.value, 296)
-        else:
-            assert ctas.value == nt.value * sp.value
+        lib.mugd_gemm_tc_query(None, C.byref(g), 132, None, C.byref(sp), None, C.byref(nt))
+        assert bn.value in (64, 128) and occ.value == 1
+        assert bn.value == 128 or g.N < 128                       # 64-wide tiles only for narrow outputs
+        assert ctas.value == nt.value * sp.value
     assert n_tc >= 190
-    if Beff == 64:
-        assert n_two >= 60                                        # the big batch runs most of its GEMM time on the two-CTA variant
-    if Beff == 8:
-        assert n_two <= 20                                        # only the widest feed-forward GEMMs have more tiles than SMs

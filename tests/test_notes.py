@@ -58,7 +58,7 @@ def test_gpu_note_kernel_equals_reference(gold):
 
 @pytest.mark.gpu
 def test_decode_to_hit_objects_end_to_end(gold, golden_dir):
-    """z (reference golden latent) -> B200 decoder -> GPU note extraction == reference decoder + reference convertor,
+    """z (reference golden latent) -> CUDA decoder -> GPU note extraction == reference decoder + reference convertor,
     except for notes whose deciding logit is within the logit tolerance of 0"""
     from mug_diffusion_b200 import synth
     from mug_diffusion_b200.sampler import MugDiffusionB200

@@ -1,7 +1,8 @@
 """mug_diffusion_b200/postprocess.py (SURVEY §8f N4: gridify + mini-jack removal) against golden vectors produced by the UNMODIFIED
-reference (tools/make_postprocess_goldens.py -> tests/golden/postprocess.json), and against the live reference where its tree exists.
+reference (tools/make_postprocess_goldens.py -> tests/golden/postprocess.json, tools/make_live_goldens.py ->
+tests/golden/postprocess_random.json.gz).
 String / integer results: the bar is equality."""
-import importlib.util
+import gzip
 import json
 import os
 import sys
@@ -37,16 +38,19 @@ def test_long_notes_are_never_moved_and_snapped_at_both_ends():
     assert len(grid) == 4 and all(l.split(",")[3] == o.split(",")[3] for l, o in zip(grid, lines))
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/mug/data/utils.py"), reason="reference tree not present")
-@pytest.mark.parametrize("seed", [11, 12, 13])
+RANDOM_SEEDS = [11, 12, 13]
+
+
+def random_chart_case(seed):
+    return dict(seed=seed, bpm=150 + 13.7 * seed % 140, offset=300 + seed, n=150, div=4 if seed % 2 else 8, jack_ratio=0.15)
+
+
+@pytest.mark.parametrize("seed", RANDOM_SEEDS)
 def test_live_reference(seed):
-    spec = importlib.util.spec_from_file_location("ref_utils", "/root/reference/mug/data/utils.py")
-    ref = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref)
-    lines = chart(seed, 150 + 13.7 * seed % 140, 300 + seed, 150, div=4 if seed % 2 else 8, jack_ratio=0.15)
-    a = ref.remove_intractable_mania_mini_jacks(lines, verbose=False)
+    with gzip.open(os.path.join(ROOT, "tests", "golden", "postprocess_random.json.gz"), "rt") as f:
+        ref = {c["seed"]: c for c in json.load(f)}[seed]
+    lines = chart(**random_chart_case(seed))
     b = pp.remove_intractable_mania_mini_jacks(lines, verbose=False)
-    assert a == b
-    ga, bpm_a, off_a = ref.gridify(a, verbose=False)
+    assert b == ref["dejack"]
     gb, bpm_b, off_b = pp.gridify(b, verbose=False)
-    assert ga == gb and float(bpm_a) == float(bpm_b) and float(off_a) == float(off_b)
+    assert gb == ref["grid"] and float(bpm_b) == ref["bpm"] and float(off_b) == ref["offset"]

@@ -1,7 +1,8 @@
 """Prompt path (SURVEY 8f N3): feature dict -> embedding ids -> [B,128,21] conditioning.
 CPU: the oracle restatement and the product's host function against ids produced by the UNMODIFIED reference
-(tests/golden/prompt.json, tools/make_goldens.py --only prompt), and against the live reference where its tree exists.
+(tests/golden/prompt.json, tools/make_goldens.py --only prompt; tests/golden/prompt_random.json.gz, tools/make_live_goldens.py).
 GPU: the gather kernel behind ``model.model.cond_stage_model`` bit-exact against the reference embedder's output."""
+import gzip
 import json
 import os
 import random
@@ -16,8 +17,6 @@ sys.path.insert(0, ROOT)
 import golden_cases as gc  # noqa: E402
 from mug_diffusion_b200 import prompt as P  # noqa: E402
 from oracle import mug_oracle as orc  # noqa: E402
-
-REF = os.environ.get("MUG_REFERENCE_ROOT", "/root/reference")
 
 # a spec that exercises what the shipped yaml does not: count > 1 and non-integer bin edges
 SPEC_COUNT = [
@@ -65,28 +64,35 @@ def test_oracle_embed_matches_reference_golden(gold, golden_dir):
     assert torch.equal(orc.prompt_embed(g["table"], ids), g["out"])
 
 
-@pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "mug")), reason="reference tree not present")
-def test_ids_match_live_reference_on_random_dicts(gold):
-    sys.path.insert(0, os.path.join(ROOT, "tools"))
-    import ref_shim
-    ref_shim.install_shims()
-    from mug.util import count_beatmap_features, feature_dict_to_embedding_ids
-    rnd = random.Random(5)
-    for spec in (gold["spec"], SPEC_COUNT):
-        assert P.count_beatmap_features(spec) == count_beatmap_features(spec)
-        for _ in range(300):
-            d = {}
-            for x in spec:
-                if rnd.random() < 0.4:
-                    continue
-                if x["type"] == "numeric":
-                    span = x["max"] - x["min"]
-                    d[x["name"]] = rnd.choice([x["min"] - 1, x["max"] + 1, x["min"] + span * rnd.random(), x["min"], x["max"]])
-                elif x["type"] == "bool":
-                    d[x["name"]] = rnd.choice([True, False, 0, 1])
-                else:
-                    d[x["name"]] = rnd.choice(x["category"])
-            want = feature_dict_to_embedding_ids(d, spec)
+def random_dicts(spec, n=300, seed=5):
+    """n seeded feature dicts over `spec`: missing keys, out-of-range, boundary and in-between values"""
+    rnd = random.Random(seed)
+    out = []
+    for _ in range(n):
+        d = {}
+        for x in spec:
+            if rnd.random() < 0.4:
+                continue
+            if x["type"] == "numeric":
+                span = x["max"] - x["min"]
+                d[x["name"]] = rnd.choice([x["min"] - 1, x["max"] + 1, x["min"] + span * rnd.random(), x["min"], x["max"]])
+            elif x["type"] == "bool":
+                d[x["name"]] = rnd.choice([True, False, 0, 1])
+            else:
+                d[x["name"]] = rnd.choice(x["category"])
+        out.append(d)
+    return out
+
+
+def test_ids_match_live_reference_on_random_dicts(gold, golden_dir):
+    """the reference's own ids for the seeded random dicts (tests/golden/prompt_random.json.gz, tools/make_live_goldens.py)"""
+    with gzip.open(os.path.join(golden_dir, "prompt_random.json.gz"), "rt") as f:
+        ref = json.load(f)
+    for spec, want_spec in zip((gold["spec"], SPEC_COUNT), ref):
+        assert P.count_beatmap_features(spec) == want_spec["count"]
+        dicts = random_dicts(spec)
+        assert len(dicts) == len(want_spec["ids"])
+        for d, want in zip(dicts, want_spec["ids"]):
             assert P.feature_dict_to_embedding_ids(d, spec) == want
             assert orc.feature_ids(d, spec) == want
 

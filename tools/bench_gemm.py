@@ -75,7 +75,7 @@ def main():
         flops = 2.0 * M * Cout * Cin * taps
         sp = C.c_int32()
         g = ops.ops[0].u.gemm
-        R.lib.mugd_gemm_tc_query(R.handle, C.byref(g), 148, None, C.byref(sp), None, None)
+        R.lib.mugd_gemm_tc_query(R.handle, C.byref(g), 132, None, C.byref(sp), None, None)
         print(f"{label:28s} {M:6d} {Cout:5d} {taps*Cin:5d} | {res[L_.GEMM_TC]:8.1f} {flops/res[L_.GEMM_TC]/1e6:8.1f} | "
               f"{res[L_.GEMM_SIMT]:8.1f} {flops/res[L_.GEMM_SIMT]/1e6:9.1f} | {sp.value}  cta0 setup/main/stage/epi us = "
               f"{stamps[0]:.1f}/{stamps[1]:.1f}/{stamps[2]:.1f}/{stamps[3]:.1f}")

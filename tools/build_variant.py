@@ -19,5 +19,5 @@ for src in B.SOURCES:
     objs.append(obj)
     procs.append(subprocess.Popen([B._nvcc(), *flags, "-c", os.path.join(B.CSRC, src), "-o", obj]))
 assert all(p.wait() == 0 for p in procs)
-subprocess.check_call([B._nvcc(), "-shared", "-o", out, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"])
+subprocess.check_call([B._nvcc(), "-shared", "-o", out, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"])
 print(out)

@@ -41,7 +41,8 @@ CASES = [dict(seed=1, bpm=187.3, offset=412, n=260), dict(seed=2, bpm=240.0, off
 
 
 def main():
-    spec = importlib.util.spec_from_file_location("ref_utils", "/root/reference/mug/data/utils.py")
+    from ref_shim import REF_ROOT
+    spec = importlib.util.spec_from_file_location("ref_utils", os.path.join(REF_ROOT, "mug", "data", "utils.py"))
     ref = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref)
     out = []

@@ -48,7 +48,7 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--gemm", default="auto")
     ap.add_argument("--fuse", type=int, default=1, help="0: stand-alone LayerNorm kernels")
-    ap.add_argument("--attn", type=int, default=1, help="0: exact-fp32 FFMA attention kernel instead of the tcgen05 one")
+    ap.add_argument("--attn", type=int, default=1, help="0: exact-fp32 FFMA attention kernel instead of the tensor-core one")
     ap.add_argument("--only", default="", help="only ops whose family name contains this")
     a = ap.parse_args()
     dev = torch.device("cuda:0")
@@ -87,9 +87,9 @@ def main():
             sp, ok, nt = C.c_int32(), C.c_int32(), C.c_int32()
             g = arr[idx[0]].u.gemm
             try:
-                eng.lib.mugd_gemm_tc_query(eng.handle, C.byref(g), 148, C.byref(ok), C.byref(sp), None, C.byref(nt))
+                eng.lib.mugd_gemm_tc_query(eng.handle, C.byref(g), 132, C.byref(ok), C.byref(sp), None, C.byref(nt))
                 bn, occ = C.c_int32(), C.c_int32()
-                eng.lib.mugd_gemm_tc_variant(C.byref(g), 148, C.byref(bn), C.byref(occ), None)
+                eng.lib.mugd_gemm_tc_variant(C.byref(g), 132, C.byref(bn), C.byref(occ), None)
                 extra = (f"tc={ok.value} tiles={nt.value} split={sp.value} bn={bn.value}x{occ.value} "
                          f"TF/s={2.0*g.M*g.N*(g.K*g.taps+g.K2)/us/1e6:.0f}")
             except Exception as e:       # noqa: BLE001
