@@ -55,9 +55,7 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
         sess = eng.session(Beff, Lz, per_sample_t=False)
         dec = eng.decoder_session(B, Lz)
         T = inp["c"].shape[2]
-        if T != sess.ctx_tokens:
-            sess.ctx_tokens = T
-            sess._build(sess.comp)
+        sess.set_ctx_tokens(T)
         # ---- staging buffers of the caller (inputs / outputs in the reference's NCL layout) ----
         st = dict(in_x=inp["x_T"].to(dev).contiguous(), in_c=inp["c"].to(dev).contiguous(), in_uc=inp["uc"].to(dev).contiguous(),
                   pred=torch.zeros(B * Lz * Cz, device=dev), out_z=torch.zeros(B, Cz, Lz, device=dev),
@@ -67,10 +65,7 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
             st[f"in_w{i}"] = w
         # per-request host tables for this S
         sess.set_timestep_table(ts.copy())
-        coef = np.stack([np.asarray(a, dtype=np.float32) for a in (sampler.ddim_alphas, sampler.ddim_alphas_prev, sampler.ddim_sigmas,
-                                                                   sampler.ddim_sqrt_one_minus_alphas)], axis=1)
-        sess.coef.zero_()
-        sess.coef[:total].copy_(torch.from_numpy(np.ascontiguousarray(coef)).to(dev))
+        sess.set_ddim_schedule(sampler.ddim_alphas, sampler.ddim_alphas_prev, sampler.ddim_sigmas, sampler.ddim_sqrt_one_minus_alphas)
 
         # ---- regions: every device allocation a plan may point into ----
         tensors: Dict[str, torch.Tensor] = dict(weights=eng.weights, weights_lo=eng.weights_lo, arena=sess.arena_t, emb_table=sess.emb_table, temb=sess.temb,
@@ -88,16 +83,7 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
         regions = [L_.Region(keep[i], _ptr(tensors[n]), tensors[n].numel() * tensors[n].element_size()) for i, n in enumerate(names)]
 
         # ---- the plans ----
-        upd = L_.DdimUpdate()
-        upd.x = sess.xin.ptr
-        upd.x_dup = sess.xin.r(B * Lz, 2 * B * Lz).ptr if cfg_on else None
-        upd.eps, upd.pred_x0, upd.coef, upd.step = sess.eps.ptr, _ptr(st["pred"]), _ptr(sess.coef), _ptr(sess.step)
-        upd.S, upd.n, upd.cfg, upd.scale, upd.temperature = total, B * Lz * Cz, int(cfg_on), float(scale), 1.0
-        adv = L_.StepAdvance()
-        adv.step = _ptr(sess.step)
-        tail = OpList()
-        tail.add(L_.OP_DDIM_UPDATE, upd)
-        tail.add(L_.OP_STEP_ADVANCE, adv)
+        tail = sess.ddim_tail(B, total, cfg_on, scale, 1.0, _ptr(st["pred"]))
         readz = OpList()
         readz.transpose(sess.xin.ptr, _ptr(st["out_z"]), sess.xin.ld, 0, B, Cz, Lz, False)
         dec_in = OpList()
@@ -140,13 +126,10 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
         sess.set_step(0)
         for name in ("emb", "ctx", "audio", "loadx"):
             plans[name].run()
-        sess.run_steps(total, tail)
+        sess.plan.launch(total, tail)
         for name in ("readz", "dec_in"):
             plans[name].run()
-        if not dec.plan.captured:
-            dec.plan.run()
-            dec.plan.capture()
-        dec.plan.replay(1)
+        dec.plan.launch()
         plans["dec_out"].run()
         torch.cuda.synchronize()
         for n in ("out_z", "out_logits"):

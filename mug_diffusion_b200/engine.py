@@ -21,7 +21,7 @@ import torch
 
 from . import lib as L_
 from .config import DecoderConfig, ModelConfig, UNetConfig
-from .netspec import Block, decoder_layout, unet_layout
+from .netspec import RES_LAYERS, Block, decoder_layout, unet_layout
 from .packer import WeightBlob, pack_model
 
 GN_EPS = 1e-6     # models.py:11
@@ -194,32 +194,49 @@ def emit_upsample_conv(ops: "OpList", blob: WeightBlob, wfn, prefix: str, x: Vie
     return idx
 
 
-def tc_weight_map(blob: WeightBlob, wbase: int) -> Dict[int, Tuple[int, int]]:
+def tc_weight_map(blob: WeightBlob, wbase: int, lo_base: Optional[int] = None) -> Dict[int, Tuple[int, int]]:
     """address of every tensor-core GEMM weight -> (hi address, lo address).  After the engine's device-side split (runtime.MugEngine)
-    hi lives where the plain weight was and lo in the engine's second buffer (``blob.lo_bases[wbase]``; 0 = this engine keeps plain
-    fp32 weights for the exact-fp32 FFMA path: empty map).  A base nobody registered (plan compilation without a device, CPU tests)
-    gets a virtual lo buffer behind the blob."""
-    lo_base = blob.lo_bases.get(wbase, wbase + 4 * blob.numel)
-    if lo_base == 0:
-        return {}
-    cached = getattr(blob, "_tc_maps", None)
-    if cached is None:
-        cached = blob._tc_maps = {}
-    key = (wbase, lo_base)
-    if key not in cached:
-        cached[key] = {wbase + 4 * off: (wbase + 4 * off, lo_base + 4 * lo) for _, off, _, lo in blob.tc}
-    return cached[key]
+    hi lives where the plain weight was and lo in the engine's second buffer at ``lo_base``.  Without one (plan compilation without
+    a device, CPU tests) lo is placed in a virtual buffer behind the blob."""
+    if lo_base is None:
+        lo_base = wbase + 4 * blob.numel
+    return {wbase + 4 * off: (wbase + 4 * off, lo_base + 4 * lo) for _, off, _, lo in blob.tc}
 
 
 # tags (profiling labels carried in mugd_op.tag)
 TAG_RES, TAG_ATTN, TAG_S4, TAG_UPDOWN, TAG_IO = 1, 2, 3, 4, 5
 
 
+def emit_res(ops: OpList, arena: Arena, wfn, b: Block, x: View, out: View, B: int, Lr: int, G: int, **emb):
+    """ResBlock of the U-Net or the decoder (netspec.RES_LAYERS): GroupNorm+SiLU -> conv3 -> GroupNorm+SiLU -> conv3 + skip.  A skip
+    with a channel change (1x1 conv) runs as extra k-steps of the last GEMM on a second source; otherwise x is added as the residual.
+    ``emb``: the U-Net's time-embedding row added after the first conv (the rowvec arguments of OpList.gemm)."""
+    norm1, conv1, norm2, conv2, _ = RES_LAYERS[b.kind]
+    p = b.prefix
+    m = arena.mark()
+    t1 = arena.alloc(x.rows, b.cin)
+    ops.groupnorm(x, t1, wfn(p + norm1 + "weight"), wfn(p + norm1 + "bias"), B, Lr, G, True, TAG_RES)
+    t2 = arena.alloc(x.rows, b.cout)
+    ops.gemm(t1, wfn(p + conv1 + "weight"), b.cout, b.cin, t2, bias=wfn(p + conv1 + "bias"), taps=3, mode=L_.CONV_SAME, Lin=Lr, Lout=Lr,
+             tag=TAG_RES, **emb)
+    t3 = arena.alloc(x.rows, b.cout)
+    ops.groupnorm(t2, t3, wfn(p + norm2 + "weight"), wfn(p + norm2 + "bias"), B, Lr, G, True, TAG_RES)
+    if b.has_skip_conv:
+        ops.gemm(t3, wfn(p + "out_skip.weight"), b.cout, b.cout, out, bias=wfn(p + "out_skip.bias"), taps=3, mode=L_.CONV_SAME,
+                 Lin=Lr, Lout=Lr, A2=x, tag=TAG_RES)
+    else:
+        ops.gemm(t3, wfn(p + conv2 + "weight"), b.cout, b.cout, out, bias=wfn(p + conv2 + "bias"), taps=3, mode=L_.CONV_SAME,
+                 Lin=Lr, Lout=Lr, residual=x, tag=TAG_RES)
+    arena.release(m)
+
+
 class UNetCompiler:
     """Emit the op list of one U-Net evaluation (unet.py:511-550) for Beff samples of length L."""
 
-    def __init__(self, cfg: UNetConfig, blob: WeightBlob, wbase: int, prefix: str = "model.unet_model."):
+    def __init__(self, cfg: UNetConfig, blob: WeightBlob, wbase: int, tc_map: Optional[Dict[int, Tuple[int, int]]] = None,
+                 prefix: str = "model.unet_model."):
         self.cfg, self.blob, self.wbase, self.prefix = cfg, blob, wbase, prefix
+        self.tc_map = tc_weight_map(blob, wbase) if tc_map is None else tc_map
         self.lay = unet_layout(cfg, prefix)
 
     def w(self, name: str) -> int:
@@ -231,7 +248,7 @@ class UNetCompiler:
         at small batches and loses slightly at large ones, so None = fold below 8192 token rows.
         False = stand-alone LayerNorm kernels (the referee path, and what the exact-fp32 FFMA GEMM uses)."""
         cfg = self.cfg
-        ops = OpList(tc_weight_map(self.blob, self.wbase))
+        ops = OpList(self.tc_map)
         nlev = cfg.levels
         assert Lz % (1 << (nlev - 1)) == 0 and (Lz >> (nlev - 1)) % 4 == 0, "z_length must be a multiple of 32"
         rows = [Beff * (Lz >> l) for l in range(nlev)]
@@ -243,9 +260,8 @@ class UNetCompiler:
         fuse_ln = fold_ln and any(k.endswith("qkv_ln.weight") for k in self.blob.entries)
 
         # ---- row-moment block: [live | zeros] fp64, `live` re-armed by the first op of every evaluation ----
-        all_blocks = [b for e in self.lay.input + [self.lay.middle] + self.lay.output if not isinstance(e, tuple) for b in e]
         lvl_of_ds = {1 << l: l for l in range(nlev)}
-        ln_rows = sum(3 * rows[lvl_of_ds[b.ds]] for b in all_blocks if b.kind == "attn")
+        ln_rows = sum(3 * rows[lvl_of_ds[b.ds]] for b in self.lay.blocks() if b.kind == "attn")
         stat_doubles = ln_rows * 2 if fuse_ln else 0
         stat_floats = (2 * stat_doubles + 63) // 64 * 64
         live = arena.alloc(1, stat_floats) if fuse_ln else None
@@ -320,28 +336,8 @@ class UNetCompiler:
             ops.groupnorm(x, y, gamma, beta, Beff, Lr, G, silu, tag)
 
         # ---- block emitters ------------------------------------------------------------------
-        def emit_res(b: Block, x: View, out: View, lvl: int):
-            Lr = lens[lvl]
-            m = arena.mark()
-            p = b.prefix
-            t1 = arena.alloc(x.rows, b.cin)
-            groupnorm(x, t1, self.w(p + "in_layers.0.weight"), self.w(p + "in_layers.0.bias"), Lr, True, TAG_RES)
-            t2 = arena.alloc(x.rows, b.cout)
-            gemm(t1, self.w(p + "in_layers.2.weight"), b.cout, b.cin, t2, bias=self.w(p + "in_layers.2.bias"), taps=3,
-                 mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, rowvec=E + 4 * emb_off[p],
-                 rowvec_b_stride=emb_total if per_sample_t else 0,
-                 rowvec_step_stride=0 if per_sample_t else emb_total, step=0 if per_sample_t else step, tag=TAG_RES)
-            t3 = arena.alloc(x.rows, b.cout)
-            groupnorm(t2, t3, self.w(p + "out_layers.0.weight"), self.w(p + "out_layers.0.bias"), Lr, True, TAG_RES)
-            if b.has_skip_conv:
-                # conv3(t3) + skip_connection(x) as ONE GEMM: the 1x1 skip runs as extra k-steps on a second source
-                gemm(t3, self.w(p + "out_skip.weight"), b.cout, b.cout, out, bias=self.w(p + "out_skip.bias"), taps=3,
-                     mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, A2=x, tag=TAG_RES)
-            else:
-                gemm(t3, self.w(p + "out_layers.3.weight"), b.cout, b.cout, out, bias=self.w(p + "out_layers.3.bias"), taps=3,
-                     mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, residual=x, tag=TAG_RES)
-            arena.release(m)
-
+        # the time-embedding row of a ResBlock: one per sample (per-sample t) or the row of the current DDIM step
+        emb_row = dict(rowvec_b_stride=emb_total) if per_sample_t else dict(rowvec_step_stride=emb_total, step=step)
         attn_index = [0]
 
         def emit_attn(b: Block, x: View, out: View, lvl: int):
@@ -424,7 +420,7 @@ class UNetCompiler:
                     continue
                 out = final_out if (last and final_out is not None) else arena.alloc(cur.rows, b.cout)
                 if b.kind == "res":
-                    emit_res(b, cur, out, lvl)
+                    emit_res(ops, arena, self.w, b, cur, out, Beff, lens[lvl], G, rowvec=E + 4 * emb_off[b.prefix], **emb_row)
                 elif b.kind == "attn":
                     emit_attn(b, cur, out, lvl)
                 elif b.kind == "s4":
@@ -496,8 +492,10 @@ class UNetCompiler:
 class DecoderCompiler:
     """Decoder.forward (autoencoder.py:329-354) on channels-last rows."""
 
-    def __init__(self, cfg: DecoderConfig, blob: WeightBlob, wbase: int, prefix: str = "model.first_stage_model.decoder."):
+    def __init__(self, cfg: DecoderConfig, blob: WeightBlob, wbase: int, tc_map: Optional[Dict[int, Tuple[int, int]]] = None,
+                 prefix: str = "model.first_stage_model.decoder."):
         self.cfg, self.blob, self.wbase, self.prefix = cfg, blob, wbase, prefix
+        self.tc_map = tc_weight_map(blob, wbase) if tc_map is None else tc_map
         self.seq = decoder_layout(cfg, prefix)
 
     def w(self, name: str) -> int:
@@ -505,7 +503,7 @@ class DecoderCompiler:
 
     def compile(self, arena: Arena, B: int, Lz: int) -> dict:
         cfg = self.cfg
-        ops = OpList(tc_weight_map(self.blob, self.wbase))
+        ops = OpList(self.tc_map)
         G = cfg.num_groups
         zin = arena.alloc(B * Lz, cfg.z_channels)
         cur = zin
@@ -520,21 +518,7 @@ class DecoderCompiler:
                 cur = o
             elif b.kind == "dec_res":
                 o = arena.alloc(B * Lr, b.cout)
-                m = arena.mark()
-                t1 = arena.alloc(B * Lr, b.cin)
-                ops.groupnorm(cur, t1, self.w(p + "norm1.weight"), self.w(p + "norm1.bias"), B, Lr, G, True, TAG_RES)
-                t2 = arena.alloc(B * Lr, b.cout)
-                ops.gemm(t1, self.w(p + "conv1.weight"), b.cout, b.cin, t2, bias=self.w(p + "conv1.bias"), taps=3,
-                         mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, tag=TAG_RES)
-                t3 = arena.alloc(B * Lr, b.cout)
-                ops.groupnorm(t2, t3, self.w(p + "norm2.weight"), self.w(p + "norm2.bias"), B, Lr, G, True, TAG_RES)
-                if b.has_skip_conv:
-                    ops.gemm(t3, self.w(p + "out_skip.weight"), b.cout, b.cout, o, bias=self.w(p + "out_skip.bias"), taps=3,
-                             mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, A2=cur, tag=TAG_RES)
-                else:
-                    ops.gemm(t3, self.w(p + "conv2.weight"), b.cout, b.cout, o, bias=self.w(p + "conv2.bias"), taps=3,
-                             mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, residual=cur, tag=TAG_RES)
-                arena.release(m)
+                emit_res(ops, arena, self.w, b, cur, o, B, Lr, G)
                 cur = o
             elif b.kind == "up":
                 o = arena.alloc(B * Lr * 2, b.cout)

@@ -36,6 +36,19 @@ class UNetLayout:
     out: Optional[Block] = None
     skip_channels: List[int] = field(default_factory=list)   # channels of every hs entry, push order
 
+    def blocks(self) -> Iterator[Block]:
+        """every Block in execution order: input, middle and output blocks (not the audio markers), then ``out``"""
+        for entry in self.input + [self.middle] + self.output:
+            if not isinstance(entry, tuple):
+                yield from entry
+        yield self.out
+
+
+# sub-layer names (norm1, conv1, norm2, conv2, 1x1 skip) of the U-Net's TimestepResBlock (unet.py:121) and the decoder's ResnetBlock
+# (models.py:94): the two compute the same thing, except that the U-Net adds a time-embedding row after conv1
+RES_LAYERS = {"res": ("in_layers.0.", "in_layers.2.", "out_layers.0.", "out_layers.3.", "skip_connection."),
+              "dec_res": ("norm1.", "conv1.", "norm2.", "conv2.", "nin_shortcut.")}
+
 
 def unet_layout(cfg: UNetConfig, prefix: str = "model.unet_model.") -> UNetLayout:
     mc = cfg.model_channels
@@ -203,13 +216,8 @@ def unet_param_specs(cfg: UNetConfig, prefix: str = "model.unet_model.") -> Dict
     out: Dict[str, Spec] = {}
     _lin(out, prefix + "time_embed.0.", cfg.model_channels, cfg.time_embed_dim)
     _lin(out, prefix + "time_embed.2.", cfg.time_embed_dim, cfg.time_embed_dim)
-    lay = unet_layout(cfg, prefix)
-    for entry in lay.input + [lay.middle] + lay.output:
-        if isinstance(entry, tuple):
-            continue
-        for b in entry:
-            _block_params(out, b, cfg)
-    _block_params(out, lay.out, cfg)
+    for b in unet_layout(cfg, prefix).blocks():
+        _block_params(out, b, cfg)
     return out
 
 
@@ -232,13 +240,3 @@ def decoder_param_specs(cfg: DecoderConfig, prefix: str = "model.first_stage_mod
             _norm(out, p + "norm_out.", b.cin)
             _conv(out, p + "conv_out.", b.cin, b.cout, 3)
     return out
-
-
-def s4_blocks(cfg: UNetConfig, prefix: str = "model.unet_model.") -> Iterator[Block]:
-    lay = unet_layout(cfg, prefix)
-    for entry in lay.input + [lay.middle] + lay.output:
-        if isinstance(entry, tuple):
-            continue
-        for b in entry:
-            if b.kind == "s4":
-                yield b

@@ -21,7 +21,7 @@ from typing import Dict, List, Tuple
 import torch
 
 from .config import DecoderConfig, UNetConfig
-from .netspec import Block, decoder_layout, unet_layout
+from .netspec import RES_LAYERS, Block, decoder_layout, unet_layout
 
 ALIGN = 64  # floats (256 B)
 
@@ -41,7 +41,6 @@ class WeightBlob:
         self.data: torch.Tensor | None = None      # finalized flat tensor (CPU, then moved)
         self.tc: List[Tuple[str, int, int, int]] = []   # tensor-core weights: (entry, blob offset, elements, offset in the lo buffer)
         self.tc_lo_numel = 0
-        self.lo_bases: Dict[int, int] = {}         # device base of an engine's weights -> device base of its lo buffer (0 = not split)
 
     def add(self, name: str, t: torch.Tensor):
         assert name not in self.entries, name
@@ -115,26 +114,17 @@ def _pack_block(blob: WeightBlob, sd: Dict[str, torch.Tensor], b: Block):
     if b.kind in ("conv_in", "dec_conv_in"):
         blob.add_shaped(p + "weight", _conv3(sd[p + "weight"]))
         blob.add_shaped(p + "bias", sd[p + "bias"])
-    elif b.kind == "res":
-        for n in ("in_layers.0.", "out_layers.0."):
+    elif b.kind in RES_LAYERS:
+        norm1, conv1, norm2, conv2, skip = RES_LAYERS[b.kind]
+        for n in (norm1, norm2):
             blob.add_shaped(p + n + "weight", sd[p + n + "weight"])
             blob.add_shaped(p + n + "bias", sd[p + n + "bias"])
-        for n in ("in_layers.2.",) + (() if b.has_skip_conv else ("out_layers.3.",)):
+        for n in (conv1,) + (() if b.has_skip_conv else (conv2,)):
             blob.add_shaped(p + n + "weight", _conv3(sd[p + n + "weight"]))
             blob.add_shaped(p + n + "bias", sd[p + n + "bias"])
         if b.has_skip_conv:
-            blob.add_shaped(p + "out_skip.weight", torch.cat([_conv3(sd[p + "out_layers.3.weight"]), _conv1(sd[p + "skip_connection.weight"])], dim=1))
-            blob.add_shaped(p + "out_skip.bias", sd[p + "out_layers.3.bias"] + sd[p + "skip_connection.bias"])
-    elif b.kind == "dec_res":
-        for n in ("norm1.", "norm2."):
-            blob.add_shaped(p + n + "weight", sd[p + n + "weight"])
-            blob.add_shaped(p + n + "bias", sd[p + n + "bias"])
-        for n in ("conv1.",) + (() if b.has_skip_conv else ("conv2.",)):
-            blob.add_shaped(p + n + "weight", _conv3(sd[p + n + "weight"]))
-            blob.add_shaped(p + n + "bias", sd[p + n + "bias"])
-        if b.has_skip_conv:
-            blob.add_shaped(p + "out_skip.weight", torch.cat([_conv3(sd[p + "conv2.weight"]), _conv1(sd[p + "nin_shortcut.weight"])], dim=1))
-            blob.add_shaped(p + "out_skip.bias", sd[p + "conv2.bias"] + sd[p + "nin_shortcut.bias"])
+            blob.add_shaped(p + "out_skip.weight", torch.cat([_conv3(sd[p + conv2 + "weight"]), _conv1(sd[p + skip + "weight"])], dim=1))
+            blob.add_shaped(p + "out_skip.bias", sd[p + conv2 + "bias"] + sd[p + skip + "bias"])
     elif b.kind == "attn":
         blob.add_shaped(p + "norm.weight", sd[p + "norm.weight"])
         blob.add_shaped(p + "norm.bias", sd[p + "norm.bias"])
@@ -207,17 +197,6 @@ def _pack_block(blob: WeightBlob, sd: Dict[str, torch.Tensor], b: Block):
         raise ValueError(b.kind)
 
 
-def all_unet_blocks(cfg: UNetConfig, prefix: str) -> List[Block]:
-    lay = unet_layout(cfg, prefix)
-    out: List[Block] = []
-    for entry in lay.input + [lay.middle] + lay.output:
-        if isinstance(entry, tuple):
-            continue
-        out.extend(entry)
-    out.append(lay.out)
-    return out
-
-
 def pack_model(sd: Dict[str, torch.Tensor], ucfg: UNetConfig, dcfg: DecoderConfig,
                unet_prefix: str = "model.unet_model.", dec_prefix: str = "model.first_stage_model.decoder.",
                tensor_core_split: bool = True, wave_cfg=None) -> WeightBlob:
@@ -226,7 +205,7 @@ def pack_model(sd: Dict[str, torch.Tensor], ucfg: UNetConfig, dcfg: DecoderConfi
     for n in ("time_embed.0.", "time_embed.2."):
         blob.add_shaped(up + n + "weight", sd[up + n + "weight"])
         blob.add_shaped(up + n + "bias", sd[up + n + "bias"])
-    blocks = all_unet_blocks(ucfg, up)
+    blocks = list(unet_layout(ucfg, up).blocks())
     # fused emb_layers: one [sum Cout, 512] matrix, per-ResBlock column offsets recorded in meta
     res = [b for b in blocks if b.kind == "res"]
     blob.add_shaped(up + "emb_all.weight", torch.cat([sd[b.prefix + "emb_layers.1.weight"] for b in res], dim=0))

@@ -4,15 +4,15 @@ from __future__ import annotations
 import ctypes as C
 import threading
 from collections import OrderedDict
-from typing import Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
+from torch.utils.weak import WeakIdKeyDictionary
 
 from . import lib as L_
 from .config import ModelConfig
 from .engine import (Arena, CTX_TOKENS_MAX, DecoderCompiler, MAX_STEPS, OpList, UNetCompiler, View, tc_weight_map)
-from .netspec import s4_blocks
 from .packer import WeightBlob, pack_model
 
 
@@ -51,12 +51,43 @@ class Plan:
     def replay(self, times: int = 1):
         L_.check(self.engine.lib.mugd_plan_replay(self.handle, times, _stream()), "plan_replay")
 
+    def launch(self, steps: int = 1, tail: Optional[OpList] = None):
+        """``steps`` replays of the plan's CUDA graph; with ``tail``, every replay is followed by the tail ops and all steps run from
+        one C call (mugd_sample).  The first call captures the graph, after a warm-up run outside capture (lazy module load,
+        cudaFuncSetAttribute)."""
+        if not self.captured:
+            self.run()
+            self.capture()
+        if tail is None:
+            self.replay(steps)
+            return
+        self.engine.attach_workspace(tail)
+        L_.check(self.engine.lib.mugd_sample(self.handle, tail.array(), len(tail.ops), steps, _stream()), "mugd_sample")
+
     def __del__(self):
         try:
             if self.handle:
                 self.engine.lib.mugd_plan_destroy(self.handle)
         except Exception:
             pass
+
+
+def compile_sized(engine: "MugEngine", compile_fn: Callable[[Arena], dict]):
+    """Compile into a zeroed device arena of exactly the size the plan needs: a dry compile measures it, the real one runs at a
+    256-byte aligned base.  compile_fn(arena) returns the compiler's result dict.  Returns (arena tensor, result, Plan)."""
+    dry = Arena(0)
+    compile_fn(dry)
+    nbytes = dry.high + 1024
+    arena_t = torch.zeros(nbytes // 4 + 64, device=engine.device)
+    base = (arena_t.data_ptr() + 255) // 256 * 256
+    res = compile_fn(Arena(base, nbytes))
+    return arena_t, res, Plan(engine, res["ops"])
+
+
+# device-resident blob tensor an engine has split in place -> its lo buffer (an entry lives as long as the tensor).  A second engine
+# over the same tensor (dist.broadcast_blob leaves the blob on the device, where .to(device) returns it unchanged) must take this lo
+# buffer: splitting again would round hi to itself and leave a zero lo.
+_SPLIT_LO = WeakIdKeyDictionary()
 
 
 class MugEngine:
@@ -79,6 +110,7 @@ class MugEngine:
         self.wbase = self.weights.data_ptr()
         self.weights_lo: Optional[torch.Tensor] = None         # the lo operands of the tensor-core weights (second buffer)
         self.tc_split_done = False
+        self.tc_map: Dict[int, Tuple[int, int]] = {}          # W -> (W_hi, W_lo) addresses; empty while the weights are plain fp32
         self.lock = threading.RLock()
         # split-K scratch of the tensor-core GEMM: all ops run in stream order, so one buffer serves every plan
         # (bound: tiles*splits < 2*SMs tiles of 128x128 fp32)
@@ -107,9 +139,10 @@ class MugEngine:
                     raise L_.MugdError("this engine's weights were split in place and no host copy exists: build a new engine for gemm_impl='simt'")
                 self.weights.copy_(self.blob.data)
                 self.tc_split_done = False
-            self.blob.lo_bases[self.wbase] = 0
+            self.tc_map = {}
         else:
             self._split_tc_weights()
+            self.tc_map = tc_weight_map(self.blob, self.wbase, self.weights_lo.data_ptr())
         L_.check(self.lib.mugd_set_tc_single_pass_tf32(self.handle, 1 if impl == "tc_tf32" else 0), "set_tc_single_pass_tf32")
         self.gemm_impl = impl
         self.sessions.clear()
@@ -117,27 +150,24 @@ class MugEngine:
 
     def _split_tc_weights(self):
         """TF32 hi / lo operands of every tensor-core weight, computed on the device: hi over the plain weight, lo in a second buffer"""
-        shared = getattr(self.blob, "_lo_tensors", None)
-        if shared is None:
-            shared = self.blob._lo_tensors = {}
-        if not self.tc_split_done and self.wbase in shared:
-            # the blob already lives on this device (broadcast_blob over NCCL) and another engine split it in place: share its lo buffer
-            self.weights_lo, self.tc_split_done = shared[self.wbase], True
-        if not self.tc_split_done:
-            if self.weights_lo is None:
-                self.weights_lo = torch.zeros(max(self.blob.tc_lo_numel, 4), device=self.device)
-            if self.weights is self.blob.data:
-                shared[self.wbase] = self.weights_lo
-            ops = OpList()
-            for _, off, n, lo in self.blob.tc:
-                d = L_.Tf32Split()
-                d.w_hi, d.lo, d.n = self.wbase + 4 * off, self.weights_lo.data_ptr() + 4 * lo, n
-                ops.add(L_.OP_TF32_SPLIT, d)
-            st = _stream()
-            for op in ops.ops:
-                L_.check(self.lib.mugd_op_run(self.handle, C.byref(op), st), "tf32_split")
-            self.tc_split_done = True
-        self.blob.lo_bases[self.wbase] = self.weights_lo.data_ptr()
+        if self.tc_split_done:
+            return
+        if self.weights in _SPLIT_LO:
+            self.weights_lo, self.tc_split_done = _SPLIT_LO[self.weights], True
+            return
+        if self.weights_lo is None:
+            self.weights_lo = torch.zeros(max(self.blob.tc_lo_numel, 4), device=self.device)
+        if self.weights is self.blob.data:
+            _SPLIT_LO[self.weights] = self.weights_lo
+        ops = OpList()
+        for _, off, n, lo in self.blob.tc:
+            d = L_.Tf32Split()
+            d.w_hi, d.lo, d.n = self.wbase + 4 * off, self.weights_lo.data_ptr() + 4 * lo, n
+            ops.add(L_.OP_TF32_SPLIT, d)
+        st = _stream()
+        for op in ops.ops:
+            L_.check(self.lib.mugd_op_run(self.handle, C.byref(op), st), "tf32_split")
+        self.tc_split_done = True
 
     def attach_workspace(self, ops: OpList):
         for op in ops.ops:
@@ -151,6 +181,21 @@ class MugEngine:
         st = _stream()
         for op in ops.ops:
             L_.check(self.lib.mugd_op_run(self.handle, C.byref(op), st), f"op kind {op.kind}")
+
+    def ncl_to_rows(self, x: torch.Tensor, rows: View):
+        """contiguous [B, C, L] device tensor (the reference's layout) -> channels-last rows [B*L, C] at ``rows``"""
+        B, Cc, Lr = x.shape
+        ops = OpList()
+        ops.transpose(_ptr(x), rows.ptr, 0, rows.ld, B, Cc, Lr, True)
+        self.run_ops(ops)
+
+    def rows_to_ncl(self, rows: View, B: int, Cc: int, Lr: int) -> torch.Tensor:
+        """channels-last rows [B*L, C] at ``rows`` -> a new [B, C, L] tensor"""
+        out = torch.empty(B, Cc, Lr, device=self.device)
+        ops = OpList()
+        ops.transpose(rows.ptr, _ptr(out), rows.ld, 0, B, Cc, Lr, False)
+        self.run_ops(ops)
+        return out
 
     def _lru_get(self, cache: OrderedDict, key, make):
         s = cache.get(key)
@@ -196,12 +241,10 @@ class Session:
         self.engine, self.Beff, self.Lz, self.per_sample_t = engine, Beff, Lz, per_sample_t
         cfg = engine.cfg.unet
         dev = engine.device
-        comp = UNetCompiler(cfg, engine.blob, engine.wbase)
-        self.comp = comp
+        self.comp = UNetCompiler(cfg, engine.blob, engine.wbase, engine.tc_map)
         emb_total = engine.blob.meta["emb_total"]
-        n_attn = sum(1 for b in _all_blocks(comp) if b.kind == "attn")
-        attn_blocks = [b for b in _all_blocks(comp) if b.kind == "attn"]
-        s4b = [b for b in _all_blocks(comp) if b.kind == "s4"]
+        attn_blocks = [b for b in self.comp.lay.blocks() if b.kind == "attn"]
+        s4b = [b for b in self.comp.lay.blocks() if b.kind == "s4"]
 
         # ---- side buffers (owned torch tensors) ----------------------------------------------
         emb_rows = Beff if per_sample_t else MAX_STEPS
@@ -216,7 +259,7 @@ class Session:
         self.ctx_tokens = 21
         self.s4_kt = {b.prefix: torch.zeros(Lz // b.ds, b.cin, device=dev) for b in s4b}
         self._gen_s4_kernels(s4b)
-        self._build(comp)
+        self._build()
 
     # S4 convolution kernels for this length: SSKernelNPLR.forward once per (model, L)  (s4.py:706-832)
     def _gen_s4_kernels(self, s4b):
@@ -262,24 +305,22 @@ class Session:
             s4_kt={p: View(_ptr(t), t.shape[1], t.shape[0], t.shape[1]) for p, t in self.s4_kt.items()},
         )
 
-    def _build(self, comp: UNetCompiler):
+    def _build(self):
         # the LayerNorm fold lives in the tensor-core GEMM epilogues; the exact-fp32 FFMA path keeps the stand-alone LayerNorm
         # kernels and doubles as the referee of the folded plan.  engine.fold_ln: None = by size, True / False = forced (A/B, tests)
         fold = False if self.engine.gemm_impl == "simt" else self.engine.fold_ln
-        dry = Arena(0)
-        comp.compile(dry, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold)
-        nbytes = dry.high + 1024
-        self.arena_t = torch.zeros(nbytes // 4 + 64, device=self.engine.device)
-        base = (self.arena_t.data_ptr() + 255) // 256 * 256
-        arena = Arena(base, nbytes)
-        res = comp.compile(arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold)
+        self.arena_t, res, self.plan = compile_sized(self.engine, lambda arena: self.comp.compile(
+            arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold))
         self.xin: View = res["xin"]
         self.eps: View = res["eps"]
         self.audio_slots = res["audio_slots"]
         self.ln_folded = res["ln_folded"]
-        self.plan = Plan(self.engine, res["ops"])
-        self.arena_bytes = nbytes
-        self._captured_for = None
+
+    def set_ctx_tokens(self, T: int):
+        """context length of the cross-attention; Lk is baked into the attention ops, so a new length recompiles the plan"""
+        if T != self.ctx_tokens:
+            self.ctx_tokens = T
+            self._build()
 
     # ---- per-request preparation ---------------------------------------------------------------
     def set_timestep_table(self, timesteps: Sequence[int]):
@@ -303,7 +344,7 @@ class Session:
         """the three GEMMs that turn R sinusoid rows (self.temb) into R rows of the fused ResBlock embedding table"""
         cfg = self.engine.cfg.unet
         eng = self.engine
-        ops = OpList(tc_weight_map(eng.blob, eng.wbase))
+        ops = OpList(eng.tc_map)
         up = self.comp.prefix
         tv = View(_ptr(self.temb), cfg.model_channels, R, cfg.model_channels)
         h1 = View(_ptr(self.emb_h1), cfg.time_embed_dim, R, cfg.time_embed_dim)
@@ -329,9 +370,7 @@ class Session:
         Bc = sum(int(c.shape[0]) for c in parts)
         _, Cd, T = parts[0].shape
         assert Bc == self.Beff and Cd == cfg.context_dim and T <= CTX_TOKENS_MAX and all(c.shape[1:] == parts[0].shape[1:] for c in parts)
-        if T != self.ctx_tokens:
-            self.ctx_tokens = T
-            self._build(self.comp)            # Lk is baked into the attention ops
+        self.set_ctx_tokens(T)
         eng.run_ops(self.context_ops([(_ptr(c), int(c.shape[0])) for c in parts], T))
         self._keep = parts
 
@@ -341,13 +380,13 @@ class Session:
         cfg = eng.cfg.unet
         Cd = cfg.context_dim
         Bc = sum(b for _, b in parts)
-        ops = OpList(tc_weight_map(eng.blob, eng.wbase))
+        ops = OpList(eng.tc_map)
         row = 0
         for addr, bpart in parts:
             ops.transpose(addr, _ptr(self.ctx) + 4 * row * Cd, 0, Cd, bpart, Cd, T, True)
             row += bpart * T
         cv = View(_ptr(self.ctx), Cd, Bc * T, Cd)
-        blocks = [b for b in _all_blocks(self.comp) if b.kind == "attn"]
+        blocks = [b for b in self.comp.lay.blocks() if b.kind == "attn"]
         for b, kv in zip(blocks, self.ctx_kv):
             o = View(_ptr(kv), kv.shape[1], Bc * T, kv.shape[1])
             ops.gemm(cv, self.comp.w(b.prefix + "transformer_blocks.0.attn2.kv.weight"), 2 * b.cin, Cd, o, Lout=T)
@@ -393,29 +432,37 @@ class Session:
         return ops
 
     def read_rows(self, view: View, B: int, Cc: int, Lr: int) -> torch.Tensor:
-        out = torch.empty(B, Cc, Lr, device=self.engine.device)
-        ops = OpList()
-        ops.transpose(view.ptr, _ptr(out), view.ld, 0, B, Cc, Lr, False)
-        self.engine.run_ops(ops)
-        return out
+        return self.engine.rows_to_ncl(view, B, Cc, Lr)
 
     def eval(self, graph: bool = True):
         if graph:
-            if not self.plan.captured:
-                self.plan.run()               # warm-up (lazy module load, cudaFuncSetAttribute) outside capture
-                self.plan.capture()
-            self.plan.replay(1)
+            self.plan.launch()
         else:
             self.plan.run()
 
-    def run_steps(self, n: int, tail: OpList):
-        """n DDIM steps from ONE C call (mugd_sample): n x {graph replay of the evaluation ; the tail ops (update, step advance)}"""
-        if not self.plan.captured:
-            self.plan.run()                   # warm-up (lazy module load, cudaFuncSetAttribute) outside capture
-            self.plan.capture()
-        self.engine.attach_workspace(tail)
-        arr = tail.array()
-        L_.check(self.engine.lib.mugd_sample(self.plan.handle, arr, len(tail.ops), n, _stream()), "mugd_sample")
+    def set_ddim_schedule(self, alphas, alphas_prev, sigmas, sqrt_one_minus_alphas):
+        """coef row i = (alpha, alpha_prev, sigma, sqrt(1 - alpha)) of DDIM step i, rows past the schedule zero"""
+        coef = np.stack([np.asarray(a, dtype=np.float32) for a in (alphas, alphas_prev, sigmas, sqrt_one_minus_alphas)], axis=1)
+        self.coef.zero_()
+        self.coef[:len(coef)].copy_(torch.from_numpy(coef).to(self.engine.device))
+
+    def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:
+        """the ops that follow each evaluation of an S-step request for B samples: the DDIM update of the xin rows (both halves
+        under classifier-free guidance) from eps, the coef row of the current step and, if ``noise`` is given, the noise rows;
+        pred_x0 receives the predicted x0 rows.  Then the step counter advances."""
+        n = B * self.Lz * self.engine.cfg.unet.in_channels
+        upd = L_.DdimUpdate()
+        upd.x = self.xin.ptr
+        upd.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        upd.eps, upd.noise, upd.pred_x0 = self.eps.ptr, noise or None, pred_x0
+        upd.coef, upd.step = _ptr(self.coef), _ptr(self.step)
+        upd.S, upd.n, upd.cfg, upd.scale, upd.temperature = S, n, int(cfg_on), float(scale), float(temperature)
+        adv = L_.StepAdvance()
+        adv.step = _ptr(self.step)
+        tail = OpList()
+        tail.add(L_.OP_DDIM_UPDATE, upd)
+        tail.add(L_.OP_STEP_ADVANCE, adv)
+        return tail
 
     def set_step(self, value: int):
         L_.check(self.engine.lib.mugd_fill_i32(_ptr(self.step), value, _stream()), "fill_i32")
@@ -424,16 +471,9 @@ class Session:
 class DecoderSession:
     def __init__(self, engine: MugEngine, B: int, Lz: int):
         self.engine, self.B, self.Lz = engine, B, Lz
-        comp = DecoderCompiler(engine.cfg.decoder, engine.blob, engine.wbase)
-        dry = Arena(0)
-        comp.compile(dry, B, Lz)
-        nbytes = dry.high + 1024
-        self.arena_t = torch.zeros(nbytes // 4 + 64, device=engine.device)
-        base = (self.arena_t.data_ptr() + 255) // 256 * 256
-        res = comp.compile(Arena(base, nbytes), B, Lz)
+        comp = DecoderCompiler(engine.cfg.decoder, engine.blob, engine.wbase, engine.tc_map)
+        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz))
         self.zin, self.logits, self.Lout = res["zin"], res["logits"], res["Lout"]
-        self.plan = Plan(engine, res["ops"])
-        self.arena_bytes = nbytes
 
     def notes(self, frame_ms: float, key_count: int = 4):
         """Note extraction on the logits of the last ``decode`` (still resident, channels-last): returns
@@ -461,19 +501,9 @@ class DecoderSession:
         z = z.to(eng.device, torch.float32)
         if cfg.scale != 1.0:
             z = z / cfg.scale                 # autoencoder.py:76
-        z = z.contiguous()
-        ops = OpList()
-        ops.transpose(_ptr(z), self.zin.ptr, 0, self.zin.ld, self.B, cfg.z_channels, self.Lz, True)
-        eng.run_ops(ops)
-        if not self.plan.captured:
-            self.plan.run()                   # warm-up (lazy module load, cudaFuncSetAttribute) outside capture
-            self.plan.capture()
-        self.plan.replay(1)
-        out = torch.empty(self.B, cfg.x_channels, self.Lout, device=eng.device)
-        ops = OpList()
-        ops.transpose(self.logits.ptr, _ptr(out), self.logits.ld, 0, self.B, cfg.x_channels, self.Lout, False)
-        eng.run_ops(ops)
-        return out
+        eng.ncl_to_rows(z.contiguous(), self.zin)
+        self.plan.launch()
+        return eng.rows_to_ncl(self.logits, self.B, cfg.x_channels, self.Lout)
 
 
 _NODE_CACHE: Dict[int, torch.Tensor] = {}
@@ -508,12 +538,3 @@ def hit_object_lines(count, start_ms, end_ms, key_count: int):
         items.sort(key=lambda t: t[1])
         charts.append([t[0] for t in items])
     return charts
-
-
-def _all_blocks(comp: UNetCompiler):
-    lay = comp.lay
-    for entry in lay.input + [lay.middle] + lay.output:
-        if isinstance(entry, tuple):
-            continue
-        for b in entry:
-            yield b

@@ -16,9 +16,8 @@ from typing import Dict, Optional, Sequence
 import numpy as np
 import torch
 
-from . import lib as L_
 from .config import DecoderConfig, ModelConfig, UNetConfig
-from .engine import OpList
+from .engine import View
 from .prompt import PromptEmbedder
 from .runtime import MugEngine, Session, _ptr
 
@@ -262,32 +261,15 @@ class DDIMSampler(object):
             # ddim.py:170-174 concatenates [uc, c] and [w, w]; here the two halves are written straight into their rows
             sess.set_context([unconditional_conditioning, c] if cfg_on else c)
             sess.set_audio(list(w)[-model.cfg.unet.levels:], dup=cfg_on)
-            coef = np.stack([np.asarray(self.ddim_alphas, dtype=np.float32), np.asarray(self.ddim_alphas_prev, dtype=np.float32),
-                             np.asarray(self.ddim_sigmas, dtype=np.float32),
-                             np.asarray(self.ddim_sqrt_one_minus_alphas, dtype=np.float32)], axis=1)
-            sess.coef[:total].copy_(torch.from_numpy(np.ascontiguousarray(coef)).to(dev))
+            sess.set_ddim_schedule(self.ddim_alphas, self.ddim_alphas_prev, self.ddim_sigmas, self.ddim_sqrt_one_minus_alphas)
             sess.load_x(x, dup=cfg_on)
             sess.set_step(0)
-            n = B * Lz * Cz
-            pred = torch.empty(n, device=dev)
+            # pred_x0 and the noise of a step: channels-last rows [B*Lz, Cz]
+            pred = torch.empty(B * Lz, Cz, device=dev)
             has_noise = bool(np.any(np.asarray(self.ddim_sigmas) != 0))
-            noise_nlc = torch.empty(n, device=dev) if has_noise else None
-
-            upd = L_.DdimUpdate()
-            upd.x = sess.xin.ptr
-            upd.x_dup = sess.xin.r(B * Lz, 2 * B * Lz).ptr if cfg_on else None
-            upd.eps = sess.eps.ptr
-            upd.noise = _ptr(noise_nlc) if has_noise else None
-            upd.pred_x0 = _ptr(pred)
-            upd.coef = _ptr(sess.coef)
-            upd.step = _ptr(sess.step)
-            upd.S, upd.n, upd.cfg = total, n, int(cfg_on)
-            upd.scale, upd.temperature = float(unconditional_guidance_scale), float(temperature)
-            adv = L_.StepAdvance()
-            adv.step = _ptr(sess.step)
-            tail = OpList()
-            tail.add(L_.OP_DDIM_UPDATE, upd)
-            tail.add(L_.OP_STEP_ADVANCE, adv)
+            noise_nlc = torch.empty(B * Lz, Cz, device=dev) if has_noise else None
+            tail = sess.ddim_tail(B, total, cfg_on, unconditional_guidance_scale, temperature, _ptr(pred),
+                                  _ptr(noise_nlc) if has_noise else 0)
 
             intermediates = {'x_inter': [x], 'pred_x0': [x]}
             iterator = time_range
@@ -300,12 +282,7 @@ class DDIMSampler(object):
                 return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
 
             def current_pred():
-                pv = L_  # noqa: F841
-                out = torch.empty(B, Cz, Lz, device=dev)
-                ops = OpList()
-                ops.transpose(_ptr(pred), _ptr(out), Cz, 0, B, Cz, Lz, False)
-                eng.run_ops(ops)
-                return out
+                return eng.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
 
             per_step_host_work = (mask is not None or has_noise or match_rng or callback is not None or img_callback is not None)
             if not per_step_host_work:
@@ -317,7 +294,7 @@ class DDIMSampler(object):
                     j = i
                     while not ((total - j - 1) % log_every_t == 0 or (total - j - 1) == total - 1):
                         j += 1
-                    sess.run_steps(j - i + 1, tail)
+                    sess.plan.launch(j - i + 1, tail)
                     for _ in range(j - i + 1):
                         next(it, None)                                          # keeps a progress bar (tqdm_class) moving
                     intermediates['x_inter'].append(current_x())
@@ -340,9 +317,7 @@ class DDIMSampler(object):
                             # dropout(sigma * n * T) == sigma * T * dropout(n): same Bernoulli draw, same 1/(1-p) scale (:193-194)
                             nz = torch.nn.functional.dropout(nz, p=noise_dropout)
                     if has_noise:
-                        ops = OpList()
-                        ops.transpose(_ptr(nz), _ptr(noise_nlc), 0, Cz, B, Cz, Lz, True)
-                        eng.run_ops(ops)
+                        eng.ncl_to_rows(nz, View(_ptr(noise_nlc), Cz, B * Lz, Cz))
                     sess.eval(graph=True)
                     eng.run_ops(tail)
                     if callback:

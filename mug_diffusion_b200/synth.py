@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from .config import DecoderConfig, ModelConfig, UNetConfig
-from .netspec import decoder_param_specs, s4_blocks, unet_param_specs
+from .netspec import decoder_param_specs, unet_layout, unet_param_specs
 
 
 def _rng(seed: int, name: str) -> np.random.Generator:
@@ -78,9 +78,10 @@ def synthetic_state_dict(z_length: int, cfg: Optional[ModelConfig] = None, seed:
     if unet:
         for name, (shape, role) in unet_param_specs(cfg.unet).items():
             sd[name] = _init(name, shape, role, seed)
-        for b in s4_blocks(cfg.unet):
-            assert z_length % b.ds == 0
-            sd[b.prefix + "s4_model.kernel.kernel.L"] = torch.tensor(z_length // b.ds, dtype=torch.int64)
+        for b in unet_layout(cfg.unet).blocks():
+            if b.kind == "s4":
+                assert z_length % b.ds == 0
+                sd[b.prefix + "s4_model.kernel.kernel.L"] = torch.tensor(z_length // b.ds, dtype=torch.int64)
     if decoder:
         for name, (shape, role) in decoder_param_specs(cfg.decoder).items():
             sd[name] = _init(name, shape, role, seed)

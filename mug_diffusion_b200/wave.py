@@ -172,8 +172,10 @@ def pack_wave(blob: WeightBlob, sd: Dict[str, torch.Tensor], cfg: WaveConfig, pr
 class WaveCompiler:
     """Launch plan of one encoder pass for B spectrograms of T frames (T divisible by 2**9)."""
 
-    def __init__(self, cfg: WaveConfig, blob: WeightBlob, wbase: int, prefix: str = WAVE_PREFIX):
+    def __init__(self, cfg: WaveConfig, blob: WeightBlob, wbase: int, tc_map: Optional[Dict[int, Tuple[int, int]]] = None,
+                 prefix: str = WAVE_PREFIX):
         self.cfg, self.blob, self.wbase, self.prefix = cfg, blob, wbase, prefix
+        self.tc_map = tc_weight_map(blob, wbase) if tc_map is None else tc_map
         self.seq = wave_layout(cfg, prefix)
 
     def w(self, name: str) -> int:
@@ -183,7 +185,7 @@ class WaveCompiler:
         cfg = self.cfg
         nlev = len(cfg.channel_mult)
         assert T % (1 << (nlev - 1)) == 0, "mel length must be a multiple of 512 frames"
-        ops = OpList(tc_weight_map(self.blob, self.wbase))
+        ops = OpList(self.tc_map)
         G, H = cfg.num_groups, cfg.num_heads
         mel = arena.alloc(B * T, cfg.n_freq)
         cur = mel
@@ -272,38 +274,21 @@ class WaveSession:
     the U-Net, unet.py:527-543) are ``None`` unless ``all_levels`` is set."""
 
     def __init__(self, engine, B: int, T: int):
-        from .runtime import Plan
+        from .runtime import compile_sized
         self.engine, self.B, self.T = engine, B, T
         cfg = engine.blob.meta["wave_cfg"]
-        comp = WaveCompiler(cfg, engine.blob, engine.wbase)
-        dry = Arena(0)
-        comp.compile(dry, B, T)
-        nbytes = dry.high + 1024
-        self.arena_t = torch.zeros(nbytes // 4 + 64, device=engine.device)
-        base = (self.arena_t.data_ptr() + 255) // 256 * 256
-        res = comp.compile(Arena(base, nbytes), B, T)
+        comp = WaveCompiler(cfg, engine.blob, engine.wbase, engine.tc_map)
+        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, T))
         self.mel, self.outs = res["mel"], res["outs"]
-        self.plan = Plan(engine, res["ops"])
         self.cfg = cfg
 
     def encode(self, mel: torch.Tensor, all_levels: bool = False) -> List[Optional[torch.Tensor]]:
         eng = self.engine
         mel = mel.to(eng.device, torch.float32).contiguous()
         assert mel.shape == (self.B, self.cfg.n_freq, self.T), mel.shape
-        ops = OpList()
-        ops.transpose(mel.data_ptr(), self.mel.ptr, 0, self.mel.ld, self.B, self.cfg.n_freq, self.T, True)
-        eng.run_ops(ops)
+        eng.ncl_to_rows(mel, self.mel)
         self.plan.run()
-        result: List[Optional[torch.Tensor]] = []
         nlev = len(self.outs)
-        ops = OpList()
-        for i, (view, ch, Lr) in enumerate(self.outs):
-            if all_levels or i >= nlev - 4:
-                t = torch.empty(self.B, ch, Lr, device=eng.device)
-                ops.transpose(view.ptr, t.data_ptr(), view.ld, 0, self.B, ch, Lr, False)
-                result.append(t)
-            else:
-                result.append(None)
-        eng.run_ops(ops)
         self._keep = mel
-        return result
+        return [eng.rows_to_ncl(view, self.B, ch, Lr) if all_levels or i >= nlev - 4 else None
+                for i, (view, ch, Lr) in enumerate(self.outs)]

@@ -145,3 +145,23 @@ def test_engine_keeps_every_weight_once_plus_the_lo_halves():
     assert torch.equal(eng.weights.cpu(), blob.data)
     eng.set_gemm_impl("auto")
     assert torch.equal(eng.weights[off:off + n].cpu(), hi_ref)
+
+
+def test_engines_over_one_device_resident_blob_share_its_split():
+    """a second engine over the same device-resident blob tensor (what dist.broadcast_blob hands every rank) takes the first engine's
+    lo buffer instead of splitting the tensor again, which would leave a zero lo; with no host copy the FFMA path is refused"""
+    from mug_diffusion_b200.config import ModelConfig
+    from mug_diffusion_b200.packer import pack_model
+    from mug_diffusion_b200.runtime import MugEngine
+    cfg = ModelConfig()
+    blob = pack_model(synth.synthetic_state_dict(96), cfg.unet, cfg.decoder)
+    host = blob.data
+    blob.data = host.cuda()
+    e1 = MugEngine(None, cfg, torch.device("cuda:0"), blob=blob)
+    e2 = MugEngine(None, cfg, torch.device("cuda:0"), blob=blob)
+    assert e1.weights is blob.data and e2.weights is blob.data and e2.weights_lo is e1.weights_lo and e2.tc_map == e1.tc_map
+    name, off, n, lo = blob.tc[len(blob.tc) // 2]
+    hi_ref, lo_ref = tf32_split(host[off:off + n])
+    assert torch.equal(blob.data[off:off + n].cpu(), hi_ref) and torch.equal(e2.weights_lo[lo:lo + n].cpu(), lo_ref)
+    with pytest.raises(L_.MugdError):
+        e2.set_gemm_impl("simt")

@@ -85,7 +85,7 @@ def test_packer_layouts(packed):
 
 
 def _fake_ext(comp, Beff, Lz):
-    blocks = [b for e in comp.lay.input + [comp.lay.middle] + comp.lay.output if not isinstance(e, tuple) for b in e]
+    blocks = list(comp.lay.blocks())
     return dict(emb_table=1 << 40, step=(1 << 40) + 4096, ctx_tokens=21,
                 ctx_kv=[View((1 << 41) + i * (1 << 24), 2 * b.cin, Beff * 21, 2 * b.cin) for i, b in enumerate(x for x in blocks if x.kind == "attn")],
                 s4_kt={b.prefix: View((1 << 42) + i * (1 << 24), b.cin, Lz // b.ds, b.cin) for i, b in enumerate(x for x in blocks if x.kind == "s4")})
