@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define MUGD_ABI_VERSION 12
+#define MUGD_ABI_VERSION 13
 
 typedef struct mugd_handle mugd_handle;   /* one device + scratch state            */
 typedef struct mugd_plan mugd_plan;       /* validated launch plan (+ CUDA graph)  */
@@ -53,7 +53,8 @@ enum mugd_op_kind {
     MUGD_OP_STEP_ADVANCE = 9,  /* *step += 1                                                                 */
     MUGD_OP_NOTES = 10,        /* decoder logits -> ordered note list (OsuManiaConvertor.array_to_objects)   */
     MUGD_OP_EMBED = 11,        /* prompt ids -> [B, H, F] embedding (BeatmapFeatureEmbedder.forward)         */
-    MUGD_OP_TF32_SPLIT = 12    /* weight preprocessing: w -> (hi in place, lo) for the 3xTF32 tensor-core GEMM */
+    MUGD_OP_TF32_SPLIT = 12,   /* weight preprocessing: w -> (hi in place, lo) for the 3xTF32 tensor-core GEMM */
+    MUGD_OP_POSTERIOR = 13     /* first-stage encoder moments -> mean / logvar / std / z (DiagonalGaussianDistribution)  */
 };
 
 /* A-operand row addressing of MUGD_OP_GEMM (rows are tokens of B samples, Lout output rows each) */
@@ -190,13 +191,26 @@ typedef struct mugd_embed {
  * every weight once; the resident copy holds hi + lo of the tensor-core weights and no plain duplicate. */
 typedef struct mugd_tf32_split { float* w_hi; float* lo; int64_t n; } mugd_tf32_split;
 
+/* Posterior of the first-stage encoder, mug/firststage/autoencoder.py:356-387 (DiagonalGaussianDistribution): mean, logvar =
+ * chunk(params, 2, dim=1); logvar = clamp(logvar, -10, 20); std = exp(0.5 * logvar); z = mean * scale (mode()) or, with noise,
+ * (mean + std * noise) * scale (sample()).  Same operation order as the reference's separate ATen ops, no FMA contraction: mean,
+ * logvar and mode() are bit-identical to torch; std and z differ from it by the ulp difference of two exp implementations.
+ * All tensors are NCL; every output may be NULL. */
+typedef struct mugd_posterior {
+    const float* params;                   /* [B, 2Z, L] encoder output (moments)                            */
+    const float* noise;                    /* [B, Z, L] standard normal draw, or NULL = mode()                */
+    float *mean, *logvar, *std, *z;        /* [B, Z, L] each                                                  */
+    float scale;                           /* AutoencoderKL.scale                                             */
+    int32_t B, Z, L;
+} mugd_posterior;
+
 typedef struct mugd_op {
     int32_t kind;
     int32_t tag;                           /* free for the host (profiling labels)                          */
     union {
         mugd_gemm gemm; mugd_groupnorm gn; mugd_layernorm ln; mugd_attention attn; mugd_s4conv s4;
         mugd_ddim_update ddim; mugd_transpose tr; mugd_copy2d cp; mugd_step_advance adv; mugd_notes notes;
-        mugd_embed embed; mugd_tf32_split split;
+        mugd_embed embed; mugd_tf32_split split; mugd_posterior post;
     } u;
 } mugd_op;
 
@@ -289,8 +303,8 @@ int  mugd_debug_set_tc_timing(long long* device_buf);
 
 /* ---- utility ---------------------------------------------------------------------------------- */
 int  mugd_fill_i32(int32_t* dst, int32_t value, void* stream);
-/* sizeof() of {mugd_op, mugd_gemm, mugd_groupnorm, mugd_layernorm, mugd_attention, mugd_s4conv,
- * mugd_ddim_update, mugd_transpose, mugd_copy2d, mugd_notes, mugd_embed, mugd_tf32_split} so a foreign-language mirror can verify its layout */
+/* sizeof() of {mugd_op, mugd_gemm, mugd_groupnorm, mugd_layernorm, mugd_attention, mugd_s4conv, mugd_ddim_update, mugd_transpose,
+ * mugd_copy2d, mugd_notes, mugd_embed, mugd_tf32_split, mugd_posterior} so a foreign-language mirror can verify its layout */
 int  mugd_abi_sizes(int32_t* out, int32_t n);
 
 #ifdef __cplusplus

@@ -6,7 +6,7 @@ live reference ``UNetModel`` / ``Decoder`` so the sampler can be built from the 
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import Tuple
+from typing import Optional, Tuple
 
 
 @dataclass(frozen=True)
@@ -87,6 +87,12 @@ class DecoderConfig:
 
 
 @dataclass(frozen=True)
+class EncoderConfig(DecoderConfig):
+    """The first-stage encoder (autoencoder.py:185-242).  It is built from the same ``ddconfig`` as the decoder, so it has the same
+    fields: it reads [B, x_channels, 2^(levels-1) L] note arrays and writes 2 * z_channels moment channels at L."""
+
+
+@dataclass(frozen=True)
 class ModelConfig:
     unet: UNetConfig = field(default_factory=UNetConfig)
     decoder: DecoderConfig = field(default_factory=DecoderConfig)
@@ -94,3 +100,4 @@ class ModelConfig:
     timesteps: int = 1000
     linear_start: float = 1e-4
     linear_end: float = 2e-2
+    encoder: Optional[EncoderConfig] = None      # None: no chart encoder (a blob with encoder weights then uses EncoderConfig())

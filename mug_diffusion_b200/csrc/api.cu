@@ -54,6 +54,7 @@ static int dispatch(mugd_handle* h, const mugd_op& op, cudaStream_t st, int* lau
         case MUGD_OP_NOTES: return launch_notes(h->dev, op.u.notes, st, launches);
         case MUGD_OP_EMBED: return launch_embed(h->dev, op.u.embed, st, launches);
         case MUGD_OP_TF32_SPLIT: return launch_tf32_split(h->dev, op.u.split, st, launches);
+        case MUGD_OP_POSTERIOR: return launch_posterior(h->dev, op.u.post, st, launches);
         default:
             set_error("unknown op kind %d", op.kind);
             return MUGD_ERR_INVALID;
@@ -206,11 +207,12 @@ int mugd_sample(mugd_plan* eval_plan, const mugd_op* tail, int32_t n_tail, int32
 }
 
 int mugd_abi_sizes(int32_t* out, int32_t n) {
-    MUGD_REQUIRE(out && n >= 12, "abi_sizes: need room for 12 entries");
+    MUGD_REQUIRE(out && n >= 13, "abi_sizes: need room for 13 entries");
     out[0] = sizeof(mugd_op); out[1] = sizeof(mugd_gemm); out[2] = sizeof(mugd_groupnorm);
     out[3] = sizeof(mugd_layernorm); out[4] = sizeof(mugd_attention); out[5] = sizeof(mugd_s4conv);
     out[6] = sizeof(mugd_ddim_update); out[7] = sizeof(mugd_transpose); out[8] = sizeof(mugd_copy2d);
     out[9] = sizeof(mugd_notes); out[10] = sizeof(mugd_embed); out[11] = sizeof(mugd_tf32_split);
+    out[12] = sizeof(mugd_posterior);
     return MUGD_OK;
 }
 

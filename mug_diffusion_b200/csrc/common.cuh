@@ -59,6 +59,7 @@ int launch_step_advance(const DeviceInfo& dev, const mugd_step_advance& a, cudaS
 int launch_notes(const DeviceInfo& dev, const mugd_notes& n, cudaStream_t st, int* launches);
 int launch_embed(const DeviceInfo& dev, const mugd_embed& e, cudaStream_t st, int* launches);
 int launch_tf32_split(const DeviceInfo& dev, const mugd_tf32_split& s, cudaStream_t st, int* launches);
+int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_t st, int* launches);
 int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, cudaStream_t st, int* launches);
 bool gemm_tc_supported(const mugd_gemm& g);
 

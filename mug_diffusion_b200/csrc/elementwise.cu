@@ -3,6 +3,7 @@
 //   transpose   : [B,C,L] <-> channels-last [B*L, ld] at the Python boundary (reference tensors are NCL)
 //   copy2d      : strided row copy (the 4 per-level tensors that live in two concat buffers)
 //   step_advance: device-side step counter so one CUDA graph serves every DDIM step
+//   posterior   : first-stage encoder moments -> mean / logvar / std / z   mug/firststage/autoencoder.py:356-387
 #include "common.cuh"
 
 namespace mugd {
@@ -243,6 +244,39 @@ int launch_embed(const DeviceInfo&, const mugd_embed& e, cudaStream_t st, int* l
     MUGD_REQUIRE(e.table && e.ids && e.out, "embed: null argument");
     MUGD_REQUIRE(e.B <= 65535, "embed: B=%d too large for one launch", e.B);
     MUGD_CHECK_CUDA(launch_k(embed_kernel, dim3(e.F, e.B), dim3(128), 0, st, e));
+    if (launches) *launches += 1;
+    return MUGD_OK;
+}
+
+// ---- posterior of the first-stage encoder (DiagonalGaussianDistribution, mug/firststage/autoencoder.py:356-387) -----------
+// One thread per latent element.  clamp -> 0.5*logvar -> expf in that order (autoencoder.py:362-364), full-precision expf; the
+// sample is mean + std*noise, then * scale (:371-372) with _rn intrinsics so no FMA contraction changes the rounding.
+__global__ void __launch_bounds__(256)
+posterior_kernel(const mugd_posterior p) {
+    pdl_trigger();
+    pdl_wait();
+    const int64_t zl = (int64_t)p.Z * p.L;
+    const int64_t n = (int64_t)p.B * zl;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t b = i / zl;
+        const float* src = p.params + b * zl + i;             // sample b starts at 2*b*zl: mean rows, then logvar rows
+        const float mean = src[0];
+        const float raw = src[zl];
+        const float lv = raw != raw ? raw : fminf(fmaxf(raw, -10.0f), 20.0f);       // torch.clamp propagates NaN
+        const float sd = expf(__fmul_rn(0.5f, lv));
+        if (p.mean) p.mean[i] = mean;
+        if (p.logvar) p.logvar[i] = lv;
+        if (p.std) p.std[i] = sd;
+        if (p.z) p.z[i] = __fmul_rn(p.noise ? __fadd_rn(mean, __fmul_rn(sd, p.noise[i])) : mean, p.scale);
+    }
+}
+
+int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_t st, int* launches) {
+    MUGD_REQUIRE(p.B > 0 && p.Z > 0 && p.L > 0 && p.params, "posterior: bad arguments B=%d Z=%d L=%d", p.B, p.Z, p.L);
+    const int64_t n = (int64_t)p.B * p.Z * p.L;
+    int blocks = (int)((n + 255) / 256);
+    if (blocks > dev.sm_count * 16) blocks = dev.sm_count * 16;
+    MUGD_CHECK_CUDA(launch_k(posterior_kernel, dim3(blocks), dim3(256), 0, st, p));
     if (launches) *launches += 1;
     return MUGD_OK;
 }

@@ -37,6 +37,8 @@ static const PtrField k_ptr_fields[] = {
     PF(MUGD_OP_NOTES, notes.logits), PF(MUGD_OP_NOTES, notes.count), PF(MUGD_OP_NOTES, notes.start_ms), PF(MUGD_OP_NOTES, notes.end_ms),
     PF(MUGD_OP_EMBED, embed.table), PF(MUGD_OP_EMBED, embed.ids), PF(MUGD_OP_EMBED, embed.out),
     PF(MUGD_OP_TF32_SPLIT, split.w_hi), PF(MUGD_OP_TF32_SPLIT, split.lo),
+    PF(MUGD_OP_POSTERIOR, post.params), PF(MUGD_OP_POSTERIOR, post.noise), PF(MUGD_OP_POSTERIOR, post.mean), PF(MUGD_OP_POSTERIOR, post.logvar),
+    PF(MUGD_OP_POSTERIOR, post.std), PF(MUGD_OP_POSTERIOR, post.z),
 };
 #undef PF
 

@@ -20,8 +20,8 @@ import numpy as np
 import torch
 
 from . import lib as L_
-from .config import DecoderConfig, ModelConfig, UNetConfig
-from .netspec import RES_LAYERS, Block, decoder_layout, unet_layout
+from .config import DecoderConfig, EncoderConfig, ModelConfig, UNetConfig
+from .netspec import RES_LAYERS, Block, decoder_layout, encoder_layout, unet_layout
 from .packer import WeightBlob, pack_model
 
 GN_EPS = 1e-6     # models.py:11
@@ -490,23 +490,29 @@ class UNetCompiler:
 
 
 class DecoderCompiler:
-    """Decoder.forward (autoencoder.py:329-354) on channels-last rows."""
+    """Decoder.forward (autoencoder.py:329-354) on channels-last rows.  The same walk runs the encoder's block list
+    (``EncoderCompiler``): its input is the first block's, its output the ``dec_out`` block's."""
 
     def __init__(self, cfg: DecoderConfig, blob: WeightBlob, wbase: int, tc_map: Optional[Dict[int, Tuple[int, int]]] = None,
                  prefix: str = "model.first_stage_model.decoder."):
         self.cfg, self.blob, self.wbase, self.prefix = cfg, blob, wbase, prefix
         self.tc_map = tc_weight_map(blob, wbase) if tc_map is None else tc_map
-        self.seq = decoder_layout(cfg, prefix)
+        self.seq = self.layout(cfg, prefix)
+
+    layout = staticmethod(decoder_layout)
 
     def w(self, name: str) -> int:
         return self.wbase + 4 * self.blob.offset(name)
 
     def compile(self, arena: Arena, B: int, Lz: int) -> dict:
+        """ops for B samples; a block of length multiplier ``mul`` runs on Lz * mul rows per sample.  Returns the input rows
+        (``inp``: [B * Lz * mul_first, cin_first]), the output rows (``out``) and their length per sample (``Lout``)."""
         cfg = self.cfg
         ops = OpList(self.tc_map)
         G = cfg.num_groups
-        zin = arena.alloc(B * Lz, cfg.z_channels)
-        cur = zin
+        first = self.seq[0]
+        inp = arena.alloc(B * Lz * first.mul, first.cin)
+        cur = inp
         out_view = None
         for b in self.seq:
             Lr = Lz * b.mul
@@ -524,10 +530,28 @@ class DecoderCompiler:
                 o = arena.alloc(B * Lr * 2, b.cout)
                 emit_upsample_conv(ops, self.blob, self.w, p, cur, o, Lr, b.cin, b.cout, TAG_UPDOWN)
                 cur = o
+            elif b.kind == "down":
+                # Downsample: right-pad 1, conv3 stride 2 (models.py:84-91)
+                o = arena.alloc(B * Lr // 2, b.cout)
+                ops.gemm(cur, self.w(p + "conv.weight"), b.cout, b.cin, o, bias=self.w(p + "conv.bias"), taps=3, mode=L_.CONV_DOWN,
+                         Lin=Lr, Lout=Lr // 2, tag=TAG_UPDOWN)
+                cur = o
             elif b.kind == "dec_out":
                 t = arena.alloc(B * Lr, b.cin)
                 ops.groupnorm(cur, t, self.w(p + "norm_out.weight"), self.w(p + "norm_out.bias"), B, Lr, G, True, TAG_IO)
                 out_view = arena.alloc(B * Lr, b.cout)
                 ops.gemm(t, self.w(p + "conv_out.weight"), b.cout, b.cin, out_view, bias=self.w(p + "conv_out.bias"), taps=3,
                          mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, tag=TAG_IO)
-        return dict(ops=ops, zin=zin, logits=out_view, Lout=Lz * self.seq[-1].mul)
+            else:
+                raise ValueError(b.kind)
+        return dict(ops=ops, inp=inp, out=out_view, Lout=Lz * self.seq[-1].mul)
+
+
+class EncoderCompiler(DecoderCompiler):
+    """Encoder.forward (autoencoder.py:244-265): [B * 2^(levels-1) Lz, x_channels] note rows -> [B * Lz, 2 * z_channels] moments."""
+
+    def __init__(self, cfg: EncoderConfig, blob: WeightBlob, wbase: int, tc_map: Optional[Dict[int, Tuple[int, int]]] = None,
+                 prefix: str = "model.first_stage_model.encoder."):
+        super().__init__(cfg, blob, wbase, tc_map, prefix)
+
+    layout = staticmethod(encoder_layout)

@@ -14,12 +14,12 @@ LIB_PATH = os.environ.get("MUGD_LIB") or os.path.join(HERE, "libmugd.so")      #
 
 # ---- enums (include/mugd.h) ------------------------------------------------------------------------
 (OP_GEMM, OP_GROUPNORM, OP_LAYERNORM, OP_ATTENTION, OP_S4CONV, OP_DDIM_UPDATE, OP_TRANSPOSE, OP_COPY2D, OP_STEP_ADVANCE, OP_NOTES, OP_EMBED,
- OP_TF32_SPLIT) = range(1, 13)
+ OP_TF32_SPLIT, OP_POSTERIOR) = range(1, 14)
 CONV_NONE, CONV_SAME, CONV_DOWN, CONV_UP, CONV_TAPS = range(5)
 ACT_NONE, ACT_SILU, ACT_GELU = range(3)
 GATE_NONE, GATE_GEGLU, GATE_GLU = range(3)
 GEMM_AUTO, GEMM_SIMT, GEMM_TC = range(3)
-ABI_VERSION = 12
+ABI_VERSION = 13
 
 _f = C.c_void_p  # device pointers travel as integers
 
@@ -94,10 +94,15 @@ class Tf32Split(C.Structure):
     _fields_ = [("w_hi", _f), ("lo", _f), ("n", C.c_int64)]
 
 
+class Posterior(C.Structure):
+    _fields_ = [("params", _f), ("noise", _f), ("mean", _f), ("logvar", _f), ("std", _f), ("z", _f), ("scale", C.c_float),
+                ("B", C.c_int32), ("Z", C.c_int32), ("L", C.c_int32)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", Gemm), ("gn", GroupNorm), ("ln", LayerNorm), ("attn", Attention), ("s4", S4Conv),
                 ("ddim", DdimUpdate), ("tr", Transpose), ("cp", Copy2D), ("adv", StepAdvance), ("notes", Notes), ("embed", Embed),
-                ("split", Tf32Split)]
+                ("split", Tf32Split), ("post", Posterior)]
 
 
 class Op(C.Structure):
@@ -105,7 +110,8 @@ class Op(C.Structure):
 
 
 _KIND_FIELD = {OP_GEMM: "gemm", OP_GROUPNORM: "gn", OP_LAYERNORM: "ln", OP_ATTENTION: "attn", OP_S4CONV: "s4",
-               OP_DDIM_UPDATE: "ddim", OP_TRANSPOSE: "tr", OP_COPY2D: "cp", OP_STEP_ADVANCE: "adv", OP_NOTES: "notes", OP_EMBED: "embed", OP_TF32_SPLIT: "split"}
+               OP_DDIM_UPDATE: "ddim", OP_TRANSPOSE: "tr", OP_COPY2D: "cp", OP_STEP_ADVANCE: "adv", OP_NOTES: "notes", OP_EMBED: "embed", OP_TF32_SPLIT: "split",
+               OP_POSTERIOR: "post"}
 
 
 def make_op(kind: int, desc, tag: int = 0) -> Op:
@@ -161,9 +167,10 @@ def load() -> C.CDLL:
     lib.mugd_abi_sizes.argtypes = [C.POINTER(C.c_int32), C.c_int32]
     if lib.mugd_abi_version() != ABI_VERSION:
         raise MugdError(f"libmugd ABI {lib.mugd_abi_version()} != binding {ABI_VERSION}: rebuild the library")
-    sizes = (C.c_int32 * 12)()
-    lib.mugd_abi_sizes(sizes, 12)
-    mine = [C.sizeof(t) for t in (Op, Gemm, GroupNorm, LayerNorm, Attention, S4Conv, DdimUpdate, Transpose, Copy2D, Notes, Embed, Tf32Split)]
+    sizes = (C.c_int32 * 13)()
+    lib.mugd_abi_sizes(sizes, 13)
+    mine = [C.sizeof(t) for t in (Op, Gemm, GroupNorm, LayerNorm, Attention, S4Conv, DdimUpdate, Transpose, Copy2D, Notes, Embed, Tf32Split,
+                                  Posterior)]
     if list(sizes) != mine:
         raise MugdError(f"struct layout mismatch: C {list(sizes)} vs ctypes {mine}")
     lib.mugd_sample.argtypes = [C.c_void_p, C.POINTER(Op), C.c_int32, C.c_int32, C.c_void_p]

@@ -3,7 +3,7 @@ state_dict key prefixes, channel counts and sequence-length divisors.
 
 This is the single source the weight packer, the launch-plan compiler and the synthetic-weight
 generator share.  It mirrors the *constructors* of the reference (mug/diffusion/unet.py:341-493 for the
-U-Net, mug/firststage/autoencoder.py:268-327 for the decoder) so that key names equal the reference's
+U-Net, mug/firststage/autoencoder.py:268-327 for the decoder, :185-242 for the encoder) so that key names equal the reference's
 ``state_dict()`` keys exactly (checked in tests/test_netspec.py against tests/golden/ref_keys.json).
 """
 from __future__ import annotations
@@ -11,7 +11,7 @@ from __future__ import annotations
 from dataclasses import dataclass, field
 from typing import Dict, Iterator, List, Optional, Tuple
 
-from .config import DecoderConfig, UNetConfig
+from .config import DecoderConfig, EncoderConfig, UNetConfig
 
 
 @dataclass
@@ -20,8 +20,8 @@ class Block:
     prefix: str               # state_dict prefix, ends with '.'
     cin: int
     cout: int
-    ds: int                   # sequence-length divisor relative to z_length (1,2,4,8); decoder: <1 via mul
-    mul: int = 1              # decoder only: length multiplier (1,2,4,8)
+    ds: int                   # sequence-length divisor relative to z_length (1,2,4,8); first stage: <1 via mul
+    mul: int = 1              # decoder / encoder only: length multiplier (1,2,4,8) of the block's input
     heads: int = 0
     has_skip_conv: bool = False
 
@@ -135,6 +135,30 @@ def decoder_layout(cfg: DecoderConfig, prefix: str = "model.first_stage_model.de
     return seq
 
 
+def encoder_layout(cfg: EncoderConfig, prefix: str = "model.first_stage_model.encoder.") -> List[Block]:
+    """Execution order of Encoder.forward (autoencoder.py:244-265): conv_in, per level the ResnetBlocks and (all but the last level)
+    a stride-2 Downsample, two mid ResnetBlocks, norm_out + SiLU + conv_out to 2 * z_channels moments.  The decoder's block kinds
+    describe every layer; ``mul`` runs 2^(levels-1) .. 1."""
+    nres = len(cfg.channel_mult)
+    mc = cfg.middle_channels
+    mul = 1 << (nres - 1)
+    seq = [Block("dec_conv_in", prefix + "conv_in.", cfg.x_channels, mc, 1, mul=mul)]
+    block_in = mc                                     # inchannel_mult = (1,) + channel_mult (:199)
+    for lvl in range(nres):
+        block_out = mc * cfg.channel_mult[lvl]
+        for b in range(cfg.num_res_blocks):
+            seq.append(Block("dec_res", f"{prefix}down.{lvl}.block.{b}.", block_in, block_out, 1, mul=mul,
+                             has_skip_conv=(block_in != block_out)))
+            block_in = block_out
+        if lvl != nres - 1:
+            seq.append(Block("down", f"{prefix}down.{lvl}.downsample.", block_in, block_in, 1, mul=mul))
+            mul //= 2
+    seq.append(Block("dec_res", prefix + "mid.block_1.", block_in, block_in, 1, mul=mul))
+    seq.append(Block("dec_res", prefix + "mid.block_2.", block_in, block_in, 1, mul=mul))
+    seq.append(Block("dec_out", prefix, block_in, 2 * cfg.z_channels, 1, mul=mul))
+    return seq
+
+
 # --------------------------------------------------------------------------------------------------
 # parameter manifest:  name -> (shape, role)
 # roles drive the synthetic initialiser only: w (fan-in scaled), b, gamma, beta, relpos, cemb, s4_*
@@ -221,9 +245,9 @@ def unet_param_specs(cfg: UNetConfig, prefix: str = "model.unet_model.") -> Dict
     return out
 
 
-def decoder_param_specs(cfg: DecoderConfig, prefix: str = "model.first_stage_model.decoder.") -> Dict[str, Spec]:
+def _first_stage_params(seq: List[Block]) -> Dict[str, Spec]:
     out: Dict[str, Spec] = {}
-    for b in decoder_layout(cfg, prefix):
+    for b in seq:
         p = b.prefix
         if b.kind == "dec_conv_in":
             _conv(out, p, b.cin, b.cout, 3)
@@ -234,9 +258,17 @@ def decoder_param_specs(cfg: DecoderConfig, prefix: str = "model.first_stage_mod
             _conv(out, p + "conv2.", b.cout, b.cout, 3)
             if b.has_skip_conv:
                 _conv(out, p + "nin_shortcut.", b.cin, b.cout, 1)
-        elif b.kind == "up":
+        elif b.kind in ("up", "down"):
             _conv(out, p + "conv.", b.cin, b.cout, 3)
         elif b.kind == "dec_out":
             _norm(out, p + "norm_out.", b.cin)
             _conv(out, p + "conv_out.", b.cin, b.cout, 3)
     return out
+
+
+def decoder_param_specs(cfg: DecoderConfig, prefix: str = "model.first_stage_model.decoder.") -> Dict[str, Spec]:
+    return _first_stage_params(decoder_layout(cfg, prefix))
+
+
+def encoder_param_specs(cfg: EncoderConfig, prefix: str = "model.first_stage_model.encoder.") -> Dict[str, Spec]:
+    return _first_stage_params(encoder_layout(cfg, prefix))

@@ -16,12 +16,12 @@ The blob is what rank 0 broadcasts over NCCL for multi-GPU runs (one collective,
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from .config import DecoderConfig, UNetConfig
-from .netspec import RES_LAYERS, Block, decoder_layout, unet_layout
+from .config import DecoderConfig, EncoderConfig, UNetConfig
+from .netspec import RES_LAYERS, Block, decoder_layout, encoder_layout, unet_layout
 
 ALIGN = 64  # floats (256 B)
 
@@ -199,7 +199,8 @@ def _pack_block(blob: WeightBlob, sd: Dict[str, torch.Tensor], b: Block):
 
 def pack_model(sd: Dict[str, torch.Tensor], ucfg: UNetConfig, dcfg: DecoderConfig,
                unet_prefix: str = "model.unet_model.", dec_prefix: str = "model.first_stage_model.decoder.",
-               tensor_core_split: bool = True, wave_cfg=None) -> WeightBlob:
+               tensor_core_split: bool = True, wave_cfg=None, encoder_cfg: Optional[EncoderConfig] = None,
+               enc_prefix: str = "model.first_stage_model.encoder.") -> WeightBlob:
     blob = WeightBlob()
     up = unet_prefix
     for n in ("time_embed.0.", "time_embed.2."):
@@ -221,6 +222,12 @@ def pack_model(sd: Dict[str, torch.Tensor], ucfg: UNetConfig, dcfg: DecoderConfi
         _pack_block(blob, sd, b)
     for b in decoder_layout(dcfg, dec_prefix):
         _pack_block(blob, sd, b)
+    if any(k.startswith(enc_prefix) for k in sd):
+        # the chart encoder (autoencoder.py:185-265), only when its weights are given: blobs without it are unchanged
+        ecfg = encoder_cfg or EncoderConfig()
+        for b in encoder_layout(ecfg, enc_prefix):
+            _pack_block(blob, sd, b)
+        blob.meta["encoder_cfg"] = ecfg
     if wave_cfg is not None or any(k.startswith("model.wave_model.") for k in sd):
         from .wave import WaveConfig, pack_wave            # SURVEY §8f N1: the audio encoder, once per request
         pack_wave(blob, sd, wave_cfg or WaveConfig())

@@ -11,8 +11,8 @@ import torch
 from torch.utils.weak import WeakIdKeyDictionary
 
 from . import lib as L_
-from .config import ModelConfig
-from .engine import (Arena, CTX_TOKENS_MAX, DecoderCompiler, MAX_STEPS, OpList, UNetCompiler, View, tc_weight_map)
+from .config import EncoderConfig, ModelConfig
+from .engine import (Arena, CTX_TOKENS_MAX, DecoderCompiler, EncoderCompiler, MAX_STEPS, OpList, UNetCompiler, View, tc_weight_map)
 from .packer import WeightBlob, pack_model
 
 
@@ -105,7 +105,7 @@ class MugEngine:
         self.lib = L_.load()
         self.handle = C.c_void_p()
         L_.check(self.lib.mugd_create(self.device.index or 0, C.byref(self.handle)), "mugd_create")
-        self.blob = blob if blob is not None else pack_model(state_dict, self.cfg.unet, self.cfg.decoder)
+        self.blob = blob if blob is not None else pack_model(state_dict, self.cfg.unet, self.cfg.decoder, encoder_cfg=self.cfg.encoder)
         self.weights = self.blob.data.to(self.device)          # every weight once, fp32 (0.56 GB); tensor-core weights become hi in place
         self.wbase = self.weights.data_ptr()
         self.weights_lo: Optional[torch.Tensor] = None         # the lo operands of the tensor-core weights (second buffer)
@@ -223,6 +223,17 @@ class MugEngine:
 
     def decoder_session(self, B: int, Lz: int) -> "DecoderSession":
         return self._lru_get(self.dec_sessions, (B, Lz), lambda: DecoderSession(self, B, Lz))
+
+    @property
+    def encoder_cfg(self) -> EncoderConfig:
+        if "encoder_cfg" not in self.blob.meta:
+            raise L_.MugdError("this engine was packed without model.first_stage_model.encoder.* weights")
+        return self.blob.meta["encoder_cfg"]
+
+    def encoder_session(self, B: int, Lz: int) -> "EncoderSession":
+        """Chart encoder plan for B note arrays of 2^(levels-1) * Lz frames (8 Lz for the shipped model); needs encoder weights."""
+        self.encoder_cfg                      # raises when the blob has no encoder
+        return self._lru_get(self.dec_sessions, ("enc", B, Lz), lambda: EncoderSession(self, B, Lz))
 
     def __del__(self):
         try:
@@ -473,7 +484,7 @@ class DecoderSession:
         self.engine, self.B, self.Lz = engine, B, Lz
         comp = DecoderCompiler(engine.cfg.decoder, engine.blob, engine.wbase, engine.tc_map)
         self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz))
-        self.zin, self.logits, self.Lout = res["zin"], res["logits"], res["Lout"]
+        self.zin, self.logits, self.Lout = res["inp"], res["out"], res["Lout"]
 
     def notes(self, frame_ms: float, key_count: int = 4):
         """Note extraction on the logits of the last ``decode`` (still resident, channels-last): returns
@@ -504,6 +515,75 @@ class DecoderSession:
         eng.ncl_to_rows(z.contiguous(), self.zin)
         self.plan.launch()
         return eng.rows_to_ncl(self.logits, self.B, cfg.x_channels, self.Lout)
+
+
+class EncoderSession:
+    """Compiled chart encoder (Encoder.forward, autoencoder.py:244-265) for B note arrays of ``frames`` = 2^(levels-1) * Lz frames."""
+
+    def __init__(self, engine: MugEngine, B: int, Lz: int):
+        self.engine, self.B, self.Lz = engine, B, Lz
+        self.cfg = engine.encoder_cfg
+        comp = EncoderCompiler(self.cfg, engine.blob, engine.wbase, engine.tc_map)
+        self.frames = Lz * comp.seq[0].mul
+        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz))
+        self.notes_rows, self.moments = res["inp"], res["out"]
+
+    def encode(self, notes: torch.Tensor) -> "DiagonalGaussianDistribution":
+        """notes [B, x_channels, frames] -> the posterior of AutoencoderKL.encode (autoencoder.py:67-73)"""
+        eng = self.engine
+        cfg = self.cfg
+        x = notes.to(eng.device, torch.float32).contiguous()
+        assert x.shape == (self.B, cfg.x_channels, self.frames), (tuple(x.shape), (self.B, cfg.x_channels, self.frames))
+        eng.ncl_to_rows(x, self.notes_rows)
+        self.plan.launch()
+        params = eng.rows_to_ncl(self.moments, self.B, 2 * cfg.z_channels, self.Lz)
+        return DiagonalGaussianDistribution(eng, params, cfg.scale)
+
+
+class DiagonalGaussianDistribution:
+    """The encoder's posterior with the surface callers use of the reference class of the same name (autoencoder.py:356-387):
+    ``parameters`` [B, 2Z, L], ``mean`` / ``logvar`` (clamped to [-10, 20]) / ``std`` / ``var`` [B, Z, L], ``mode()`` and ``sample()``.
+    All are device tensors; mean, logvar, std, mode() and sample() come from the posterior kernel (MUGD_OP_POSTERIOR)."""
+
+    def __init__(self, engine: MugEngine, parameters: torch.Tensor, scale: float):
+        self.engine, self.parameters, self.scale = engine, parameters, float(scale)
+        B, C2, L = parameters.shape
+        self.mean, self.logvar, self.std = (torch.empty(B, C2 // 2, L, device=parameters.device) for _ in range(3))
+        self._var: Optional[torch.Tensor] = None
+        self._run(mean=self.mean, logvar=self.logvar, std=self.std)
+
+    def _run(self, noise: Optional[torch.Tensor] = None, **outs: torch.Tensor):
+        B, Z, L = self.mean.shape
+        d = L_.Posterior()
+        d.params, d.noise = _ptr(self.parameters), _ptr(noise) if noise is not None else None
+        for name, t in outs.items():
+            setattr(d, name, _ptr(t))
+        d.scale, d.B, d.Z, d.L = self.scale, B, Z, L
+        ops = OpList()
+        ops.add(L_.OP_POSTERIOR, d)
+        with self.engine.lock:
+            self.engine.run_ops(ops)
+
+    @property
+    def var(self) -> torch.Tensor:
+        """exp(logvar) (autoencoder.py:365); only the KL term reads it, so it is formed on first use"""
+        if self._var is None:
+            self._var = torch.exp(self.logvar)
+        return self._var
+
+    def mode(self) -> torch.Tensor:
+        """mean * scale (autoencoder.py:386-387)"""
+        z = torch.empty_like(self.mean)
+        self._run(z=z)
+        return z
+
+    def sample(self) -> torch.Tensor:
+        """(mean + std * n) * scale with n = torch.randn(mean.shape) drawn on the CPU generator, as the reference draws it
+        (autoencoder.py:370-372): after torch.manual_seed(s) the result matches the reference's for the same s."""
+        noise = torch.randn(self.mean.shape).to(self.mean.device)
+        z = torch.empty_like(self.mean)
+        self._run(noise, z=z)
+        return z
 
 
 _NODE_CACHE: Dict[int, torch.Tensor] = {}

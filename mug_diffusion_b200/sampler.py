@@ -5,6 +5,7 @@ Reference surface kept (SURVEY §8b):
     samples, inter = sampler.sample(S, c, w, batch_size, ...)     mug/diffusion/ddim.py:56-107
     eps    = model.model.forward(x, t, c, w)                      mug/diffusion/diffusion.py:52-54
     logits = model.model.decode(z)                                mug/diffusion/diffusion.py:49-50
+    post   = model.model.encode({'note': notes})                  mug/diffusion/diffusion.py:46-47
 ``model`` is a ``MugDiffusionB200`` (build it with ``from_reference(ddpm)`` from a loaded reference DDPM, or
 ``from_state_dict``).  Every per-step op runs in libmugd; this file only does what the reference does on
 the host: the beta/alpha schedule tables, argument plumbing, callbacks and the RNG draw for eta > 0.
@@ -16,10 +17,12 @@ from typing import Dict, Optional, Sequence
 import numpy as np
 import torch
 
-from .config import DecoderConfig, ModelConfig, UNetConfig
+from .config import DecoderConfig, EncoderConfig, ModelConfig, UNetConfig
 from .engine import View
+from .lib import MugdError
+from .postprocess import objects_to_array
 from .prompt import PromptEmbedder
-from .runtime import MugEngine, Session, _ptr
+from .runtime import DiagonalGaussianDistribution, MugEngine, Session, _ptr
 
 try:  # the reference falls back to tqdm when no tqdm_class is given (ddim.py:133-135)
     from tqdm import tqdm as _tqdm
@@ -64,7 +67,7 @@ PROMPT_TABLE_KEY = "model.cond_stage_model.embedding.weight"
 
 
 class _Wrapper:
-    """Stands where ``MugDiffusionWrapper`` stands: ``.forward(x, t, c, w)`` and ``.decode(z)``."""
+    """Stands where ``MugDiffusionWrapper`` stands: ``.forward(x, t, c, w)``, ``.decode(z)`` and ``.encode(batch)``."""
 
     def __init__(self, owner: "MugDiffusionB200"):
         self._o = owner
@@ -93,6 +96,28 @@ class _Wrapper:
             B, _, Lz = z.shape
             return o.engine.decoder_session(B, Lz).decode(z)
 
+
+    @torch.no_grad()
+    def encode(self, batch) -> DiagonalGaussianDistribution:
+        """AutoencoderKL.encode of ``batch['note']`` [B, 16, 8L] (diffusion.py:46-47, autoencoder.py:67-73): the chart encoder on the
+        GPU.  Returns the posterior (``mode()`` is the latent of the chart, ``sample()`` draws from it)."""
+        o = self._o
+        notes = batch["note"]
+        with o.engine.lock:
+            f = 1 << (len(o.engine.encoder_cfg.channel_mult) - 1)        # note frames per latent frame
+            B, _, T = notes.shape
+            if T % f:
+                raise ValueError(f"note array length {T} is not a multiple of {f}")
+            return o.engine.encoder_session(B, T // f).encode(notes)
+
+    @torch.no_grad()
+    def encode_hit_objects(self, charts: Sequence[Sequence[str]], frame_ms: float, key_count: int = 4) -> DiagonalGaussianDistribution:
+        """The mirror of ``decode_to_hit_objects``: per chart a list of .osu hit-object lines -> note arrays of 8 * z_length frames
+        (OsuManiaConvertor.objects_to_array on the host, convertor.py:266-320) -> ``encode``.  Returns the posterior."""
+        o = self._o
+        T = (1 << (len(o.engine.encoder_cfg.channel_mult) - 1)) * o.z_length
+        notes = np.stack([objects_to_array(lines, key_count, frame_ms, T)[0] for lines in charts])
+        return self.encode({"note": torch.from_numpy(notes).to(o.device)})
 
     @torch.no_grad()
     def cond_stage_model(self, feature: torch.Tensor) -> torch.Tensor:
@@ -179,9 +204,27 @@ class MugDiffusionB200:
         dcfg = DecoderConfig(x_channels=sd_all[pre + "conv_out.weight"].shape[0], middle_channels=mid,
                              z_channels=sd_all[pre + "conv_in.weight"].shape[1], num_groups=groups,
                              channel_mult=mult, num_res_blocks=dd.num_res_blocks, scale=float(fs.scale))
+        if getattr(fs, "log_var", None) is not None:
+            # AutoencoderKL(constant_var=...) replaces the encoder's logvar by one parameter (autoencoder.py:34-36,69-72)
+            raise MugdError("first-stage models built with constant_var are not supported (the shipped config does not use it)")
+        ecfg = None
+        epre = "model.first_stage_model.encoder."
+        if epre + "conv_in.weight" in sd_all:
+            # recover the encoder's ddconfig from its conv shapes (autoencoder.py:185-242)
+            emid, xch = (int(n) for n in sd_all[epre + "conv_in.weight"].shape[:2])
+            nlev = 0
+            while f"{epre}down.{nlev}.block.0.conv1.weight" in sd_all:
+                nlev += 1
+            nrb = 0
+            while f"{epre}down.0.block.{nrb}.conv1.weight" in sd_all:
+                nrb += 1
+            emult = tuple(int(sd_all[f"{epre}down.{l}.block.0.conv1.weight"].shape[0]) // emid for l in range(nlev))
+            egroups = fs.encoder.norm_out.num_groups if hasattr(fs, "encoder") else groups
+            ecfg = EncoderConfig(x_channels=xch, middle_channels=emid, z_channels=int(sd_all[epre + "conv_out.weight"].shape[0]) // 2,
+                                 num_groups=egroups, channel_mult=emult, num_res_blocks=nrb, scale=float(fs.scale))
         cfg = ModelConfig(unet=UNetConfig.from_module(unet), decoder=dcfg, z_channels=int(ddpm.z_channels),
                           timesteps=int(ddpm.num_timesteps), linear_start=float(ddpm.linear_start),
-                          linear_end=float(ddpm.linear_end))
+                          linear_end=float(ddpm.linear_end), encoder=ecfg)
         return sd_all, cfg
 
     # the reference's q_sample, used only by the inpainting (mask) branch of ddim_sampling (ddim.py:141-144)

@@ -19,8 +19,8 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 import torch
 
-from .config import DecoderConfig, ModelConfig, UNetConfig
-from .netspec import decoder_param_specs, unet_layout, unet_param_specs
+from .config import DecoderConfig, EncoderConfig, ModelConfig, UNetConfig
+from .netspec import decoder_param_specs, encoder_param_specs, unet_layout, unet_param_specs
 
 
 def _rng(seed: int, name: str) -> np.random.Generator:
@@ -86,6 +86,11 @@ def synthetic_state_dict(z_length: int, cfg: Optional[ModelConfig] = None, seed:
         for name, (shape, role) in decoder_param_specs(cfg.decoder).items():
             sd[name] = _init(name, shape, role, seed)
     return sd
+
+
+def synthetic_encoder_state_dict(cfg: Optional[EncoderConfig] = None, seed: int = 0) -> Dict[str, torch.Tensor]:
+    """``model.first_stage_model.encoder.*`` tensors of the chart encoder, same per-name seeded initialiser as the rest."""
+    return {name: _init(name, shape, role, seed) for name, (shape, role) in encoder_param_specs(cfg or EncoderConfig()).items()}
 
 
 def _gauss(rng: np.random.Generator, shape) -> torch.Tensor:

@@ -2,7 +2,7 @@
 tools/ref_shim.py) on the seeded synthetic weights/inputs of mug_diffusion_b200.synth.
 
 Run in the build container only (the GPU box has no /root/reference):
-    python tools/make_goldens.py [--only blocks|unet|ddim]
+    python tools/make_goldens.py [--only blocks|unet|ddim|s4len|wave|notes|prompt|encoder|objects]
 """
 import argparse
 import os
@@ -17,6 +17,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
+import encoder_cases as ec  # noqa: E402
 import golden_cases as gc  # noqa: E402
 import ref_shim  # noqa: E402
 from mug_diffusion_b200 import synth  # noqa: E402
@@ -182,6 +183,49 @@ def make_hit_objects():
     print("wrote hit_objects.json", {k: (len(v) if isinstance(v, list) else v) for k, v in out.items()}, [len(c) for c in out["synthetic"]])
 
 
+def _reference_convertor(frame_ms, max_frame, rate=1.0, offset_ms=0.0):
+    ref_shim.install_shims()
+    from mug.data.convertor import BeatmapMeta, OsuManiaConvertor
+    return OsuManiaConvertor(frame_ms=frame_ms, max_frame=max_frame, rate=rate, offset_ms=offset_ms), BeatmapMeta
+
+
+@torch.no_grad()
+def make_encoder():
+    """AutoencoderKL.encode of the UNMODIFIED reference (autoencoder.py:67-73, 185-265, 356-387) with the synthetic encoder weights on
+    two note arrays of 8 * 96 frames: the reference's objects_to_array of the first ddim_L96_B2_S10_cfg5 chart, and a dense uniform
+    array.  sample() runs after torch.manual_seed(SAMPLE_SEED)."""
+    model, _ = ref_shim.load_reference_model()
+    esd = synth.synthetic_encoder_state_dict(seed=ec.ENCODER_SEED)
+    missing, unexpected = model.load_state_dict(esd, strict=False)
+    assert not [k for k in missing if k.startswith("model.first_stage_model.encoder.")] and not unexpected
+    frames = 8 * ec.ENCODER_L
+    conv, Meta = _reference_convertor(ec.golden_charts()["frame_ms"], frames)
+    chart, _ = conv.objects_to_array(ec.encoder_chart_lines(), Meta(path="", cs=4))
+    notes = torch.from_numpy(np.stack([chart, ec.dense_notes(frames)]).astype(np.float32))
+    post = model.model.encode({"note": notes})
+    mode = post.mode()
+    torch.manual_seed(ec.SAMPLE_SEED)
+    sample = post.sample()
+    save(f"encoder_L{ec.ENCODER_L}_B{ec.ENCODER_B}", parameters=post.parameters.numpy(), mean=post.mean.numpy(),
+         logvar=post.logvar.numpy(), std=post.std.numpy(), mode=mode.numpy(), sample=sample.numpy())
+
+
+def make_objects():
+    """OsuManiaConvertor.objects_to_array of the UNMODIFIED reference on every case of tests/encoder_cases.py: the note array and
+    valid_flag (only outputs are stored; the inputs are listed in encoder_cases.py)."""
+    import gzip
+    import json
+    out = {}
+    for c in ec.objects_cases():
+        conv, Meta = _reference_convertor(c["frame_ms"], c["max_frame"], c["rate"], c["offset_ms"])
+        arr, valid = conv.objects_to_array(c["lines"], Meta(path="", cs=c["key_count"]))
+        assert arr.dtype == np.float32
+        out[c["name"]] = dict(array=arr.tolist(), valid_flag=valid.tolist())
+    with gzip.open(os.path.join(GOLD, "objects_to_array.json.gz"), "wt") as f:
+        json.dump(out, f, separators=(",", ":"))
+    print("wrote objects_to_array.json.gz", len(out), "cases")
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", default=None)
@@ -202,5 +246,9 @@ if __name__ == "__main__":
         make_hit_objects()
     if a.only in (None, "prompt"):
         make_prompt()
+    if a.only in (None, "encoder"):
+        make_encoder()
+    if a.only in (None, "objects"):
+        make_objects()
 
 
