@@ -40,9 +40,10 @@ namespace mugd {
 const std::vector<mugd_op>& plan_ops(const mugd_plan* p) { return p->ops; }
 int plan_from_ops(mugd_handle* h, const mugd_op* ops, int32_t n, mugd_plan** out) { return mugd_plan_create(h, ops, n, out); }
 
-static int dispatch(mugd_handle* h, const mugd_op& op, cudaStream_t st, int* launches) {
+// next_tc: the next tensor-core GEMM after `op` in its plan (NULL outside a plan): a GEMM op prefetches its weights
+static int dispatch(mugd_handle* h, const mugd_op& op, cudaStream_t st, int* launches, const mugd_gemm* next_tc = nullptr) {
     switch (op.kind) {
-        case MUGD_OP_GEMM: return launch_gemm(h->dev, op.u.gemm, h->default_gemm_impl, st, launches);
+        case MUGD_OP_GEMM: return launch_gemm(h->dev, op.u.gemm, h->default_gemm_impl, next_tc, st, launches);
         case MUGD_OP_GROUPNORM: return launch_groupnorm(h->dev, op.u.gn, st, launches);
         case MUGD_OP_LAYERNORM: return launch_layernorm(h->dev, op.u.ln, st, launches);
         case MUGD_OP_ATTENTION: return launch_attention(h->dev, op.u.attn, st, launches);
@@ -149,8 +150,14 @@ int mugd_plan_create(mugd_handle* h, const mugd_op* ops, int32_t n_ops, mugd_pla
 int mugd_plan_run(mugd_plan* p, void* stream) {
     MUGD_REQUIRE(p, "null plan");
     int launches = 0;
-    for (size_t i = 0; i < p->ops.size(); ++i) {
-        int rc = dispatch(p->h, p->ops[i], (cudaStream_t)stream, &launches);
+    const size_t n = p->ops.size();
+    std::vector<const mugd_gemm*> next_tc(n, nullptr);
+    for (size_t i = n; i-- > 1;) {
+        const mugd_op& o = p->ops[i];
+        next_tc[i - 1] = o.kind == MUGD_OP_GEMM && gemm_runs_tc(o.u.gemm, p->h->default_gemm_impl) ? &o.u.gemm : next_tc[i];
+    }
+    for (size_t i = 0; i < n; ++i) {
+        int rc = dispatch(p->h, p->ops[i], (cudaStream_t)stream, &launches, next_tc[i]);
         if (rc != MUGD_OK) {
             char prev[900];
             strncpy(prev, g_err, sizeof(prev) - 1);

@@ -47,7 +47,9 @@ struct DeviceInfo {
 
 // per-family launchers (each validates its descriptor and enqueues kernels on `st`);
 // they return the number of kernels launched through *launches (may be null)
-int launch_gemm(const DeviceInfo& dev, const mugd_gemm& g, int default_impl, cudaStream_t st, int* launches);
+// next: the plan's next GEMM that runs on the tensor cores (or NULL); a tensor-core GEMM prefetches its weights into L2
+int launch_gemm(const DeviceInfo& dev, const mugd_gemm& g, int default_impl, const mugd_gemm* next, cudaStream_t st, int* launches);
+bool gemm_runs_tc(const mugd_gemm& g, int default_impl);
 int launch_groupnorm(const DeviceInfo& dev, const mugd_groupnorm& g, cudaStream_t st, int* launches);
 int launch_layernorm(const DeviceInfo& dev, const mugd_layernorm& g, cudaStream_t st, int* launches);
 int launch_attention(const DeviceInfo& dev, const mugd_attention& a, cudaStream_t st, int* launches);
@@ -60,7 +62,7 @@ int launch_notes(const DeviceInfo& dev, const mugd_notes& n, cudaStream_t st, in
 int launch_embed(const DeviceInfo& dev, const mugd_embed& e, cudaStream_t st, int* launches);
 int launch_tf32_split(const DeviceInfo& dev, const mugd_tf32_split& s, cudaStream_t st, int* launches);
 int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_t st, int* launches);
-int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, cudaStream_t st, int* launches);
+int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, cudaStream_t st, int* launches);
 bool gemm_tc_supported(const mugd_gemm& g);
 
 // Programmatic dependent launch (PDL): every hot-path kernel is launched with the programmatic-stream-serialization

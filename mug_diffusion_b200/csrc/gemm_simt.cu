@@ -243,12 +243,16 @@ static int validate_gemm(const mugd_gemm& g) {
     return MUGD_OK;
 }
 
-int launch_gemm(const DeviceInfo& dev, const mugd_gemm& g, int default_impl, cudaStream_t st, int* launches) {
+bool gemm_runs_tc(const mugd_gemm& g, int default_impl) {
+    return (g.impl == MUGD_GEMM_AUTO ? default_impl : g.impl) == MUGD_GEMM_TC && gemm_tc_supported(g);
+}
+
+int launch_gemm(const DeviceInfo& dev, const mugd_gemm& g, int default_impl, const mugd_gemm* next, cudaStream_t st, int* launches) {
     int rc = validate_gemm(g);
     if (rc != MUGD_OK) return rc;
     int impl = g.impl == MUGD_GEMM_AUTO ? default_impl : g.impl;
     if (impl == MUGD_GEMM_TC) {
-        if (gemm_tc_supported(g)) return launch_gemm_tc(dev, g, st, launches);
+        if (gemm_tc_supported(g)) return launch_gemm_tc(dev, g, next, st, launches);
         MUGD_REQUIRE(g.impl != MUGD_GEMM_TC, "gemm: tensor-core path requested but shape unsupported (M=%d N=%d K=%d)", g.M, g.N, g.K);
     }
     // a weight that was split in place (W_hi == W) no longer holds fp32 values: the FFMA kernel must never read it

@@ -15,9 +15,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;       // SWIZZLE_128B needs 1024-B alignment
     const TcBars<BN> B(base);
-#ifdef MUGD_TC_TIMELINE
-    if (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0) p.dbg[0] = gtimer();
-#endif
+    TC_STAMP(p, 0, blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0);
     // ---- one-time setup: barriers; nothing here touches memory written by the previous kernel ----
     if (threadIdx.x < 32) {
         B.init_parallel((int)threadIdx.x);
@@ -28,6 +26,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
     }
     __syncthreads();
+    TC_STAMP(p, 1, blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0);
     gemm_tc_tile<BN, true, EPI>(&tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p, blockIdx.x, blockIdx.y, blockIdx.z, base);
 }
 
@@ -143,7 +142,7 @@ TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split) {
     return t;
 }
 
-int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, TcPlanned* out) {
+int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, TcPlanned* out) {
     MUGD_REQUIRE(gemm_tc_supported(g), "gemm_tc: unsupported shape/operands");
     {
         const int rc = tc_validate_fusions(g);
@@ -221,6 +220,11 @@ int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, TcPlanned* out) {
     p.it_rem = t.total_it % t.splits;
     p.hot = {p.Lrows, p.Bs, p.box_l, p.box_b, p.tiles_per_sample, p.it_base, p.it_rem, p.it_main, p.kblocks, p.total_it, p.splits, p.single_pass,
              g.conv_mode, g.tap_shift, g.tap_dilation, p.gx};
+    if (next) {
+        p.pf_hi = next->W_hi;
+        p.pf_lo = p.single_pass ? nullptr : next->W_lo;
+        p.pf_bytes = (int64_t)next->N * ((int64_t)next->taps * next->K + next->K2) * 4;
+    }
 #ifdef MUGD_TC_TIMELINE
     p.dbg = g_tc_dbg;
 #endif
@@ -266,9 +270,9 @@ static int tc_launch_bn(const TcPlanned& pl, cudaStream_t st) {
     }
 }
 
-int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, cudaStream_t st, int* launches) {
+int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, cudaStream_t st, int* launches) {
     TcPlanned pl;
-    int rc = tc_plan(dev, g, &pl);
+    int rc = tc_plan(dev, g, next, &pl);
     if (rc != MUGD_OK) return rc;
     if (pl.p.BN == 128) rc = tc_launch_bn<128>(pl, st);
     else rc = tc_launch_bn<64>(pl, st);

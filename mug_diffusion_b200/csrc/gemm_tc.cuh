@@ -11,7 +11,9 @@
 //                  W_hi / W_lo tiles; completion on an mbarrier, release of a stage by one arrival per warp.
 //   warpgroups   : warpgroup w owns tile rows 64w..64w+63.  Each thread reads its A fragment out of the swizzled raw tile, splits
 //                  it into a_hi / a_lo (cvt.rna.tf32) in registers and issues 12 wgmma.m64nBNk8.tf32 per k-step (A from
-//                  registers, B = weight tile through a shared-memory descriptor); the next stage is split while they run.
+//                  registers, B = weight tile through a shared-memory descriptor); the next stage is split while they run, and one
+//                  k-step of MMAs stays in flight across the k-step boundary.
+//   prefetch     : the producer lane also pulls its CTA's slice of the NEXT tensor-core GEMM's weights into L2.
 //   epilogue 1   : accumulator registers -> shared memory (row pitch BN+4), over the then idle pipeline buffers
 //   epilogue 2   : all warps: bias / time-embedding row / SiLU / GELU / GEGLU / GLU / residual, row-contiguous coalesced stores;
 //                  with split-K the partial tile goes to an L2-resident workspace and tc_reduce_item() sums the splits in fixed
@@ -53,8 +55,14 @@ struct TcParams {
     int32_t sm_count;
     double ln_invK;           // 1 / K (folded LayerNorm: moments -> mean / variance)
     int32_t it_base, it_rem;  // split z owns k-steps [z*it_base + min(z, it_rem), +it_base + (z < it_rem)): no division on the device
+    // W_hi / W_lo of the next tensor-core GEMM of the plan (pf_lo NULL in single-pass mode, pf_bytes 0 = none), prefetched into L2
+    // while this GEMM runs: the next launch then reads its first stages from L2 instead of HBM.  Weights are written once, when the
+    // engine is built, so the prefetch cannot race with a producer.
+    const float* pf_hi;
+    const float* pf_lo;
+    int64_t pf_bytes;
 #ifdef MUGD_TC_TIMELINE
-    long long* dbg;           // CTA (0,0,0) writes globaltimer stamps (tools/gemm_timeline.py)
+    long long* dbg;           // CTA (0,0,0) writes globaltimer stamps (TC_STAMP, tools/bench_gemm.py)
 #endif
 };
 
@@ -65,6 +73,13 @@ __device__ __forceinline__ long long gtimer() {
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory");
     return t;
 }
+// Phase stamps of CTA (0,0,0), thread 0 (MUGD_TC_TIMELINE builds): [0] entry, [1] barriers armed, [2] main loop done, [3] tile staged
+// in shared memory, [4] tile stored.  tools/bench_gemm.py prints the differences as setup / main / stage / epi.
+#ifdef MUGD_TC_TIMELINE
+#define TC_STAMP(p, k, cta0) do { if ((p).dbg && (cta0) && threadIdx.x == 0) (p).dbg[k] = gtimer(); } while (0)
+#else
+#define TC_STAMP(p, k, cta0) do { } while (0)
+#endif
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -108,6 +123,9 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
         : "memory");
+}
+__device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {     // p 16-byte aligned, bytes a multiple of 16
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(p)), "r"(bytes) : "memory");
 }
 // One lane of a converged warp: cp.async.bulk.tensor is a uniform-datapath instruction; issued from a lane-divergent branch
 // (`if (lane == 0)`) ptxas wraps it in an elect-and-branch loop, guarded by elect.sync in a converged warp it issues directly.
@@ -420,6 +438,16 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
             for (int i = 0; i < pro; ++i) issue_w(i);
             if (PDL) pdl_wait();                 // activations written by the previous kernel are touched from here on
             for (int i = 0; i < pro; ++i) issue_a(i);
+            if (p.pf_bytes > 0) {                // after this CTA's own loads: CTA c prefetches slice c of the next GEMM's weights
+                const int64_t ncta = (int64_t)p.gx * p.gy * p.splits;
+                const int64_t per = (p.pf_bytes / ncta + 15) & ~(int64_t)15;
+                const int64_t off = (((int64_t)bz * p.gy + by) * p.gx + bx) * per;
+                const int64_t n = min(per, p.pf_bytes - off);
+                if (n > 0) {
+                    prefetch_l2(reinterpret_cast<const char*>(p.pf_hi) + off, (uint32_t)n);
+                    if (p.pf_lo) prefetch_l2(reinterpret_cast<const char*>(p.pf_lo) + off, (uint32_t)n);
+                }
+            }
         }
         __syncwarp();
     }
@@ -450,48 +478,64 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     }
 
     // ===================================== main loop (both warpgroups) =====================================
+    // One k-step of MMAs stays in flight.  Step i reads one of two A-fragment register sets; once it is issued, step i-1 is retired
+    // (wgmma_wait<1>), which frees the other set for step i+1's split and lets this warp release step i-1's stage.  Warp 0 refills
+    // that stage when both warpgroups have released it: at that point its own warpgroup still has step i queued on the tensor cores,
+    // so neither warpgroup drains its MMAs to wait for the other.
     const int wg = warp >> 2, g8 = lane >> 2, t4 = lane & 3;
     const int r0 = wg * 64 + (warp & 3) * 16 + g8;                 // this thread's first fragment row (the second is r0 + 8)
     float acc[NACC];
 #pragma unroll
     for (int j = 0; j < NACC; ++j) acc[j] = 0.f;
-    TcAFrag fa;
+    TcAFrag f0, f1;
     if (nit > 0) {
         mbar_wait(B.full(0), 0u);
-        tc_load_split(a_raw(0), r0, t4, fa);
+        tc_load_split(a_raw(0), r0, t4, f0);
     }
-    for (int i = 0; i < nit; ++i) {
-        const int s = i % STAGES;
-        const uint64_t dbh = wgmma_desc(b_hi(s)), dbl = wgmma_desc(b_lo(s));
-        wgmma_fence();
+    auto main_loop = [&](auto single_tag) {
+        constexpr bool SINGLE = decltype(single_tag)::value;
+        auto kstep = [&](int i, const TcAFrag& cur, TcAFrag& nxt) {
+            const int s = i % STAGES;
+            const uint64_t dbh = wgmma_desc(b_hi(s)), dbl = wgmma_desc(b_lo(s));
+            wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < TC_BK / 8; ++kk) {
-            const uint64_t ko = (uint64_t)(kk * 2);          // 8 fp32 = 32 bytes = 2 x 16-byte units
-            if (h.single_pass) {
-                Wgmma<BN>::mma(acc, fa.hi[kk], dbh + ko);
-            } else {
-                Wgmma<BN>::mma(acc, fa.lo[kk], dbh + ko);
-                Wgmma<BN>::mma(acc, fa.hi[kk], dbl + ko);
-                Wgmma<BN>::mma(acc, fa.hi[kk], dbh + ko);
+            for (int kk = 0; kk < TC_BK / 8; ++kk) {
+                const uint64_t ko = (uint64_t)(kk * 2);      // 8 fp32 = 32 bytes = 2 x 16-byte units
+                if constexpr (SINGLE) {
+                    Wgmma<BN>::mma(acc, cur.hi[kk], dbh + ko);
+                } else {
+                    Wgmma<BN>::mma(acc, cur.lo[kk], dbh + ko);
+                    Wgmma<BN>::mma(acc, cur.hi[kk], dbl + ko);
+                    Wgmma<BN>::mma(acc, cur.hi[kk], dbh + ko);
+                }
             }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (i > 0) {
+                const int j = i - 1, sj = j % STAGES;
+                __syncwarp();
+                if (lane == 0) mbar_arrive(B.empty(sj));
+                if (warp == 0 && j + STAGES < nit) {
+                    mbar_wait(B.empty(sj), (uint32_t)(j / STAGES) & 1u);    // both warpgroups are done with stage sj: refill it
+                    if (elect_one()) { issue_w(j + STAGES); issue_a(j + STAGES); }
+                    __syncwarp();
+                }
+            }
+            // the next stage's activations are split while the tensor cores work on this one
+            if (i + 1 < nit) {
+                mbar_wait(B.full((i + 1) % STAGES), (uint32_t)((i + 1) / STAGES) & 1u);
+                tc_load_split(a_raw((i + 1) % STAGES), r0, t4, nxt);
+            }
+        };
+        for (int i = 0; i < nit; i += 2) {
+            kstep(i, f0, f1);
+            if (i + 1 < nit) kstep(i + 1, f1, f0);
         }
-        wgmma_commit();
-        // the next stage's activations are split while the tensor cores work on this one
-        TcAFrag fn;
-        if (i + 1 < nit) {
-            mbar_wait(B.full((i + 1) % STAGES), (uint32_t)((i + 1) / STAGES) & 1u);
-            tc_load_split(a_raw((i + 1) % STAGES), r0, t4, fn);
-        }
-        wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(B.empty(s));
-        if (warp == 0 && i + STAGES < nit) {
-            mbar_wait(B.empty(s), (uint32_t)(i / STAGES) & 1u);      // both warpgroups are done with stage s: refill it
-            if (elect_one()) { issue_w(i + STAGES); issue_a(i + STAGES); }
-            __syncwarp();
-        }
-        if (i + 1 < nit) fa = fn;
-    }
+    };
+    if (h.single_pass) main_loop(std::true_type{});
+    else main_loop(std::false_type{});
+    wgmma_wait<0>();
+    TC_STAMP(p, 2, bx == 0 && by == 0 && bz == 0);
     // LayerNorm folded into this GEMM: the moments of tile row threadIdx.x -> mean / rstd
     float2 lnrow = make_float2(0.f, 1.f);
     if constexpr (TcEpiTraits<EPI>::MODE == TC_EPI_LN) lnrow = tc_ln_from_moments(ln_s, ln_ss, p.ln_invK, g.ln_eps);
@@ -513,6 +557,7 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     }
     // ---- phase 2 (all 8 warps): consecutive threads take consecutive float4 of a row -> coalesced global traffic.
     __syncthreads();
+    TC_STAMP(p, 3, bx == 0 && by == 0 && bz == 0);
     {
         const float* rowvec = g.rowvec ? g.rowvec + (int64_t)epi_step * g.rowvec_step_stride : nullptr;
         if (p.splits > 1) {
@@ -538,6 +583,7 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
             tc_store_tile<BN, E::ACT, E::GATE, E::MODE>(g, base, m_base, n0, rows_valid, rowvec, base + S::TILE_BYTES - 1024u, epi_bias, epi_cs);
         }
     }
+    TC_STAMP(p, 4, bx == 0 && by == 0 && bz == 0);
 }
 
 // split-K second pass.  One call = one thread's share of reduce block `blk`: TC_RED_R output rows x one 4-column group.  A block of
@@ -630,6 +676,7 @@ struct alignas(64) TcPlanned {
     TcParams p;
 };
 TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split);
-int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, TcPlanned* out);     // validates, picks the geometry, encodes the maps
+// validates, picks the geometry, encodes the maps; `next` (or NULL): the tensor-core GEMM whose weights this one prefetches into L2
+int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, TcPlanned* out);
 
 }  // namespace mugd
