@@ -9,7 +9,7 @@
  * and the entry points below are what a ctypes binding on the reference side would call
  * (INTEGRATION.md shows that binding).  Plain pointers and sizes only: every pointer is a DEVICE pointer
  * into memory the caller owns (torch allocations in the Python host), `stream` is a cudaStream_t passed
- * as void*.  No CPU fallback exists: mugd_create fails on anything that is not compute capability 10.x.
+ * as void*.  No CPU fallback exists: mugd_create fails on anything that is not compute capability 9.0.
  *
  * Execution model: the host "compiles" a network evaluation into a flat launch plan (array of mugd_op,
  * pointers fully resolved), the library validates it, optionally captures it into a CUDA graph, and

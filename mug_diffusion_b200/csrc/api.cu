@@ -89,12 +89,17 @@ int mugd_create(int device, mugd_handle** out) {
         return MUGD_ERR_NO_DEVICE;
     }
     MUGD_CHECK_CUDA(cudaSetDevice(device));
+    const int smem_optin = (int)prop.sharedMemPerBlockOptin;
+    MUGD_CHECK_CUDA(gemm_tc_allow_smem(smem_optin));
+    MUGD_CHECK_CUDA(attention_tc_allow_smem(smem_optin));
+    MUGD_CHECK_CUDA(attention_allow_smem(smem_optin));
+    MUGD_CHECK_CUDA(s4_allow_smem(smem_optin));
     mugd_handle* h = new mugd_handle();
     h->dev.device = device;
     h->dev.sm_count = prop.multiProcessorCount;
     h->dev.cc_major = prop.major;
     h->dev.cc_minor = prop.minor;
-    h->dev.max_smem_optin = (int)prop.sharedMemPerBlockOptin;
+    h->dev.max_smem_optin = smem_optin;
     *out = h;
     return MUGD_OK;
 }

@@ -46,7 +46,6 @@ attention_kernel(const mugd_attention a) {
     const int P = a.pos_max, NT = 2 * P + 1;
     float* cg = rel + NT;
 
-    pdl_trigger();
     pdl_wait();
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
     const int b = blockIdx.z, h = blockIdx.y;
@@ -167,14 +166,13 @@ attention_kernel(const mugd_attention a) {
     }
 }
 
+cudaError_t attention_allow_smem(int bytes) {
+    return allow_dynamic_smem(bytes, attention_kernel<32>, attention_kernel<48>, attention_kernel<64>);
+}
+
 template <int D>
 static int attention_launch(const mugd_attention& a, cudaStream_t st) {
     const size_t bytes = sizeof(float) * (AttSmem<D>::FLOATS + 2 * (2 * a.pos_max + 1));
-    static size_t configured = 0;
-    if (bytes > configured) {
-        MUGD_CHECK_CUDA(cudaFuncSetAttribute(attention_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-        configured = bytes;
-    }
     dim3 grid((a.Lq + AT_BQ - 1) / AT_BQ, a.H, a.B);
     MUGD_CHECK_CUDA(launch_k(attention_kernel<D>, grid, dim3(AT_THREADS), bytes, st, a));
     return MUGD_OK;

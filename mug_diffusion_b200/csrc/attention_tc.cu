@@ -35,62 +35,6 @@ constexpr int BQ = 128;
 constexpr int BKV = 128;
 constexpr uint32_t SLAB = BKV * 128;          // 128 keys x (32 fp32 channels = 128 B): one swizzle-atom column of a tile
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// bounded wait: a protocol bug traps (CUDA error) instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-    const long long t0 = clock64();
-    while (true) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(bar), "r"(parity)
-            : "memory");
-        if (done) break;
-        if (clock64() - t0 > 4000000000LL) __trap();
-    }
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-// one lane of a converged warp (see gemm_tc.cuh: uniform-datapath instructions must not sit in a lane-divergent branch)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-        "elect.sync rx|px, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, px;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ float to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
-}
-__device__ __forceinline__ float4 lds_f4(uint32_t addr) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
-__device__ __forceinline__ void sts_f1(uint32_t addr, float v) {
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
-}
-__device__ __forceinline__ void sts_f4(uint32_t addr, float4 v) {
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-
 template <int D>
 struct Smem {
     static constexpr int KSLABS = (D + 31) / 32;           // 32-channel slabs per head slice (head dim 48: 1.5 used)
@@ -130,10 +74,9 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     const int qa = q0 + rq, qb = qa + 8;
     const int ntiles = (a.Lk + BKV - 1) / BKV;
 
-    pdl_trigger();
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) mbar_init(bar_full(s), 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init_fence();
     }
     __syncthreads();
     pdl_wait();
@@ -322,57 +265,34 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qr;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qr) == cudaSuccess && qr == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
 // (channel, key, sample) view of a [B*Lk, ld] row-major buffer whose first H*D columns are the head slices
-static int encode_kv(EncodeTiledFn enc, CUtensorMap* tm, const float* p, int64_t ld, int cols, int Lk, int B) {
-    cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)Lk, (cuuint64_t)B};
-    cuuint64_t strides[2] = {(cuuint64_t)ld * 4, (cuuint64_t)Lk * (cuuint64_t)ld * 4};
-    cuuint32_t box[3] = {32, (cuuint32_t)BKV, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(p), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    MUGD_REQUIRE(r == CUDA_SUCCESS, "attention_tc: cuTensorMapEncodeTiled failed with %d (cols=%d Lk=%d B=%d ld=%lld)", (int)r, cols, Lk, B,
-                 (long long)ld);
-    return MUGD_OK;
+static int encode_kv(CUtensorMap* tm, const float* p, int64_t ld, int cols, int Lk, int B) {
+    const cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)Lk, (cuuint64_t)B};
+    const cuuint64_t strides[2] = {(cuuint64_t)ld * 4, (cuuint64_t)Lk * (cuuint64_t)ld * 4};
+    const cuuint32_t box[3] = {32, (cuuint32_t)BKV, 1};
+    return encode_f32_tma(tm, p, 3, dims, strides, box, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "attention_tc");
 }
 
 static float* g_dbg = nullptr;      // debugging aid: CTA (0,0,0) dumps the raw logits of its first key tile (16 of each row's 40 floats)
 
 template <int D>
 static int launch(const mugd_attention& a, cudaStream_t st) {
-    EncodeTiledFn enc = get_encode();
-    MUGD_REQUIRE(enc != nullptr, "attention_tc: cuTensorMapEncodeTiled entry point not available");
     CUtensorMap tmK, tmV;
-    int rc = encode_kv(enc, &tmK, a.k, a.ldk, a.H * D, a.Lk, a.B);
+    int rc = encode_kv(&tmK, a.k, a.ldk, a.H * D, a.Lk, a.B);
     if (rc != MUGD_OK) return rc;
-    rc = encode_kv(enc, &tmV, a.v, a.ldv, a.H * D, a.Lk, a.B);
+    rc = encode_kv(&tmV, a.v, a.ldv, a.H * D, a.Lk, a.B);
     if (rc != MUGD_OK) return rc;
     const size_t bytes = Smem<D>::total(a.pos_max);
-    static size_t configured = 0;
-    if (bytes > configured) {
-        MUGD_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-        configured = bytes;
-    }
     dim3 grid((a.Lq + BQ - 1) / BQ, a.H, a.B);
     MUGD_CHECK_CUDA(launch_k(attention_tc_kernel<D>, grid, dim3(THREADS), bytes, st, tmK, tmV, a, g_dbg));
     return MUGD_OK;
 }
 
 }  // namespace atc
+
+cudaError_t attention_tc_allow_smem(int bytes) {
+    return allow_dynamic_smem(bytes, atc::attention_tc_kernel<32>, atc::attention_tc_kernel<48>, atc::attention_tc_kernel<64>);
+}
 
 int launch_attention_tc(const DeviceInfo&, const mugd_attention& a, cudaStream_t st) {
     return (a.D == 32) ? atc::launch<32>(a, st) : (a.D == 48) ? atc::launch<48>(a, st) : atc::launch<64>(a, st);

@@ -65,11 +65,19 @@ int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_
 int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, cudaStream_t st, int* launches);
 bool gemm_tc_supported(const mugd_gemm& g);
 
+// Kernels that need more than 48 KB of dynamic shared memory are allowed the device's opt-in maximum (`bytes`) by mugd_create, after
+// its cudaSetDevice: the attribute belongs to the current device's context, so it is set once for every device a handle is created
+// on.  A launch still asks for only its own byte count, so occupancy and the shared-memory carve-out do not change.  Each kernel
+// file lists its own instantiations.
+cudaError_t gemm_tc_allow_smem(int bytes);
+cudaError_t attention_tc_allow_smem(int bytes);
+cudaError_t attention_allow_smem(int bytes);
+cudaError_t s4_allow_smem(int bytes);
+
 // Programmatic dependent launch (PDL): every hot-path kernel is launched with the programmatic-stream-serialization
-// attribute, signals `launch_dependents` at entry and executes `griddepcontrol.wait` before its first global-memory
-// access.  The next kernel's launch latency and prologue (block scheduling, barrier init,
-// tensor-map fetch) then overlap the tail of the current one; data hazards are unchanged because the wait
-// only returns when the prerequisite grid has completed and flushed.
+// attribute and executes `griddepcontrol.wait` (pdl_wait) before its first access to memory the previous kernel wrote.  The next
+// kernel's launch latency and prologue (block scheduling, barrier init, tensor-map fetch) then overlap the tail of the current one;
+// data hazards are unchanged because the wait only returns when the prerequisite grid has completed and flushed.
 extern bool g_use_pdl;
 
 #ifdef __CUDACC__
@@ -87,10 +95,16 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
     cfg.numAttrs = g_use_pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
+// Lets each kernel launch with up to `bytes` of dynamic shared memory on the current device.
+template <typename... Kernels>
+inline cudaError_t allow_dynamic_smem(int bytes, Kernels... kernels) {
+    cudaError_t e = cudaSuccess;
+    ((e = (e == cudaSuccess) ? cudaFuncSetAttribute(kernels, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) : e), ...);
+    return e;
+}
 // No kernel signals launch_dependents explicitly: the trigger is implicit at grid completion, so PDL only overlaps the dependent's
 // launch with this grid's memory flush.  Explicit triggers
 // (at entry, in the short kernels only, after the GEMM main loop) were tried and not kept.
-__device__ __forceinline__ void pdl_trigger() {}
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // ---- device helpers ---------------------------------------------------------------------------

@@ -5,6 +5,7 @@
 //   step_advance: device-side step counter so one CUDA graph serves every DDIM step
 //   posterior   : first-stage encoder moments -> mean / logvar / std / z   mug/firststage/autoencoder.py:356-387
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace mugd {
 
@@ -13,7 +14,6 @@ namespace mugd {
 // ATen ops (no FMA contraction), so given identical eps the update is bit-identical.
 __global__ void __launch_bounds__(256)
 ddim_update_kernel(const mugd_ddim_update d) {
-    pdl_trigger();
     pdl_wait();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= d.n) return;
@@ -50,7 +50,6 @@ int launch_ddim_update(const DeviceInfo&, const mugd_ddim_update& d, cudaStream_
 __global__ void __launch_bounds__(256)
 transpose_kernel(const mugd_transpose t) {
     __shared__ float tile[32][33];
-    pdl_trigger();
     pdl_wait();
     const int b = blockIdx.z;
     const int c0 = blockIdx.y * 32, l0 = blockIdx.x * 32;
@@ -99,7 +98,6 @@ int launch_transpose(const DeviceInfo&, const mugd_transpose& t, cudaStream_t st
 
 __global__ void __launch_bounds__(256)
 copy2d_kernel(const mugd_copy2d c) {
-    pdl_trigger();
     pdl_wait();
     const int q = c.cols >> 2;
     const int64_t total = (int64_t)c.rows * q;
@@ -126,12 +124,8 @@ __global__ void __launch_bounds__(256)
 tf32_split_kernel(float* __restrict__ w_hi, float* __restrict__ lo, int64_t n4) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
         const float4 w = ld_f4(w_hi + i * 4);
-        float4 h, l;
-        uint32_t r;
-#define MUGD_RNA(dst, src) asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(src)); dst = __uint_as_float(r)
-        MUGD_RNA(h.x, w.x); MUGD_RNA(h.y, w.y); MUGD_RNA(h.z, w.z); MUGD_RNA(h.w, w.w);
-        MUGD_RNA(l.x, w.x - h.x); MUGD_RNA(l.y, w.y - h.y); MUGD_RNA(l.z, w.z - h.z); MUGD_RNA(l.w, w.w - h.w);
-#undef MUGD_RNA
+        const float4 h = make_float4(to_tf32(w.x), to_tf32(w.y), to_tf32(w.z), to_tf32(w.w));
+        const float4 l = make_float4(to_tf32(w.x - h.x), to_tf32(w.y - h.y), to_tf32(w.z - h.z), to_tf32(w.w - h.w));
         st_f4(w_hi + i * 4, h);
         st_f4(lo + i * 4, l);
     }
@@ -148,7 +142,6 @@ int launch_tf32_split(const DeviceInfo& dev, const mugd_tf32_split& s, cudaStrea
 }
 
 __global__ void step_advance_kernel(int32_t* step) {
-    pdl_trigger();
     pdl_wait();
     *step += 1;
 }
@@ -166,7 +159,6 @@ int launch_step_advance(const DeviceInfo&, const mugd_step_advance& a, cudaStrea
 // compacted with a ballot/prefix scan so the output is ordered by frame like the reference's np.where loop.
 __global__ void __launch_bounds__(256)
 notes_kernel(const mugd_notes n) {
-    pdl_trigger();
     pdl_wait();
     const int c = blockIdx.x, b = blockIdx.y;
     const int K = n.K, T = n.T;
@@ -230,7 +222,6 @@ int launch_notes(const DeviceInfo&, const mugd_notes& n, cudaStream_t st, int* l
 // sample: 10 KB per request, latency only).
 __global__ void __launch_bounds__(128)
 embed_kernel(const mugd_embed e) {
-    pdl_trigger();
     pdl_wait();
     const int f = blockIdx.x, b = blockIdx.y;
     const int id = e.ids[b * e.F + f];
@@ -253,7 +244,6 @@ int launch_embed(const DeviceInfo&, const mugd_embed& e, cudaStream_t st, int* l
 // sample is mean + std*noise, then * scale (:371-372) with _rn intrinsics so no FMA contraction changes the rounding.
 __global__ void __launch_bounds__(256)
 posterior_kernel(const mugd_posterior p) {
-    pdl_trigger();
     pdl_wait();
     const int64_t zl = (int64_t)p.Z * p.L;
     const int64_t n = (int64_t)p.B * zl;

@@ -1,5 +1,4 @@
-// wgmma implicit GEMM: stand-alone kernels + host side (geometry planner, tensor-map encoding, launch).
-// The device code lives in gemm_tc.cuh (shared with other kernels that embed GEMM tiles).
+// wgmma implicit GEMM: kernels + host side (geometry planner, tensor-map encoding, launch).  The device code lives in gemm_tc.cuh.
 //
 // Reference call sites are the same as gemm_simt.cu (which remains the exact-fp32 referee and the fallback for
 // shapes this kernel does not take: K % 32 != 0, N < 16, generic upsampling addressing).
@@ -27,42 +26,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     __syncthreads();
     TC_STAMP(p, 1, blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0);
-    gemm_tc_tile<BN, true, EPI>(&tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p, blockIdx.x, blockIdx.y, blockIdx.z, base);
+    gemm_tc_tile<BN, EPI>(&tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p, blockIdx.x, blockIdx.y, blockIdx.z, base);
 }
 
-// split-K second pass: fully parallel over the GPU and L2-resident (see tc_reduce_rows).
+// split-K second pass: fully parallel over the GPU and L2-resident (see tc_reduce).
 template <int BN, int EPI>
 __global__ void __launch_bounds__(TC_THREADS)
 gemm_tc_reduce_kernel(const __grid_constant__ TcParams p) {
-    tc_reduce_block<BN, EPI>(p, blockIdx.x);           // waits for the GEMM (griddepcontrol.wait) after requesting its weight-side operands
+    tc_reduce<BN, EPI>(p, blockIdx.x);                 // waits for the GEMM (griddepcontrol.wait) after requesting its weight-side operands
 }
 
 #ifdef MUGD_TC_TIMELINE
 static long long* g_tc_dbg = nullptr;
 #endif
-// planner constants: us per k-step of a 128-wide tile, (unused) second tile-width slot, us per split-K round trip (workspace + reduce
-// launch), (unused) fourth slot.  They are relative weights of the tile-width / K-split decision; mugd_debug_set_tc_cost for sweeps.
-static float g_tc_cost[4] = {0.55f, 0.9f, 3.0f, 0.f};
+// planner constants: relative weights of the tile-width / K-split decision (mugd_debug_set_tc_cost for sweeps)
+static float g_tc_kstep128 = 0.55f;  // per k-step of a 128-wide tile
+static float g_tc_split = 3.0f;      // per split-K round trip (workspace + reduce launch)
 static int g_tc_force_bn = 0;        // experiments: 0 = cost model, 64 / 128 = force the tile width where legal
 
 // =====================================================================================================
 // host side
 // =====================================================================================================
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qr;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qr) == cudaSuccess && qr == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
 static bool tc_shape_ok(const mugd_gemm& g) {
     if (!(g.conv_mode == MUGD_CONV_NONE || g.conv_mode == MUGD_CONV_SAME || g.conv_mode == MUGD_CONV_DOWN ||
           g.conv_mode == MUGD_CONV_TAPS)) return false;
@@ -93,24 +77,27 @@ static int tc_validate_fusions(const mugd_gemm& g) {
 }
 
 TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split) {
-    TcGeometry t;
+    TcGeometry t = {};
+    TcParams::Hot& h = t.hot;
     t.BN = (g.N >= 128) ? 128 : 64;
-    if (g.conv_mode == MUGD_CONV_NONE) { t.Lrows = g.M; t.Bs = 1; }
-    else { t.Lrows = g.Lout; t.Bs = g.M / g.Lout; }
-    if (t.Lrows >= TC_BM) {
-        t.box_l = TC_BM; t.box_b = 1;
-        t.tiles_per_sample = (t.Lrows + TC_BM - 1) / TC_BM;
-        t.gy = t.tiles_per_sample * t.Bs;
+    if (g.conv_mode == MUGD_CONV_NONE) { h.Lrows = g.M; h.Bs = 1; }
+    else { h.Lrows = g.Lout; h.Bs = g.M / g.Lout; }
+    if (h.Lrows >= TC_BM) {
+        h.box_l = TC_BM; h.box_b = 1;
+        h.tiles_per_sample = (h.Lrows + TC_BM - 1) / TC_BM;
+        t.gy = h.tiles_per_sample * h.Bs;
     } else {
-        t.box_l = t.Lrows;
-        t.box_b = TC_BM / t.Lrows;
-        if (t.box_b > t.Bs) t.box_b = t.Bs;
-        t.tiles_per_sample = 1;
-        t.gy = (t.Bs + t.box_b - 1) / t.box_b;
+        h.box_l = h.Lrows;
+        h.box_b = TC_BM / h.Lrows;
+        if (h.box_b > h.Bs) h.box_b = h.Bs;
+        h.tiles_per_sample = 1;
+        t.gy = (h.Bs + h.box_b - 1) / h.box_b;
     }
-    t.total_it = g.taps * (g.K / TC_BK) + g.K2 / TC_BK;
-    // Cost model: a CTA needs ~1 unit to fill its pipeline and g_tc_cost[0] per k-step of a 128-wide tile (0.4 with 64-wide tiles);
-    // splitting K adds the workspace round trip and a second (reduce) launch, g_tc_cost[2].
+    h.kblocks = g.K / TC_BK;
+    h.it_main = g.taps * h.kblocks;
+    h.total_it = h.it_main + g.K2 / TC_BK;
+    // Cost model: a CTA needs ~1 unit to fill its pipeline and g_tc_kstep128 per k-step of a 128-wide tile (0.4 with 64-wide tiles);
+    // splitting K adds the workspace round trip and a second (reduce) launch, g_tc_split.
     // Candidates: tile width 64 (narrow N, or forced), 128 when N allows it, each with its best K split.
     int splits = 1;
     float best = 1e30f;
@@ -122,138 +109,116 @@ TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split) {
         if (g_tc_force_bn && bn != g_tc_force_bn && !(g_tc_force_bn > g.N && bn == 64)) continue;
         const int gx = (g.N + bn - 1) / bn;
         const int tiles = gx * t.gy;
-        const float kstep = bn == 128 ? g_tc_cost[0] : 0.4f;
+        const float kstep = bn == 128 ? g_tc_kstep128 : 0.4f;
         const int sp_max = forced_split > 0 ? forced_split : (tiles < sm_count ? 16 : 1);
-        for (int sp = forced_split > 0 ? forced_split : 1; sp <= sp_max && sp <= t.total_it; ++sp) {
-            const int per = (t.total_it + sp - 1) / sp;
+        for (int sp = forced_split > 0 ? forced_split : 1; sp <= sp_max && sp <= h.total_it; ++sp) {
+            const int per = (h.total_it + sp - 1) / sp;
             if (forced_split <= 0 && sp > 1 && per < 2) break;
             if (forced_split <= 0 && sp > 1 && tiles * sp > 2 * sm_count) break;   // bounds the workspace: < 2*SMs partial tiles
             const int waves = (tiles * sp + sm_count - 1) / sm_count;
-            const float est = waves * (1.0f + kstep * per) + (sp > 1 ? g_tc_cost[2] : 0.0f);
+            const float est = waves * (1.0f + kstep * per) + (sp > 1 ? g_tc_split : 0.0f);
             if (est < best - 0.25f) { best = est; splits = sp; t.BN = bn; }
         }
     }
-    t.gx = (g.N + t.BN - 1) / t.BN;
-    const int tiles = t.gx * t.gy;
-    if (splits > t.total_it) splits = t.total_it;
+    h.gx = (g.N + t.BN - 1) / t.BN;
+    if (splits > h.total_it) splits = h.total_it;
     if (splits < 1) splits = 1;
-    t.splits = splits;
-    t.ws_floats = splits > 1 ? (int64_t)tiles * splits * TC_BM * t.BN : 0;
+    h.splits = splits;
+    h.it_base = h.total_it / splits;
+    h.it_rem = h.total_it % splits;
+    h.conv_mode = g.conv_mode;
+    h.tap_shift = g.tap_shift;
+    h.tap_dilation = g.tap_dilation;
+    t.ws_floats = splits > 1 ? (int64_t)h.gx * t.gy * splits * TC_BM * t.BN : 0;
     return t;
 }
 
 int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, TcPlanned* out) {
     MUGD_REQUIRE(gemm_tc_supported(g), "gemm_tc: unsupported shape/operands");
-    {
-        const int rc = tc_validate_fusions(g);
-        if (rc != MUGD_OK) return rc;
-    }
-    EncodeTiledFn enc = get_encode();
-    MUGD_REQUIRE(enc != nullptr, "gemm_tc: cuTensorMapEncodeTiled not available from the driver");
+    int rc = tc_validate_fusions(g);
+    if (rc != MUGD_OK) return rc;
     const TcGeometry t = tc_geometry(g, dev.sm_count, g.split_k);
-    if (t.splits > 1) {
+    const TcParams::Hot& h = t.hot;
+    if (h.splits > 1) {
         MUGD_REQUIRE(g.workspace, "gemm_tc: split-K needs a workspace");
         MUGD_REQUIRE(g.workspace_bytes >= t.ws_floats * 4, "gemm_tc: workspace too small (%lld < %lld)", (long long)g.workspace_bytes,
                      (long long)t.ws_floats * 4);
     }
+    const cuuint32_t a_box[3] = {(cuuint32_t)TC_BK, (cuuint32_t)h.box_l, (cuuint32_t)h.box_b};
     for (int tap = 0; tap < 3; ++tap) {
         if (tap > 0 && g.conv_mode != MUGD_CONV_DOWN) { out->maps[tap] = out->maps[0]; continue; }
         const bool down = g.conv_mode == MUGD_CONV_DOWN;
         // DOWN: row l of the map of tap t is source row 2l+t; the last row of tap 2 is the right padding -> out of bounds
-        const cuuint64_t rows = down ? (cuuint64_t)(t.Lrows - (tap == 2 ? 1 : 0)) : (cuuint64_t)t.Lrows;
-        const cuuint64_t sample_rows = down ? (cuuint64_t)g.Lin : (cuuint64_t)t.Lrows;
-        cuuint64_t dims[3] = {(cuuint64_t)g.K, rows, (cuuint64_t)t.Bs};
-        cuuint64_t strides[2] = {(cuuint64_t)g.lda * 4 * (down ? 2 : 1), sample_rows * (cuuint64_t)g.lda * 4};
-        cuuint32_t box[3] = {(cuuint32_t)TC_BK, (cuuint32_t)t.box_l, (cuuint32_t)t.box_b};
-        cuuint32_t estr[3] = {1, 1, 1};
-        const float* basep = g.A + (down ? (int64_t)tap * g.lda : 0);
-        CUresult r = enc(&out->maps[tap], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(basep), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        MUGD_REQUIRE(r == CUDA_SUCCESS, "gemm_tc: cuTensorMapEncodeTiled(A) failed with %d (K=%d L=%d B=%d lda=%lld)", (int)r, g.K,
-                     t.Lrows, t.Bs, (long long)g.lda);
+        const cuuint64_t rows = down ? (cuuint64_t)(h.Lrows - (tap == 2 ? 1 : 0)) : (cuuint64_t)h.Lrows;
+        const cuuint64_t sample_rows = down ? (cuuint64_t)g.Lin : (cuuint64_t)h.Lrows;
+        const cuuint64_t dims[3] = {(cuuint64_t)g.K, rows, (cuuint64_t)h.Bs};
+        const cuuint64_t strides[2] = {(cuuint64_t)g.lda * 4 * (down ? 2 : 1), sample_rows * (cuuint64_t)g.lda * 4};
+        rc = encode_f32_tma(&out->maps[tap], g.A + (down ? (int64_t)tap * g.lda : 0), 3, dims, strides, a_box, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                            "gemm_tc A");
+        if (rc != MUGD_OK) return rc;
     }
     if (g.K2 > 0) {
         // second source: same row structure as the output (Lrows rows per sample), no tap shift
-        cuuint64_t dims[3] = {(cuuint64_t)g.K2, (cuuint64_t)t.Lrows, (cuuint64_t)t.Bs};
-        cuuint64_t strides[2] = {(cuuint64_t)g.lda2 * 4, (cuuint64_t)t.Lrows * (cuuint64_t)g.lda2 * 4};
-        cuuint32_t box[3] = {(cuuint32_t)TC_BK, (cuuint32_t)t.box_l, (cuuint32_t)t.box_b};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&out->maps[3], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(g.A2), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        MUGD_REQUIRE(r == CUDA_SUCCESS, "gemm_tc: cuTensorMapEncodeTiled(A2) failed with %d (K2=%d lda2=%lld)", (int)r, g.K2, (long long)g.lda2);
+        const cuuint64_t dims[3] = {(cuuint64_t)g.K2, (cuuint64_t)h.Lrows, (cuuint64_t)h.Bs};
+        const cuuint64_t strides[2] = {(cuuint64_t)g.lda2 * 4, (cuuint64_t)h.Lrows * (cuuint64_t)g.lda2 * 4};
+        rc = encode_f32_tma(&out->maps[3], g.A2, 3, dims, strides, a_box, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "gemm_tc A2");
+        if (rc != MUGD_OK) return rc;
     } else {
         out->maps[3] = out->maps[0];
     }
+    const cuuint64_t ktot = (cuuint64_t)g.taps * g.K + g.K2;
+    const cuuint64_t w_dims[2] = {ktot, (cuuint64_t)g.N};
+    const cuuint64_t w_strides[1] = {ktot * 4};
+    const cuuint32_t w_box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)t.BN};
     for (int w = 0; w < 2; ++w) {
-        const cuuint64_t ktot = (cuuint64_t)g.taps * g.K + g.K2;
-        cuuint64_t dims[2] = {ktot, (cuuint64_t)g.N};
-        cuuint64_t strides[1] = {ktot * 4};
-        cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)t.BN};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&out->maps[4 + w], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(w == 0 ? g.W_hi : g.W_lo), dims,
-                         strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        MUGD_REQUIRE(r == CUDA_SUCCESS, "gemm_tc: cuTensorMapEncodeTiled(W) failed with %d", (int)r);
+        rc = encode_f32_tma(&out->maps[4 + w], w == 0 ? g.W_hi : g.W_lo, 2, w_dims, w_strides, w_box, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            "gemm_tc W");
+        if (rc != MUGD_OK) return rc;
     }
     TcParams& p = out->p;
     memset(&p, 0, sizeof(p));
+    p.hot = h;
+    p.hot.single_pass = dev.tc_single_pass ? 1 : 0;
     p.g = g;
     p.ws = (float*)g.workspace;
-    p.splits = t.splits;
-    p.total_it = t.total_it;
-    p.kblocks = g.K / TC_BK;
-    p.it_main = g.taps * (g.K / TC_BK);
-    p.Lrows = t.Lrows;
-    p.Bs = t.Bs;
-    p.box_l = t.box_l;
-    p.box_b = t.box_b;
-    p.tiles_per_sample = t.tiles_per_sample;
-    p.single_pass = dev.tc_single_pass ? 1 : 0;
-    p.BN = t.BN;
-    p.sm_count = dev.sm_count;
-    p.gx = t.gx;
     p.gy = t.gy;
     p.ln_invK = 1.0 / (double)g.K;
-    p.it_base = t.total_it / t.splits;
-    p.it_rem = t.total_it % t.splits;
-    p.hot = {p.Lrows, p.Bs, p.box_l, p.box_b, p.tiles_per_sample, p.it_base, p.it_rem, p.it_main, p.kblocks, p.total_it, p.splits, p.single_pass,
-             g.conv_mode, g.tap_shift, g.tap_dilation, p.gx};
     if (next) {
         p.pf_hi = next->W_hi;
-        p.pf_lo = p.single_pass ? nullptr : next->W_lo;
+        p.pf_lo = p.hot.single_pass ? nullptr : next->W_lo;
         p.pf_bytes = (int64_t)next->N * ((int64_t)next->taps * next->K + next->K2) * 4;
     }
 #ifdef MUGD_TC_TIMELINE
     p.dbg = g_tc_dbg;
 #endif
+    out->BN = t.BN;
     return MUGD_OK;
 }
 
 template <int BN, int EPI>
 static int tc_launch(const TcPlanned& pl, cudaStream_t st) {
     const TcParams& p = pl.p;
-    if (p.splits > 1) {
+    const TcParams::Hot& h = p.hot;
+    if (h.splits > 1) {
         // the main kernel only writes partial tiles: it runs the smallest instantiation, the epilogue variant lives in the reduce
-        static bool configured = false;
-        if (!configured) {
-            MUGD_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, TC_E_NONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcSmem<BN>::TOTAL));
-            configured = true;
-        }
-        MUGD_CHECK_CUDA(launch_k(gemm_tc_kernel<BN, TC_E_NONE>, dim3(p.gx, p.gy, p.splits), dim3(TC_THREADS), TcSmem<BN>::TOTAL, st, pl.maps[0],
+        MUGD_CHECK_CUDA(launch_k(gemm_tc_kernel<BN, TC_E_NONE>, dim3(h.gx, p.gy, h.splits), dim3(TC_THREADS), TcSmem<BN>::TOTAL, st, pl.maps[0],
                                  pl.maps[1], pl.maps[2], pl.maps[3], pl.maps[4], pl.maps[5], p));
-        MUGD_CHECK_CUDA(launch_k(gemm_tc_reduce_kernel<BN, EPI>, dim3((unsigned)(p.gx * p.gy * TcReduceGeom<BN>::BPT)), dim3(TC_THREADS), 0, st, p));
+        MUGD_CHECK_CUDA(launch_k(gemm_tc_reduce_kernel<BN, EPI>, dim3((unsigned)(h.gx * p.gy * (TC_BM / TC_RED_ROWS<BN>))), dim3(TC_THREADS), 0,
+                                 st, p));
         return MUGD_OK;
     }
-    static bool configured = false;
-    if (!configured) {
-        MUGD_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcSmem<BN>::TOTAL));
-        configured = true;
-    }
-    MUGD_CHECK_CUDA(launch_k(gemm_tc_kernel<BN, EPI>, dim3(p.gx, p.gy, 1), dim3(TC_THREADS), TcSmem<BN>::TOTAL, st, pl.maps[0], pl.maps[1],
+    MUGD_CHECK_CUDA(launch_k(gemm_tc_kernel<BN, EPI>, dim3(h.gx, p.gy, 1), dim3(TC_THREADS), TcSmem<BN>::TOTAL, st, pl.maps[0], pl.maps[1],
                              pl.maps[2], pl.maps[3], pl.maps[4], pl.maps[5], p));
     return MUGD_OK;
+}
+
+template <int BN, int... EPI>
+static cudaError_t allow_smem_bn(int bytes, std::integer_sequence<int, EPI...>) {
+    return allow_dynamic_smem(bytes, gemm_tc_kernel<BN, EPI>...);
+}
+cudaError_t gemm_tc_allow_smem(int bytes) {
+    const cudaError_t e = allow_smem_bn<64>(bytes, std::make_integer_sequence<int, TC_E_COUNT>{});
+    return e != cudaSuccess ? e : allow_smem_bn<128>(bytes, std::make_integer_sequence<int, TC_E_COUNT>{});
 }
 
 template <int BN>
@@ -274,20 +239,21 @@ int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* n
     TcPlanned pl;
     int rc = tc_plan(dev, g, next, &pl);
     if (rc != MUGD_OK) return rc;
-    if (pl.p.BN == 128) rc = tc_launch_bn<128>(pl, st);
+    if (pl.BN == 128) rc = tc_launch_bn<128>(pl, st);
     else rc = tc_launch_bn<64>(pl, st);
     if (rc != MUGD_OK) return rc;
-    if (launches) *launches += pl.p.splits > 1 ? 2 : 1;
+    if (launches) *launches += pl.p.hot.splits > 1 ? 2 : 1;
     return MUGD_OK;
 }
 
 }  // namespace mugd
 
+// kstep256_us and two_cta_fixed_us are accepted for ABI compatibility and ignored: no such kernel variant exists
 extern "C" int mugd_debug_set_tc_cost(float kstep128_us, float kstep256_us, float split_us, float two_cta_fixed_us) {
-    if (two_cta_fixed_us != 0.f) mugd::g_tc_cost[3] = two_cta_fixed_us;
-    if (kstep128_us > 0.f) mugd::g_tc_cost[0] = kstep128_us;
-    if (kstep256_us > 0.f) mugd::g_tc_cost[1] = kstep256_us;
-    if (split_us > 0.f) mugd::g_tc_cost[2] = split_us;
+    (void)kstep256_us;
+    (void)two_cta_fixed_us;
+    if (kstep128_us > 0.f) mugd::g_tc_kstep128 = kstep128_us;
+    if (split_us > 0.f) mugd::g_tc_split = split_us;
     return MUGD_OK;
 }
 
@@ -318,10 +284,9 @@ extern "C" int mugd_gemm_tc_variant(const mugd_gemm* g, int32_t sm_count, int32_
     }
     const int sms = sm_count > 0 ? sm_count : 132;
     const TcGeometry t = tc_geometry(*g, sms, g->split_k);
-    const int tiles = t.gx * t.gy;
     if (tile_n) *tile_n = t.BN;
     if (ctas_per_sm) *ctas_per_sm = 1;
-    if (grid_ctas) *grid_ctas = tiles * t.splits;
+    if (grid_ctas) *grid_ctas = t.hot.gx * t.gy * t.hot.splits;
     return MUGD_OK;
 }
 
@@ -338,8 +303,8 @@ extern "C" int mugd_gemm_tc_query(mugd_handle*, const mugd_gemm* g, int32_t sm_c
         return MUGD_OK;
     }
     const TcGeometry t = tc_geometry(*g, sm_count > 0 ? sm_count : 132, g->split_k);
-    if (splits) *splits = t.splits;
+    if (splits) *splits = t.hot.splits;
     if (workspace_bytes) *workspace_bytes = t.ws_floats * 4;
-    if (n_tiles) *n_tiles = t.gx * t.gy;
+    if (n_tiles) *n_tiles = t.hot.gx * t.gy;
     return MUGD_OK;
 }

@@ -1,5 +1,5 @@
-// Device side of the wgmma (Hopper warpgroup MMA) implicit GEMM, shared by the stand-alone kernels of gemm_tc.cu and any kernel
-// that embeds GEMM tiles.  fp32 in / fp32 out with the 3xTF32 split so results stay at fp32 accuracy (DESIGN.md §4 "Precision"):
+// Device side of the wgmma (Hopper warpgroup MMA) implicit GEMM of gemm_tc.cu.  fp32 in / fp32 out with the 3xTF32 split so results
+// stay at fp32 accuracy (DESIGN.md §4 "Precision"):
 //
 //     a = a_hi + a_lo (both exactly representable in TF32, round-to-nearest),   w = w_hi + w_lo
 //     acc += a_lo*w_hi + a_hi*w_lo + a_hi*w_hi          (fp32 accumulation in registers, dropped term ~2^-22)
@@ -10,16 +10,17 @@
 //                  is the TMA out-of-bounds zero fill on the l axis, so no im2col / padding copy exists -- plus the pre-split
 //                  W_hi / W_lo tiles; completion on an mbarrier, release of a stage by one arrival per warp.
 //   warpgroups   : warpgroup w owns tile rows 64w..64w+63.  Each thread reads its A fragment out of the swizzled raw tile, splits
-//                  it into a_hi / a_lo (cvt.rna.tf32) in registers and issues 12 wgmma.m64nBNk8.tf32 per k-step (A from
+//                  it into a_hi / a_lo (to_tf32) in registers and issues 12 wgmma.m64nBNk8.tf32 per k-step (A from
 //                  registers, B = weight tile through a shared-memory descriptor); the next stage is split while they run, and one
 //                  k-step of MMAs stays in flight across the k-step boundary.
 //   prefetch     : the producer lane also pulls its CTA's slice of the NEXT tensor-core GEMM's weights into L2.
 //   epilogue 1   : accumulator registers -> shared memory (row pitch BN+4), over the then idle pipeline buffers
 //   epilogue 2   : all warps: bias / time-embedding row / SiLU / GELU / GEGLU / GLU / residual, row-contiguous coalesced stores;
-//                  with split-K the partial tile goes to an L2-resident workspace and tc_reduce_item() sums the splits in fixed
+//                  with split-K the partial tile goes to an L2-resident workspace and tc_reduce() sums the splits in fixed
 //                  order (deterministic) and runs the same fused epilogue.
 #pragma once
 #include <cuda.h>
+#include <stddef.h>
 
 #include <type_traits>
 
@@ -36,25 +37,24 @@ constexpr uint32_t TC_A_BYTES = TC_BM * TC_BK * 4;   // 16 KB
 struct TcParams {
     // What the tile prologue and the TMA producer read before the first load leaves, packed into the first 64 bytes: kernel
     // parameters live in constant memory, a fresh launch misses on every line it touches, and those misses are serial on the
-    // producer's critical path.
+    // producer's critical path.  Filled by tc_geometry() (single_pass: by tc_plan()).
     struct Hot {
-        int32_t Lrows, Bs, box_l, box_b, tiles_per_sample, it_base, it_rem, it_main, kblocks, total_it, splits, single_pass,
-            conv_mode, tap_shift, tap_dilation, gx;
+        int32_t Lrows, Bs;        // row structure of the A tensor map (Lrows = rows per sample, Bs samples)
+        int32_t box_l, box_b;     // TMA box: box_l rows of box_b consecutive samples (box_l*box_b <= 128)
+        int32_t tiles_per_sample; // when Lrows >= 128
+        int32_t it_base, it_rem;  // split z owns k-steps [z*it_base + min(z, it_rem), +it_base + (z < it_rem)): no division on the device
+        int32_t it_main;          // taps * K / 32: k-steps >= it_main read the second source (A2, 1x1 term)
+        int32_t kblocks;          // K / 32
+        int32_t total_it;         // (taps * K + K2) / 32
+        int32_t splits;
+        int32_t single_pass;      // 1: plain TF32 (a_hi*w_hi only, ~2^-11 relative) -- opt-in speed mode, NOT used for parity/bench
+        int32_t conv_mode, tap_shift, tap_dilation;
+        int32_t gx;               // column tiles (grid: gx x gy x splits)
     } hot;
     mugd_gemm g;
-    float* ws;                // split-K partial tiles [tile][split][128][BN]
-    int32_t splits;
-    int32_t total_it;         // (taps * K + K2) / 32
-    int32_t kblocks;          // K / 32
-    int32_t it_main;          // taps * K / 32: k-steps >= it_main read the second source (A2, 1x1 term)
-    int32_t Lrows, Bs;        // row structure of the A tensor map (Lrows = rows per sample, Bs samples)
-    int32_t box_l, box_b;     // TMA box: box_l rows of box_b consecutive samples (box_l*box_b <= 128)
-    int32_t tiles_per_sample; // when Lrows >= 128
-    int32_t single_pass;      // 1: plain TF32 (a_hi*w_hi only, ~2^-11 relative) -- opt-in speed mode, NOT used for parity/bench
-    int32_t BN, gx, gy;       // tile width and tile grid (gx column tiles x gy row tiles x splits)
-    int32_t sm_count;
-    double ln_invK;           // 1 / K (folded LayerNorm: moments -> mean / variance)
-    int32_t it_base, it_rem;  // split z owns k-steps [z*it_base + min(z, it_rem), +it_base + (z < it_rem)): no division on the device
+    float* ws;                    // split-K partial tiles [tile][split][128][BN]
+    int32_t gy;                   // row tiles
+    double ln_invK;               // 1 / K (folded LayerNorm: moments -> mean / variance)
     // W_hi / W_lo of the next tensor-core GEMM of the plan (pf_lo NULL in single-pass mode, pf_bytes 0 = none), prefetched into L2
     // while this GEMM runs: the next launch then reads its first stages from L2 instead of HBM.  Weights are written once, when the
     // engine is built, so the prefetch cannot race with a producer.
@@ -62,12 +62,12 @@ struct TcParams {
     const float* pf_lo;
     int64_t pf_bytes;
 #ifdef MUGD_TC_TIMELINE
-    long long* dbg;           // CTA (0,0,0) writes globaltimer stamps (TC_STAMP, tools/bench_gemm.py)
+    long long* dbg;               // CTA (0,0,0) writes globaltimer stamps (TC_STAMP, tools/bench_gemm.py)
 #endif
 };
+static_assert(sizeof(TcParams::Hot) == 64 && offsetof(TcParams, hot) == 0, "the hot fields are the first 64 bytes of the parameters");
 
 #ifdef __CUDACC__
-// ---- raw PTX helpers ---------------------------------------------------------------------------------
 __device__ __forceinline__ long long gtimer() {
     long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory");
@@ -80,69 +80,6 @@ __device__ __forceinline__ long long gtimer() {
 #else
 #define TC_STAMP(p, k, cta0) do { } while (0)
 #endif
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_inval(uint32_t bar) {
-    asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// bounded wait: a protocol bug traps (CUDA error) instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-    long long t0 = 0;                 // the clock is read only after a probe has failed: the common case costs one try_wait
-    while (true) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(bar), "r"(parity)
-            : "memory");
-        if (done) break;
-        const long long now = clock64();
-        if (t0 == 0) t0 = now;
-        else if (now - t0 > 4000000000LL) __trap();
-    }
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {     // p 16-byte aligned, bytes a multiple of 16
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(p)), "r"(bytes) : "memory");
-}
-// One lane of a converged warp: cp.async.bulk.tensor is a uniform-datapath instruction; issued from a lane-divergent branch
-// (`if (lane == 0)`) ptxas wraps it in an elect-and-branch loop, guarded by elect.sync in a converged warp it issues directly.
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-        "elect.sync rx|px, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, px;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ float to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
-}
 // Pipeline of one CTA: STAGES x (raw A tile + W_hi tile + W_lo tile), filled by TMA, consumed by both warpgroups.
 template <int BN>
 struct TcSmem {
@@ -285,12 +222,9 @@ __device__ __forceinline__ void tc_store_tile(const mugd_gemm& g, uint32_t stage
                 const int row = row0 + (i0 + u) * RPP;
                 const int m = m_base + row;
                 const bool ok = FULL || (row < n_rows && col_ok);
-                float4 acc;
-                asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(acc.x), "=f"(acc.y), "=f"(acc.z), "=f"(acc.w)
-                             : "r"(stage + (uint32_t)(row * SP + c4 * 4) * 4u));
+                const float4 acc = lds_f4(stage + (uint32_t)(row * SP + c4 * 4) * 4u);
                 float2 ln = make_float2(0.f, 1.f);
-                if constexpr (MODE == TC_EPI_LN)
-                    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ln.x), "=f"(ln.y) : "r"(rowstat + (uint32_t)row * 8u));
+                if constexpr (MODE == TC_EPI_LN) ln = lds_f2(rowstat + (uint32_t)row * 8u);
                 float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (ok) o = tc_finish4<ACT, GATE, MODE == TC_EPI_LN>(g, cp + (int64_t)(i0 + u) * c_step, acc, bia, rvv[u], res[u], cs, ln, m, no);
                 if constexpr (MODE == TC_EPI_SINK) tc_row_sink<SEG>(g.row_moments, ok ? m : -1, o);
@@ -353,7 +287,7 @@ struct TcBars {
     __device__ __forceinline__ void init_parallel(int t) const {
         if (t >= COUNT) return;
         mbar_init(bars + 8u * t, t < S::STAGES ? 1u : (uint32_t)(TC_THREADS / 32));    // empty: one arrival per warp
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init_fence();
     }
 };
 
@@ -369,8 +303,7 @@ __device__ __forceinline__ void tc_load_split(uint32_t a_tile, int r0, int t, Tc
         for (int e = 0; e < 4; ++e) {
             const int r = r0 + (e & 1) * 8;                  // a[0] / a[2]: row g, a[1] / a[3]: row g + 8
             const int chunk = 2 * kk + (e >> 1);             // a[2] / a[3]: column t + 4
-            float x;
-            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a_tile + (uint32_t)r * 128u + (uint32_t)((chunk ^ (r & 7)) << 4) + (uint32_t)t * 4u));
+            const float x = lds_f1(a_tile + (uint32_t)r * 128u + (uint32_t)((chunk ^ (r & 7)) << 4) + (uint32_t)t * 4u);
             const float h = to_tf32(x);
             f.hi[kk][e] = __float_as_uint(h);
             f.lo[kk][e] = __float_as_uint(to_tf32(x - h));
@@ -383,8 +316,7 @@ __device__ __forceinline__ void tc_load_split(uint32_t a_tile, int r0, int t, Tc
 // threads call it: warpgroup w computes rows 64w..64w+63 with wgmma (A = the split activation rows from registers, B = the weight
 // tiles from shared memory); one elected lane of warp 0 also drives the TMA ring.  On return every TMA has landed, every MMA has
 // retired, and the tile (or its split-K partial) is on its way to global memory.
-// PDL: stand-alone launches pass true -- the producer executes griddepcontrol.wait before it loads activations.
-template <int BN, bool PDL, int EPI>
+template <int BN, int EPI>
 __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUtensorMap* tmA1, const CUtensorMap* tmA2, const CUtensorMap* tmB,
                                              const CUtensorMap* tmWhi, const CUtensorMap* tmWlo, const TcParams& p, int bx, int by, int bz,
                                              uint32_t base) {
@@ -397,14 +329,14 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     auto b_lo = [&](int s) { return b_hi(s) + S::B_BYTES; };
 
     const mugd_gemm& g = p.g;
+    const TcParams::Hot& h = p.hot;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n0 = bx * BN;
     int b_base, l_base, rows_valid;
     tc_tile_rows(p, by, b_base, l_base, rows_valid);
-    const int m_base = b_base * p.hot.Lrows + l_base;
-    const int it_begin = bz * p.hot.it_base + min(bz, p.hot.it_rem);
-    const int nit = p.hot.it_base + (bz < p.hot.it_rem ? 1 : 0);
-    const TcParams::Hot& h = p.hot;
+    const int m_base = b_base * h.Lrows + l_base;
+    const int it_begin = bz * h.it_base + min(bz, h.it_rem);
+    const int nit = h.it_base + (bz < h.it_rem ? 1 : 0);
     const uint32_t a_tx = (uint32_t)(h.box_l * h.box_b) * TC_BK * 4;
     const uint32_t w_tx = (h.single_pass ? 1u : 2u) * S::B_BYTES;
 
@@ -436,12 +368,12 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
         if (elect_one()) {
             const int pro = nit < STAGES ? nit : STAGES;
             for (int i = 0; i < pro; ++i) issue_w(i);
-            if (PDL) pdl_wait();                 // activations written by the previous kernel are touched from here on
+            pdl_wait();                          // activations written by the previous kernel are touched from here on
             for (int i = 0; i < pro; ++i) issue_a(i);
             if (p.pf_bytes > 0) {                // after this CTA's own loads: CTA c prefetches slice c of the next GEMM's weights
-                const int64_t ncta = (int64_t)p.gx * p.gy * p.splits;
+                const int64_t ncta = (int64_t)h.gx * p.gy * h.splits;
                 const int64_t per = (p.pf_bytes / ncta + 15) & ~(int64_t)15;
-                const int64_t off = (((int64_t)bz * p.gy + by) * p.gx + bx) * per;
+                const int64_t off = (((int64_t)bz * p.gy + by) * h.gx + bx) * per;
                 const int64_t n = min(per, p.pf_bytes - off);
                 if (n > 0) {
                     prefetch_l2(reinterpret_cast<const char*>(p.pf_hi) + off, (uint32_t)n);
@@ -459,8 +391,8 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     float4 epi_bias = make_float4(0.f, 0.f, 0.f, 0.f), epi_cs = epi_bias;
     double ln_s = 0.0, ln_ss = 0.0;
     {
-        if constexpr (PDL) pdl_wait();                       // the step counter / LayerNorm moments are written by the previous kernels
-        if (p.hot.splits == 1) {
+        pdl_wait();                                          // the step counter / LayerNorm moments are written by the previous kernels
+        if (h.splits == 1) {
             const int nn = n0 + ((int)threadIdx.x % (BN / 4)) * 4;
             if (g.step) epi_step = *g.step;
             if (g.bias && nn < g.N) epi_bias = ld_f4(g.bias + nn);
@@ -546,23 +478,20 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
         const int c = j * 8 + 2 * t4;
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + (uint32_t)(r0 * SP + c) * 4u), "f"(acc[4 * j]), "f"(acc[4 * j + 1]) : "memory");
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + (uint32_t)((r0 + 8) * SP + c) * 4u), "f"(acc[4 * j + 2]), "f"(acc[4 * j + 3])
-                     : "memory");
+        sts_f2(base + (uint32_t)(r0 * SP + c) * 4u, acc[4 * j], acc[4 * j + 1]);
+        sts_f2(base + (uint32_t)((r0 + 8) * SP + c) * 4u, acc[4 * j + 2], acc[4 * j + 3]);
     }
     if constexpr (TcEpiTraits<EPI>::MODE == TC_EPI_LN) {     // (mean, rstd) of tile row r for phase 2, in the last KB of the pipeline buffers
-        if (threadIdx.x < TC_BM)
-            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(base + S::TILE_BYTES - 1024u + (uint32_t)threadIdx.x * 8u), "f"(lnrow.x), "f"(lnrow.y)
-                         : "memory");
+        if (threadIdx.x < TC_BM) sts_f2(base + S::TILE_BYTES - 1024u + (uint32_t)threadIdx.x * 8u, lnrow.x, lnrow.y);
     }
     // ---- phase 2 (all 8 warps): consecutive threads take consecutive float4 of a row -> coalesced global traffic.
     __syncthreads();
     TC_STAMP(p, 3, bx == 0 && by == 0 && bz == 0);
     {
         const float* rowvec = g.rowvec ? g.rowvec + (int64_t)epi_step * g.rowvec_step_stride : nullptr;
-        if (p.splits > 1) {
-            const int tile_lin = by * p.gx + bx;
-            float* wsp = p.ws + ((int64_t)tile_lin * p.splits + bz) * (TC_BM * BN);
+        if (h.splits > 1) {
+            const int tile_lin = by * h.gx + bx;
+            float* wsp = p.ws + ((int64_t)tile_lin * h.splits + bz) * (TC_BM * BN);
             constexpr int C4 = BN / 4;
             constexpr int U = 8;
 #pragma unroll 1
@@ -572,8 +501,7 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
                 for (int u = 0; u < U; ++u) {
                     const int idx = i0 + u * TC_THREADS + (int)threadIdx.x;
                     const int row = idx / C4, c4 = idx - row * C4;
-                    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(a4[u].x), "=f"(a4[u].y), "=f"(a4[u].z), "=f"(a4[u].w)
-                                 : "r"(base + (uint32_t)(row * SP + c4 * 4) * 4u));
+                    a4[u] = lds_f4(base + (uint32_t)(row * SP + c4 * 4) * 4u);
                 }
 #pragma unroll
                 for (int u = 0; u < U; ++u) st_f4(wsp + (i0 + u * TC_THREADS + (int)threadIdx.x) * 4, a4[u]);   // [row][BN] dense
@@ -586,34 +514,27 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     TC_STAMP(p, 4, bx == 0 && by == 0 && bz == 0);
 }
 
-// split-K second pass.  One call = one thread's share of reduce block `blk`: TC_RED_R output rows x one 4-column group.  A block of
-// 256 threads covers RPB = TC_RED_R * (256 / (BN/4)) rows of one tile; the partial tiles are summed in fixed split order
-// (deterministic), then the fused epilogue (+ row-moment sink / folded LayerNorm) runs.  One row per thread: the reduce of a small
-// GEMM is latency-bound, more and smaller blocks finish sooner.
-constexpr int TC_RED_R = 1;
-template <int BN>
-struct TcReduceGeom {
-    static constexpr int C4 = BN / 4;
-    static constexpr int RPP = TC_THREADS / C4;       // rows per pass
-    static constexpr int RPB = TC_RED_R * RPP;        // rows per block
-    static constexpr int BPT = TC_BM / RPB;           // blocks per tile
-    static_assert(TC_BM % RPB == 0, "reduce geometry");
-};
+// split-K second pass, one output row x one 4-column group per thread: a block of TC_THREADS covers TC_RED_ROWS<BN> rows of one tile
+// (the reduce of a small GEMM is latency-bound, more and smaller blocks finish sooner).  The partial tiles are summed in fixed split
+// order (deterministic), then the fused epilogue (+ row-moment sink / folded LayerNorm) runs.
+template <int BN> constexpr int TC_RED_ROWS = TC_THREADS / (BN / 4);
 
-template <int BN, int ACT, int GATE, int MODE>
-__device__ __forceinline__ void tc_reduce_rows(const TcParams& p, int tile_lin, int rb) {
-    using G = TcReduceGeom<BN>;
-    static_assert(TC_RED_R == 1, "one output row per thread");
-    constexpr int C4 = G::C4;
+template <int BN, int EPI>
+__device__ __forceinline__ void tc_reduce(const TcParams& p, int blk) {
+    constexpr int ACT = TcEpiTraits<EPI>::ACT, GATE = TcEpiTraits<EPI>::GATE, MODE = TcEpiTraits<EPI>::MODE;
+    constexpr int C4 = BN / 4;
+    constexpr int BPT = TC_BM / TC_RED_ROWS<BN>;       // blocks per tile
     constexpr int SEG = C4 < 32 ? C4 : 32;
     constexpr int ZU = 8;                              // partial tiles in flight per thread
     const mugd_gemm& g = p.g;
-    const int bx = tile_lin % p.gx, by = tile_lin / p.gx;
+    const TcParams::Hot& h = p.hot;
+    const int tile_lin = blk / BPT;
+    const int bx = tile_lin % h.gx, by = tile_lin / h.gx;
     int b_base, l_base, rows_valid;
     tc_tile_rows(p, by, b_base, l_base, rows_valid);
-    const int m_base = b_base * p.Lrows + l_base;
+    const int m_base = b_base * h.Lrows + l_base;
     const int c4 = (int)threadIdx.x % C4;
-    const int r = rb * G::RPB + (int)threadIdx.x / C4;
+    const int r = (blk % BPT) * TC_RED_ROWS<BN> + (int)threadIdx.x / C4;
     const int n = bx * BN + c4 * 4;
     const int m = m_base + r;
     const bool ok = r < rows_valid && m < g.M && n < g.N;
@@ -633,14 +554,14 @@ __device__ __forceinline__ void tc_reduce_rows(const TcParams& p, int tile_lin, 
     if constexpr (MODE == TC_EPI_LN) {
         if (ok) mo = *reinterpret_cast<const double2*>(g.ln_stats + (int64_t)m * 2);
     }
-    const float* src = p.ws + ((long long)tile_lin * p.splits) * (TC_BM * BN) + (long long)r * BN + c4 * 4;
+    const float* src = p.ws + ((long long)tile_lin * h.splits) * (TC_BM * BN) + (long long)r * BN + c4 * 4;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int z0 = 0; z0 < p.splits; z0 += ZU) {                            // fixed order -> deterministic
+    for (int z0 = 0; z0 < h.splits; z0 += ZU) {                            // fixed order -> deterministic
         float4 t4[ZU];
 #pragma unroll
         for (int u = 0; u < ZU; ++u) {
             t4[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (ok && z0 + u < p.splits) t4[u] = __ldcg(reinterpret_cast<const float4*>(src + (long long)(z0 + u) * (TC_BM * BN)));
+            if (ok && z0 + u < h.splits) t4[u] = __ldcg(reinterpret_cast<const float4*>(src + (long long)(z0 + u) * (TC_BM * BN)));
         }
         if (z0 == 0 && g.rowvec && ok)                                      // needs the step counter: by now it has arrived
             rvv = ld_f4(g.rowvec + (int64_t)step * g.rowvec_step_stride + (int64_t)(m / g.Lout) * g.rowvec_b_stride + n);
@@ -657,23 +578,19 @@ __device__ __forceinline__ void tc_reduce_rows(const TcParams& p, int tile_lin, 
     if constexpr (MODE == TC_EPI_SINK) tc_row_sink<SEG>(g.row_moments, ok ? m : -1, o);
 }
 
-template <int BN, int EPI>
-__device__ __forceinline__ void tc_reduce_block(const TcParams& p, int blk) {
-    using G = TcReduceGeom<BN>;
-    using E = TcEpiTraits<EPI>;
-    tc_reduce_rows<BN, E::ACT, E::GATE, E::MODE>(p, blk / G::BPT, blk % G::BPT);
-}
 #endif  // __CUDACC__
 
 // ---- host side (gemm_tc.cu) -------------------------------------------------------------------------
 struct TcGeometry {
-    int BN, splits, gx, gy, Lrows, Bs, box_l, box_b, tiles_per_sample, total_it;
+    TcParams::Hot hot;        // every field but single_pass (a per-handle switch)
+    int BN, gy;
     int64_t ws_floats;
 };
-// one planned tensor-core GEMM: kernel parameters + its six tensor maps (A taps 0..2, second source, W_hi, W_lo)
+// one planned tensor-core GEMM: kernel parameters + its six tensor maps (A taps 0..2, second source, W_hi, W_lo) + the tile width
 struct alignas(64) TcPlanned {
     CUtensorMap maps[6];
     TcParams p;
+    int BN;
 };
 TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split);
 // validates, picks the geometry, encodes the maps; `next` (or NULL): the tensor-core GEMM whose weights this one prefetches into L2

@@ -129,12 +129,6 @@ int launch_s4conv(const DeviceInfo& dev, const mugd_s4conv& s, cudaStream_t st, 
     const int Lpad = (s.L + 2 * S4_R - 1) / (2 * S4_R) * (2 * S4_R);
     const size_t smem = ((size_t)(S4_PAD + Lpad) + (size_t)(Lpad + 3 * S4_R)) * S4_PITCH * sizeof(float);
     MUGD_REQUIRE((int)smem <= dev.max_smem_optin, "s4conv: L=%d needs %zu B of shared memory (max %d)", s.L, smem, dev.max_smem_optin);
-    static bool configured = false;
-    if (!configured) {
-        MUGD_CHECK_CUDA(cudaFuncSetAttribute(s4conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dev.max_smem_optin));
-        MUGD_CHECK_CUDA(cudaFuncSetAttribute(s4conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dev.max_smem_optin));
-        configured = true;
-    }
     const int base = (s.H / S4_CH) * s.B;
     const int npairs = (Lpad / (2 * S4_R) + 1) / 2;
     int nsplit = 1;
@@ -245,6 +239,8 @@ __global__ void s4_irfft_kernel(const double2* __restrict__ kf, int H, int Lint,
     }
 }
 
+cudaError_t s4_allow_smem(int bytes) { return allow_dynamic_smem(bytes, s4conv_kernel<true>, s4conv_kernel<false>, s4_irfft_kernel); }
+
 }  // namespace mugd
 
 extern "C" int mugd_s4_kernel_gen(mugd_handle*, const float* log_dt, const float* Bri, const float* Cri,
@@ -265,8 +261,6 @@ extern "C" int mugd_s4_kernel_gen(mugd_handle*, const float* log_dt, const float
     MUGD_CHECK_CUDA(cudaGetLastError());
     const size_t smem = sizeof(double2) * (size_t)(nf + L_internal);
     MUGD_REQUIRE(smem <= 200 * 1024, "s4_kernel_gen: L_internal=%d too long for the one-shot DFT", L_internal);
-    if (smem > 48 * 1024)
-        MUGD_CHECK_CUDA(cudaFuncSetAttribute(s4_irfft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     s4_irfft_kernel<<<H, 256, smem, st>>>(kf, H, L_internal, L_out, Kt);
     MUGD_CHECK_CUDA(cudaGetLastError());
     return MUGD_OK;

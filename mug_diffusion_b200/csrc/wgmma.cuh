@@ -4,12 +4,113 @@
 // Register fragments (warp w of the warpgroup owns rows 16w..16w+15; g = lane / 4, t = lane % 4):
 //   A (4 x b32):      a[0] = A[g][t]   a[1] = A[g+8][t]   a[2] = A[g][t+4]   a[3] = A[g+8][t+4]
 //   D (N/2 x f32):    d[4j+0] = D[g][8j+2t]   d[4j+1] = D[g][8j+2t+1]   d[4j+2] = D[g+8][8j+2t]   d[4j+3] = D[g+8][8j+2t+1]
+//
+// Also the one home of the other sm_90a primitives the two tensor-core kernels (gemm_tc.cuh, attention_tc.cu) share: mbarriers,
+// TMA loads and the L2 bulk prefetch, one-lane election, the TF32 rounding, shared-memory vector loads / stores, and on the host the
+// fp32 tensor-map encoder.
 #pragma once
+#include <cuda.h>
 #include <stdint.h>
+
+#include "common.cuh"
 
 namespace mugd {
 
 #ifdef __CUDACC__
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// ---- mbarriers (shared-memory addresses) ----
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+// after the last mbar_init of a thread: makes its initialised barriers visible to the async proxy (TMA) and the other threads
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// bounded wait: a protocol bug traps (CUDA error) instead of hanging the GPU
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    uint32_t done = 0;
+    long long t0 = 0;                 // the clock is read only after a probe has failed: the common case costs one try_wait
+    while (true) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(done)
+            : "r"(bar), "r"(parity)
+            : "memory");
+        if (done) break;
+        const long long now = clock64();
+        if (t0 == 0) t0 = now;
+        else if (now - t0 > 4000000000LL) __trap();
+    }
+}
+
+// ---- TMA: tile loads through a tensor map (completion on mbarrier `bar`), L2 bulk prefetch ----
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+__device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {     // p 16-byte aligned, bytes a multiple of 16
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(p)), "r"(bytes) : "memory");
+}
+
+// One lane of a converged warp: cp.async.bulk.tensor is a uniform-datapath instruction; issued from a lane-divergent branch
+// (`if (lane == 0)`) ptxas wraps it in an elect-and-branch loop, guarded by elect_one() in a converged warp it issues directly.
+__device__ __forceinline__ bool elect_one() {
+    uint32_t pred = 0;
+    asm volatile(
+        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
+        "elect.sync rx|px, 0xffffffff;\n\t"
+        "selp.u32 %0, 1, 0, px;\n\t}"
+        : "=r"(pred));
+    return pred != 0;
+}
+// round to the nearest TF32 value (kept in an fp32 register): x - to_tf32(x) is the exact low part of the 3xTF32 split
+__device__ __forceinline__ float to_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return __uint_as_float(r);
+}
+
+// ---- shared-memory loads / stores by 32-bit shared address ----
+__device__ __forceinline__ float lds_f1(uint32_t addr) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ float2 lds_f2(uint32_t addr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ float4 lds_f4(uint32_t addr) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ void sts_f1(uint32_t addr, float v) {
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
+__device__ __forceinline__ void sts_f2(uint32_t addr, float x, float y) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ void sts_f4(uint32_t addr, float4 v) {
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
 // K-major SWIZZLE_128B descriptor: rows of 128 bytes, 8-row groups 1024 B apart (stride byte offset), leading byte offset unused (1),
 // layout type 1 = 128-byte swizzle.  The operand must start 1024-byte aligned; a k offset inside the swizzle atom is added to the
 // start address (k8 of fp32 = 32 bytes = 2 units of 16 bytes).
@@ -72,5 +173,29 @@ template <> struct Wgmma<128> {
 };
 
 #endif  // __CUDACC__
+
+// ---- host: fp32 tensor maps with 128-byte swizzle (the layout every TMA load above expects), no out-of-bounds fill value (zeros) ----
+// `what` names the caller in the error text.  The driver entry point is looked up once per process.
+inline int encode_f32_tma(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                          const cuuint32_t* box, CUtensorMapL2promotion l2, const char* what) {
+    typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                      const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    static const EncodeTiledFn enc = [] {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult qr;
+        const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qr) == cudaSuccess &&
+                        qr == cudaDriverEntryPointSuccess;
+        return ok ? (EncodeTiledFn)p : nullptr;
+    }();
+    MUGD_REQUIRE(enc != nullptr, "%s: the driver has no tensor-map encoder", what);
+    const cuuint32_t estr[3] = {1, 1, 1};
+    const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, estr,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    MUGD_REQUIRE(r == CUDA_SUCCESS, "%s: tensor-map encoding failed with CUresult %d (dims %llu x %llu x %llu, row stride %llu B)", what, (int)r,
+                 (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 1),
+                 (unsigned long long)strides[0]);
+    return MUGD_OK;
+}
 
 }  // namespace mugd

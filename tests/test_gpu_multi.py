@@ -77,3 +77,60 @@ def test_two_rank_sharded_sampling_equals_single_gpu(tmp_path):
     single = torch.cat(chunks)
     assert gathered.shape == single.shape == (B, 16, 8 * L)
     assert torch.equal(gathered, single)
+
+
+def test_ops_bit_identical_on_two_devices_of_one_process():
+    """One process, one handle per device: the tensor-core GEMM, the tensor-core attention and the S4 convolution (each needs more than
+    48 KB of shared memory, an attribute of the device's context) run on cuda:0 and cuda:1 and agree bit for bit."""
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs 2 GPUs")
+    import ctypes as C
+    import math
+
+    import torch.nn.functional as F
+    from gpu_util import ptr, rel_err, view
+    from mug_diffusion_b200 import lib as L_
+    from mug_diffusion_b200 import synth
+    from mug_diffusion_b200.engine import OpList
+    from mug_diffusion_b200.packer import tf32_split
+
+    def g(name, shape):
+        return synth._gauss(synth._rng(13, name), shape)
+
+    M, K, N = 1024, 256, 384                              # GEMM
+    B, H, D, L = 2, 8, 64, 256                            # attention: 256 keys -> tensor-core kernel
+    Bs, Ls, Hs = 2, 512, 128                              # S4 convolution
+    x, w = g("x", (M, K)), g("w", (N, K)) / math.sqrt(K)
+    w_hi, w_lo = tf32_split(w)
+    q, k, v = g("q", (B * L, H * D)), g("k", (B * L, H * D)), g("v", (B * L, H * D))
+    rel, cg = 0.5 * g("rel", (129, H)), 1 + 0.1 * g("cg", (129, H))
+    u, kt, dsk = g("u", (Bs * Ls, Hs)), g("kt", (Ls, Hs)) * 0.05, g("d", (Hs,))
+    lib = L_.load()
+    results = []
+    for dev in (0, 1):
+        with torch.cuda.device(dev):
+            handle = C.c_void_p()
+            L_.check(lib.mugd_create(dev, C.byref(handle)), f"mugd_create({dev})")
+            try:
+                xc, wc, hc, lc = (t.to(f"cuda:{dev}") for t in (x, w, w_hi, w_lo))
+                qc, kc, vc, relc, cgc = (t.to(f"cuda:{dev}") for t in (q, k, v, rel, cg))
+                uc, ktc, dc = (t.to(f"cuda:{dev}") for t in (u, kt, dsk))
+                ws = torch.zeros(16 * 1024 * 1024, device=f"cuda:{dev}")
+                out_g = torch.zeros(M, N, device=f"cuda:{dev}")
+                out_a = torch.zeros(B * L, H * D, device=f"cuda:{dev}")
+                out_s = torch.zeros(Bs * Ls, Hs, device=f"cuda:{dev}")
+                ops = OpList()
+                ops.gemm(view(xc), ptr(wc), N, K, view(out_g), W_hi=ptr(hc), W_lo=ptr(lc), impl=L_.GEMM_TC)
+                ops.ops[0].u.gemm.workspace, ops.ops[0].u.gemm.workspace_bytes = ws.data_ptr(), ws.numel() * 4
+                ops.attention(view(qc), view(kc), view(vc), view(out_a), ptr(relc), ptr(cgc), B, H, L, L, 64)
+                ops.s4conv(view(uc), ptr(ktc), ptr(dc), view(out_s), Bs, Ls)
+                st = torch.cuda.current_stream().cuda_stream
+                for op in ops.ops:
+                    L_.check(lib.mugd_op_run(handle, C.byref(op), st), f"op {op.kind} on cuda:{dev}")
+                torch.cuda.synchronize()
+                results.append([t.cpu() for t in (out_g, out_a, out_s)])
+            finally:
+                lib.mugd_destroy(handle)
+    assert rel_err(results[0][0], F.linear(x.double(), w.double())) < 1e-5
+    for a, b in zip(*results):
+        assert torch.equal(a, b)

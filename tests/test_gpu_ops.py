@@ -182,7 +182,7 @@ def attn_ref(q, k, v, rel, cg, H, pos_max=64):
     return (attn @ vh).permute(0, 2, 1, 3).reshape(B, Lq, inner)
 
 
-@pytest.mark.parametrize("impl", [1, 0], ids=["tcgen05", "ffma"])
+@pytest.mark.parametrize("impl", [1, 0], ids=["wgmma", "ffma"])
 @pytest.mark.parametrize("B,H,D,Lq,Lk", [(2, 8, 32, 48, 48), (2, 8, 48, 24, 21), (1, 8, 64, 200, 200), (2, 8, 32, 256, 256),
                                          (1, 8, 64, 124, 124), (3, 8, 48, 130, 21), (1, 8, 32, 496, 496), (1, 8, 48, 300, 300),
                                          (2, 8, 64, 12, 12), (1, 4, 64, 129, 257), (8, 8, 64, 64, 21), (8, 8, 32, 256, 21), (2, 8, 48, 128, 32),
