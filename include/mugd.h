@@ -278,7 +278,8 @@ int  mugd_gemm_tc_variant(const mugd_gemm* g, int32_t sm_count, int32_t* tile_n,
 /* ---- per-handle switches -------------------------------------------------------------------------
  * OPT-IN speed mode of the tensor-core GEMM: 1 = plain TF32 products (a_hi*w_hi only, ~2^-11 relative error per product, like
  * cuDNN's allow_tf32 that the reference's own GPU path uses for convs); 0 (default) = 3xTF32, fp32-accurate.  Parity tests and
- * bench.py use 0.  Plans created (and graphs captured) earlier keep the mode they were created with. */
+ * bench.py use 0.  The mode is read when a GEMM is launched: mugd_op_run and mugd_plan_run use the mode current at the call, whenever
+ * the plan was created; a captured graph keeps the mode that was current at mugd_plan_capture. */
 int  mugd_set_tc_single_pass_tf32(mugd_handle* h, int enabled);
 
 /* attention kernel: 1 (default) = QK^T and PV on the wgmma tensor cores (3xTF32, fp32 accuracy); 0 = exact-fp32 FFMA kernel
