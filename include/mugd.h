@@ -267,6 +267,20 @@ int  mugd_s4_kernel_gen(mugd_handle* h,
                         void* workspace, int64_t workspace_bytes, /* >= 16*H*(L_internal/2+1) bytes */
                         void* stream);
 
+/* ---- log-mel spectrogram of decoded audio: load_audio_without_cache, mug/util.py:138-143 (once per request) ----------------
+ * out[b*T_out + t][m] = fp16-rounded log1p(sum_k mel[m][k] |STFT(y_b)[k][t]|^2) for t < T = 1 + n/hop, 0 for T <= t < T_out (webui's
+ * pad to 64 * z_length frames, webui.py:360-365), with librosa >= 0.10's STFT: center=True, zero padding, n_fft = 512 only.
+ * window [n_fft] and twiddle [n_fft/2][2] = exp(-2 pi i k / n_fft) are fp64 device tables; band m of the filterbank is
+ * weights[sum of band_len[<m]] .. over rfft bins band_start[m] .. band_start[m] + band_len[m] - 1.  band_start and band_len are
+ * HOST arrays of n_mels entries (read by the call and checked before the launch); y, weights and out are device memory. */
+int  mugd_melspec(mugd_handle* h,
+                  const float* y, int64_t n, int64_t ldy, int32_t B,  /* [B][ldy] mono samples at the model's rate    */
+                  const double* window, const double* twiddle, int32_t n_fft,
+                  const int32_t* band_start, const int32_t* band_len, const float* weights, int32_t n_mels,
+                  int32_t hop,
+                  float* out, int64_t ldo, int32_t T_out,              /* [B*T_out][ldo] channels-last, T_out >= 1+n/hop */
+                  void* stream);
+
 /* ---- tensor-core GEMM planning: is this GEMM taken by the wgmma kernel, with which K split, and how much
  * split-K workspace / how many tile counters does it need (the host allocates them once per plan) ------ */
 int  mugd_gemm_tc_query(mugd_handle* h, const mugd_gemm* g, int32_t sm_count, int32_t* supported, int32_t* splits,

@@ -140,6 +140,25 @@ class _Wrapper:
             return o.engine.wave_session(B, T).encode(mel)
 
     @torch.no_grad()
+    def melspectrogram(self, y) -> torch.Tensor:
+        """Stands where ``load_audio_without_cache`` stands after decoding (mug/util.py:138-143): float32 samples at 22050 Hz,
+        ``[n]`` or ``[B, n]`` (numpy, or torch on any device) -> log1p mel ``[B, 128, 1 + n // 128]`` on the device, every value
+        representable in fp16.  One kernel (librosa >= 0.10 defaults, DESIGN §2); librosa is not needed."""
+        o = self._o
+        with o.engine.lock:
+            return o.mel_frontend.melspectrogram(y)
+
+    @torch.no_grad()
+    def audio_features(self, y, count: int = 1):
+        """webui.py:349-377 from decoded samples ``[n]`` (float32, 22050 Hz): returns ``(w, z_length)``, the audio encoder's
+        10-entry list for ``count`` identical samples and webui's z_length for this audio.  The mel is written, zero-padded to
+        64 * z_length frames, straight into the encoder's input rows; the encoder runs once.  The caller sets
+        ``model.z_length = z_length`` as webui does (webui.py:356).  Needs ``model.wave_model.*`` weights."""
+        o = self._o
+        with o.engine.lock:
+            return o.mel_frontend.audio_features(y, count, o.cfg.unet.levels)
+
+    @torch.no_grad()
     def decode_to_hit_objects(self, z: torch.Tensor, frame_ms: float, key_count: int = 4):
         """decode(z) followed by OsuManiaConvertor.array_to_objects (convertor.py:232-264) on the GPU: the [B,16,8L] logits
         never leave the device, only the compact note lists do.  Returns one list of .osu hit-object lines per chart."""
@@ -170,6 +189,15 @@ class MugDiffusionB200:
         emb = None if state_dict is None else state_dict.get(PROMPT_TABLE_KEY)
         self.prompt_embedder = PromptEmbedder(self.engine, emb) if emb is not None else None
         self.model = _Wrapper(self)
+        self._mel_frontend = None
+
+    @property
+    def mel_frontend(self):
+        """the audio front-end's device tables, built on first use"""
+        if self._mel_frontend is None:
+            from .audio import MelFrontEnd
+            self._mel_frontend = MelFrontEnd(self.engine)
+        return self._mel_frontend
 
     def set_prompt_table(self, weight: torch.Tensor):
         """attach / replace the [n_embed, 128] prompt embedding table (``cond_stage_model.embedding.weight``)"""

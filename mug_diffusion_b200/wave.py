@@ -283,12 +283,21 @@ class WaveSession:
         self.cfg = cfg
 
     def encode(self, mel: torch.Tensor, all_levels: bool = False) -> List[Optional[torch.Tensor]]:
+        self.load(mel)
+        return self.run(all_levels)
+
+    def load(self, mel: torch.Tensor):
+        """NCL mel [B, n_freq, T] -> the plan's channels-last input rows ``self.mel``"""
         eng = self.engine
         mel = mel.to(eng.device, torch.float32).contiguous()
         assert mel.shape == (self.B, self.cfg.n_freq, self.T), mel.shape
         eng.ncl_to_rows(mel, self.mel)
+        self._keep = mel
+
+    def run(self, all_levels: bool = False) -> List[Optional[torch.Tensor]]:
+        """One encoder pass over whatever the input rows hold (``load``, or the mel kernel writing them directly)."""
+        eng = self.engine
         self.plan.run()
         nlev = len(self.outs)
-        self._keep = mel
         return [eng.rows_to_ncl(view, self.B, ch, Lr) if all_levels or i >= nlev - 4 else None
                 for i, (view, ch, Lr) in enumerate(self.outs)]
