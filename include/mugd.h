@@ -281,6 +281,23 @@ int  mugd_melspec(mugd_handle* h,
                   float* out, int64_t ldo, int32_t T_out,              /* [B*T_out][ldo] channels-last, T_out >= 1+n/hop */
                   void* stream);
 
+/* ---- chart timing: one scan of the BPM / offset search of gridify, mug/data/utils.py:46-101 (postprocess.search_timing) ---------
+ * For each chart c, the first trial in the reference loop's order whose score n_on / bpm beats best_score[c].  The trials are rows
+ * of 6: row 0 holds head_len[c] <= 5 phases (head_bpm[c], head_off[c*5 + j]) in slots 1 + j; row r >= 1 is candidate
+ * k = k0[c] + r - 1, slot 0 = (cands[k], first[c]) and slot 1 + j = (cands[k], np.arange(best_off, best_off - beat, -beat/4)[j]),
+ * beat = 60000 / cands[k].  A trial counts the notes t with |pos - rint(pos)| < 10 / step, step = 60000 / bpm, pos = (t - off) / step
+ * (t - off in float32 for slot 0, in fp64 otherwise), all IEEE round-to-nearest, so results are bit-equal to the numpy loop.
+ * times: device float32 note times of all charts, chart c at chart_start[c] .. chart_start[c+1] - 1; cands: device fp64 candidate
+ * table [n_cands].  chart_start [n_charts + 1], k0, head_len, best_off, best_score, first, head_bpm [n_charts] and head_off
+ * [n_charts * 5] are HOST arrays (read by the call and checked before the launch; every chart needs >= 1 note, 0 <= k0 <= n_cands).
+ * workspace: device scratch of 8 * n_charts bytes.  Outputs (device): out_i[c*3 + {0,1,2}] = position row * 6 + slot (-1: no trial
+ * improves), kind (0 head, 1 candidate, 2 phase; -1), n_on; out_d[c*3 + {0,1,2}] = bpm, offset, score of that trial. */
+int  mugd_grid_scan(mugd_handle* h, const float* times, const int32_t* chart_start, int32_t n_charts,
+                    const double* cands, int32_t n_cands,
+                    const int32_t* k0, const int32_t* head_len, const double* best_off, const double* best_score,
+                    const float* first, const double* head_bpm, const double* head_off,
+                    void* workspace, int32_t* out_i, double* out_d, void* stream);
+
 /* ---- tensor-core GEMM planning: is this GEMM taken by the wgmma kernel, with which K split, and how much
  * split-K workspace / how many tile counters does it need (the host allocates them once per plan) ------ */
 int  mugd_gemm_tc_query(mugd_handle* h, const mugd_gemm* g, int32_t sm_count, int32_t* supported, int32_t* splits,

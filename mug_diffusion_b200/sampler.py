@@ -158,6 +158,15 @@ class _Wrapper:
         with o.engine.lock:
             return o.mel_frontend.audio_features(y, count, o.cfg.unet.levels)
 
+    def gridify(self, charts: Sequence[Sequence[str]]):
+        """webui's ``custom_gridify`` step (webui.py:401-407, mug/data/utils.py:46-143) for a batch of charts: returns
+        ``[(lines, bpm, offset), ...]`` equal to ``[postprocess.gridify(c, verbose=False) for c in charts]``, numpy scalar types
+        included.  The BPM / offset search scans its trials on the GPU, all charts in lockstep; the few refits and the snapping
+        run on the host.  An empty chart raises ValueError before anything runs."""
+        o = self._o
+        with o.engine.lock:
+            return o.grid_scanner.gridify(charts)
+
     @torch.no_grad()
     def decode_to_hit_objects(self, z: torch.Tensor, frame_ms: float, key_count: int = 4):
         """decode(z) followed by OsuManiaConvertor.array_to_objects (convertor.py:232-264) on the GPU: the [B,16,8L] logits
@@ -190,6 +199,7 @@ class MugDiffusionB200:
         self.prompt_embedder = PromptEmbedder(self.engine, emb) if emb is not None else None
         self.model = _Wrapper(self)
         self._mel_frontend = None
+        self._grid_scanner = None
 
     @property
     def mel_frontend(self):
@@ -198,6 +208,14 @@ class MugDiffusionB200:
             from .audio import MelFrontEnd
             self._mel_frontend = MelFrontEnd(self.engine)
         return self._mel_frontend
+
+    @property
+    def grid_scanner(self):
+        """the chart-timing scan's device tables, built on first use"""
+        if self._grid_scanner is None:
+            from .gridscan import GridScanner
+            self._grid_scanner = GridScanner(self.engine)
+        return self._grid_scanner
 
     def set_prompt_table(self, weight: torch.Tensor):
         """attach / replace the [n_embed, 128] prompt embedding table (``cond_stage_model.embedding.weight``)"""
