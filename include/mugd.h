@@ -298,6 +298,29 @@ int  mugd_grid_scan(mugd_handle* h, const float* times, const int32_t* chart_sta
                     const float* first, const double* head_bpm, const double* head_off,
                     void* workspace, int32_t* out_i, double* out_d, void* stream);
 
+/* ---- chart clean-up: gridify's snapping, mug/data/utils.py:120-139 (postprocess.snap_lines) ------------------------------------
+ * out[i] = the snapped time of note time times[i] of chart c (chart_start[c] <= i < chart_start[c+1]): for div in
+ * (1, 2, 4, 3, 6, 8, 16, 32), step = 60000 / (bpm[c] * div), pos = (t - offset[c]) / step, k = rint(pos); the first div with
+ * |pos - k| < 10 / step gives (int64)(k * step + offset[c]) (truncated toward zero); no div keeps t.  All IEEE round-to-nearest
+ * with no contraction, so results equal the numpy-scalar loop.  offset_is_f32[c] = 1 when gridify's offset is an np.float32: then
+ * t - offset is a float32 subtraction of t rounded to float32, as NumPy 2 evaluates int - np.float32.  times (int32) and out
+ * (int64) are device memory; chart_start [n_charts + 1], bpm, offset and offset_is_f32 [n_charts] are HOST arrays (read by the
+ * call and checked before the launch: chart_start[0] = 0 and non-decreasing, 0 < bpm <= 1e9, |offset| < 2^52, a float32-flagged
+ * offset is a float32 value).  Empty charts are allowed. */
+int  mugd_chart_snap(mugd_handle* h, const int32_t* times, const int32_t* chart_start, int32_t n_charts,
+                     const double* bpm, const double* offset, const int32_t* offset_is_f32, int64_t* out, void* stream);
+
+/* ---- chart clean-up: remove_intractable_mania_mini_jacks(lines, verbose=False, jack_interval), mug/data/utils.py:142-268 ------
+ * Runs the reference's greedy loop over every chart's notes in list order (one warp per chart).  Per note i (device memory):
+ * start[i] = float(f[2]); end[i] = float(f[5].split(":")[0]) when is_long[i] (int(f[3]) == 128; end is not read otherwise);
+ * x[i] = int(float(f[0])), with |x| < 2^30 (columns are x / 128 truncated toward zero, so negative and out-of-range columns
+ * behave as in the reference).  On return x[i] is the note's final x and state[i] is 0 (dropped), 1 (kept) or 2 (kept and moved:
+ * f[0] becomes str(x[i])).  workspace: device scratch of 8 * chart_start[n_charts] bytes.  chart_start [n_charts + 1] is a HOST
+ * array (chart_start[0] = 0, non-decreasing; empty charts are allowed); jack_interval must not be NaN. */
+int  mugd_remove_mini_jacks(mugd_handle* h, const int32_t* chart_start, int32_t n_charts, double jack_interval,
+                            const double* start, const double* end, const uint8_t* is_long, int32_t* x, uint8_t* state,
+                            void* workspace, void* stream);
+
 /* ---- tensor-core GEMM planning: is this GEMM taken by the wgmma kernel, with which K split, and how much
  * split-K workspace / how many tile counters does it need (the host allocates them once per plan) ------ */
 int  mugd_gemm_tc_query(mugd_handle* h, const mugd_gemm* g, int32_t sm_count, int32_t* supported, int32_t* splits,

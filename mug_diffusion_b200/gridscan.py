@@ -93,14 +93,3 @@ class GridScanner:
         """postprocess.search_timing over these charts with the scans on the device: [(bpm, offset)]"""
         self.load(times_list)
         return pp.search_timing(times_list, self.scan, self.cands_host)
-
-    def gridify(self, charts: Sequence[Sequence[str]]):
-        """[postprocess.gridify(lines, verbose=False) for lines in charts], the timing search batched over the charts"""
-        for i, lines in enumerate(charts):
-            if len(lines) == 0:
-                raise ValueError(f"chart {i} is empty: gridify needs at least one hit object")
-        if not charts:
-            return []
-        times = [pp.note_times(lines) for lines in charts]
-        timing = self.search(times)
-        return [(pp.snap_lines(lines, bpm, off), bpm, off) for lines, (bpm, off) in zip(charts, timing)]

@@ -162,6 +162,8 @@ def load() -> C.CDLL:
                                  C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_int32, C.c_int32,
                                  C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]
     lib.mugd_grid_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p] * 11
+    lib.mugd_chart_snap.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p] * 5
+    lib.mugd_remove_mini_jacks.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_double] + [C.c_void_p] * 7
     lib.mugd_gemm_tc_variant.argtypes =[C.POINTER(Gemm), C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     lib.mugd_gemm_tc_query.argtypes = [C.c_void_p, C.POINTER(Gemm), C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                        C.POINTER(C.c_int64), C.POINTER(C.c_int32)]
@@ -212,5 +214,5 @@ EXPORTED_SYMBOLS = [
     "mugd_plan_launch_count", "mugd_plan_destroy", "mugd_s4_kernel_gen", "mugd_fill_i32", "mugd_abi_sizes", "mugd_gemm_tc_query",
     "mugd_set_pdl", "mugd_set_tc_single_pass_tf32", "mugd_set_attention_impl", "mugd_debug_set_tc_tile_n", "mugd_debug_set_tc_cost", "mugd_gemm_tc_variant",
     "mugd_debug_set_attention_dump", "mugd_debug_set_tc_timing", "mugd_sample", "mugd_plan_save", "mugd_plan_load", "mugd_plan_regions", "mugd_plan_ops",
-    "mugd_melspec", "mugd_grid_scan",
+    "mugd_melspec", "mugd_grid_scan", "mugd_chart_snap", "mugd_remove_mini_jacks",
 ]

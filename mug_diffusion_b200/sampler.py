@@ -161,11 +161,30 @@ class _Wrapper:
     def gridify(self, charts: Sequence[Sequence[str]]):
         """webui's ``custom_gridify`` step (webui.py:401-407, mug/data/utils.py:46-143) for a batch of charts: returns
         ``[(lines, bpm, offset), ...]`` equal to ``[postprocess.gridify(c, verbose=False) for c in charts]``, numpy scalar types
-        included.  The BPM / offset search scans its trials on the GPU, all charts in lockstep; the few refits and the snapping
-        run on the host.  An empty chart raises ValueError before anything runs."""
+        included.  The BPM / offset search scans its trials on the GPU, all charts in lockstep, with its few refits on the host;
+        the snapping runs on the GPU.  An empty chart raises ValueError before anything runs."""
+        from . import chartpost
         o = self._o
         with o.engine.lock:
-            return o.grid_scanner.gridify(charts)
+            return chartpost.gridify(o.grid_scanner, o.chart_post, charts)
+
+    def remove_mini_jacks(self, charts: Sequence[Sequence[str]], jack_interval=90):
+        """``[postprocess.remove_intractable_mania_mini_jacks(c, verbose=False, jack_interval=jack_interval) for c in charts]``
+        (mug/data/utils.py:142-268) with the greedy loop on the GPU, one warp per chart.  An empty chart gives []."""
+        from . import chartpost
+        o = self._o
+        with o.engine.lock:
+            return chartpost.remove_mini_jacks(o.chart_post, charts, jack_interval)
+
+    def postprocess_charts(self, charts: Sequence[Sequence[str]], auto_snap: bool = True, jack_interval=90):
+        """webui's ``custom_gridify`` (webui.py:401-407) for every chart: returns ``[(bpm, offset, lines), ...]``, equal to
+        gridify(c, verbose=False), its snapped lines kept if ``auto_snap``, then remove_intractable_mania_mini_jacks(...,
+        verbose=False, jack_interval).  The timing search runs as in ``gridify``; snapping and mini-jack removal run on the
+        GPU; the lines are parsed once and formatted once.  An empty chart raises ValueError before anything runs."""
+        from . import chartpost
+        o = self._o
+        with o.engine.lock:
+            return chartpost.postprocess_charts(o.grid_scanner, o.chart_post, charts, auto_snap, jack_interval)
 
     @torch.no_grad()
     def decode_to_hit_objects(self, z: torch.Tensor, frame_ms: float, key_count: int = 4):
@@ -200,6 +219,7 @@ class MugDiffusionB200:
         self.model = _Wrapper(self)
         self._mel_frontend = None
         self._grid_scanner = None
+        self._chart_post = None
 
     @property
     def mel_frontend(self):
@@ -216,6 +236,14 @@ class MugDiffusionB200:
             from .gridscan import GridScanner
             self._grid_scanner = GridScanner(self.engine)
         return self._grid_scanner
+
+    @property
+    def chart_post(self):
+        """the chart clean-up kernels (snapping, mini-jack removal), set up on first use"""
+        if self._chart_post is None:
+            from .chartpost import ChartPost
+            self._chart_post = ChartPost(self.engine)
+        return self._chart_post
 
     def set_prompt_table(self, weight: torch.Tensor):
         """attach / replace the [n_embed, 128] prompt embedding table (``cond_stage_model.embedding.weight``)"""
