@@ -5,6 +5,8 @@
  *   examples/host_c/sample_host <bundle dir>
  *
  * manifest.txt lines:  region <name> <bytes> zero|file <file>   |  plan <file> run|graph  |  sample <eval> <tail> <steps>
+ *                      stage <field> <region> <offset>          (one pointer of the mugd_stage of the next `staged` line)
+ *                      staged <eval> <tail> <steps> <q_coef file>|- <B> <C> <L>   (inpainting / eta > 0: mugd_sample_staged)
  *                      expect <region> <bytes> <file>           (outputs to compare; exit status 1 on mismatch)
  * This mirrors what DDIMSampler.sample + model.decode do in the reference (mug/diffusion/ddim.py:56-196, diffusion.py:49-50). */
 #include <cuda_runtime.h>
@@ -59,7 +61,8 @@ int main(int argc, char** argv) {
     CK(cudaEventCreate(&e1));
     int bad = 0;
     float sample_ms = 0.f;
-    int sample_steps = 0;
+    mugd_stage stage;
+    memset(&stage, 0, sizeof(stage));
 
     while (fgets(line, sizeof(line), mf)) {
         char a[64], b[256], c[256], d[256];
@@ -93,9 +96,32 @@ int main(int argc, char** argv) {
             CK(cudaStreamSynchronize(st));
             printf("ran %-12s (%s, %d launches)\n", b, c, mugd_plan_launch_count(p));
             mugd_plan_destroy(p);
-        } else if (strcmp(a, "sample") == 0) {
+        } else if (strcmp(a, "stage") == 0) {
+            long long off = 0;
+            if (sscanf(line, "%*s %63s %255s %lld", d, b, &off) != 3) { fprintf(stderr, "bad line: %s", line); return 2; }
+            mugd_region* r = find_region(b);
+            if (off < 0 || off >= r->bytes) { fprintf(stderr, "offset outside region %s: %s", b, line); return 2; }
+            void* p = (char*)r->base + off;
+            if (strcmp(d, "x") == 0) stage.x = (float*)p;
+            else if (strcmp(d, "x_dup") == 0) stage.x_dup = (float*)p;
+            else if (strcmp(d, "x0") == 0) stage.x0 = (const float*)p;
+            else if (strcmp(d, "mask") == 0) stage.mask = (const float*)p;
+            else if (strcmp(d, "q_noise") == 0) stage.q_noise = (const float*)p;
+            else if (strcmp(d, "noise") == 0) stage.noise = (const float*)p;
+            else if (strcmp(d, "noise_rows") == 0) stage.noise_rows = (float*)p;
+            else { fprintf(stderr, "unknown stage field: %s", line); return 2; }
+        } else if (strcmp(a, "sample") == 0 || strcmp(a, "staged") == 0) {
+            const int staged = strcmp(a, "staged") == 0;
             int steps = 0;
-            if (sscanf(line, "%*s %255s %255s %d", b, c, &steps) != 3) { fprintf(stderr, "bad line: %s", line); return 2; }
+            float* q_coef = NULL;
+            if (staged) {
+                if (sscanf(line, "%*s %255s %255s %d %255s %d %d %d", b, c, &steps, d, &stage.B, &stage.C, &stage.L) != 7 || steps < 0) {
+                    fprintf(stderr, "bad line: %s", line);
+                    return 2;
+                }
+                if (strcmp(d, "-") != 0) q_coef = (float*)read_file(dir, d, 8LL * steps);   /* host array [steps][2] */
+                stage.q_coef = q_coef;
+            } else if (sscanf(line, "%*s %255s %255s %d", b, c, &steps) != 3) { fprintf(stderr, "bad line: %s", line); return 2; }
             mugd_plan *pe = NULL, *pt = NULL;
             snprintf(path, sizeof(path), "%s/%s", dir, b);
             MK(mugd_plan_load(h, path, regions, n_regions, &pe));
@@ -116,13 +142,15 @@ int main(int argc, char** argv) {
             CK(cudaMemcpy(arena->base, snap, (size_t)arena->bytes, cudaMemcpyDeviceToDevice));
             CK(cudaFree(snap));
             CK(cudaEventRecord(e0, st));
-            MK(mugd_sample(pe, tail, n_tail, steps, st));   /* the whole DDIM loop: one call, no synchronisation inside */
+            /* the whole DDIM loop: one call, no synchronisation inside */
+            if (staged) MK(mugd_sample_staged(pe, &stage, tail, n_tail, steps, st));
+            else MK(mugd_sample(pe, tail, n_tail, steps, st));
             CK(cudaEventRecord(e1, st));
             CK(cudaStreamSynchronize(st));
             CK(cudaEventElapsedTime(&sample_ms, e0, e1));
-            sample_steps = steps;
-            printf("sampled %d DDIM steps in %.3f ms (%.1f steps/s, %d launches per evaluation)\n", steps, sample_ms, 1000.0 * steps / sample_ms,
-                   mugd_plan_launch_count(pe));
+            printf("sampled %d DDIM steps in %.3f ms (%.1f steps/s, %d launches per evaluation)%s\n", steps, sample_ms, 1000.0 * steps / sample_ms,
+                   mugd_plan_launch_count(pe), staged ? (q_coef ? ", staged: inpainting" : ", staged: step noise") : "");
+            free(q_coef);
             mugd_plan_destroy(pe);
             mugd_plan_destroy(pt);
         } else if (strcmp(a, "expect") == 0) {
@@ -148,7 +176,6 @@ int main(int argc, char** argv) {
         }
     }
     fclose(mf);
-    (void)sample_steps;
     mugd_destroy(h);
     return bad;
 }

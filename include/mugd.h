@@ -240,6 +240,32 @@ void mugd_plan_destroy(mugd_plan* p);
  * step-dependent rows (time embedding, DDIM coefficients) are selected on the device by the counter.  `eval_plan` must be captured. */
 int  mugd_sample(mugd_plan* eval_plan, const mugd_op* tail, int32_t n_tail, int32_t n_steps, void* stream);
 
+/* ---- the same loop for inpainting and eta > 0 requests: what the host stages in front of each step ---------------------------
+ * Step i of a mugd_sample_staged call first runs one stage kernel over the dense x rows [B*L, C] that MUGD_OP_DDIM_UPDATE updates:
+ *   inpainting blend (ddim.py:141-144, diffusion.py:327-333), when x0 is given:
+ *       xo = a_i * x0 + b_i * q_noise[i];   x <- xo * mask + (1 - mask) * x   (written to x and, if given, x_dup)
+ *     in torch's eager operation order with IEEE round-to-nearest and no contraction, so the result is bit-identical to those ops;
+ *   step noise, when noise is given: noise_rows <- noise[i] transposed to rows (the DDIM op's `noise`).
+ * x0, mask, q_noise and noise are device NCL tensors as torch holds them ([B, C, L]; the tables [n_steps][B, C, L], row i for step i of
+ * this call); the mask is expanded to [B, C, L].  q_coef is a HOST array [n_steps][2] = (sqrt_alphas_cumprod[t_i],
+ * sqrt_one_minus_alphas_cumprod[t_i]) read by the call.  Either part may be absent (NULL); x0, mask, q_noise and q_coef go together,
+ * as do noise and noise_rows. */
+typedef struct mugd_stage {
+    float* x; float* x_dup;                /* [B*L, C] dense rows; x_dup = the CFG copy or NULL                  */
+    const float* x0;                       /* [B, C, L] or NULL (no blend)                                     */
+    const float* mask;                     /* [B, C, L]                                                        */
+    const float* q_noise;                  /* [n_steps][B, C, L] q_sample's randn_like(x0) per step            */
+    const float* q_coef;                   /* HOST [n_steps][2]                                                */
+    const float* noise;                    /* [n_steps][B, C, L] randn(shape) [+ dropout] per step, or NULL    */
+    float* noise_rows;                     /* [B*L, C] the DDIM op's noise rows                                */
+    int32_t B, C, L, reserved_;
+} mugd_stage;
+/* n_steps x { stage kernel for step i ; replay of the captured evaluation plan ; the tail ops }.  Every argument is checked before the
+ * first launch: each MUGD_OP_DDIM_UPDATE of the tail must update the same rows (x, x_dup, n = B*C*L) and, with noise, read noise_rows.
+ * A standalone entry point: the ABI version is unchanged. */
+int  mugd_sample_staged(mugd_plan* eval_plan, const mugd_stage* stage, const mugd_op* tail, int32_t n_tail, int32_t n_steps,
+                        void* stream);
+
 /* ---- plans on disk: a host without Python (examples/host_c) loads what the Python plan compiler produced ---------------------
  * Every pointer of a plan lies in one of a few device allocations ("regions": weight blob, activation arena, side tables, the
  * caller's staging buffers).  mugd_plan_save stores each pointer as (region, offset); mugd_plan_load resolves them against the

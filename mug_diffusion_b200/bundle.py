@@ -1,6 +1,7 @@
 """Export one compiled sampling request as a bundle a host WITHOUT Python can run (examples/host_c/sample_host.c):
 
     python -m mug_diffusion_b200.bundle --out /tmp/bundle --L 96 --B 1 --S 10 --scale 5
+    python -m mug_diffusion_b200.bundle --out /tmp/bundle --L 96 --B 2 --S 10 --scale 5 --eta 1 --inpaint     (regenerate half a chart)
 
 The network -> launch-plan compiler is Python (engine.py); what it produces is plain data: arrays of mugd_op whose pointers fall
 into a handful of device allocations.  The bundle holds
@@ -11,13 +12,16 @@ into a handful of device allocations.  The bundle holds
 Request flow = DDIMSampler.sample + model.decode (ddim.py:56-196, diffusion.py:49-50):
     emb (time-embedding table) -> ctx (cross-attention K|V) -> audio (concat slots) -> loadx -> S x {eval graph ; update ; advance}
     -> readz -> decode -> readlogits
+An inpainting or eta > 0 request stages x0, the mask and the random numbers of every step (drawn up front from torch's CUDA generator in
+the sampler's order) as input regions, with the q_sample coefficients in stage_coef.bin, and runs its loop as one mugd_sample_staged
+call: `stage <field> <region> <offset>` lines describe the mugd_stage, `staged eval.plan tail.plan <steps> <coef file> <B> <C> <L>` runs it.
 """
 from __future__ import annotations
 
 import argparse
 import ctypes as C
 import os
-from typing import Dict, List
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -25,6 +29,7 @@ import torch
 from . import lib as L_
 from .engine import OpList
 from .runtime import Plan, _ptr
+from .sampler import draw_step_noise
 
 
 def _save_plan(eng, ops: OpList, regions: List[L_.Region], path: str) -> Plan:
@@ -34,9 +39,11 @@ def _save_plan(eng, ops: OpList, regions: List[L_.Region], path: str) -> Plan:
     return pl
 
 
-def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out_dir: str) -> Dict[str, torch.Tensor]:
-    """Compile the request (inp: x_T, c, uc, w[4] on the host), write the bundle, run it once through the very same plans and
-    return the results (z, logits) that the C host must reproduce."""
+def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out_dir: str, eta: float = 0.0, temperature: float = 1.0,
+                  noise_dropout: float = 0.0, inpaint: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
+    """Compile the request (inp: x_T, c, uc, w[4] on the host; inpaint: (x0, mask) of DDIMSampler.sample), write the bundle, run it
+    once through the very same plans and return the results (z, logits) that the C host must reproduce.  The random numbers of an
+    eta > 0 or inpainting request are drawn here from the CUDA generator as DDIMSampler.sample draws them."""
     from .sampler import DDIMSampler
 
     os.makedirs(out_dir, exist_ok=True)
@@ -47,7 +54,7 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
     cfg_on = scale != 1.0
     Beff = 2 * B if cfg_on else B
     sampler = DDIMSampler(model)
-    sampler.make_schedule(S, verbose=False)
+    sampler.make_schedule(S, ddim_eta=eta, verbose=False)
     ts = np.flip(sampler.ddim_timesteps)
     total = len(ts)
 
@@ -63,6 +70,21 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
         w4 = [w.to(dev).contiguous() for w in list(inp["w"])[-cfg.unet.levels:]]
         for i, w in enumerate(w4):
             st[f"in_w{i}"] = w
+        # the staged loop's operands: x0, the expanded mask and one [B, C, L] row per step of each noise table
+        has_noise = bool(np.any(np.asarray(sampler.ddim_sigmas) != 0))
+        staged = has_noise or inpaint is not None
+        shape = (B, Cz, Lz)
+        if has_noise:
+            st["noise_rows"] = torch.zeros(B * Lz * Cz, device=dev)
+            st["in_noise"] = torch.empty((total,) + shape, device=dev)
+        if inpaint is not None:
+            st["in_x0"] = inpaint[0].to(dev, torch.float32).contiguous()
+            st["in_mask"] = inpaint[1].to(dev, torch.float32).expand(shape).contiguous()
+            st["in_qnoise"] = torch.empty((total,) + shape, device=dev)
+            sac, s1m = model.sqrt_alphas_cumprod.cpu(), model.sqrt_one_minus_alphas_cumprod.cpu()
+            qcoef = np.ascontiguousarray(np.stack([sac[ts.copy()].numpy(), s1m[ts.copy()].numpy()], 1), dtype=np.float32)
+            qcoef.tofile(os.path.join(out_dir, "stage_coef.bin"))
+        draw_step_noise(total, shape, st.get("in_x0"), st.get("in_qnoise"), has_noise, st.get("in_noise"), noise_dropout, dev)
         # per-request host tables for this S
         sess.set_timestep_table(ts.copy())
         sess.set_ddim_schedule(sampler.ddim_alphas, sampler.ddim_alphas_prev, sampler.ddim_sigmas, sampler.ddim_sqrt_one_minus_alphas)
@@ -83,7 +105,15 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
         regions = [L_.Region(keep[i], _ptr(tensors[n]), tensors[n].numel() * tensors[n].element_size()) for i, n in enumerate(names)]
 
         # ---- the plans ----
-        tail = sess.ddim_tail(B, total, cfg_on, scale, 1.0, _ptr(st["pred"]))
+        tail = sess.ddim_tail(B, total, cfg_on, scale, temperature, _ptr(st["pred"]), _ptr(st["noise_rows"]) if has_noise else 0)
+        stage = None
+        if staged:
+            stage = sess.ddim_stage(B, cfg_on, _ptr(st["noise_rows"]) if has_noise else 0)
+            if has_noise:
+                stage.noise = _ptr(st["in_noise"])
+            if inpaint is not None:
+                stage.x0, stage.mask, stage.q_noise = _ptr(st["in_x0"]), _ptr(st["in_mask"]), _ptr(st["in_qnoise"])
+                stage.q_coef = qcoef.ctypes.data
         readz = OpList()
         readz.transpose(sess.xin.ptr, _ptr(st["out_z"]), sess.xin.ld, 0, B, Cz, Lz, False)
         dec_in = OpList()
@@ -117,7 +147,14 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
             plans[name] = pl
             if mode == "tail":
                 continue
-            if name == "eval":
+            if name == "eval" and staged:
+                for field in ("x", "x_dup", "x0", "mask", "q_noise", "noise", "noise_rows"):
+                    ptr = getattr(stage, field)
+                    if ptr:
+                        region = next(n for n in names if 0 <= ptr - _ptr(tensors[n]) < tensors[n].numel() * tensors[n].element_size())
+                        lines.append(f"stage {field} {region} {ptr - _ptr(tensors[region])}")
+                lines.append(f"staged eval.plan tail.plan {total} {'stage_coef.bin' if inpaint is not None else '-'} {B} {Cz} {Lz}")
+            elif name == "eval":
                 lines.append(f"sample eval.plan tail.plan {total}")
             else:
                 lines.append(f"plan {name}.plan {mode}")
@@ -126,7 +163,7 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
         sess.set_step(0)
         for name in ("emb", "ctx", "audio", "loadx"):
             plans[name].run()
-        sess.plan.launch(total, tail)
+        sess.plan.launch(total, tail, stage)
         for name in ("readz", "dec_in"):
             plans[name].run()
         dec.plan.launch()
@@ -149,10 +186,17 @@ def main():
     ap.add_argument("--B", type=int, default=1)
     ap.add_argument("--S", type=int, default=10)
     ap.add_argument("--scale", type=float, default=5.0)
+    ap.add_argument("--eta", type=float, default=0.0)
+    ap.add_argument("--temperature", type=float, default=1.0)
+    ap.add_argument("--noise-dropout", type=float, default=0.0)
+    ap.add_argument("--inpaint", action="store_true", help="keep the first half of a synthetic chart latent, regenerate the rest")
+    ap.add_argument("--seed", type=int, default=0, help="torch CUDA generator seed of the staged random numbers")
     a = ap.parse_args()
     model = MugDiffusionB200.from_state_dict(synth.synthetic_state_dict(a.L), z_length=a.L)
     inp = synth.synthetic_inputs(a.B, a.L)
-    res = export_bundle(model, inp, a.S, a.scale, a.out)
+    torch.cuda.manual_seed(a.seed)
+    res = export_bundle(model, inp, a.S, a.scale, a.out, eta=a.eta, temperature=a.temperature, noise_dropout=a.noise_dropout,
+                        inpaint=synth.synthetic_inpainting(a.B, a.L) if a.inpaint else None)
     print("bundle written to", a.out, "| z", tuple(res["z"].shape), "logits", tuple(res["logits"].shape))
 
 

@@ -218,6 +218,40 @@ int mugd_sample(mugd_plan* eval_plan, const mugd_op* tail, int32_t n_tail, int32
     return MUGD_OK;
 }
 
+int mugd_sample_staged(mugd_plan* eval_plan, const mugd_stage* stage, const mugd_op* tail, int32_t n_tail, int32_t n_steps,
+                       void* stream) {
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_staged: the evaluation plan must be captured (mugd_plan_capture)");
+    MUGD_REQUIRE(stage, "mugd_sample_staged: null stage");
+    MUGD_REQUIRE(n_steps >= 0, "mugd_sample_staged: n_steps=%d < 0", n_steps);
+    MUGD_REQUIRE(n_tail >= 0 && (n_tail == 0 || tail), "mugd_sample_staged: bad tail (n_tail=%d)", n_tail);
+    const mugd_stage& s = *stage;
+    int rc = check_stage(s, n_steps);
+    if (rc != MUGD_OK) return rc;
+    const int64_t n = (int64_t)s.B * s.C * s.L;
+    for (int k = 0; k < n_tail; ++k) {
+        if (tail[k].kind != MUGD_OP_DDIM_UPDATE) continue;
+        const mugd_ddim_update& d = tail[k].u.ddim;
+        MUGD_REQUIRE(d.x == s.x && d.x_dup == s.x_dup, "mugd_sample_staged: tail op %d updates other rows than the stage's x / x_dup", k);
+        MUGD_REQUIRE(d.n == n, "mugd_sample_staged: tail op %d updates n=%d elements, the stage B*C*L=%lld", k, d.n, (long long)n);
+        MUGD_REQUIRE(!s.noise || d.noise == s.noise_rows, "mugd_sample_staged: tail op %d reads its noise from other rows than noise_rows",
+                     k);
+    }
+    const bool staged = s.x0 || s.noise;
+    cudaStream_t st = (cudaStream_t)stream;
+    for (int i = 0; i < n_steps; ++i) {
+        if (staged) {
+            rc = launch_stage(s, i, st);
+            if (rc != MUGD_OK) return rc;
+        }
+        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
+        for (int k = 0; k < n_tail; ++k) {
+            rc = dispatch(eval_plan->h, tail[k], st, nullptr);
+            if (rc != MUGD_OK) return rc;
+        }
+    }
+    return MUGD_OK;
+}
+
 int mugd_abi_sizes(int32_t* out, int32_t n) {
     MUGD_REQUIRE(out && n >= 13, "abi_sizes: need room for 13 entries");
     out[0] = sizeof(mugd_op); out[1] = sizeof(mugd_gemm); out[2] = sizeof(mugd_groupnorm);

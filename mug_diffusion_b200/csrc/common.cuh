@@ -62,6 +62,9 @@ int launch_notes(const DeviceInfo& dev, const mugd_notes& n, cudaStream_t st, in
 int launch_embed(const DeviceInfo& dev, const mugd_embed& e, cudaStream_t st, int* launches);
 int launch_tf32_split(const DeviceInfo& dev, const mugd_tf32_split& s, cudaStream_t st, int* launches);
 int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_t st, int* launches);
+// mugd_sample_staged: check_stage validates a stage for n_steps (host arrays included); launch_stage runs step i of it
+int check_stage(const mugd_stage& s, int32_t n_steps);
+int launch_stage(const mugd_stage& s, int32_t i, cudaStream_t st);
 int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, cudaStream_t st, int* launches);
 bool gemm_tc_supported(const mugd_gemm& g);
 

@@ -1,5 +1,6 @@
 // Small fused elementwise kernels of the sampler loop:
 //   ddim_update : classifier-free-guidance combine + DDIM x_{t-1} update   mug/diffusion/ddim.py:170-195
+//   stage       : inpainting blend + step noise in front of a step of mugd_sample_staged   ddim.py:141-144,192-194
 //   transpose   : [B,C,L] <-> channels-last [B*L, ld] at the Python boundary (reference tensors are NCL)
 //   copy2d      : strided row copy (the 4 per-level tensors that live in two concat buffers)
 //   step_advance: device-side step counter so one CUDA graph serves every DDIM step
@@ -43,6 +44,74 @@ int launch_ddim_update(const DeviceInfo&, const mugd_ddim_update& d, cudaStream_
     MUGD_REQUIRE(d.n > 0 && d.S > 0 && d.x && d.eps && d.coef, "ddim_update: bad arguments");
     MUGD_CHECK_CUDA(launch_k(ddim_update_kernel, dim3((d.n + 255) / 256), dim3(256), 0, st, d));
     if (launches) *launches += 1;
+    return MUGD_OK;
+}
+
+// Stage of one step of mugd_sample_staged: the inpainting blend on the x rows and the step noise into the DDIM op's noise rows.
+// 32x32 tiles as in transpose_kernel: the NCL operands are read coalesced along L, the rows written along C.  The blend restates
+// `a * x0 + b * noise` (q_sample) and `x_orig * mask + (1. - mask) * x` (ddim.py:141-144) op for op with _rn intrinsics.
+__global__ void __launch_bounds__(256)
+stage_kernel(const mugd_stage s, const float* __restrict__ qn, const float* __restrict__ nz, float a, float b) {
+    __shared__ float t_x0[32][33], t_m[32][33], t_q[32][33], t_n[32][33];
+    pdl_wait();
+    const int bb = blockIdx.z;
+    const int c0 = blockIdx.y * 32, l0 = blockIdx.x * 32;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;   // 32 x 8
+    const int C = s.C, L = s.L;
+    const int64_t base = (int64_t)bb * C * L;
+#pragma unroll
+    for (int r = ty; r < 32; r += 8) {
+        const int c = c0 + r, l = l0 + tx;
+        if (c < C && l < L) {
+            const int64_t j = base + (int64_t)c * L + l;
+            if (s.x0) {
+                t_x0[r][tx] = s.x0[j];
+                t_m[r][tx] = s.mask[j];
+                t_q[r][tx] = qn[j];
+            }
+            if (nz) t_n[r][tx] = nz[j];
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = ty; r < 32; r += 8) {
+        const int l = l0 + r, c = c0 + tx;
+        if (c >= C || l >= L) continue;
+        const int64_t row = ((int64_t)bb * L + l) * C + c;
+        if (s.x0) {
+            const float m = t_m[tx][r];
+            const float xo = __fadd_rn(__fmul_rn(a, t_x0[tx][r]), __fmul_rn(b, t_q[tx][r]));
+            const float v = __fadd_rn(__fmul_rn(xo, m), __fmul_rn(__fsub_rn(1.0f, m), s.x[row]));
+            s.x[row] = v;
+            if (s.x_dup) s.x_dup[row] = v;
+        }
+        if (nz) s.noise_rows[row] = t_n[tx][r];
+    }
+}
+
+int check_stage(const mugd_stage& s, int32_t n_steps) {
+    MUGD_REQUIRE(s.x, "sample_staged: stage.x is NULL");
+    MUGD_REQUIRE(s.B > 0 && s.C > 0 && s.L > 0 && (int64_t)s.B * s.C * s.L <= INT32_MAX, "sample_staged: bad shape B=%d C=%d L=%d",
+                 s.B, s.C, s.L);
+    MUGD_REQUIRE(s.B <= 65535 && (s.C + 31) / 32 <= 65535, "sample_staged: B=%d / C=%d too large for one launch", s.B, s.C);
+    MUGD_REQUIRE(!s.q_coef || s.q_noise, "sample_staged: q_coef given without a q-noise table");
+    MUGD_REQUIRE(!s.q_noise || s.x0, "sample_staged: q-noise table given without x0");
+    MUGD_REQUIRE(!s.mask || s.x0, "sample_staged: mask given without x0");
+    MUGD_REQUIRE(!s.x0 || (s.mask && s.q_noise && s.q_coef), "sample_staged: x0 needs mask, q_noise and q_coef");
+    MUGD_REQUIRE(!s.noise == !s.noise_rows, "sample_staged: noise and noise_rows go together");
+    if (s.q_coef)
+        for (int32_t i = 0; i < 2 * n_steps; ++i)
+            MUGD_REQUIRE(isfinite(s.q_coef[i]), "sample_staged: q_coef[%d][%d] = %g is not finite", i / 2, i % 2, s.q_coef[i]);
+    return MUGD_OK;
+}
+
+int launch_stage(const mugd_stage& s, int32_t i, cudaStream_t st) {
+    const int64_t n = (int64_t)s.B * s.C * s.L;
+    const float* qn = s.q_noise ? s.q_noise + i * n : nullptr;
+    const float* nz = s.noise ? s.noise + i * n : nullptr;
+    const float a = s.q_coef ? s.q_coef[2 * i] : 0.0f, b = s.q_coef ? s.q_coef[2 * i + 1] : 0.0f;
+    const dim3 grid((s.L + 31) / 32, (s.C + 31) / 32, s.B);
+    MUGD_CHECK_CUDA(launch_k(stage_kernel, grid, dim3(256), 0, st, s, qn, nz, a, b));
     return MUGD_OK;
 }
 

@@ -51,10 +51,10 @@ class Plan:
     def replay(self, times: int = 1):
         L_.check(self.engine.lib.mugd_plan_replay(self.handle, times, _stream()), "plan_replay")
 
-    def launch(self, steps: int = 1, tail: Optional[OpList] = None):
+    def launch(self, steps: int = 1, tail: Optional[OpList] = None, stage: Optional[L_.Stage] = None):
         """``steps`` replays of the plan's CUDA graph; with ``tail``, every replay is followed by the tail ops and all steps run from
-        one C call (mugd_sample).  The first call captures the graph, after a warm-up run outside capture (lazy module load,
-        cudaFuncSetAttribute)."""
+        one C call (mugd_sample); with ``stage`` as well, each step starts with the stage kernel (mugd_sample_staged: inpainting blend,
+        step noise).  The first call captures the graph, after a warm-up run outside capture (lazy module load, cudaFuncSetAttribute)."""
         if not self.captured:
             self.run()
             self.capture()
@@ -62,7 +62,11 @@ class Plan:
             self.replay(steps)
             return
         self.engine.attach_workspace(tail)
-        L_.check(self.engine.lib.mugd_sample(self.handle, tail.array(), len(tail.ops), steps, _stream()), "mugd_sample")
+        if stage is None:
+            L_.check(self.engine.lib.mugd_sample(self.handle, tail.array(), len(tail.ops), steps, _stream()), "mugd_sample")
+        else:
+            L_.check(self.engine.lib.mugd_sample_staged(self.handle, C.byref(stage), tail.array(), len(tail.ops), steps, _stream()),
+                     "mugd_sample_staged")
 
     def __del__(self):
         try:
@@ -474,6 +478,16 @@ class Session:
         tail.add(L_.OP_DDIM_UPDATE, upd)
         tail.add(L_.OP_STEP_ADVANCE, adv)
         return tail
+
+    def ddim_stage(self, B: int, cfg_on: bool, noise: int = 0) -> L_.Stage:
+        """the stage of mugd_sample_staged over the rows ddim_tail updates (x, and its copy under classifier-free guidance);
+        ``noise`` = the tail's noise rows.  The caller fills in x0 / mask / q_noise / q_coef and the noise table."""
+        s = L_.Stage()
+        s.x = self.xin.ptr
+        s.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        s.noise_rows = noise or None
+        s.B, s.C, s.L = B, self.engine.cfg.unet.in_channels, self.Lz
+        return s
 
     def set_step(self, value: int):
         L_.check(self.engine.lib.mugd_fill_i32(_ptr(self.step), value, _stream()), "fill_i32")

@@ -61,6 +61,50 @@ def ddim_parameters(alphas_cumprod: torch.Tensor, ts: np.ndarray, eta: float):
 
 
 # --------------------------------------------------------------------------------------------------
+# the device loop's staged random numbers (mugd_sample_staged)
+# --------------------------------------------------------------------------------------------------
+# Each noise table of one mugd_sample_staged call holds at most this many bytes (one [B, C, L] float32 tensor per step, at least one
+# step); a longer stretch is split into several calls, which changes no result.  B=4, L=512 needs 128 KiB per step.
+STAGE_TABLE_BYTES = 64 << 20
+
+
+def draw_step_noise(steps: int, shape, x0: Optional[torch.Tensor], q_table: Optional[torch.Tensor], draw_noise: bool,
+                    noise_table: Optional[torch.Tensor], noise_dropout: float, device):
+    """The random numbers of ``steps`` DDIM steps, drawn in the per-step loop's order from the device's default generator: per step
+    q_sample's randn_like(x0) into q_table[k] (when q_table is given, ddim.py:142), then randn(shape) [+ dropout] (when draw_noise,
+    ddim.py:192-194) into noise_table[k], or discarded when noise_table is None.  Same values, same generator state afterwards."""
+    for k in range(steps):
+        if q_table is not None:
+            q_table[k].copy_(torch.randn_like(x0))
+        if draw_noise:
+            nz = torch.randn(shape, device=device)
+            if noise_dropout > 0.:
+                nz = torch.nn.functional.dropout(nz, p=noise_dropout)
+            if noise_table is not None:
+                noise_table[k].copy_(nz)
+
+
+def takes_device_loop(shape, device, mask=None, x0=None, callback=None, img_callback=None) -> bool:
+    """True when ddim_sampling runs the request from mugd_sample / mugd_sample_staged calls.  Callbacks need the per-step loop; so do
+    inpainting operands on which the per-step ops would promote or raise: a mask or x0 that is not a float32 tensor on the model's
+    device, an x0 that is not of ``shape``, a mask that does not broadcast to exactly ``shape``."""
+    if callback is not None or img_callback is not None:
+        return False
+    if mask is None:
+        return True
+    shape = tuple(shape)
+    for t in (mask, x0):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != torch.device(device):
+            return False
+    if tuple(x0.shape) != shape:
+        return False
+    try:
+        return tuple(torch.broadcast_shapes(mask.shape, shape)) == shape
+    except RuntimeError:
+        return False
+
+
+# --------------------------------------------------------------------------------------------------
 # model holder with the attributes the callers read
 # --------------------------------------------------------------------------------------------------
 PROMPT_TABLE_KEY = "model.cond_stage_model.embedding.weight"
@@ -401,17 +445,47 @@ class DDIMSampler(object):
             def current_pred():
                 return eng.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
 
-            per_step_host_work = (mask is not None or has_noise or match_rng or callback is not None or img_callback is not None)
-            if not per_step_host_work:
-                # nothing on the host between steps: run the stretches between two recorded intermediates from ONE C call each
-                # (mugd_sample: n x {graph replay, CFG/DDIM update, step advance}, no synchronisation)
+            if takes_device_loop(shape, x.device, mask, x0, callback, img_callback):
+                # nothing on the host between steps: run the stretches between two recorded intermediates from one C call each
+                # (mugd_sample: n x {graph replay, CFG/DDIM update, step advance}, no synchronisation).  Inpainting and eta > 0 draw a
+                # stretch's random numbers up front, in the per-step loop's order, and stage them in front of every step
+                # (mugd_sample_staged); match_reference_rng alone only draws and discards.
+                blend = mask is not None
+                draw = has_noise or match_rng
+                stage, q_tab, n_tab, qcoef = None, None, None, None
+                per_call = max(1, STAGE_TABLE_BYTES // (4 * B * Cz * Lz))
+                if blend or has_noise:
+                    stage = sess.ddim_stage(B, cfg_on, _ptr(noise_nlc) if has_noise else 0)
+                    tab_steps = min(per_call, total)
+                    if blend:
+                        x0c = x0.contiguous()
+                        mask_e = mask.expand(shape).contiguous()                # the blend's mask, expanded once per request
+                        q_tab = torch.empty((tab_steps,) + tuple(shape), device=dev)
+                        sac, s1m = model.sqrt_alphas_cumprod.cpu(), model.sqrt_one_minus_alphas_cumprod.cpu()
+                        qcoef = np.ascontiguousarray(np.stack([sac[time_range.copy()].numpy(), s1m[time_range.copy()].numpy()], 1),
+                                                     dtype=np.float32)
+                        stage.x0, stage.mask, stage.q_noise = _ptr(x0c), _ptr(mask_e), _ptr(q_tab)
+                    if has_noise:
+                        n_tab = torch.empty((tab_steps,) + tuple(shape), device=dev)
+                        stage.noise = _ptr(n_tab)
                 it = iter(iterator)
                 i = 0
                 while i < total:
                     j = i
                     while not ((total - j - 1) % log_every_t == 0 or (total - j - 1) == total - 1):
                         j += 1
-                    sess.plan.launch(j - i + 1, tail)
+                    k = i
+                    while k <= j:
+                        n = min(per_call, j - k + 1)
+                        if blend or draw:
+                            draw_step_noise(n, shape, x0, q_tab, draw, n_tab, noise_dropout, dev)
+                        if stage is None:
+                            sess.plan.launch(n, tail)
+                        else:
+                            if blend:
+                                stage.q_coef = qcoef[k:].ctypes.data
+                            sess.plan.launch(n, tail, stage)
+                        k += n
                     for _ in range(j - i + 1):
                         next(it, None)                                          # keeps a progress bar (tqdm_class) moving
                     intermediates['x_inter'].append(current_x())
@@ -419,6 +493,7 @@ class DDIMSampler(object):
                     i = j + 1
                 for _ in it:
                     pass
+                self.last_launches_per_step = sess.plan.launches + (3 if stage is not None else 2)
             else:
                 for i, step in enumerate(iterator):
                     index = total - i - 1
@@ -444,5 +519,5 @@ class DDIMSampler(object):
                     if index % log_every_t == 0 or index == total - 1:
                         intermediates['x_inter'].append(current_x())
                         intermediates['pred_x0'].append(current_pred())
-            self.last_launches_per_step = sess.plan.launches + 2
+                self.last_launches_per_step = sess.plan.launches + 2
             return current_x(), intermediates

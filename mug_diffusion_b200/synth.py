@@ -120,6 +120,16 @@ def synthetic_inputs(B: int, z_length: int, cfg: Optional[ModelConfig] = None, s
     return out
 
 
+def synthetic_inpainting(B: int, z_length: int, z_channels: int = 16, seed: int = 31):
+    """(x0 ``[B,16,L]``, mask ``[B,1,L]``) of an inpainting request: keep the first half of every latent chart, with a soft edge
+    (0.5) over the next eighth, and regenerate the rest."""
+    x0 = _gauss(_rng(seed, "x0"), (B, z_channels, z_length))
+    mask = torch.zeros(B, 1, z_length)
+    mask[:, :, :z_length // 2] = 1.0
+    mask[:, :, z_length // 2:z_length // 2 + z_length // 8] = 0.5
+    return x0, mask
+
+
 def wave_list(w4: Sequence[torch.Tensor]) -> List[torch.Tensor]:
     """The reference passes the 10-entry wave-encoder output list; only the last 4 are read
     (unet.py:527-543).  Pad the front with empty placeholders."""
