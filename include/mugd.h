@@ -266,6 +266,36 @@ typedef struct mugd_stage {
 int  mugd_sample_staged(mugd_plan* eval_plan, const mugd_stage* stage, const mugd_op* tail, int32_t n_tail, int32_t n_steps,
                         void* stream);
 
+/* ---- the PLMS sampler loop: PLMSSampler.plms_sampling / p_sample_plms, mug/diffusion/plms.py:115-236 (eta = 0 only) -----------
+ * n = B*L*C elements of the dense x rows.  Step i of an S-step request:
+ *   replay the evaluation plan; combine: e_t = eps rows (CFG: e_u + scale * (e_c - e_u), uncond half first, :182-186), written to
+ *   slot i mod 3 of `hist` (old_eps keeps the last 3, :160-162), and e' into e_prime by the Adams-Bashforth order min(i, 3):
+ *   (3 e_t - o1) / 2, (23 e_t - 16 o1 + 5 o2) / 12, (55 e_t - 59 o1 + 37 o2 - 9 o3) / 24 (:224-232, o_k = e_t of step i - k);
+ *   then `update` (x_{t-1} from e', :199-216) and *update.step += 1.
+ * Step 0 (pseudo improved Euler, :219-223) evaluates twice:
+ *   1. replay at t (timestep row 0); combine with e' = e_t; 2. x_stash <- x; 3. `update` (coefficient row 0) writes the Euler x_prev into
+ *   x and x_dup; 4. *step <- 1 (0 when S = 1: t_next = time_range[min(1, S - 1)], :145) and replay, so the time-embedding rows follow;
+ *   5. x <- x_stash; 6. Heun combine: e' = (e_t + e_t_next) / 2, e_t read from slot 0; 7. *step <- 0, `update`, *step += 1.
+ * Every intermediate is one IEEE round-to-nearest in torch's CUDA eager order (a division by a Python scalar is torch's multiply by
+ * the float reciprocal), no contraction: bit-identical to the torch expressions.
+ * The ring and the step counter live on the device, so a request can run as several calls (first_step = steps already run, the
+ * counter holding first_step) with intermediates recorded between them. */
+typedef struct mugd_plms {
+    mugd_ddim_update update;               /* the x update on e': cfg = 0, eps = e_prime, noise = NULL; x, x_dup, pred_x0, coef, step
+                                              and S as for mugd_sample (coef rows at eta = 0)                                    */
+    const float* eps;                      /* [Beff*L, C] the evaluation plan's output rows; Beff = 2B when cfg                   */
+    float* e_prime;                        /* [n] e' of the current step                                                         */
+    float* hist;                           /* [3][n] e_t of the last three steps (slot j mod 3 for step j)                      */
+    float* x_stash;                        /* [n] x across step 0's second evaluation                                           */
+    int32_t cfg; float scale;              /* classifier-free guidance: cfg = 1 and its scale                                  */
+} mugd_plms;
+/* steps first_step .. first_step + n_steps - 1 of the update's S-step request, no host synchronisation.  Every argument is checked before
+ * the first launch.  Launches per step: the plan's graph, the combine kernel, the update and the advance (step 0: one more graph replay,
+ * combine and update, two counter fills and two copies).  A standalone entry point: the ABI version is unchanged. */
+int  mugd_sample_plms(mugd_plan* eval_plan, const mugd_plms* p, int32_t first_step, int32_t n_steps, void* stream);
+/* the combine kernel alone for step `step` (heun = 1: step 0's second combine), for a host that runs the PLMS steps one by one */
+int  mugd_plms_combine(const mugd_plms* p, int32_t step, int32_t heun, void* stream);
+
 /* ---- plans on disk: a host without Python (examples/host_c) loads what the Python plan compiler produced ---------------------
  * Every pointer of a plan lies in one of a few device allocations ("regions": weight blob, activation arena, side tables, the
  * caller's staging buffers).  mugd_plan_save stores each pointer as (region, offset); mugd_plan_load resolves them against the

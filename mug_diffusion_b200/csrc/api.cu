@@ -252,6 +252,40 @@ int mugd_sample_staged(mugd_plan* eval_plan, const mugd_stage* stage, const mugd
     return MUGD_OK;
 }
 
+int mugd_sample_plms(mugd_plan* eval_plan, const mugd_plms* p, int32_t first_step, int32_t n_steps, void* stream) {
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_plms: the evaluation plan must be captured (mugd_plan_capture)");
+    MUGD_REQUIRE(p, "mugd_sample_plms: null plms");
+    int rc = check_plms(*p);
+    if (rc != MUGD_OK) return rc;
+    const mugd_ddim_update& u = p->update;
+    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= u.S,
+                 "mugd_sample_plms: first_step=%d, n_steps=%d outside the S=%d steps of the request", first_step, n_steps, u.S);
+    const DeviceInfo& dev = eval_plan->h->dev;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t xbytes = sizeof(float) * (size_t)u.n;
+    int32_t* const step = const_cast<int32_t*>(u.step);      // the update reads the counter this loop sets and advances
+    mugd_step_advance adv;
+    adv.step = step;
+    for (int32_t i = first_step; i < first_step + n_steps; ++i) {
+        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
+        if ((rc = launch_plms_combine(*p, i, 0, st)) != MUGD_OK) return rc;
+        if (i == 0) {
+            // pseudo improved Euler (plms.py:219-223): the Euler x_prev of e_t goes into both CFG halves of the input rows, the plan
+            // evaluates it at t_next = time_range[min(1, S - 1)] (:145), then x is restored and e' = (e_t + e_t_next) / 2
+            MUGD_CHECK_CUDA(cudaMemcpyAsync(p->x_stash, u.x, xbytes, cudaMemcpyDeviceToDevice, st));
+            if ((rc = launch_ddim_update(dev, u, st, nullptr)) != MUGD_OK) return rc;
+            if ((rc = mugd_fill_i32(step, u.S > 1 ? 1 : 0, stream)) != MUGD_OK) return rc;
+            MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
+            MUGD_CHECK_CUDA(cudaMemcpyAsync(u.x, p->x_stash, xbytes, cudaMemcpyDeviceToDevice, st));
+            if ((rc = launch_plms_combine(*p, 0, 1, st)) != MUGD_OK) return rc;
+            if ((rc = mugd_fill_i32(step, 0, stream)) != MUGD_OK) return rc;
+        }
+        if ((rc = launch_ddim_update(dev, u, st, nullptr)) != MUGD_OK) return rc;
+        if ((rc = launch_step_advance(dev, adv, st, nullptr)) != MUGD_OK) return rc;
+    }
+    return MUGD_OK;
+}
+
 int mugd_abi_sizes(int32_t* out, int32_t n) {
     MUGD_REQUIRE(out && n >= 13, "abi_sizes: need room for 13 entries");
     out[0] = sizeof(mugd_op); out[1] = sizeof(mugd_gemm); out[2] = sizeof(mugd_groupnorm);

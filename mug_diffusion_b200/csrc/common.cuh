@@ -65,6 +65,10 @@ int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_
 // mugd_sample_staged: check_stage validates a stage for n_steps (host arrays included); launch_stage runs step i of it
 int check_stage(const mugd_stage& s, int32_t n_steps);
 int launch_stage(const mugd_stage& s, int32_t i, cudaStream_t st);
+// mugd_sample_plms / mugd_plms_combine: check_plms validates the descriptor; launch_plms_combine runs the combine of step `step`
+// (heun = 1: the second half of step 0)
+int check_plms(const mugd_plms& p);
+int launch_plms_combine(const mugd_plms& p, int32_t step, int heun, cudaStream_t st);
 int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, cudaStream_t st, int* launches);
 bool gemm_tc_supported(const mugd_gemm& g);
 

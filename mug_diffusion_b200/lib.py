@@ -104,6 +104,11 @@ class Stage(C.Structure):
                 ("B", C.c_int32), ("C", C.c_int32), ("L", C.c_int32), ("reserved_", C.c_int32)]
 
 
+class Plms(C.Structure):
+    _fields_ = [("update", DdimUpdate), ("eps", _f), ("e_prime", _f), ("hist", _f), ("x_stash", _f), ("cfg", C.c_int32),
+                ("scale", C.c_float)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", Gemm), ("gn", GroupNorm), ("ln", LayerNorm), ("attn", Attention), ("s4", S4Conv),
                 ("ddim", DdimUpdate), ("tr", Transpose), ("cp", Copy2D), ("adv", StepAdvance), ("notes", Notes), ("embed", Embed),
@@ -186,6 +191,8 @@ def load() -> C.CDLL:
         raise MugdError(f"struct layout mismatch: C {list(sizes)} vs ctypes {mine}")
     lib.mugd_sample.argtypes = [C.c_void_p, C.POINTER(Op), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_sample_staged.argtypes = [C.c_void_p, C.POINTER(Stage), C.POINTER(Op), C.c_int32, C.c_int32, C.c_void_p]
+    lib.mugd_sample_plms.argtypes = [C.c_void_p, C.POINTER(Plms), C.c_int32, C.c_int32, C.c_void_p]
+    lib.mugd_plms_combine.argtypes = [C.POINTER(Plms), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_plan_save.argtypes = [C.c_void_p, C.POINTER(Region), C.c_int32, C.c_char_p]
     lib.mugd_plan_load.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(Region), C.c_int32, C.POINTER(C.c_void_p)]
     lib.mugd_set_tc_single_pass_tf32.argtypes = [C.c_void_p, C.c_int]
@@ -221,5 +228,5 @@ EXPORTED_SYMBOLS = [
     "mugd_set_pdl", "mugd_set_tc_single_pass_tf32", "mugd_set_attention_impl", "mugd_debug_set_tc_tile_n", "mugd_debug_set_tc_cost", "mugd_gemm_tc_variant",
     "mugd_debug_set_attention_dump", "mugd_debug_set_tc_timing", "mugd_sample", "mugd_plan_save", "mugd_plan_load", "mugd_plan_regions", "mugd_plan_ops",
     "mugd_melspec", "mugd_grid_scan", "mugd_chart_snap", "mugd_remove_mini_jacks",
-    "mugd_sample_staged",
+    "mugd_sample_staged", "mugd_sample_plms", "mugd_plms_combine",
 ]

@@ -51,13 +51,21 @@ class Plan:
     def replay(self, times: int = 1):
         L_.check(self.engine.lib.mugd_plan_replay(self.handle, times, _stream()), "plan_replay")
 
+    def ensure_captured(self):
+        if not self.captured:
+            self.run()
+            self.capture()
+
+    def launch_plms(self, plms: L_.Plms, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a PLMS request from one C call (mugd_sample_plms)"""
+        self.ensure_captured()
+        L_.check(self.engine.lib.mugd_sample_plms(self.handle, C.byref(plms), first_step, steps, _stream()), "mugd_sample_plms")
+
     def launch(self, steps: int = 1, tail: Optional[OpList] = None, stage: Optional[L_.Stage] = None):
         """``steps`` replays of the plan's CUDA graph; with ``tail``, every replay is followed by the tail ops and all steps run from
         one C call (mugd_sample); with ``stage`` as well, each step starts with the stage kernel (mugd_sample_staged: inpainting blend,
         step noise).  The first call captures the graph, after a warm-up run outside capture (lazy module load, cudaFuncSetAttribute)."""
-        if not self.captured:
-            self.run()
-            self.capture()
+        self.ensure_captured()
         if tail is None:
             self.replay(steps)
             return
@@ -461,10 +469,8 @@ class Session:
         self.coef.zero_()
         self.coef[:len(coef)].copy_(torch.from_numpy(coef).to(self.engine.device))
 
-    def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:
-        """the ops that follow each evaluation of an S-step request for B samples: the DDIM update of the xin rows (both halves
-        under classifier-free guidance) from eps, the coef row of the current step and, if ``noise`` is given, the noise rows;
-        pred_x0 receives the predicted x0 rows.  Then the step counter advances."""
+    def ddim_update(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> L_.DdimUpdate:
+        """the DDIM update of ddim_tail"""
         n = B * self.Lz * self.engine.cfg.unet.in_channels
         upd = L_.DdimUpdate()
         upd.x = self.xin.ptr
@@ -472,6 +478,26 @@ class Session:
         upd.eps, upd.noise, upd.pred_x0 = self.eps.ptr, noise or None, pred_x0
         upd.coef, upd.step = _ptr(self.coef), _ptr(self.step)
         upd.S, upd.n, upd.cfg, upd.scale, upd.temperature = S, n, int(cfg_on), float(scale), float(temperature)
+        return upd
+
+    def plms(self, B: int, S: int, cfg_on: bool, scale: float, pred_x0: int, work: torch.Tensor) -> L_.Plms:
+        """the mugd_sample_plms descriptor of an S-step request for B samples: the combine reads eps (both halves under
+        classifier-free guidance), the update (cfg = 0, no noise) runs on e' and writes the xin rows of both halves and pred_x0.
+        ``work``: a [5, B*Lz*C] device tensor owned by the caller = e', the ring of the last three e_t, the x stash."""
+        n = B * self.Lz * self.engine.cfg.unet.in_channels
+        assert work.shape == (5, n) and work.dtype == torch.float32 and work.is_contiguous()
+        p = L_.Plms()
+        p.update = self.ddim_update(B, S, cfg_on, 1.0, 1.0, pred_x0)
+        p.update.cfg, p.update.eps = 0, _ptr(work[0])
+        p.eps, p.e_prime, p.hist, p.x_stash = self.eps.ptr, _ptr(work[0]), _ptr(work[1]), _ptr(work[4])
+        p.cfg, p.scale = int(cfg_on), float(scale)
+        return p
+
+    def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:
+        """the ops that follow each evaluation of an S-step request for B samples: the DDIM update of the xin rows (both halves
+        under classifier-free guidance) from eps, the coef row of the current step and, if ``noise`` is given, the noise rows;
+        pred_x0 receives the predicted x0 rows.  Then the step counter advances."""
+        upd = self.ddim_update(B, S, cfg_on, scale, temperature, pred_x0, noise)
         adv = L_.StepAdvance()
         adv.step = _ptr(self.step)
         tail = OpList()

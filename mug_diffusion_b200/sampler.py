@@ -2,6 +2,7 @@
 
 Reference surface kept (SURVEY §8b):
     sampler = DDIMSampler(model)                                  mug/diffusion/ddim.py:12
+    sampler = PLMSSampler(model)                                  mug/diffusion/plms.py:11 (scripts/mapping.py --plms)
     samples, inter = sampler.sample(S, c, w, batch_size, ...)     mug/diffusion/ddim.py:56-107
     eps    = model.model.forward(x, t, c, w)                      mug/diffusion/diffusion.py:52-54
     logits = model.model.decode(z)                                mug/diffusion/diffusion.py:49-50
@@ -12,13 +13,15 @@ the host: the beta/alpha schedule tables, argument plumbing, callbacks and the R
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Dict, Optional, Sequence
 
 import numpy as np
 import torch
 
+from . import lib as L_
 from .config import DecoderConfig, EncoderConfig, ModelConfig, UNetConfig
-from .engine import View
+from .engine import OpList, View
 from .lib import MugdError
 from .postprocess import objects_to_array
 from .prompt import PromptEmbedder
@@ -397,6 +400,27 @@ class DDIMSampler(object):
                                   unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class,
                                   match_reference_rng=bool(kwargs.get("match_reference_rng", False)))
 
+    def _load_request(self, w, c, shape, x_T, scale, uc):
+        """Once per request, both samplers: x_T (drawn when not given), whether classifier-free guidance is on, and the session of
+        this shape with the timestep table (row i = i-th loop iteration), context, audio, coefficient rows of make_schedule and x
+        loaded, its step counter at 0.  Returns (x, cfg_on, session, time_range)."""
+        model = self.model
+        dev = self.device
+        B, Cz, Lz = shape
+        x = torch.randn(shape, device=dev) if x_T is None else x_T.to(dev, torch.float32)
+        cfg_on = not (uc is None or scale == 1.)
+        Beff = 2 * B if cfg_on else B
+        time_range = np.flip(self.ddim_timesteps)
+        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False)
+        sess.set_timestep_table(time_range.copy())
+        # ddim.py:170-174 concatenates [uc, c] and [w, w]; here the two halves are written straight into their rows
+        sess.set_context([uc, c] if cfg_on else c)
+        sess.set_audio(list(w)[-model.cfg.unet.levels:], dup=cfg_on)
+        sess.set_ddim_schedule(self.ddim_alphas, self.ddim_alphas_prev, self.ddim_sigmas, self.ddim_sqrt_one_minus_alphas)
+        sess.load_x(x, dup=cfg_on)
+        sess.set_step(0)
+        return x, cfg_on, sess, time_range
+
     @torch.no_grad()
     def ddim_sampling(self, w, c, shape, x_T=None, callback=None, mask=None, x0=None, img_callback=None,
                       log_every_t=100, temperature=1., noise_dropout=0., unconditional_guidance_scale=1.,
@@ -409,22 +433,8 @@ class DDIMSampler(object):
         # draw is skipped here unless it can change the result or the caller asks for the same global-RNG consumption
         match_rng = bool(match_reference_rng)
         with eng.lock:
-            x = torch.randn(shape, device=dev) if x_T is None else x_T.to(dev, torch.float32)
-            cfg_on = not (unconditional_conditioning is None or unconditional_guidance_scale == 1.)
-            Beff = 2 * B if cfg_on else B
-            ts = self.ddim_timesteps
-            total = ts.shape[0]
-            time_range = np.flip(ts)
-            sess: Session = eng.session(Beff, Lz, per_sample_t=False)
-
-            # ---- once per request -----------------------------------------------------------
-            sess.set_timestep_table(time_range.copy())                      # row i = i-th loop iteration
-            # ddim.py:170-174 concatenates [uc, c] and [w, w]; here the two halves are written straight into their rows
-            sess.set_context([unconditional_conditioning, c] if cfg_on else c)
-            sess.set_audio(list(w)[-model.cfg.unet.levels:], dup=cfg_on)
-            sess.set_ddim_schedule(self.ddim_alphas, self.ddim_alphas_prev, self.ddim_sigmas, self.ddim_sqrt_one_minus_alphas)
-            sess.load_x(x, dup=cfg_on)
-            sess.set_step(0)
+            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, unconditional_guidance_scale, unconditional_conditioning)
+            total = time_range.shape[0]
             # pred_x0 and the noise of a step: channels-last rows [B*Lz, Cz]
             pred = torch.empty(B * Lz, Cz, device=dev)
             has_noise = bool(np.any(np.asarray(self.ddim_sigmas) != 0))
@@ -520,4 +530,181 @@ class DDIMSampler(object):
                         intermediates['x_inter'].append(current_x())
                         intermediates['pred_x0'].append(current_pred())
                 self.last_launches_per_step = sess.plan.launches + 2
+            return current_x(), intermediates
+
+
+# --------------------------------------------------------------------------------------------------
+# PLMS sampler
+# --------------------------------------------------------------------------------------------------
+class PLMSSampler(DDIMSampler):
+    """The reference's second sampler, PLMSSampler (mug/diffusion/plms.py): pseudo linear multistep, a 4th-order Adams-Bashforth
+    combination of the last four noise predictions with a two-evaluation improved-Euler first step, at eta = 0.  Same constructor,
+    schedule tables and per-request loading as DDIMSampler; each step is one U-Net evaluation (step 0: two), the combine kernel
+    and the DDIM update on e'."""
+
+    def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=True):
+        if ddim_eta != 0:
+            raise ValueError('ddim_eta must be 0 for PLMS')                    # plms.py:25-26
+        super().make_schedule(ddim_num_steps, ddim_discretize, ddim_eta, verbose)
+
+    @torch.no_grad()
+    def sample(self, S, c=None, w=None, batch_size=None, shape=None, callback=None, img_callback=None, eta=0., mask=None, x0=None,
+               temperature=1., noise_dropout=0., verbose=True, x_T=None, log_every_t=100, unconditional_guidance_scale=1.,
+               unconditional_conditioning=None, tqdm_class=None, conditioning=None, **kwargs):
+        """The call scripts/mapping.py:476-483 makes (``c`` may also be given as the reference's ``conditioning``).  Returns
+        ``(samples, {'x_inter', 'pred_x0'})`` with plms.py:134,166-168's logging rule.  Every argument is checked before any GPU
+        work.  Requests without callback / img_callback / mask run from mugd_sample_plms calls, one per stretch between two recorded
+        intermediates; the others run the steps one by one.  ``match_reference_rng=True``: the CUDA generator consumes what the
+        reference's discarded step noise consumes (randn(shape) [+ dropout], twice at step 0 and once per later step; for B > 1 the
+        reference's noise_like receives a [B, B, C, L] shape from its [b, 1, 1, 1] coefficients, this draws [B, C, L])."""
+        if eta != 0:
+            raise ValueError('ddim_eta must be 0 for PLMS')
+        if conditioning is not None:
+            if c is not None:
+                raise TypeError("give the conditioning as c or as conditioning, not both")
+            c = conditioning
+        size = self._check_request(S, c, w, batch_size, shape, x_T, mask, x0, unconditional_guidance_scale, unconditional_conditioning,
+                                   log_every_t)
+        self.make_schedule(ddim_num_steps=S, ddim_eta=eta, verbose=verbose)
+        if verbose:
+            print(f'Data shape for PLMS sampling is {size}')
+        return self.plms_sampling(w, c, size, x_T=x_T, callback=callback, img_callback=img_callback, mask=mask, x0=x0,
+                                  log_every_t=log_every_t, noise_dropout=noise_dropout,
+                                  unconditional_guidance_scale=unconditional_guidance_scale,
+                                  unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class,
+                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)))
+
+    def _check_request(self, S, c, w, batch_size, shape, x_T, mask, x0, scale, uc, log_every_t):
+        """the request's [B, C, L] shape; ValueError / TypeError for what the device path cannot take"""
+        if c is None or w is None:
+            raise TypeError("PLMSSampler.sample needs the conditioning c and the audio features w")
+        if isinstance(S, bool) or not isinstance(S, (int, np.integer)) or not 0 < S <= self.ddpm_num_timesteps:
+            raise ValueError(f"S={S!r}: the number of steps must be an integer in [1, {self.ddpm_num_timesteps}]")
+        last = int(ddim_timesteps_uniform(int(S), self.ddpm_num_timesteps)[-1])
+        if last >= self.ddpm_num_timesteps:
+            # e.g. S = 3: range(0, 1000, 333) + 1 ends at 1000, past the schedule (the reference's table lookup fails there too)
+            raise ValueError(f"S={S}: the uniform schedule reaches timestep {last}, outside the {self.ddpm_num_timesteps}-step schedule")
+        if isinstance(batch_size, bool) or not isinstance(batch_size, (int, np.integer)) or batch_size < 1:
+            raise ValueError(f"batch_size={batch_size!r} must be a positive integer")
+        if isinstance(log_every_t, bool) or not isinstance(log_every_t, (int, np.integer)) or log_every_t < 1:
+            raise ValueError(f"log_every_t={log_every_t!r} must be a positive integer")
+        if shape is None:
+            size = (int(batch_size), self.model.z_channels, self.model.z_length)
+        elif len(shape) != 2:
+            raise ValueError(f"shape={tuple(shape)}: a latent is (channels, length)")
+        else:
+            size = (int(batch_size), int(shape[0]), int(shape[1]))
+        if size[1] != self.model.z_channels:
+            raise ValueError(f"shape {size}: the model's latents have {self.model.z_channels} channels")
+        cfg_on = not (uc is None or scale == 1.)
+        for name, t in (("c", c), ("unconditional_conditioning", uc if cfg_on else None)):
+            if t is not None and (not isinstance(t, torch.Tensor) or t.dim() != 3 or t.shape[0] != size[0]):
+                raise ValueError(f"{name} must be a [batch_size={size[0]}, channels, tokens] tensor")
+        if x_T is not None and tuple(x_T.shape) != size:
+            raise ValueError(f"x_T has shape {tuple(x_T.shape)}, the request {size}")
+        if mask is not None:
+            if x0 is None or tuple(x0.shape) != size:
+                raise ValueError(f"inpainting needs x0 of shape {size} with the mask")
+            try:
+                torch.broadcast_shapes(tuple(mask.shape), size)
+            except RuntimeError:
+                raise ValueError(f"mask of shape {tuple(mask.shape)} does not broadcast to {size}") from None
+        return size
+
+    @torch.no_grad()
+    def plms_sampling(self, w, c, shape, x_T=None, callback=None, mask=None, x0=None, img_callback=None, log_every_t=100,
+                      noise_dropout=0., unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None,
+                      progress=True, match_reference_rng=False):
+        """plms.py:115-170 (and p_sample_plms, :172-236) on the GPU."""
+        model = self.model
+        eng = model.engine
+        dev = self.device
+        B, Cz, Lz = shape
+        match_rng = bool(match_reference_rng)
+        scale = unconditional_guidance_scale
+
+        def draw(k):
+            # the reference's step noise at sigma = 0 (plms.py:212-214): values discarded, generator advanced
+            if match_rng:
+                draw_step_noise(k, shape, None, None, True, None, noise_dropout, dev)
+
+        with eng.lock:
+            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, scale, unconditional_conditioning)
+            total = time_range.shape[0]
+            pred = torch.empty(B * Lz, Cz, device=dev)
+            work = torch.empty(5, B * Lz * Cz, device=dev)                    # e', the e_t ring [3], the x stash
+            plms = sess.plms(B, total, cfg_on, scale, _ptr(pred), work)
+
+            intermediates = {'x_inter': [x], 'pred_x0': [x]}
+            iterator = time_range
+            if progress:
+                cls = tqdm_class if tqdm_class is not None else _tqdm
+                if cls is not None:
+                    iterator = cls(time_range, desc='Charting, using PLMS Sampler', total=total)
+
+            def current_x():
+                return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+
+            def current_pred():
+                return eng.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
+
+            def logged(i):
+                index = total - i - 1
+                return index % log_every_t == 0 or index == total - 1              # plms.py:166
+
+            if callback is None and img_callback is None and mask is None:
+                # one mugd_sample_plms call per stretch between two recorded intermediates: the e_t ring and the step counter stay on
+                # the device, so a call may start inside the warm-up
+                it = iter(iterator)
+                i = 0
+                while i < total:
+                    j = i
+                    while not logged(j):
+                        j += 1
+                    draw(j - i + 1 + (i == 0))
+                    sess.plan.launch_plms(plms, i, j - i + 1)
+                    for _ in range(j - i + 1):
+                        next(it, None)                                          # keeps a progress bar (tqdm_class) moving
+                    intermediates['x_inter'].append(current_x())
+                    intermediates['pred_x0'].append(current_pred())
+                    i = j + 1
+                for _ in it:
+                    pass
+            else:
+                # one step at a time from the same kernels: the referee of the device loop
+                update = OpList()
+                update.add(L_.OP_DDIM_UPDATE, plms.update)
+                adv = L_.StepAdvance()
+                adv.step = _ptr(sess.step)
+                tail = OpList()
+                tail.add(L_.OP_DDIM_UPDATE, plms.update)
+                tail.add(L_.OP_STEP_ADVANCE, adv)
+                stream = torch.cuda.current_stream().cuda_stream
+                for i, step in enumerate(iterator):
+                    if mask is not None:
+                        assert x0 is not None
+                        tsb = torch.full((B,), int(step), device=dev, dtype=torch.long)
+                        x_orig = model.q_sample(x0.to(dev), tsb)                    # plms.py:147-150
+                        sess.load_x(x_orig * mask + (1. - mask) * current_x(), dup=cfg_on)
+                    sess.eval(graph=True)
+                    L_.check(eng.lib.mugd_plms_combine(C.byref(plms), i, 0, stream), "mugd_plms_combine")
+                    if i == 0:
+                        x_t = current_x()                                       # pseudo improved Euler, plms.py:219-223
+                        draw(1)
+                        eng.run_ops(update)                                     # x_prev of e_t into both halves
+                        sess.set_step(1 if total > 1 else 0)                    # t_next, plms.py:145
+                        sess.eval(graph=True)
+                        sess.load_x(x_t, dup=False)
+                        L_.check(eng.lib.mugd_plms_combine(C.byref(plms), 0, 1, stream), "mugd_plms_combine")
+                        sess.set_step(0)
+                    draw(1)
+                    eng.run_ops(tail)
+                    if callback:
+                        callback(i)
+                    if img_callback:
+                        img_callback(current_pred(), i)
+                    if logged(i):
+                        intermediates['x_inter'].append(current_x())
+                        intermediates['pred_x0'].append(current_pred())
+            self.last_launches_per_step = sess.plan.launches + 3
             return current_x(), intermediates
