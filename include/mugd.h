@@ -296,6 +296,40 @@ int  mugd_sample_plms(mugd_plan* eval_plan, const mugd_plms* p, int32_t first_st
 /* the combine kernel alone for step `step` (heun = 1: step 0's second combine), for a host that runs the PLMS steps one by one */
 int  mugd_plms_combine(const mugd_plms* p, int32_t step, int32_t heun, void* stream);
 
+/* ---- the DDPM ancestral sampler loop: DDPM.log_beatmap, mug/diffusion/diffusion.py:255-282 (parameterization "eps") ------------
+ * Step i of a T-step request (timestep t = T - 1 - i, the device counter holding i): replay the evaluation plan, then one update kernel
+ *   e       = eps rows; with cfg: e_u + scale * (e_c - e_u), uncond half first (an extension: the reference loop has no guidance;
+ *             the combine is ddim.py:175's)
+ *   x_recon = coef[t][0] * x - coef[t][1] * e;  with clip: x_recon = clamp(x_recon, -10, 10), NaN kept        (:260-267, :211-215)
+ *   x       = coef[t][2] * x_recon + coef[t][3] * x + coef[t][4] * noise                                        (:268-277)
+ * written to x (and x_dup), x_recon to pred_x0 (if given); then *step += 1.  Every intermediate is one IEEE round-to-nearest in
+ * torch's eager order, no contraction: with equal eps and noise the result is bit-identical to the reference's torch expressions.
+ * coef is a device table [T][5] = (sqrt_recip_alphas_cumprod, sqrt_recipm1_alphas_cumprod, posterior_mean_coef1,
+ * posterior_mean_coef2, sigma) of the model's float32 schedule buffers, where sigma[t] = (1 - (t == 0)) * exp(0.5 *
+ * posterior_log_variance_clipped[t]) evaluated in float32 by torch's CUDA ops (the Python host builds the column with them, so exp is
+ * torch's; another host must reproduce torch's CUDA expf to stay bit-identical).  noise is a device table [n_steps][B, C, L] (NCL, as
+ * torch draws it): row k is the noise of step first_step + k of a mugd_sample_ddpm call; mugd_ddpm_update reads row 0.  The step
+ * counter lives on the device, so a request can run as several calls with intermediates recorded between them. */
+#define MUGD_MAX_STEPS 1000                /* rows of the time-embedding table a sampling session holds: T <= MUGD_MAX_STEPS  */
+typedef struct mugd_ddpm {
+    float* x; float* x_dup;                /* [B*L, C] dense rows in place; x_dup = the CFG copy (given exactly when cfg = 1)     */
+    const float* eps;                      /* [Beff*L, C] the evaluation plan's output rows; Beff = 2B when cfg                  */
+    float* pred_x0;                        /* [B*L, C] x_recon of the step, or NULL                                             */
+    const float* noise;                    /* [n_steps][B, C, L]                                                                */
+    const float* coef;                     /* [T][5]                                                                            */
+    int32_t* step;                         /* device step counter i                                                             */
+    int32_t T, B, C, L;
+    int32_t cfg; float scale;              /* classifier-free guidance: cfg = 1 and its scale                                  */
+    int32_t clip;                          /* 1 = clip_denoised                                                                 */
+    int32_t reserved_;
+} mugd_ddpm;
+/* steps first_step .. first_step + n_steps - 1 of the T-step request, no host synchronisation: n_steps x { graph replay, update with
+ * noise row k, *step += 1 }, the same launches per step as mugd_sample.  Every argument is checked before the first launch
+ * (first_step + n_steps <= T <= MUGD_MAX_STEPS).  A standalone entry point: the ABI version is unchanged. */
+int  mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_step, int32_t n_steps, void* stream);
+/* the update kernel alone (noise row 0, the counter not advanced), for a host that runs the DDPM steps one by one */
+int  mugd_ddpm_update(const mugd_ddpm* d, void* stream);
+
 /* ---- plans on disk: a host without Python (examples/host_c) loads what the Python plan compiler produced ---------------------
  * Every pointer of a plan lies in one of a few device allocations ("regions": weight blob, activation arena, side tables, the
  * caller's staging buffers).  mugd_plan_save stores each pointer as (region, offset); mugd_plan_load resolves them against the

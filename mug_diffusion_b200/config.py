@@ -101,3 +101,8 @@ class ModelConfig:
     linear_start: float = 1e-4
     linear_end: float = 2e-2
     encoder: Optional[EncoderConfig] = None      # None: no chart encoder (a blob with encoder weights then uses EncoderConfig())
+    # the DDPM sampler's settings (diffusion.py:75-85): x_recon clamped to [-10, 10], the posterior variance's share of beta, and what
+    # the U-Net predicts (only "eps" is supported)
+    clip_denoised: bool = True
+    v_posterior: float = 0.0
+    parameterization: str = "eps"

@@ -286,6 +286,25 @@ int mugd_sample_plms(mugd_plan* eval_plan, const mugd_plms* p, int32_t first_ste
     return MUGD_OK;
 }
 
+int mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_step, int32_t n_steps, void* stream) {
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_ddpm: the evaluation plan must be captured (mugd_plan_capture)");
+    MUGD_REQUIRE(d, "mugd_sample_ddpm: null ddpm");
+    int rc = check_ddpm(*d);
+    if (rc != MUGD_OK) return rc;
+    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= d->T,
+                 "mugd_sample_ddpm: first_step=%d, n_steps=%d outside the T=%d steps of the request", first_step, n_steps, d->T);
+    const DeviceInfo& dev = eval_plan->h->dev;
+    cudaStream_t st = (cudaStream_t)stream;
+    mugd_step_advance adv;
+    adv.step = d->step;
+    for (int32_t k = 0; k < n_steps; ++k) {
+        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
+        if ((rc = launch_ddpm_update(*d, k, st)) != MUGD_OK) return rc;
+        if ((rc = launch_step_advance(dev, adv, st, nullptr)) != MUGD_OK) return rc;
+    }
+    return MUGD_OK;
+}
+
 int mugd_abi_sizes(int32_t* out, int32_t n) {
     MUGD_REQUIRE(out && n >= 13, "abi_sizes: need room for 13 entries");
     out[0] = sizeof(mugd_op); out[1] = sizeof(mugd_gemm); out[2] = sizeof(mugd_groupnorm);

@@ -61,6 +61,12 @@ class Plan:
         self.ensure_captured()
         L_.check(self.engine.lib.mugd_sample_plms(self.handle, C.byref(plms), first_step, steps, _stream()), "mugd_sample_plms")
 
+    def launch_ddpm(self, ddpm: L_.Ddpm, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a DDPM request from one C call (mugd_sample_ddpm); row k of the descriptor's
+        noise table is the noise of step first_step + k"""
+        self.ensure_captured()
+        L_.check(self.engine.lib.mugd_sample_ddpm(self.handle, C.byref(ddpm), first_step, steps, _stream()), "mugd_sample_ddpm")
+
     def launch(self, steps: int = 1, tail: Optional[OpList] = None, stage: Optional[L_.Stage] = None):
         """``steps`` replays of the plan's CUDA graph; with ``tail``, every replay is followed by the tail ops and all steps run from
         one C call (mugd_sample); with ``stage`` as well, each step starts with the stage kernel (mugd_sample_staged: inpainting blend,
@@ -492,6 +498,19 @@ class Session:
         p.eps, p.e_prime, p.hist, p.x_stash = self.eps.ptr, _ptr(work[0]), _ptr(work[1]), _ptr(work[4])
         p.cfg, p.scale = int(cfg_on), float(scale)
         return p
+
+    def ddpm(self, B: int, T: int, cfg_on: bool, scale: float, clip: bool, pred_x0: int, noise: int, coef: torch.Tensor) -> L_.Ddpm:
+        """the mugd_sample_ddpm descriptor of a T-step request for B samples: the update reads eps (both halves under
+        classifier-free guidance), ``coef`` (the model's [T, 5] table, kept alive by the caller) and the noise table at ``noise``
+        ([n][B, C, Lz]), and writes the xin rows of both halves and pred_x0"""
+        assert coef.shape == (T, 5) and coef.dtype == torch.float32 and coef.is_contiguous()
+        d = L_.Ddpm()
+        d.x = self.xin.ptr
+        d.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        d.eps, d.pred_x0, d.noise, d.coef, d.step = self.eps.ptr, pred_x0 or None, noise, _ptr(coef), _ptr(self.step)
+        d.T, d.B, d.C, d.L = T, B, self.engine.cfg.unet.in_channels, self.Lz
+        d.cfg, d.scale, d.clip = int(cfg_on), float(scale), int(bool(clip))
+        return d
 
     def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:
         """the ops that follow each evaluation of an S-step request for B samples: the DDIM update of the xin rows (both halves
