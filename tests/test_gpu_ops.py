@@ -172,43 +172,7 @@ def test_gemm_rejects_bad_shapes(R):
 
 
 # ---------------------------------------------------------------------------------------------------
-def attn_ref(q, k, v, rel, cg, H, pos_max=64):
-    B, Lq, inner = q.shape
-    Lk, d = k.shape[1], inner // H
-    qh, kh, vh = (t.view(B, -1, H, d).permute(0, 2, 1, 3) for t in (q, k, v))
-    idx = (torch.arange(Lk)[None, :] - torch.arange(Lq)[:, None]).clamp(-pos_max, pos_max) + pos_max
-    sim = (qh @ kh.transpose(-1, -2) + rel[idx].permute(2, 0, 1)[None]) * d ** -0.5
-    attn = sim.softmax(-1) * cg[idx].permute(2, 0, 1)[None]
-    return (attn @ vh).permute(0, 2, 1, 3).reshape(B, Lq, inner)
-
-
-@pytest.mark.parametrize("impl", [1, 0], ids=["wgmma", "ffma"])
-@pytest.mark.parametrize("B,H,D,Lq,Lk", [(2, 8, 32, 48, 48), (2, 8, 48, 24, 21), (1, 8, 64, 200, 200), (2, 8, 32, 256, 256),
-                                         (1, 8, 64, 124, 124), (3, 8, 48, 130, 21), (1, 8, 32, 496, 496), (1, 8, 48, 300, 300),
-                                         (2, 8, 64, 12, 12), (1, 4, 64, 129, 257), (8, 8, 64, 64, 21), (8, 8, 32, 256, 21), (2, 8, 48, 128, 32),
-                                         (1, 8, 32, 70, 1), (2, 8, 64, 33, 33)])
-def test_attention(R, B, H, D, Lq, Lk, impl):
-    """the attention kernels (tensor-core 3xTF32, lane-per-key for <= 32 keys, and the exact FFMA referee) against the fp64 formula;
-    covers several key tiles, ragged last tiles (Lk % 16 != 0), Lq < one tile, the 21-token prompt context, 1 / 32 / 33 keys"""
-    R.lib.mugd_set_attention_impl(R.handle, impl)
-    C = H * D
-    q, k, v = g("aq", (B, Lq, C)), g("ak", (B, Lk, C)), g("av", (B, Lk, C))
-    rel, cg = 0.5 * g("ar", (129, H)), 1 + 0.1 * g("ac", (129, H))
-    ref = attn_ref(q, k, v, rel, cg, H)
-    qkv = torch.zeros(B * Lq, 3 * C).cuda()                      # q packed as a column window like the fused qkv buffer
-    qkv[:, :C] = q.reshape(B * Lq, C).cuda()
-    kc, vc = k.reshape(B * Lk, C).cuda(), v.reshape(B * Lk, C).cuda()
-    out = torch.zeros(B * Lq, C).cuda()
-    relc, cgc = rel.cuda(), cg.cuda()
-    ops = OpList()
-    ops.attention(view(qkv, 0, C), view(kc), view(vc), view(out), ptr(relc), ptr(cgc), B, H, Lq, Lk, 64)
-    try:
-        R.run(ops)
-    finally:
-        R.lib.mugd_set_attention_impl(R.handle, 1)
-    assert rel_err(out.view(B, Lq, C), ref) < 2e-5
-
-
+# the attention kernels on their own: test_gpu_attention.py
 @pytest.mark.parametrize("name", list(gc.ATTN_CORE_CASES))
 def test_attention_vs_reference_golden(R, name, golden_dir):
     """whole CrossAttention module (to_q/k/v GEMMs + attention + to_out) against the reference's output"""

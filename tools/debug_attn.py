@@ -1,4 +1,7 @@
-"""dump the first key tile of CTA (0,0,0) of the tensor-core attention kernel (debugging aid)"""
+"""dump the raw logits of the first key tile of the tensor-core attention kernel (debugging aid)
+
+CTA (0,0,0) writes logits 0..15 (keys 0..15, before bias and scale) of query rows r with r % 16 < 8 into a [128, 40] buffer; they
+are printed next to q . k of the same rows.  usage: python tools/debug_attn.py [head dim: 32 | 48 | 64]"""
 import ctypes as C, os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -19,19 +22,14 @@ R.lib.mugd_debug_set_attention_dump(dbg.data_ptr())
 ops = OpList()
 relc, cgc = rel.cuda(), cg.cuda()
 ops.attention(view(qc), view(kc), view(vc), view(out), ptr(relc), ptr(cgc), B, H, Lq, Lk, 64)
-R.run(ops)
-torch.cuda.synchronize()
+try:
+    R.run(ops)
+finally:
+    R.lib.mugd_debug_set_attention_dump(None)
 d = dbg.cpu().view(128, 40)
-S_ref = (q[0, :, :D] @ k[0, :, :D].t())
-print("S raw row0 kernel:", d[0, :8].tolist())
-print("S raw row0 ref   :", S_ref[0, :8].tolist())
-print("S raw row5 kernel:", d[5, :8].tolist())
-print("S raw row5 ref   :", S_ref[5, :8].tolist())
-print("K smem rows 0,1 first4:", d[0, 30:34].tolist(), d[1, 30:34].tolist(), " ref:", k[0, 0, :4].tolist(), k[0, 1, :4].tolist())
-print("V smem rows 0,1 first4:", d[0, 26:30].tolist(), d[1, 26:30].tolist(), " ref:", v[0, 0, :4].tolist(), v[0, 1, :4].tolist())
-P = torch.softmax(S_ref * D ** -0.5, -1)
-O_ref = P @ v[0, :, :D]
-print("m,l row0:", d[0, 24:26].tolist(), " ref l:", float(torch.exp(S_ref[0] * D ** -0.5 - (S_ref[0] * D ** -0.5).max()).sum()))
-print("O tile row0 kernel (unnormalised):", d[0, 16:24].tolist())
-print("O row0 ref (normalised)          :", O_ref[0, :8].tolist())
-print("out row0:", out[0, :8].tolist())
+S_ref = q[0, :, :D].double() @ k[0, :, :D].double().t()
+for r in (0, 5, 16, 37):
+    print(f"row {r:2d} kernel:", [round(x, 5) for x in d[r, :16].tolist()])
+    print(f"row {r:2d} ref   :", [round(x, 5) for x in S_ref[r, :16].tolist()])
+print("max |kernel - ref| over the dumped logits:", float((d[[r for r in range(Lq) if r % 16 < 8], :16].double()
+                                                         - S_ref[[r for r in range(Lq) if r % 16 < 8], :16]).abs().max()))
