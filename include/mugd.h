@@ -330,6 +330,39 @@ int  mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_st
 /* the update kernel alone (noise row 0, the counter not advanced), for a host that runs the DDPM steps one by one */
 int  mugd_ddpm_update(const mugd_ddpm* d, void* stream);
 
+/* ---- remixing an existing chart (SDEdit / img2img): DDIMSampler.stochastic_encode and decode with a per-chart start ---------------
+ * mugd_stochastic_encode: out[b] = sqrt_a[t[b]] * x0[b] + sqrt_1ma[t[b]] * noise[b], each product and the sum one IEEE
+ * round-to-nearest (no contraction), bit-identical to torch's extract_into_tensor expressions.  x0, noise and out are device NCL
+ * [B, C, L]; t is a device [B] int64 array of table rows; sqrt_a / sqrt_1ma are device tables of n rows (sqrt(ddim_alphas) and
+ * ddim_sqrt_one_minus_alphas, or the model's sqrt_alphas_cumprod / sqrt_one_minus_alphas_cumprod).  The host checks the indices
+ * before the call; an index outside [0, n) writes NaN for that sample and never reads past the tables.  One launch. */
+typedef struct mugd_q_encode {
+    const float* x0; const float* noise;   /* [B, C, L]                                                        */
+    const int64_t* t;                      /* [B] table rows                                                   */
+    const float* sqrt_a; const float* sqrt_1ma;  /* [n]                                                        */
+    float* out;                            /* [B, C, L]                                                        */
+    int32_t B, C, L, n;
+} mugd_q_encode;
+int  mugd_stochastic_encode(const mugd_q_encode* d, void* stream);
+
+/* mugd_sample_join: the mugd_sample loop with one join kernel in front of each step, for charts that enter the loop at different
+ * iterations.  Chart b joins at iteration join[b]: while the device step counter (the tail's MUGD_OP_DDIM_UPDATE `step`) is <= join[b],
+ * the join kernel sets chart b's dense x rows [L, C] (and its CFG copy in x_dup) to x_latent[b] (NCL).  From its join on, chart b
+ * follows the coefficient rows of a run that started from x_latent[b] with S - join[b] steps.  A chart with join[b] >= S never runs;
+ * its rows hold whatever the last update wrote, and the host returns x_latent[b] for it. */
+typedef struct mugd_join {
+    float* x; float* x_dup;                /* [B*L, C] dense rows; x_dup = the CFG copy or NULL                  */
+    const float* x_latent;                 /* [B, C, L]                                                        */
+    const int32_t* join;                   /* [B] device: the iteration at which chart b joins                 */
+    int32_t B, C, L, reserved_;
+} mugd_join;
+/* steps first_step .. first_step + n_steps - 1 (the counter holding first_step): n_steps x { join kernel ; replay of the captured
+ * evaluation plan ; the tail ops }, no host synchronisation: one launch per step more than mugd_sample.  Every argument is checked
+ * before the first launch: the tail holds exactly one MUGD_OP_DDIM_UPDATE, on the join's x / x_dup with n = B*C*L, and
+ * first_step + n_steps <= its S.  A standalone entry point: the ABI version is unchanged. */
+int  mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
+                      int32_t n_steps, void* stream);
+
 /* ---- plans on disk: a host without Python (examples/host_c) loads what the Python plan compiler produced ---------------------
  * Every pointer of a plan lies in one of a few device allocations ("regions": weight blob, activation arena, side tables, the
  * caller's staging buffers).  mugd_plan_save stores each pointer as (region, offset); mugd_plan_load resolves them against the

@@ -305,6 +305,39 @@ int mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_ste
     return MUGD_OK;
 }
 
+int mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
+                     int32_t n_steps, void* stream) {
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_join: the evaluation plan must be captured (mugd_plan_capture)");
+    MUGD_REQUIRE(join, "mugd_sample_join: null join");
+    MUGD_REQUIRE(n_tail >= 0 && (n_tail == 0 || tail), "mugd_sample_join: bad tail (n_tail=%d)", n_tail);
+    const mugd_join& j = *join;
+    int rc = check_join(j);
+    if (rc != MUGD_OK) return rc;
+    const int64_t n = (int64_t)j.B * j.C * j.L;
+    const mugd_ddim_update* upd = nullptr;
+    for (int k = 0; k < n_tail; ++k) {
+        if (tail[k].kind != MUGD_OP_DDIM_UPDATE) continue;
+        MUGD_REQUIRE(!upd, "mugd_sample_join: the tail holds more than one DDIM update (op %d)", k);
+        upd = &tail[k].u.ddim;
+        MUGD_REQUIRE(upd->x == j.x && upd->x_dup == j.x_dup, "mugd_sample_join: tail op %d updates other rows than the join's x / x_dup", k);
+        MUGD_REQUIRE(upd->n == n, "mugd_sample_join: tail op %d updates n=%d elements, the join B*C*L=%lld", k, upd->n, (long long)n);
+        MUGD_REQUIRE(upd->step, "mugd_sample_join: tail op %d has no device step counter", k);
+    }
+    MUGD_REQUIRE(upd, "mugd_sample_join: the tail holds no DDIM update");
+    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= upd->S,
+                 "mugd_sample_join: first_step=%d, n_steps=%d outside the S=%d steps of the request", first_step, n_steps, upd->S);
+    cudaStream_t st = (cudaStream_t)stream;
+    for (int i = 0; i < n_steps; ++i) {
+        if ((rc = launch_join(j, upd->step, st)) != MUGD_OK) return rc;
+        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
+        for (int k = 0; k < n_tail; ++k) {
+            rc = dispatch(eval_plan->h, tail[k], st, nullptr);
+            if (rc != MUGD_OK) return rc;
+        }
+    }
+    return MUGD_OK;
+}
+
 int mugd_abi_sizes(int32_t* out, int32_t n) {
     MUGD_REQUIRE(out && n >= 13, "abi_sizes: need room for 13 entries");
     out[0] = sizeof(mugd_op); out[1] = sizeof(mugd_gemm); out[2] = sizeof(mugd_groupnorm);

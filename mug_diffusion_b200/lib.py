@@ -115,6 +115,16 @@ class Ddpm(C.Structure):
                 ("clip", C.c_int32), ("reserved_", C.c_int32)]
 
 
+class QEncode(C.Structure):
+    _fields_ = [("x0", _f), ("noise", _f), ("t", _f), ("sqrt_a", _f), ("sqrt_1ma", _f), ("out", _f),
+                ("B", C.c_int32), ("C", C.c_int32), ("L", C.c_int32), ("n", C.c_int32)]
+
+
+class Join(C.Structure):
+    _fields_ = [("x", _f), ("x_dup", _f), ("x_latent", _f), ("join", _f),
+                ("B", C.c_int32), ("C", C.c_int32), ("L", C.c_int32), ("reserved_", C.c_int32)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", Gemm), ("gn", GroupNorm), ("ln", LayerNorm), ("attn", Attention), ("s4", S4Conv),
                 ("ddim", DdimUpdate), ("tr", Transpose), ("cp", Copy2D), ("adv", StepAdvance), ("notes", Notes), ("embed", Embed),
@@ -201,6 +211,8 @@ def load() -> C.CDLL:
     lib.mugd_plms_combine.argtypes = [C.POINTER(Plms), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_sample_ddpm.argtypes = [C.c_void_p, C.POINTER(Ddpm), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_ddpm_update.argtypes = [C.POINTER(Ddpm), C.c_void_p]
+    lib.mugd_stochastic_encode.argtypes = [C.POINTER(QEncode), C.c_void_p]
+    lib.mugd_sample_join.argtypes = [C.c_void_p, C.POINTER(Join), C.POINTER(Op), C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_plan_save.argtypes = [C.c_void_p, C.POINTER(Region), C.c_int32, C.c_char_p]
     lib.mugd_plan_load.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(Region), C.c_int32, C.POINTER(C.c_void_p)]
     lib.mugd_set_tc_single_pass_tf32.argtypes = [C.c_void_p, C.c_int]
@@ -237,5 +249,5 @@ EXPORTED_SYMBOLS = [
     "mugd_debug_set_attention_dump", "mugd_debug_set_tc_timing", "mugd_sample", "mugd_plan_save", "mugd_plan_load", "mugd_plan_regions", "mugd_plan_ops",
     "mugd_melspec", "mugd_grid_scan", "mugd_chart_snap", "mugd_remove_mini_jacks",
     "mugd_sample_staged", "mugd_sample_plms", "mugd_plms_combine",
-    "mugd_sample_ddpm", "mugd_ddpm_update",
+    "mugd_sample_ddpm", "mugd_ddpm_update", "mugd_stochastic_encode", "mugd_sample_join",
 ]

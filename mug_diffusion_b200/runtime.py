@@ -67,6 +67,14 @@ class Plan:
         self.ensure_captured()
         L_.check(self.engine.lib.mugd_sample_ddpm(self.handle, C.byref(ddpm), first_step, steps, _stream()), "mugd_sample_ddpm")
 
+    def launch_join(self, join: L_.Join, tail: OpList, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a decode request whose charts join at different iterations, from one C call
+        (mugd_sample_join: the join kernel, the graph replay and the tail per step)"""
+        self.ensure_captured()
+        self.engine.attach_workspace(tail)
+        L_.check(self.engine.lib.mugd_sample_join(self.handle, C.byref(join), tail.array(), len(tail.ops), first_step, steps, _stream()),
+                 "mugd_sample_join")
+
     def launch(self, steps: int = 1, tail: Optional[OpList] = None, stage: Optional[L_.Stage] = None):
         """``steps`` replays of the plan's CUDA graph; with ``tail``, every replay is followed by the tail ops and all steps run from
         one C call (mugd_sample); with ``stage`` as well, each step starts with the stage kernel (mugd_sample_staged: inpainting blend,
@@ -533,6 +541,16 @@ class Session:
         s.noise_rows = noise or None
         s.B, s.C, s.L = B, self.engine.cfg.unet.in_channels, self.Lz
         return s
+
+    def join(self, B: int, cfg_on: bool, x_latent: int, join: int) -> L_.Join:
+        """the mugd_sample_join descriptor over the rows ddim_tail updates (x, and its copy under classifier-free guidance):
+        ``x_latent`` = the device address of the [B, C, Lz] start latents, ``join`` = that of the [B] int32 join iterations"""
+        j = L_.Join()
+        j.x = self.xin.ptr
+        j.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        j.x_latent, j.join = x_latent, join
+        j.B, j.C, j.L = B, self.engine.cfg.unet.in_channels, self.Lz
+        return j
 
     def set_step(self, value: int):
         L_.check(self.engine.lib.mugd_fill_i32(_ptr(self.step), value, _stream()), "fill_i32")

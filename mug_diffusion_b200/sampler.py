@@ -72,6 +72,17 @@ def ddim_timesteps_uniform(S: int, T: int) -> np.ndarray:
     return np.asarray(list(range(0, T, T // S))) + 1
 
 
+def ddim_subset_end(k, n: int) -> int:
+    """The slice end of the DDIM timesteps that ddim_sampling / plms_sampling run for ``timesteps=k`` (ddim.py:126, plms.py:131), the
+    reference's Python float expression with its quirks: k gives k - 1 steps, k = 1 none, k > n gives n - 1, and the product can
+    round down (n = 50, k = 29: int(28.999999999999996) - 1 = 27 steps)."""
+    return int(min(k / n, 1) * n) - 1
+
+
+ORIGINAL_STEPS = ("the original-steps schedule (ddim_use_original_steps / use_original_steps=True) is not supported: the reference's "
+                  "p_sample_ddim reads model.ddim_sigmas_for_original_num_steps, which its DDPM does not define")
+
+
 def ddim_parameters(alphas_cumprod: torch.Tensor, ts: np.ndarray, eta: float):
     ac = alphas_cumprod.detach().cpu()
     alphas = ac[ts]
@@ -449,10 +460,25 @@ class DDIMSampler(object):
                                   unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class,
                                   match_reference_rng=bool(kwargs.get("match_reference_rng", False)))
 
-    def _load_request(self, w, c, shape, x_T, scale, uc):
-        """Once per request, both samplers: _load_session over the DDIM timesteps, with the coefficient rows of make_schedule.
+    def _schedule_subset(self, timesteps, ddim_use_original_steps) -> np.ndarray:
+        """the DDIM timesteps a request runs: all of make_schedule's, or ddim_timesteps[:ddim_subset_end(k, n)] for timesteps=k
+        (ddim.py:123-127, plms.py:128-132).  ValueError, before any GPU work, for the original-steps schedule and a k that is not a
+        finite real number."""
+        if ddim_use_original_steps:
+            raise ValueError(ORIGINAL_STEPS)
+        if timesteps is None:
+            return self.ddim_timesteps
+        if (isinstance(timesteps, bool) or not isinstance(timesteps, (int, float, np.integer, np.floating))
+                or not np.isfinite(timesteps)):
+            raise ValueError(f"timesteps={timesteps!r} must be a finite number")
+        return self.ddim_timesteps[:ddim_subset_end(timesteps, self.ddim_timesteps.shape[0])]
+
+    def _load_request(self, w, c, shape, x_T, scale, uc, timesteps=None):
+        """Once per request, all DDIM-schedule samplers: _load_session over the DDIM timesteps (or the prefix ``timesteps`` of them),
+        with the coefficient rows of make_schedule (a request of n steps reads rows n - 1 .. 0, the prefix's).
         Returns (x, cfg_on, session, time_range)."""
-        x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, uc, np.flip(self.ddim_timesteps))
+        ts = self.ddim_timesteps if timesteps is None else timesteps
+        x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, uc, np.flip(ts))
         sess.set_ddim_schedule(self.ddim_alphas, self.ddim_alphas_prev, self.ddim_sigmas, self.ddim_sqrt_one_minus_alphas)
         return x, cfg_on, sess, time_range
 
@@ -475,18 +501,26 @@ class DDIMSampler(object):
         return x, cfg_on, sess, time_range
 
     @torch.no_grad()
-    def ddim_sampling(self, w, c, shape, x_T=None, callback=None, mask=None, x0=None, img_callback=None,
-                      log_every_t=100, temperature=1., noise_dropout=0., unconditional_guidance_scale=1.,
+    def ddim_sampling(self, w, c, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None, mask=None, x0=None,
+                      img_callback=None, log_every_t=100, temperature=1., noise_dropout=0., unconditional_guidance_scale=1.,
                       unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False):
+        """ddim.py:110-159 on the GPU.  ``timesteps=k`` runs the reference's truncated schedule, the last, low-noise
+        ddim_timesteps[:ddim_subset_end(k, n)] from x_T; when that is empty, x_T comes back with both intermediate lists [x_T].
+        ``ddim_use_original_steps=True`` raises ValueError before any GPU work (see ORIGINAL_STEPS)."""
         model = self.model
         eng = model.engine
         dev = self.device
         B, Cz, Lz = shape
+        ts = self._schedule_subset(timesteps, ddim_use_original_steps)
+        if ts.shape[0] == 0:
+            x = torch.randn(shape, device=dev) if x_T is None else x_T.to(dev, torch.float32)
+            return x, {'x_inter': [x], 'pred_x0': [x]}
         # the reference draws (and, with noise_dropout, masks) noise every step even when sigma == 0 (ddim.py:192-194); the
         # draw is skipped here unless it can change the result or the caller asks for the same global-RNG consumption
         match_rng = bool(match_reference_rng)
         with eng.lock:
-            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, unconditional_guidance_scale, unconditional_conditioning)
+            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, unconditional_guidance_scale, unconditional_conditioning,
+                                                             ts)
             total = time_range.shape[0]
             # pred_x0 and the noise of a step: channels-last rows [B*Lz, Cz]
             pred = torch.empty(B * Lz, Cz, device=dev)
@@ -585,6 +619,128 @@ class DDIMSampler(object):
                 self.last_launches_per_step = sess.plan.launches + 2
             return current_x(), intermediates
 
+    # ---- remixing an existing chart (SDEdit / img2img): stochastic_encode + decode, as upstream Stable Diffusion's DDIMSampler --------
+    def _require_schedule(self, what: str):
+        if getattr(self, "ddim_timesteps", None) is None:
+            raise ValueError(f"{what} needs the DDIM schedule: call make_schedule(S) first")
+
+    @torch.no_grad()
+    def stochastic_encode(self, x0, t, use_original_steps=False, noise=None):
+        """Noise the latent ``x0`` [B, C, L] to DDIM index ``t[b]`` per chart: sqrt(ddim_alphas)[t] * x0 + ddim_sqrt_one_minus_alphas[t]
+        * noise (Stable Diffusion's formulation), with noise = torch.randn_like(x0) when not given (the generator ends where randn_like
+        leaves it).  ``t``: a [B] integer tensor (or sequence) of indices into make_schedule's tables; ``use_original_steps=True``
+        indexes the model's sqrt_alphas_cumprod / sqrt_one_minus_alphas_cumprod instead.  One kernel, bit-identical to those torch
+        expressions on CUDA (the square root is torch's).  ValueError, before any GPU work, for malformed arguments and indices
+        outside the table."""
+        model = self.model
+        dev = self.device
+        if not use_original_steps:
+            self._require_schedule("stochastic_encode")
+        n = int(model.sqrt_alphas_cumprod.shape[0] if use_original_steps else len(self.ddim_alphas))
+        if not isinstance(x0, torch.Tensor) or x0.dim() != 3 or x0.dtype != torch.float32 or x0.device != torch.device(dev):
+            raise ValueError(f"x0 must be a float32 [B, C, L] tensor on {dev}")
+        B = x0.shape[0]
+        tt = torch.as_tensor(t)
+        if tt.dtype in (torch.bool,) or tt.is_floating_point() or tt.is_complex() or tuple(tt.shape) != (B,):
+            raise ValueError(f"t must be {B} integer table indices, one per chart (got dtype {tt.dtype}, shape {tuple(tt.shape)})")
+        th = tt.cpu()
+        if B and (int(th.min()) < 0 or int(th.max()) > n - 1):
+            raise ValueError(f"t={th.tolist()}: indices must lie in [0, {n - 1}]")
+        if noise is not None and (not isinstance(noise, torch.Tensor) or noise.shape != x0.shape or noise.dtype != torch.float32
+                                  or noise.device != x0.device):
+            raise ValueError(f"noise must be a float32 tensor of x0's shape {tuple(x0.shape)} on {dev}")
+        if noise is None:
+            noise = torch.randn_like(x0)
+        if use_original_steps:
+            sa, s1m = model.sqrt_alphas_cumprod, model.sqrt_one_minus_alphas_cumprod
+        else:
+            sa = torch.sqrt(torch.as_tensor(self.ddim_alphas).to(dev, torch.float32))
+            s1m = torch.as_tensor(self.ddim_sqrt_one_minus_alphas).to(dev, torch.float32)
+        out = torch.empty(x0.shape, device=dev)
+        if out.numel() == 0:
+            return out
+        x0c, nc = x0.contiguous(), noise.contiguous()
+        td = th.to(dev, torch.int64)
+        d = L_.QEncode()
+        d.x0, d.noise, d.t, d.sqrt_a, d.sqrt_1ma, d.out = _ptr(x0c), _ptr(nc), _ptr(td), _ptr(sa), _ptr(s1m), _ptr(out)
+        d.B, d.C, d.L, d.n = B, x0.shape[1], x0.shape[2], n
+        with model.engine.lock:
+            L_.check(model.engine.lib.mugd_stochastic_encode(C.byref(d), torch.cuda.current_stream().cuda_stream), "mugd_stochastic_encode")
+        return out
+
+    def _decode_starts(self, x_latent, t_start):
+        """the per-chart start indices of a decode request; ValueError for malformed ones"""
+        n = self.ddim_timesteps.shape[0]
+        B = x_latent.shape[0]
+        if isinstance(t_start, (int, np.integer)) and not isinstance(t_start, bool):
+            starts = [int(t_start)] * B
+        elif isinstance(t_start, (list, tuple, np.ndarray, torch.Tensor)):
+            starts = list(t_start.tolist() if isinstance(t_start, (np.ndarray, torch.Tensor)) else t_start)
+            if len(starts) != B:
+                raise ValueError(f"t_start has {len(starts)} entries for {B} charts")
+            if any(isinstance(s, bool) or not isinstance(s, (int, np.integer)) for s in starts):
+                raise ValueError(f"t_start={starts!r}: the starts must be integers")
+            starts = [int(s) for s in starts]
+        else:
+            raise ValueError(f"t_start={t_start!r} must be an integer or one integer per chart")
+        if any(s < 0 or s > n for s in starts):
+            raise ValueError(f"t_start={starts}: every start must lie in [0, {n}] (n = len(ddim_timesteps))")
+        return starts
+
+    @torch.no_grad()
+    def decode(self, x_latent, c, w, t_start, unconditional_guidance_scale=1., unconditional_conditioning=None,
+               use_original_steps=False, tqdm_class=None):
+        """Stable Diffusion's DDIMSampler.decode with Mug's (c, w) conditioning: denoise ``x_latent`` [B, C, L] (e.g. from
+        stochastic_encode) over ddim_timesteps[:t_start] flipped, at index = t_start - i - 1 and eta = 0, and return the final latent.
+        With a scalar t_start = s it equals ddim_sampling(w, c, shape, x_T=x_latent, timesteps=s + 1) wherever that subset has s steps;
+        s = 0 returns x_latent itself.  ``t_start`` may also give one start per chart: one device loop of m = max(t_start)
+        iterations in which chart b joins at iteration m - t_start[b] from x_latent[b] (a join kernel holds its rows until then) and
+        then follows the coefficient rows of its own scalar run; a chart with t_start[b] = 0 comes back as x_latent[b].  Charts with a
+        smaller start still occupy their batch rows for all m iterations: group charts by strength into separate calls to avoid the
+        idle rows.  Every argument is checked before any GPU work (ValueError): the schedule must be make_schedule's at eta = 0."""
+        model = self.model
+        eng = model.engine
+        dev = self.device
+        if use_original_steps:
+            raise ValueError(ORIGINAL_STEPS)
+        self._require_schedule("decode")
+        if np.any(np.asarray(self.ddim_sigmas) != 0):
+            raise ValueError("decode runs at eta = 0: call make_schedule(S, ddim_eta=0.)")
+        if not isinstance(x_latent, torch.Tensor) or x_latent.dim() != 3 or x_latent.shape[0] < 1 or x_latent.shape[1] != model.z_channels:
+            raise ValueError(f"x_latent must be a [B, {model.z_channels}, L] tensor"
+                             + (f", got {tuple(x_latent.shape)}" if isinstance(x_latent, torch.Tensor) else ""))
+        starts = self._decode_starts(x_latent, t_start)
+        scale, uc = unconditional_guidance_scale, unconditional_conditioning
+        B, Cz, Lz = (int(v) for v in x_latent.shape)
+        shape = (B, Cz, Lz)
+        request_size(model, c, B, (Cz, Lz), x_latent, None, None, scale, uc, 1)
+        if w is None:
+            raise ValueError("decode needs the audio features w")
+        m = max(starts)
+        if m == 0:
+            return x_latent
+        with eng.lock:
+            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_latent, scale, uc, self.ddim_timesteps[:m])
+            pred = torch.empty(B * Lz, Cz, device=dev)
+            tail = sess.ddim_tail(B, m, cfg_on, scale, 1.0, _ptr(pred))
+            if len(set(starts)) == 1:
+                sess.plan.launch(m, tail)
+                self.last_launches_per_step = sess.plan.launches + 2
+            else:
+                xl = x.contiguous()
+                joins = torch.tensor([m - s for s in starts], dtype=torch.int32, device=dev)
+                sess.plan.launch_join(sess.join(B, cfg_on, _ptr(xl), _ptr(joins)), tail, 0, m)
+                self.last_launches_per_step = sess.plan.launches + 3
+            cls = tqdm_class if tqdm_class is not None else _tqdm
+            if cls is not None:
+                for _ in cls(time_range, desc='Decoding image', total=m):      # keeps a progress bar moving
+                    pass
+            z = sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+            idle = [b for b, s in enumerate(starts) if s == 0]
+            if idle:
+                z[idle] = x[idle]
+            return z
+
 
 def request_size(model, c, batch_size, shape, x_T, mask, x0, scale, uc, log_every_t):
     """the [B, C, L] latent shape of a PLMS or DDPM request; ValueError for malformed arguments, before any GPU work"""
@@ -670,14 +826,19 @@ class PLMSSampler(DDIMSampler):
         return request_size(self.model, c, batch_size, shape, x_T, mask, x0, scale, uc, log_every_t)
 
     @torch.no_grad()
-    def plms_sampling(self, w, c, shape, x_T=None, callback=None, mask=None, x0=None, img_callback=None, log_every_t=100,
-                      noise_dropout=0., unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None,
-                      progress=True, match_reference_rng=False):
-        """plms.py:115-170 (and p_sample_plms, :172-236) on the GPU."""
+    def plms_sampling(self, w, c, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None, mask=None, x0=None,
+                      img_callback=None, log_every_t=100, noise_dropout=0., unconditional_guidance_scale=1.,
+                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False):
+        """plms.py:115-170 (and p_sample_plms, :172-236) on the GPU.  ``timesteps=k`` runs the truncated schedule of plms.py:128-136
+        (t_next and the warm-up follow it); ``ddim_use_original_steps=True`` raises as in ddim_sampling."""
         model = self.model
         eng = model.engine
         dev = self.device
         B, Cz, Lz = shape
+        ts = self._schedule_subset(timesteps, ddim_use_original_steps)
+        if ts.shape[0] == 0:
+            x = torch.randn(shape, device=dev) if x_T is None else x_T.to(dev, torch.float32)
+            return x, {'x_inter': [x], 'pred_x0': [x]}
         match_rng = bool(match_reference_rng)
         scale = unconditional_guidance_scale
 
@@ -687,7 +848,7 @@ class PLMSSampler(DDIMSampler):
                 draw_step_noise(k, shape, None, None, True, None, noise_dropout, dev)
 
         with eng.lock:
-            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, scale, unconditional_conditioning)
+            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, scale, unconditional_conditioning, ts)
             total = time_range.shape[0]
             pred = torch.empty(B * Lz, Cz, device=dev)
             work = torch.empty(5, B * Lz * Cz, device=dev)                    # e', the e_t ring [3], the x stash
