@@ -330,6 +330,35 @@ int  mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_st
 /* the update kernel alone (noise row 0, the counter not advanced), for a host that runs the DDPM steps one by one */
 int  mugd_ddpm_update(const mugd_ddpm* d, void* stream);
 
+/* ---- the DPM-Solver++ multistep sampler loop (data prediction; Stable Diffusion 2's DPM_Solver(predict_x0=True), "multistep") ----
+ * n = B*L*C elements of the dense x rows.  Step i of an S-step request (the device counter holding i): replay the evaluation plan
+ * (timestep row i = the model time of t_i), then one update kernel with coefficient row i = coef[8i .. 8i+7] = (alpha_i, sigma_i,
+ * A, c0, c1, c2, order, unused):
+ *   e  = eps rows; with cfg: e_u + scale * (e_c - e_u), uncond half first (the DDIM combine)
+ *   m0 = (x - sigma_i * e) / alpha_i                                                    the data prediction at t_i
+ *   x  = ((A * x + c0 * m0) + c1 * m1) + c2 * m2   (the c1 term only for order >= 2, c2 only for order 3)
+ * where m1 / m2 are the predictions of steps i-1 / i-2, read from ring slots (i-1) mod 3 / (i-2) mod 3; m0 goes to slot i mod 3 and
+ * to pred_x0 (if given), x to x and x_dup; then *step += 1.  Every intermediate is one IEEE round-to-nearest in this order, no
+ * contraction.  The rows come from the host (mug_diffusion_b200/dpm_solver.py), which expands the solver's D-form updates in float64.
+ * The ring and the counter live on the device, so a request can run as several calls (first_step = steps already run, the counter
+ * holding first_step), including a split inside the warm-up. */
+typedef struct mugd_dpm {
+    float* x; float* x_dup;                /* [B*L, C] dense rows in place; x_dup = the CFG copy (given exactly when cfg = 1)     */
+    const float* eps;                      /* [Beff*L, C] the evaluation plan's output rows; Beff = 2B when cfg                  */
+    float* pred_x0;                        /* [n] the data prediction m0 of the step, or NULL                                  */
+    float* ring;                           /* [3][n] m0 of the last three steps (slot j mod 3 for step j)                      */
+    const float* coef;                     /* [S][8] coefficient rows                                                           */
+    int32_t* step;                         /* device step counter i                                                             */
+    int32_t n, S;                          /* elements of x; steps of the request (S <= MUGD_MAX_STEPS)                         */
+    int32_t cfg; float scale;              /* classifier-free guidance: cfg = 1 and its scale                                  */
+} mugd_dpm;
+/* steps first_step .. first_step + n_steps - 1 of the S-step request, no host synchronisation: n_steps x { graph replay, update,
+ * *step += 1 }, the same launches per step as mugd_sample.  Every argument is checked before the first launch
+ * (first_step + n_steps <= S <= MUGD_MAX_STEPS).  A standalone entry point: the ABI version is unchanged. */
+int  mugd_sample_dpm(mugd_plan* eval_plan, const mugd_dpm* d, int32_t first_step, int32_t n_steps, void* stream);
+/* the update kernel alone (the counter not advanced), for a host that runs the DPM-Solver++ steps one by one */
+int  mugd_dpm_update(const mugd_dpm* d, void* stream);
+
 /* ---- remixing an existing chart (SDEdit / img2img): DDIMSampler.stochastic_encode and decode with a per-chart start ---------------
  * mugd_stochastic_encode: out[b] = sqrt_a[t[b]] * x0[b] + sqrt_1ma[t[b]] * noise[b], each product and the sum one IEEE
  * round-to-nearest (no contraction), bit-identical to torch's extract_into_tensor expressions.  x0, noise and out are device NCL

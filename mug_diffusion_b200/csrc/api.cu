@@ -305,6 +305,25 @@ int mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_ste
     return MUGD_OK;
 }
 
+int mugd_sample_dpm(mugd_plan* eval_plan, const mugd_dpm* d, int32_t first_step, int32_t n_steps, void* stream) {
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_dpm: the evaluation plan must be captured (mugd_plan_capture)");
+    MUGD_REQUIRE(d, "mugd_sample_dpm: null dpm");
+    int rc = check_dpm(*d);
+    if (rc != MUGD_OK) return rc;
+    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= d->S,
+                 "mugd_sample_dpm: first_step=%d, n_steps=%d outside the S=%d steps of the request", first_step, n_steps, d->S);
+    const DeviceInfo& dev = eval_plan->h->dev;
+    cudaStream_t st = (cudaStream_t)stream;
+    mugd_step_advance adv;
+    adv.step = d->step;
+    for (int32_t k = 0; k < n_steps; ++k) {
+        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
+        if ((rc = launch_dpm_update(*d, st)) != MUGD_OK) return rc;
+        if ((rc = launch_step_advance(dev, adv, st, nullptr)) != MUGD_OK) return rc;
+    }
+    return MUGD_OK;
+}
+
 int mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
                      int32_t n_steps, void* stream) {
     MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_join: the evaluation plan must be captured (mugd_plan_capture)");

@@ -72,6 +72,9 @@ int launch_plms_combine(const mugd_plms& p, int32_t step, int heun, cudaStream_t
 // mugd_sample_ddpm / mugd_ddpm_update: check_ddpm validates the descriptor; launch_ddpm_update runs the update on noise row k
 int check_ddpm(const mugd_ddpm& d);
 int launch_ddpm_update(const mugd_ddpm& d, int32_t k, cudaStream_t st);
+// mugd_sample_dpm / mugd_dpm_update: check_dpm validates the descriptor; launch_dpm_update runs the update of the counter's step
+int check_dpm(const mugd_dpm& d);
+int launch_dpm_update(const mugd_dpm& d, cudaStream_t st);
 // mugd_sample_join: check_join validates the descriptor; launch_join runs the join kernel against the device step counter
 int check_join(const mugd_join& j);
 int launch_join(const mugd_join& j, const int32_t* step, cudaStream_t st);

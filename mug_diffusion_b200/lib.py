@@ -115,6 +115,11 @@ class Ddpm(C.Structure):
                 ("clip", C.c_int32), ("reserved_", C.c_int32)]
 
 
+class Dpm(C.Structure):
+    _fields_ = [("x", _f), ("x_dup", _f), ("eps", _f), ("pred_x0", _f), ("ring", _f), ("coef", _f), ("step", _f),
+                ("n", C.c_int32), ("S", C.c_int32), ("cfg", C.c_int32), ("scale", C.c_float)]
+
+
 class QEncode(C.Structure):
     _fields_ = [("x0", _f), ("noise", _f), ("t", _f), ("sqrt_a", _f), ("sqrt_1ma", _f), ("out", _f),
                 ("B", C.c_int32), ("C", C.c_int32), ("L", C.c_int32), ("n", C.c_int32)]
@@ -211,6 +216,8 @@ def load() -> C.CDLL:
     lib.mugd_plms_combine.argtypes = [C.POINTER(Plms), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_sample_ddpm.argtypes = [C.c_void_p, C.POINTER(Ddpm), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_ddpm_update.argtypes = [C.POINTER(Ddpm), C.c_void_p]
+    lib.mugd_sample_dpm.argtypes = [C.c_void_p, C.POINTER(Dpm), C.c_int32, C.c_int32, C.c_void_p]
+    lib.mugd_dpm_update.argtypes = [C.POINTER(Dpm), C.c_void_p]
     lib.mugd_stochastic_encode.argtypes = [C.POINTER(QEncode), C.c_void_p]
     lib.mugd_sample_join.argtypes = [C.c_void_p, C.POINTER(Join), C.POINTER(Op), C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_plan_save.argtypes = [C.c_void_p, C.POINTER(Region), C.c_int32, C.c_char_p]
@@ -250,4 +257,5 @@ EXPORTED_SYMBOLS = [
     "mugd_melspec", "mugd_grid_scan", "mugd_chart_snap", "mugd_remove_mini_jacks",
     "mugd_sample_staged", "mugd_sample_plms", "mugd_plms_combine",
     "mugd_sample_ddpm", "mugd_ddpm_update", "mugd_stochastic_encode", "mugd_sample_join",
+    "mugd_sample_dpm", "mugd_dpm_update",
 ]

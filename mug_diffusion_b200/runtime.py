@@ -67,6 +67,11 @@ class Plan:
         self.ensure_captured()
         L_.check(self.engine.lib.mugd_sample_ddpm(self.handle, C.byref(ddpm), first_step, steps, _stream()), "mugd_sample_ddpm")
 
+    def launch_dpm(self, dpm: L_.Dpm, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a DPM-Solver++ request from one C call (mugd_sample_dpm)"""
+        self.ensure_captured()
+        L_.check(self.engine.lib.mugd_sample_dpm(self.handle, C.byref(dpm), first_step, steps, _stream()), "mugd_sample_dpm")
+
     def launch_join(self, join: L_.Join, tail: OpList, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a decode request whose charts join at different iterations, from one C call
         (mugd_sample_join: the join kernel, the graph replay and the tail per step)"""
@@ -363,10 +368,15 @@ class Session:
     def set_timestep_table(self, timesteps: Sequence[int]):
         """Time-embedding MLP + all ResBlock emb projections for the given timesteps, one row each
         (unet.py:335-339, 166-172; model/util.py:156-176).  The sinusoid is evaluated on the host exactly
-        as the reference does; the three GEMMs run on the GPU."""
+        as the reference does; the three GEMMs run on the GPU.  Integer timesteps go through a long tensor as the samplers' t does;
+        float times (the DPM-Solver's model times) are taken as float32, the dtype the sinusoid computes in."""
         cfg = self.engine.cfg.unet
         eng = self.engine
-        t = torch.as_tensor(np.asarray(timesteps), dtype=torch.long)
+        ts = np.asarray(timesteps)
+        if ts.dtype.kind == "f":
+            t = torch.as_tensor(ts.astype(np.float32))
+        else:
+            t = torch.as_tensor(ts, dtype=torch.long)
         R = t.shape[0]
         assert R <= self.temb.shape[0]
         half = cfg.model_channels // 2
@@ -518,6 +528,20 @@ class Session:
         d.eps, d.pred_x0, d.noise, d.coef, d.step = self.eps.ptr, pred_x0 or None, noise, _ptr(coef), _ptr(self.step)
         d.T, d.B, d.C, d.L = T, B, self.engine.cfg.unet.in_channels, self.Lz
         d.cfg, d.scale, d.clip = int(cfg_on), float(scale), int(bool(clip))
+        return d
+
+    def dpm(self, B: int, S: int, cfg_on: bool, scale: float, pred_x0: int, ring: torch.Tensor, coef: torch.Tensor) -> L_.Dpm:
+        """the mugd_sample_dpm descriptor of an S-step request for B samples: the update reads eps (both halves under
+        classifier-free guidance) and ``coef`` (the request's [S, 8] coefficient rows), keeps the last three data predictions in
+        ``ring`` ([3, B*Lz*C]), and writes the xin rows of both halves and pred_x0.  The caller keeps both tensors alive."""
+        n = B * self.Lz * self.engine.cfg.unet.in_channels
+        assert coef.shape == (S, 8) and coef.dtype == torch.float32 and coef.is_contiguous()
+        assert ring.shape == (3, n) and ring.dtype == torch.float32 and ring.is_contiguous()
+        d = L_.Dpm()
+        d.x = self.xin.ptr
+        d.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        d.eps, d.pred_x0, d.ring, d.coef, d.step = self.eps.ptr, pred_x0 or None, _ptr(ring), _ptr(coef), _ptr(self.step)
+        d.n, d.S, d.cfg, d.scale = n, S, int(cfg_on), float(scale)
         return d
 
     def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:

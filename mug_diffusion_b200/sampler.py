@@ -4,6 +4,7 @@ Reference surface kept (SURVEY §8b):
     sampler = DDIMSampler(model)                                  mug/diffusion/ddim.py:12
     sampler = PLMSSampler(model)                                  mug/diffusion/plms.py:11 (scripts/mapping.py --plms)
     sampler = DDPMSampler(model)                                  DDPM.log_beatmap's loop, mug/diffusion/diffusion.py:255-282
+    sampler = DPMSolverSampler(model)                             DPM-Solver++ multistep (Stable Diffusion 2's DPMSolverSampler)
     samples, inter = sampler.sample(S, c, w, batch_size, ...)     mug/diffusion/ddim.py:56-107
     eps    = model.model.forward(x, t, c, w)                      mug/diffusion/diffusion.py:52-54
     logits = model.model.decode(z)                                mug/diffusion/diffusion.py:49-50
@@ -20,9 +21,10 @@ from typing import Dict, Optional, Sequence
 import numpy as np
 import torch
 
+from . import dpm_solver
 from . import lib as L_
 from .config import DecoderConfig, EncoderConfig, ModelConfig, UNetConfig
-from .engine import OpList, View
+from .engine import MAX_STEPS, OpList, View
 from .lib import MugdError
 from .postprocess import objects_to_array
 from .prompt import PromptEmbedder
@@ -155,7 +157,7 @@ class _Wrapper:
             s = o.engine.session(B, Lz, per_sample_t=True)
             if t.dim() == 2:
                 t = t[:, 0]
-            s.set_timestep_table(t.detach().cpu().numpy())
+            s.set_timestep_table(t.detach().cpu().long().numpy())
             s.set_context(c)
             s.set_audio(w)
             s.load_x(x, dup=False)
@@ -1049,6 +1051,155 @@ class DDPMSampler(DDIMSampler):
                     sess.eval(graph=True)
                     draw_step_noise(1, shape, None, None, True, table, 0., dev)   # noise_like, diffusion.py:274
                     L_.check(eng.lib.mugd_ddpm_update(C.byref(ddpm), stream), "mugd_ddpm_update")
+                    eng.run_ops(advance)
+                    if callback:
+                        callback(i)
+                    if img_callback:
+                        img_callback(current_pred(), i)
+                    if logged(i):
+                        intermediates['x_inter'].append(current_x())
+                        intermediates['pred_x0'].append(current_pred())
+            self.last_launches_per_step = sess.plan.launches + 2
+            return current_x(), intermediates
+
+
+# --------------------------------------------------------------------------------------------------
+# DPM-Solver++ multistep sampler
+# --------------------------------------------------------------------------------------------------
+def alphas_cumprod_f64(cfg: ModelConfig) -> np.ndarray:
+    """the model's alphas_cumprod in float64: register_schedule's arithmetic before its float32 cast"""
+    return np.cumprod(1. - beta_schedule_linear(cfg.timesteps, cfg.linear_start, cfg.linear_end), axis=0)
+
+
+class DPMSolverSampler(DDIMSampler):
+    """DPM-Solver++ multistep (Lu et al., 2022): a 1st- to 3rd-order solver of the probability-flow ODE in data-prediction form, the
+    ``DPMSolverSampler`` of Stable Diffusion 2 with the ``sample(S, ...)`` shape of DDIMSampler and PLMSSampler.  15-25 steps of
+    order 2 are the usual replacement for 50-100 DDIM steps.  Same constructor as DDIMSampler; each step is one batched U-Net
+    evaluation at a float model time and one update kernel (csrc/dpm.cu) whose coefficient rows come from ``dpm_solver``.
+    Deterministic (no noise is drawn apart from x_T when it is not given)."""
+
+    # what DDIMSampler.sample takes and the deterministic multistep solver has no counterpart for, with the value that means "not used"
+    _NOT_IN_DPM = dict(mask=None, x0=None, eta=0., temperature=1., noise_dropout=0.)
+
+    def make_dpm_schedule(self, S, order=2, skip_type="time_uniform", solver_type="dpmsolver", lower_order_final=True,
+                          t_grid=None) -> dpm_solver.DPMSchedule:
+        """the coefficient rows and model times of an S-step request (``t_grid``: an explicit continuous-time grid of S + 1 points
+        from 1 down to 1/N instead of ``skip_type``'s)"""
+        if isinstance(S, bool) or not isinstance(S, (int, np.integer)) or not 0 < S <= MAX_STEPS:
+            raise ValueError(f"S={S!r}: the number of steps must be an integer in [1, {MAX_STEPS}]")
+        if isinstance(order, bool) or not isinstance(order, (int, np.integer)) or order not in dpm_solver.ORDERS:
+            raise ValueError(f"order={order!r}: DPM-Solver++ multistep runs order 1, 2 or 3")
+        if S < order:
+            raise ValueError(f"S={S}: order {order} needs at least {order} steps")
+        if t_grid is None and skip_type not in dpm_solver.SKIP_TYPES:
+            raise ValueError(f"skip_type={skip_type!r}: one of {dpm_solver.SKIP_TYPES}")
+        if solver_type not in dpm_solver.SOLVER_TYPES:
+            raise ValueError(f"solver_type={solver_type!r}: one of {dpm_solver.SOLVER_TYPES}")
+        if lower_order_final not in (True, False):
+            raise ValueError(f"lower_order_final={lower_order_final!r} must be True or False")
+        return dpm_solver.multistep_schedule(alphas_cumprod_f64(self.model.cfg), int(S), int(order), skip_type, solver_type,
+                                             bool(lower_order_final), t_grid)
+
+    @torch.no_grad()
+    def sample(self, S, c=None, w=None, batch_size=None, shape=None, x_T=None, order=2, skip_type="time_uniform",
+               solver_type="dpmsolver", lower_order_final=True, callback=None, img_callback=None, log_every_t=100,
+               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True, conditioning=None,
+               **kwargs):
+        """S steps of DPM-Solver++ multistep of ``order`` from x_T (drawn when not given) to t = 1/N; ``c`` may also be given as
+        ``conditioning``.  Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then x and the data prediction m of every step i with
+        ``(S - i - 1) % log_every_t == 0`` or i = 0 (DDIM's rule).  Every argument is checked before any GPU work (ValueError; TypeError
+        for missing or unknown ones); inpainting (mask / x0), eta, temperature and noise dropout are refused.  Without callbacks the
+        steps run from mugd_sample_dpm calls, one per stretch between two recorded intermediates; with ``callback`` / ``img_callback``
+        they run one by one through mugd_dpm_update."""
+        for name, off in self._NOT_IN_DPM.items():
+            v = kwargs.pop(name, off)
+            if off is None:
+                bad = v is not None
+            else:
+                bad = isinstance(v, bool) or not isinstance(v, (int, float)) or v != off
+            if bad:
+                raise ValueError(f"{name}={v!r}: DPM-Solver++ multistep is a deterministic solver without {name}")
+        if kwargs:
+            raise TypeError(f"DPMSolverSampler.sample got unexpected arguments {sorted(kwargs)}")
+        if conditioning is not None:
+            if c is not None:
+                raise TypeError("give the conditioning as c or as conditioning, not both")
+            c = conditioning
+        if c is None or w is None:
+            raise TypeError("DPMSolverSampler.sample needs the conditioning c and the audio features w")
+        scale = unconditional_guidance_scale
+        if isinstance(scale, bool) or not isinstance(scale, (int, float, np.floating)) or not np.isfinite(scale):
+            raise ValueError(f"unconditional_guidance_scale={scale!r} must be a finite number")
+        sched = self.make_dpm_schedule(S, order, skip_type, solver_type, lower_order_final)
+        size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
+        if verbose:
+            print(f'Data shape for DPM-Solver++ sampling is {size}, {S} steps of order {order} ({skip_type}, {solver_type})')
+        return self.dpm_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
+                                 unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
+                                 tqdm_class=tqdm_class)
+
+    @torch.no_grad()
+    def dpm_sampling(self, w, c, shape, sched: dpm_solver.DPMSchedule, x_T=None, callback=None, img_callback=None, log_every_t=100,
+                     unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True):
+        """the request of ``sched`` (make_dpm_schedule) on the GPU"""
+        model = self.model
+        eng = model.engine
+        dev = self.device
+        B, Cz, Lz = shape
+        total = sched.S
+        scale = unconditional_guidance_scale
+        self.last_schedule = sched
+        with eng.lock:
+            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times)
+            coef = torch.from_numpy(sched.rows_f32()).to(dev)
+            ring = torch.empty(3, B * Lz * Cz, device=dev)                     # the data predictions of the last three steps
+            pred = torch.empty(B * Lz, Cz, device=dev)
+            dpm = sess.dpm(B, total, cfg_on, scale, _ptr(pred), ring, coef)
+
+            intermediates = {'x_inter': [x], 'pred_x0': [x]}
+            iterator = time_range
+            if progress:
+                cls = tqdm_class if tqdm_class is not None else _tqdm
+                if cls is not None:
+                    iterator = cls(time_range, desc='Charting, using DPM-Solver++ Sampler', total=total)
+
+            def current_x():
+                return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+
+            def current_pred():
+                return eng.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
+
+            def logged(i):
+                index = total - i - 1
+                return index % log_every_t == 0 or index == total - 1              # DDIM's rule, ddim.py:154
+
+            if callback is None and img_callback is None:
+                # one mugd_sample_dpm call per stretch between two recorded intermediates: the ring and the step counter stay on the
+                # device, so a call may start inside the warm-up
+                it = iter(iterator)
+                i = 0
+                while i < total:
+                    j = i
+                    while not logged(j):
+                        j += 1
+                    sess.plan.launch_dpm(dpm, i, j - i + 1)
+                    for _ in range(j - i + 1):
+                        next(it, None)                                          # keeps a progress bar (tqdm_class) moving
+                    intermediates['x_inter'].append(current_x())
+                    intermediates['pred_x0'].append(current_pred())
+                    i = j + 1
+                for _ in it:
+                    pass
+            else:
+                # one step at a time from the same kernel: the referee of the device loop
+                adv = L_.StepAdvance()
+                adv.step = _ptr(sess.step)
+                advance = OpList()
+                advance.add(L_.OP_STEP_ADVANCE, adv)
+                stream = torch.cuda.current_stream().cuda_stream
+                for i, _ in enumerate(iterator):
+                    sess.eval(graph=True)
+                    L_.check(eng.lib.mugd_dpm_update(C.byref(dpm), stream), "mugd_dpm_update")
                     eng.run_ops(advance)
                     if callback:
                         callback(i)
