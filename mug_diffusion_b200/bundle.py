@@ -29,7 +29,7 @@ import torch
 from . import lib as L_
 from .engine import OpList
 from .runtime import Plan, _ptr
-from .sampler import draw_step_noise
+from .sampler import draw_step_noise, q_coef_table
 
 
 def _save_plan(eng, ops: OpList, regions: List[L_.Region], path: str) -> Plan:
@@ -81,8 +81,7 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
             st["in_x0"] = inpaint[0].to(dev, torch.float32).contiguous()
             st["in_mask"] = inpaint[1].to(dev, torch.float32).expand(shape).contiguous()
             st["in_qnoise"] = torch.empty((total,) + shape, device=dev)
-            sac, s1m = model.sqrt_alphas_cumprod.cpu(), model.sqrt_one_minus_alphas_cumprod.cpu()
-            qcoef = np.ascontiguousarray(np.stack([sac[ts.copy()].numpy(), s1m[ts.copy()].numpy()], 1), dtype=np.float32)
+            qcoef = q_coef_table(model, ts)
             qcoef.tofile(os.path.join(out_dir, "stage_coef.bin"))
         draw_step_noise(total, shape, st.get("in_x0"), st.get("in_qnoise"), has_noise, st.get("in_noise"), noise_dropout, dev)
         # per-request host tables for this S

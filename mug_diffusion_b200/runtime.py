@@ -56,21 +56,22 @@ class Plan:
             self.run()
             self.capture()
 
+    def _launch_steps(self, entry: str, desc, first_step: int, steps: int):
+        self.ensure_captured()
+        L_.check(getattr(self.engine.lib, entry)(self.handle, C.byref(desc), first_step, steps, _stream()), entry)
+
     def launch_plms(self, plms: L_.Plms, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a PLMS request from one C call (mugd_sample_plms)"""
-        self.ensure_captured()
-        L_.check(self.engine.lib.mugd_sample_plms(self.handle, C.byref(plms), first_step, steps, _stream()), "mugd_sample_plms")
+        self._launch_steps("mugd_sample_plms", plms, first_step, steps)
 
     def launch_ddpm(self, ddpm: L_.Ddpm, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a DDPM request from one C call (mugd_sample_ddpm); row k of the descriptor's
         noise table is the noise of step first_step + k"""
-        self.ensure_captured()
-        L_.check(self.engine.lib.mugd_sample_ddpm(self.handle, C.byref(ddpm), first_step, steps, _stream()), "mugd_sample_ddpm")
+        self._launch_steps("mugd_sample_ddpm", ddpm, first_step, steps)
 
     def launch_dpm(self, dpm: L_.Dpm, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a DPM-Solver++ request from one C call (mugd_sample_dpm)"""
-        self.ensure_captured()
-        L_.check(self.engine.lib.mugd_sample_dpm(self.handle, C.byref(dpm), first_step, steps, _stream()), "mugd_sample_dpm")
+        self._launch_steps("mugd_sample_dpm", dpm, first_step, steps)
 
     def launch_join(self, join: L_.Join, tail: OpList, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a decode request whose charts join at different iterations, from one C call
@@ -493,12 +494,16 @@ class Session:
         self.coef.zero_()
         self.coef[:len(coef)].copy_(torch.from_numpy(coef).to(self.engine.device))
 
+    def _x_rows(self, B: int, cfg_on: bool):
+        """the device addresses of the x rows a step updates: the first B samples' xin rows, and under classifier-free guidance
+        their copy in the second half (else None)"""
+        return self.xin.ptr, (self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None)
+
     def ddim_update(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> L_.DdimUpdate:
         """the DDIM update of ddim_tail"""
         n = B * self.Lz * self.engine.cfg.unet.in_channels
         upd = L_.DdimUpdate()
-        upd.x = self.xin.ptr
-        upd.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        upd.x, upd.x_dup = self._x_rows(B, cfg_on)
         upd.eps, upd.noise, upd.pred_x0 = self.eps.ptr, noise or None, pred_x0
         upd.coef, upd.step = _ptr(self.coef), _ptr(self.step)
         upd.S, upd.n, upd.cfg, upd.scale, upd.temperature = S, n, int(cfg_on), float(scale), float(temperature)
@@ -523,8 +528,7 @@ class Session:
         ([n][B, C, Lz]), and writes the xin rows of both halves and pred_x0"""
         assert coef.shape == (T, 5) and coef.dtype == torch.float32 and coef.is_contiguous()
         d = L_.Ddpm()
-        d.x = self.xin.ptr
-        d.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        d.x, d.x_dup = self._x_rows(B, cfg_on)
         d.eps, d.pred_x0, d.noise, d.coef, d.step = self.eps.ptr, pred_x0 or None, noise, _ptr(coef), _ptr(self.step)
         d.T, d.B, d.C, d.L = T, B, self.engine.cfg.unet.in_channels, self.Lz
         d.cfg, d.scale, d.clip = int(cfg_on), float(scale), int(bool(clip))
@@ -538,8 +542,7 @@ class Session:
         assert coef.shape == (S, 8) and coef.dtype == torch.float32 and coef.is_contiguous()
         assert ring.shape == (3, n) and ring.dtype == torch.float32 and ring.is_contiguous()
         d = L_.Dpm()
-        d.x = self.xin.ptr
-        d.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        d.x, d.x_dup = self._x_rows(B, cfg_on)
         d.eps, d.pred_x0, d.ring, d.coef, d.step = self.eps.ptr, pred_x0 or None, _ptr(ring), _ptr(coef), _ptr(self.step)
         d.n, d.S, d.cfg, d.scale = n, S, int(cfg_on), float(scale)
         return d
@@ -560,8 +563,7 @@ class Session:
         """the stage of mugd_sample_staged over the rows ddim_tail updates (x, and its copy under classifier-free guidance);
         ``noise`` = the tail's noise rows.  The caller fills in x0 / mask / q_noise / q_coef and the noise table."""
         s = L_.Stage()
-        s.x = self.xin.ptr
-        s.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        s.x, s.x_dup = self._x_rows(B, cfg_on)
         s.noise_rows = noise or None
         s.B, s.C, s.L = B, self.engine.cfg.unet.in_channels, self.Lz
         return s
@@ -570,8 +572,7 @@ class Session:
         """the mugd_sample_join descriptor over the rows ddim_tail updates (x, and its copy under classifier-free guidance):
         ``x_latent`` = the device address of the [B, C, Lz] start latents, ``join`` = that of the [B] int32 join iterations"""
         j = L_.Join()
-        j.x = self.xin.ptr
-        j.x_dup = self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None
+        j.x, j.x_dup = self._x_rows(B, cfg_on)
         j.x_latent, j.join = x_latent, join
         j.B, j.C, j.L = B, self.engine.cfg.unet.in_channels, self.Lz
         return j

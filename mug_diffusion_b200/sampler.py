@@ -117,6 +117,13 @@ def draw_step_noise(steps: int, shape, x0: Optional[torch.Tensor], q_table: Opti
                 noise_table[k].copy_(nz)
 
 
+def q_coef_table(model, time_range: np.ndarray) -> np.ndarray:
+    """The inpainting blend's host table [n][2] = (sqrt_alphas_cumprod[t_i], sqrt_one_minus_alphas_cumprod[t_i]) at the request's
+    timesteps t_i (q_sample's coefficients, ddim.py:142), as mugd_sample_staged reads it."""
+    sac, s1m = model.sqrt_alphas_cumprod.cpu(), model.sqrt_one_minus_alphas_cumprod.cpu()
+    return np.ascontiguousarray(np.stack([sac[time_range.copy()].numpy(), s1m[time_range.copy()].numpy()], 1), dtype=np.float32)
+
+
 def takes_device_loop(shape, device, mask=None, x0=None, callback=None, img_callback=None) -> bool:
     """True when ddim_sampling runs the request from mugd_sample / mugd_sample_staged calls.  Callbacks need the per-step loop; so do
     inpainting operands on which the per-step ops would promote or raise: a mask or x0 that is not a float32 tensor on the model's
@@ -419,9 +426,11 @@ class MugDiffusionB200:
 
 
 # --------------------------------------------------------------------------------------------------
-# DDIM sampler
+# what every sampler shares: the request's session and the request loop
 # --------------------------------------------------------------------------------------------------
-class DDIMSampler(object):
+class _DeviceLoopSampler:
+    """The constructor, the per-request session load and the request loop (``_run_request``) of every sampler here."""
+
     def __init__(self, model, schedule="linear", **kwargs):
         if not isinstance(model, MugDiffusionB200):
             model = MugDiffusionB200.from_reference(model)
@@ -431,6 +440,141 @@ class DDIMSampler(object):
         self.device = model.device
         self.last_launches_per_step = 0
 
+    def _x_T(self, shape, x_T):
+        """the request's start latent: x_T on the device, or drawn from its generator when not given"""
+        return torch.randn(shape, device=self.device) if x_T is None else x_T.to(self.device, torch.float32)
+
+    def _load_session(self, w, c, shape, x_T, scale, uc, time_range):
+        """x_T (drawn when not given), whether classifier-free guidance is on, and the session of this shape with the timestep table
+        (row i = time_range[i], the i-th loop iteration), context, audio and x loaded, its step counter at 0."""
+        model = self.model
+        B, Cz, Lz = shape
+        x = self._x_T(shape, x_T)
+        cfg_on = not (uc is None or scale == 1.)
+        Beff = 2 * B if cfg_on else B
+        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False)
+        sess.set_timestep_table(time_range.copy())
+        # ddim.py:170-174 concatenates [uc, c] and [w, w]; here the two halves are written straight into their rows
+        sess.set_context([uc, c] if cfg_on else c)
+        sess.set_audio(list(w)[-model.cfg.unet.levels:], dup=cfg_on)
+        sess.load_x(x, dup=cfg_on)
+        sess.set_step(0)
+        return x, cfg_on, sess, time_range
+
+    @staticmethod
+    def _progress(iterable, desc, total, tqdm_class, progress=True):
+        """``iterable`` in a progress bar: tqdm_class, else tqdm when it is installed; none when ``progress`` is False"""
+        cls = (tqdm_class if tqdm_class is not None else _tqdm) if progress else None
+        return iterable if cls is None else cls(iterable, desc=desc, total=total)
+
+    def _read_x(self, sess: Session, shape) -> torch.Tensor:
+        B, Cz, Lz = shape
+        return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+
+    def _read_pred(self, pred: torch.Tensor, shape) -> torch.Tensor:
+        B, Cz, Lz = shape
+        return self.model.engine.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
+
+    def _run_request(self, sess: Session, x, shape, pred, time_range, total, log_every_t, desc, tqdm_class, progress, callback,
+                     img_callback, device_loop, launch, step, tail_launches, chunk=None):
+        """Run a loaded request of ``total`` steps and return ``(z, {'x_inter', 'pred_x0'})``: x_T (``x``) first, then x and the
+        prediction (``pred``, channels-last rows [B*Lz, Cz]) after every step i with ``(total - i - 1) % log_every_t == 0`` or
+        i = 0 (ddim.py:154).
+        ``device_loop``: nothing runs on the host between steps.  The steps between two recorded intermediates form a stretch,
+        cut into calls of at most ``chunk`` steps; ``launch(first, n)`` runs steps first .. first + n - 1 from one C call.
+        Otherwise ``step(i, t)`` runs step i at time_range[i], followed by ``callback(i)`` and ``img_callback(pred, i)``.
+        ``tail_launches``: the launches each step adds to the U-Net plan's (``last_launches_per_step``)."""
+        iterator = self._progress(time_range, desc, total, tqdm_class, progress)
+        intermediates = {'x_inter': [x], 'pred_x0': [x]}
+
+        def record():
+            intermediates['x_inter'].append(self._read_x(sess, shape))
+            intermediates['pred_x0'].append(self._read_pred(pred, shape))
+
+        def logged(i):
+            index = total - i - 1
+            return index % log_every_t == 0 or index == total - 1
+
+        if device_loop:
+            it = iter(iterator)
+            i = 0
+            while i < total:
+                j = i
+                while not logged(j):
+                    j += 1
+                k = i
+                while k <= j:
+                    n = j - k + 1 if chunk is None else min(chunk, j - k + 1)
+                    launch(k, n)
+                    k += n
+                for _ in range(j - i + 1):
+                    next(it, None)                                              # keeps a progress bar (tqdm_class) moving
+                record()
+                i = j + 1
+            for _ in it:
+                pass
+        else:
+            for i, t in enumerate(iterator):
+                step(i, t)
+                if callback:
+                    callback(i)
+                if img_callback:
+                    img_callback(self._read_pred(pred, shape), i)
+                if logged(i):
+                    record()
+        self.last_launches_per_step = sess.plan.launches + tail_launches
+        return self._read_x(sess, shape), intermediates
+
+
+def _step_ops(sess: Session, update: Optional[L_.DdimUpdate] = None) -> OpList:
+    """the per-step loop's ops after a sampler's own update: ``update`` (a DDIM update, when given), then the step advance"""
+    adv = L_.StepAdvance()
+    adv.step = _ptr(sess.step)
+    ops = OpList()
+    if update is not None:
+        ops.add(L_.OP_DDIM_UPDATE, update)
+    ops.add(L_.OP_STEP_ADVANCE, adv)
+    return ops
+
+
+# what DDIMSampler.sample takes and the DDPM and DPM-Solver++ samplers have no counterpart for, with the value that means "not used"
+_DDIM_ONLY = dict(mask=None, x0=None, eta=0., temperature=1., noise_dropout=0.)
+
+
+def _refuse_ddim_only(kwargs: dict, sampler: str, why: str):
+    """pop _DDIM_ONLY's arguments from a sample() call's ``kwargs``: ValueError "<name>=<value>: <why with the name>" for the first one
+    that is used, TypeError for anything else left"""
+    for name, off in _DDIM_ONLY.items():
+        v = kwargs.pop(name, off)
+        if off is None:
+            bad = v is not None
+        else:
+            bad = isinstance(v, bool) or not isinstance(v, (int, float)) or v != off
+        if bad:
+            raise ValueError(f"{name}={v!r}: {why.format(name)}")
+    if kwargs:
+        raise TypeError(f"{sampler}.sample got unexpected arguments {sorted(kwargs)}")
+
+
+def _conditioning(c, conditioning):
+    """``c``, which may also be given as the reference's ``conditioning``"""
+    if conditioning is None:
+        return c
+    if c is not None:
+        raise TypeError("give the conditioning as c or as conditioning, not both")
+    return conditioning
+
+
+def _finite_scale(scale):
+    if isinstance(scale, bool) or not isinstance(scale, (int, float, np.floating)) or not np.isfinite(scale):
+        raise ValueError(f"unconditional_guidance_scale={scale!r} must be a finite number")
+    return scale
+
+
+# --------------------------------------------------------------------------------------------------
+# DDIM sampler
+# --------------------------------------------------------------------------------------------------
+class DDIMSampler(_DeviceLoopSampler):
     def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=True):
         if ddim_discretize != "uniform":
             raise NotImplementedError(f'There is no ddim discretization method called "{ddim_discretize}"')
@@ -484,23 +628,10 @@ class DDIMSampler(object):
         sess.set_ddim_schedule(self.ddim_alphas, self.ddim_alphas_prev, self.ddim_sigmas, self.ddim_sqrt_one_minus_alphas)
         return x, cfg_on, sess, time_range
 
-    def _load_session(self, w, c, shape, x_T, scale, uc, time_range):
-        """x_T (drawn when not given), whether classifier-free guidance is on, and the session of this shape with the timestep table
-        (row i = time_range[i], the i-th loop iteration), context, audio and x loaded, its step counter at 0."""
-        model = self.model
-        dev = self.device
-        B, Cz, Lz = shape
-        x = torch.randn(shape, device=dev) if x_T is None else x_T.to(dev, torch.float32)
-        cfg_on = not (uc is None or scale == 1.)
-        Beff = 2 * B if cfg_on else B
-        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False)
-        sess.set_timestep_table(time_range.copy())
-        # ddim.py:170-174 concatenates [uc, c] and [w, w]; here the two halves are written straight into their rows
-        sess.set_context([uc, c] if cfg_on else c)
-        sess.set_audio(list(w)[-model.cfg.unet.levels:], dup=cfg_on)
-        sess.load_x(x, dup=cfg_on)
-        sess.set_step(0)
-        return x, cfg_on, sess, time_range
+    def _empty_request(self, shape, x_T):
+        """the result of a request whose timestep subset is empty: x_T (drawn when not given), which is also both intermediate lists"""
+        x = self._x_T(shape, x_T)
+        return x, {'x_inter': [x], 'pred_x0': [x]}
 
     @torch.no_grad()
     def ddim_sampling(self, w, c, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None, mask=None, x0=None,
@@ -515,111 +646,68 @@ class DDIMSampler(object):
         B, Cz, Lz = shape
         ts = self._schedule_subset(timesteps, ddim_use_original_steps)
         if ts.shape[0] == 0:
-            x = torch.randn(shape, device=dev) if x_T is None else x_T.to(dev, torch.float32)
-            return x, {'x_inter': [x], 'pred_x0': [x]}
+            return self._empty_request(shape, x_T)
         # the reference draws (and, with noise_dropout, masks) noise every step even when sigma == 0 (ddim.py:192-194); the
         # draw is skipped here unless it can change the result or the caller asks for the same global-RNG consumption
-        match_rng = bool(match_reference_rng)
+        has_noise = bool(np.any(np.asarray(self.ddim_sigmas) != 0))
+        blend, draw = mask is not None, has_noise or bool(match_reference_rng)
         with eng.lock:
             x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, unconditional_guidance_scale, unconditional_conditioning,
                                                              ts)
             total = time_range.shape[0]
             # pred_x0 and the noise of a step: channels-last rows [B*Lz, Cz]
             pred = torch.empty(B * Lz, Cz, device=dev)
-            has_noise = bool(np.any(np.asarray(self.ddim_sigmas) != 0))
             noise_nlc = torch.empty(B * Lz, Cz, device=dev) if has_noise else None
             tail = sess.ddim_tail(B, total, cfg_on, unconditional_guidance_scale, temperature, _ptr(pred),
                                   _ptr(noise_nlc) if has_noise else 0)
+            device_loop = takes_device_loop(shape, x.device, mask, x0, callback, img_callback)
+            # the device loop: mugd_sample, n x {graph replay, CFG/DDIM update, step advance}.  Inpainting and eta > 0 draw a call's
+            # random numbers up front, in the per-step loop's order, and stage them in front of every step (mugd_sample_staged);
+            # match_reference_rng alone only draws and discards.
+            stage, q_tab, n_tab, qcoef = None, None, None, None
+            per_call = max(1, STAGE_TABLE_BYTES // (4 * B * Cz * Lz))
+            if device_loop and (blend or has_noise):
+                stage = sess.ddim_stage(B, cfg_on, _ptr(noise_nlc) if has_noise else 0)
+                tab_steps = min(per_call, total)
+                if blend:
+                    x0c = x0.contiguous()
+                    mask_e = mask.expand(shape).contiguous()                    # the blend's mask, expanded once per request
+                    q_tab = torch.empty((tab_steps,) + tuple(shape), device=dev)
+                    qcoef = q_coef_table(model, time_range)
+                    stage.x0, stage.mask, stage.q_noise = _ptr(x0c), _ptr(mask_e), _ptr(q_tab)
+                if has_noise:
+                    n_tab = torch.empty((tab_steps,) + tuple(shape), device=dev)
+                    stage.noise = _ptr(n_tab)
 
-            intermediates = {'x_inter': [x], 'pred_x0': [x]}
-            iterator = time_range
-            if progress:
-                cls = tqdm_class if tqdm_class is not None else _tqdm
-                if cls is not None:
-                    iterator = cls(time_range, desc='Charting, using DDIM Sampler', total=total)
-
-            def current_x():
-                return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
-
-            def current_pred():
-                return eng.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
-
-            if takes_device_loop(shape, x.device, mask, x0, callback, img_callback):
-                # nothing on the host between steps: run the stretches between two recorded intermediates from one C call each
-                # (mugd_sample: n x {graph replay, CFG/DDIM update, step advance}, no synchronisation).  Inpainting and eta > 0 draw a
-                # stretch's random numbers up front, in the per-step loop's order, and stage them in front of every step
-                # (mugd_sample_staged); match_reference_rng alone only draws and discards.
-                blend = mask is not None
-                draw = has_noise or match_rng
-                stage, q_tab, n_tab, qcoef = None, None, None, None
-                per_call = max(1, STAGE_TABLE_BYTES // (4 * B * Cz * Lz))
-                if blend or has_noise:
-                    stage = sess.ddim_stage(B, cfg_on, _ptr(noise_nlc) if has_noise else 0)
-                    tab_steps = min(per_call, total)
+            def launch(first, n):
+                if blend or draw:
+                    draw_step_noise(n, shape, x0, q_tab, draw, n_tab, noise_dropout, dev)
+                if stage is None:
+                    sess.plan.launch(n, tail)
+                else:
                     if blend:
-                        x0c = x0.contiguous()
-                        mask_e = mask.expand(shape).contiguous()                # the blend's mask, expanded once per request
-                        q_tab = torch.empty((tab_steps,) + tuple(shape), device=dev)
-                        sac, s1m = model.sqrt_alphas_cumprod.cpu(), model.sqrt_one_minus_alphas_cumprod.cpu()
-                        qcoef = np.ascontiguousarray(np.stack([sac[time_range.copy()].numpy(), s1m[time_range.copy()].numpy()], 1),
-                                                     dtype=np.float32)
-                        stage.x0, stage.mask, stage.q_noise = _ptr(x0c), _ptr(mask_e), _ptr(q_tab)
-                    if has_noise:
-                        n_tab = torch.empty((tab_steps,) + tuple(shape), device=dev)
-                        stage.noise = _ptr(n_tab)
-                it = iter(iterator)
-                i = 0
-                while i < total:
-                    j = i
-                    while not ((total - j - 1) % log_every_t == 0 or (total - j - 1) == total - 1):
-                        j += 1
-                    k = i
-                    while k <= j:
-                        n = min(per_call, j - k + 1)
-                        if blend or draw:
-                            draw_step_noise(n, shape, x0, q_tab, draw, n_tab, noise_dropout, dev)
-                        if stage is None:
-                            sess.plan.launch(n, tail)
-                        else:
-                            if blend:
-                                stage.q_coef = qcoef[k:].ctypes.data
-                            sess.plan.launch(n, tail, stage)
-                        k += n
-                    for _ in range(j - i + 1):
-                        next(it, None)                                          # keeps a progress bar (tqdm_class) moving
-                    intermediates['x_inter'].append(current_x())
-                    intermediates['pred_x0'].append(current_pred())
-                    i = j + 1
-                for _ in it:
-                    pass
-                self.last_launches_per_step = sess.plan.launches + (3 if stage is not None else 2)
-            else:
-                for i, step in enumerate(iterator):
-                    index = total - i - 1
-                    if mask is not None:
-                        assert x0 is not None
-                        tsb = torch.full((B,), int(step), device=dev, dtype=torch.long)
-                        x_orig = model.q_sample(x0.to(dev), tsb)
-                        xm = x_orig * mask + (1. - mask) * current_x()
-                        sess.load_x(xm, dup=cfg_on)
-                    if has_noise or match_rng:
-                        nz = torch.randn(shape, device=dev)                      # ddim.py:192
-                        if noise_dropout > 0.:
-                            # dropout(sigma * n * T) == sigma * T * dropout(n): same Bernoulli draw, same 1/(1-p) scale (:193-194)
-                            nz = torch.nn.functional.dropout(nz, p=noise_dropout)
-                    if has_noise:
-                        eng.ncl_to_rows(nz, View(_ptr(noise_nlc), Cz, B * Lz, Cz))
-                    sess.eval(graph=True)
-                    eng.run_ops(tail)
-                    if callback:
-                        callback(i)
-                    if img_callback:
-                        img_callback(current_pred(), i)
-                    if index % log_every_t == 0 or index == total - 1:
-                        intermediates['x_inter'].append(current_x())
-                        intermediates['pred_x0'].append(current_pred())
-                self.last_launches_per_step = sess.plan.launches + 2
-            return current_x(), intermediates
+                        stage.q_coef = qcoef[first:].ctypes.data
+                    sess.plan.launch(n, tail, stage)
+
+            def step(i, t):
+                if blend:
+                    assert x0 is not None
+                    tsb = torch.full((B,), int(t), device=dev, dtype=torch.long)
+                    x_orig = model.q_sample(x0.to(dev), tsb)
+                    sess.load_x(x_orig * mask + (1. - mask) * self._read_x(sess, shape), dup=cfg_on)
+                if draw:
+                    nz = torch.randn(shape, device=dev)                          # ddim.py:192
+                    if noise_dropout > 0.:
+                        # dropout(sigma * n * T) == sigma * T * dropout(n): same Bernoulli draw, same 1/(1-p) scale (:193-194)
+                        nz = torch.nn.functional.dropout(nz, p=noise_dropout)
+                if has_noise:
+                    eng.ncl_to_rows(nz, View(_ptr(noise_nlc), Cz, B * Lz, Cz))
+                sess.eval(graph=True)
+                eng.run_ops(tail)
+
+            return self._run_request(sess, x, shape, pred, time_range, total, log_every_t, 'Charting, using DDIM Sampler', tqdm_class,
+                                     progress, callback, img_callback, device_loop, launch, step, 3 if stage is not None else 2,
+                                     chunk=per_call)
 
     # ---- remixing an existing chart (SDEdit / img2img): stochastic_encode + decode, as upstream Stable Diffusion's DDIMSampler --------
     def _require_schedule(self, what: str):
@@ -733,11 +821,9 @@ class DDIMSampler(object):
                 joins = torch.tensor([m - s for s in starts], dtype=torch.int32, device=dev)
                 sess.plan.launch_join(sess.join(B, cfg_on, _ptr(xl), _ptr(joins)), tail, 0, m)
                 self.last_launches_per_step = sess.plan.launches + 3
-            cls = tqdm_class if tqdm_class is not None else _tqdm
-            if cls is not None:
-                for _ in cls(time_range, desc='Decoding image', total=m):      # keeps a progress bar moving
-                    pass
-            z = sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+            for _ in self._progress(time_range, 'Decoding image', m, tqdm_class):      # keeps a progress bar moving
+                pass
+            z = self._read_x(sess, shape)
             idle = [b for b, s in enumerate(starts) if s == 0]
             if idle:
                 z[idle] = x[idle]
@@ -800,10 +886,7 @@ class PLMSSampler(DDIMSampler):
         reference's noise_like receives a [B, B, C, L] shape from its [b, 1, 1, 1] coefficients, this draws [B, C, L])."""
         if eta != 0:
             raise ValueError('ddim_eta must be 0 for PLMS')
-        if conditioning is not None:
-            if c is not None:
-                raise TypeError("give the conditioning as c or as conditioning, not both")
-            c = conditioning
+        c = _conditioning(c, conditioning)
         size = self._check_request(S, c, w, batch_size, shape, x_T, mask, x0, unconditional_guidance_scale, unconditional_conditioning,
                                    log_every_t)
         self.make_schedule(ddim_num_steps=S, ddim_eta=eta, verbose=verbose)
@@ -839,8 +922,7 @@ class PLMSSampler(DDIMSampler):
         B, Cz, Lz = shape
         ts = self._schedule_subset(timesteps, ddim_use_original_steps)
         if ts.shape[0] == 0:
-            x = torch.randn(shape, device=dev) if x_T is None else x_T.to(dev, torch.float32)
-            return x, {'x_inter': [x], 'pred_x0': [x]}
+            return self._empty_request(shape, x_T)
         match_rng = bool(match_reference_rng)
         scale = unconditional_guidance_scale
 
@@ -856,92 +938,50 @@ class PLMSSampler(DDIMSampler):
             work = torch.empty(5, B * Lz * Cz, device=dev)                    # e', the e_t ring [3], the x stash
             plms = sess.plms(B, total, cfg_on, scale, _ptr(pred), work)
 
-            intermediates = {'x_inter': [x], 'pred_x0': [x]}
-            iterator = time_range
-            if progress:
-                cls = tqdm_class if tqdm_class is not None else _tqdm
-                if cls is not None:
-                    iterator = cls(time_range, desc='Charting, using PLMS Sampler', total=total)
+            def launch(first, n):
+                # the e_t ring and the step counter stay on the device, so a call may start inside the warm-up
+                draw(n + (first == 0))
+                sess.plan.launch_plms(plms, first, n)
 
-            def current_x():
-                return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+            # the per-step loop runs the same kernels: the referee of the device loop
+            update = OpList()
+            update.add(L_.OP_DDIM_UPDATE, plms.update)
+            tail = _step_ops(sess, plms.update)
+            stream = torch.cuda.current_stream().cuda_stream
 
-            def current_pred():
-                return eng.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
-
-            def logged(i):
-                index = total - i - 1
-                return index % log_every_t == 0 or index == total - 1              # plms.py:166
-
-            if callback is None and img_callback is None and mask is None:
-                # one mugd_sample_plms call per stretch between two recorded intermediates: the e_t ring and the step counter stay on
-                # the device, so a call may start inside the warm-up
-                it = iter(iterator)
-                i = 0
-                while i < total:
-                    j = i
-                    while not logged(j):
-                        j += 1
-                    draw(j - i + 1 + (i == 0))
-                    sess.plan.launch_plms(plms, i, j - i + 1)
-                    for _ in range(j - i + 1):
-                        next(it, None)                                          # keeps a progress bar (tqdm_class) moving
-                    intermediates['x_inter'].append(current_x())
-                    intermediates['pred_x0'].append(current_pred())
-                    i = j + 1
-                for _ in it:
-                    pass
-            else:
-                # one step at a time from the same kernels: the referee of the device loop
-                update = OpList()
-                update.add(L_.OP_DDIM_UPDATE, plms.update)
-                adv = L_.StepAdvance()
-                adv.step = _ptr(sess.step)
-                tail = OpList()
-                tail.add(L_.OP_DDIM_UPDATE, plms.update)
-                tail.add(L_.OP_STEP_ADVANCE, adv)
-                stream = torch.cuda.current_stream().cuda_stream
-                for i, step in enumerate(iterator):
-                    if mask is not None:
-                        assert x0 is not None
-                        tsb = torch.full((B,), int(step), device=dev, dtype=torch.long)
-                        x_orig = model.q_sample(x0.to(dev), tsb)                    # plms.py:147-150
-                        sess.load_x(x_orig * mask + (1. - mask) * current_x(), dup=cfg_on)
-                    sess.eval(graph=True)
-                    L_.check(eng.lib.mugd_plms_combine(C.byref(plms), i, 0, stream), "mugd_plms_combine")
-                    if i == 0:
-                        x_t = current_x()                                       # pseudo improved Euler, plms.py:219-223
-                        draw(1)
-                        eng.run_ops(update)                                     # x_prev of e_t into both halves
-                        sess.set_step(1 if total > 1 else 0)                    # t_next, plms.py:145
-                        sess.eval(graph=True)
-                        sess.load_x(x_t, dup=False)
-                        L_.check(eng.lib.mugd_plms_combine(C.byref(plms), 0, 1, stream), "mugd_plms_combine")
-                        sess.set_step(0)
+            def step(i, t):
+                if mask is not None:
+                    assert x0 is not None
+                    tsb = torch.full((B,), int(t), device=dev, dtype=torch.long)
+                    x_orig = model.q_sample(x0.to(dev), tsb)                    # plms.py:147-150
+                    sess.load_x(x_orig * mask + (1. - mask) * self._read_x(sess, shape), dup=cfg_on)
+                sess.eval(graph=True)
+                L_.check(eng.lib.mugd_plms_combine(C.byref(plms), i, 0, stream), "mugd_plms_combine")
+                if i == 0:
+                    x_t = self._read_x(sess, shape)                             # pseudo improved Euler, plms.py:219-223
                     draw(1)
-                    eng.run_ops(tail)
-                    if callback:
-                        callback(i)
-                    if img_callback:
-                        img_callback(current_pred(), i)
-                    if logged(i):
-                        intermediates['x_inter'].append(current_x())
-                        intermediates['pred_x0'].append(current_pred())
-            self.last_launches_per_step = sess.plan.launches + 3
-            return current_x(), intermediates
+                    eng.run_ops(update)                                         # x_prev of e_t into both halves
+                    sess.set_step(1 if total > 1 else 0)                        # t_next, plms.py:145
+                    sess.eval(graph=True)
+                    sess.load_x(x_t, dup=False)
+                    L_.check(eng.lib.mugd_plms_combine(C.byref(plms), 0, 1, stream), "mugd_plms_combine")
+                    sess.set_step(0)
+                draw(1)
+                eng.run_ops(tail)
+
+            device_loop = callback is None and img_callback is None and mask is None
+            return self._run_request(sess, x, shape, pred, time_range, total, log_every_t, 'Charting, using PLMS Sampler', tqdm_class,
+                                     progress, callback, img_callback, device_loop, launch, step, 3)
 
 
 # --------------------------------------------------------------------------------------------------
 # DDPM sampler
 # --------------------------------------------------------------------------------------------------
-class DDPMSampler(DDIMSampler):
+class DDPMSampler(_DeviceLoopSampler):
     """The reference's ancestral DDPM loop, the one its DDPM.log_beatmap runs (mug/diffusion/diffusion.py:255-282): all
     ``num_timesteps`` steps, each drawing fresh noise, with the model's posterior tables.  Same constructor as DDIMSampler; each step
     is one batched U-Net evaluation and one update kernel.  Classifier-free guidance is an extension (the reference's loop has
     none): with it, e = e_u + scale * (e_c - e_u) as in DDIM (ddim.py:170-175) before the posterior step."""
-
-    # what DDIMSampler.sample takes and the reference's DDPM loop has no counterpart for, with the value that means "not used"
-    _NOT_IN_DDPM = dict(mask=None, x0=None, eta=0., temperature=1., noise_dropout=0.)
 
     @torch.no_grad()
     def sample(self, c, w, batch_size, shape=None, x_T=None, callback=None, img_callback=None, log_every_t=100, clip_denoised=None,
@@ -950,32 +990,20 @@ class DDPMSampler(DDIMSampler):
         model's).  ``clip_denoised=None`` takes the model's.  Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then the x and
         x_recon of every step whose timestep i has ``i % log_every_t == 0 or i == T - 1`` (diffusion.py:279).  Every argument is
         checked before any GPU work; ``S`` (if given) must be T, and inpainting, eta, temperature and noise dropout are refused.
-        Without callbacks the steps run from mugd_sample_ddpm calls, one per stretch between two recorded intermediates (split so
-        that no noise table exceeds STAGE_TABLE_BYTES), each stretch's noise drawn up front in the per-step order; with
-        ``callback`` / ``img_callback`` they run one by one.  Both draw one randn(shape) per step from the device's generator (and
-        x_T first when it is not given), as the reference does."""
+        Without callbacks the steps run from mugd_sample_ddpm calls (each call's noise table at most STAGE_TABLE_BYTES), with them
+        one by one.  Both draw one randn(shape) per step from the device's generator (and x_T first when it is not given), as the
+        reference does."""
         T = self.ddpm_num_timesteps
         S = kwargs.pop("S", None)
         if S is not None and (isinstance(S, bool) or S != T):
             raise ValueError(f"S={S!r}: the DDPM sampler runs all T={T} steps of the model's schedule")
-        for name, off in self._NOT_IN_DDPM.items():
-            v = kwargs.pop(name, off)
-            if off is None:
-                bad = v is not None
-            else:
-                bad = isinstance(v, bool) or not isinstance(v, (int, float)) or v != off
-            if bad:
-                raise ValueError(f"{name}={v!r}: the reference's DDPM loop has no {name}")
-        if kwargs:
-            raise TypeError(f"DDPMSampler.sample got unexpected arguments {sorted(kwargs)}")
+        _refuse_ddim_only(kwargs, "DDPMSampler", "the reference's DDPM loop has no {}")
         if c is None or w is None:
             raise TypeError("DDPMSampler.sample needs the conditioning c and the audio features w")
         clip = self.model.clip_denoised if clip_denoised is None else clip_denoised
         if clip not in (True, False):
             raise ValueError(f"clip_denoised={clip_denoised!r} must be True, False or None")
-        scale = unconditional_guidance_scale
-        if isinstance(scale, bool) or not isinstance(scale, (int, float, np.floating)) or not np.isfinite(scale):
-            raise ValueError(f"unconditional_guidance_scale={scale!r} must be a finite number")
+        scale = _finite_scale(unconditional_guidance_scale)
         size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
         if verbose:
             print(f'Data shape for DDPM sampling is {size}, {T} steps')
@@ -1001,66 +1029,24 @@ class DDPMSampler(DDIMSampler):
             table = torch.empty((min(per_call, T),) + tuple(shape), device=dev)
             ddpm = sess.ddpm(B, T, cfg_on, scale, clip_denoised, _ptr(pred), _ptr(table), coef)
 
-            intermediates = {'x_inter': [x], 'pred_x0': [x]}
-            iterator = time_range
-            if progress:
-                cls = tqdm_class if tqdm_class is not None else _tqdm
-                if cls is not None:
-                    iterator = cls(time_range, desc='Sampling t', total=T)
+            def launch(first, n):
+                # the noise of a call is drawn up front, in the per-step loop's order
+                draw_step_noise(n, shape, None, None, True, table, 0., dev)
+                sess.plan.launch_ddpm(ddpm, first, n)
 
-            def current_x():
-                return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+            # the per-step loop runs the same kernel: the referee of the device loop
+            advance = _step_ops(sess)
+            stream = torch.cuda.current_stream().cuda_stream
 
-            def current_pred():
-                return eng.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
+            def step(i, t):
+                sess.eval(graph=True)
+                draw_step_noise(1, shape, None, None, True, table, 0., dev)       # noise_like, diffusion.py:274
+                L_.check(eng.lib.mugd_ddpm_update(C.byref(ddpm), stream), "mugd_ddpm_update")
+                eng.run_ops(advance)
 
-            def logged(i):
-                t = T - 1 - i
-                return t % log_every_t == 0 or t == T - 1                      # diffusion.py:279
-
-            if callback is None and img_callback is None:
-                # one mugd_sample_ddpm call per stretch between two recorded intermediates (more when a stretch's noise would exceed
-                # STAGE_TABLE_BYTES); the noise of a call is drawn up front, in the per-step loop's order
-                it = iter(iterator)
-                i = 0
-                while i < T:
-                    j = i
-                    while not logged(j):
-                        j += 1
-                    k = i
-                    while k <= j:
-                        n = min(per_call, j - k + 1)
-                        draw_step_noise(n, shape, None, None, True, table, 0., dev)
-                        sess.plan.launch_ddpm(ddpm, k, n)
-                        k += n
-                    for _ in range(j - i + 1):
-                        next(it, None)                                          # keeps a progress bar (tqdm_class) moving
-                    intermediates['x_inter'].append(current_x())
-                    intermediates['pred_x0'].append(current_pred())
-                    i = j + 1
-                for _ in it:
-                    pass
-            else:
-                # one step at a time from the same kernel: the referee of the device loop
-                adv = L_.StepAdvance()
-                adv.step = _ptr(sess.step)
-                advance = OpList()
-                advance.add(L_.OP_STEP_ADVANCE, adv)
-                stream = torch.cuda.current_stream().cuda_stream
-                for i, _ in enumerate(iterator):
-                    sess.eval(graph=True)
-                    draw_step_noise(1, shape, None, None, True, table, 0., dev)   # noise_like, diffusion.py:274
-                    L_.check(eng.lib.mugd_ddpm_update(C.byref(ddpm), stream), "mugd_ddpm_update")
-                    eng.run_ops(advance)
-                    if callback:
-                        callback(i)
-                    if img_callback:
-                        img_callback(current_pred(), i)
-                    if logged(i):
-                        intermediates['x_inter'].append(current_x())
-                        intermediates['pred_x0'].append(current_pred())
-            self.last_launches_per_step = sess.plan.launches + 2
-            return current_x(), intermediates
+            # log_every_t's rule on timestep T - 1 - i is diffusion.py:279's on step i
+            return self._run_request(sess, x, shape, pred, time_range, T, log_every_t, 'Sampling t', tqdm_class, progress, callback,
+                                     img_callback, callback is None and img_callback is None, launch, step, 2, chunk=per_call)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -1071,15 +1057,12 @@ def alphas_cumprod_f64(cfg: ModelConfig) -> np.ndarray:
     return np.cumprod(1. - beta_schedule_linear(cfg.timesteps, cfg.linear_start, cfg.linear_end), axis=0)
 
 
-class DPMSolverSampler(DDIMSampler):
+class DPMSolverSampler(_DeviceLoopSampler):
     """DPM-Solver++ multistep (Lu et al., 2022): a 1st- to 3rd-order solver of the probability-flow ODE in data-prediction form, the
     ``DPMSolverSampler`` of Stable Diffusion 2 with the ``sample(S, ...)`` shape of DDIMSampler and PLMSSampler.  15-25 steps of
     order 2 are the usual replacement for 50-100 DDIM steps.  Same constructor as DDIMSampler; each step is one batched U-Net
     evaluation at a float model time and one update kernel (csrc/dpm.cu) whose coefficient rows come from ``dpm_solver``.
     Deterministic (no noise is drawn apart from x_T when it is not given)."""
-
-    # what DDIMSampler.sample takes and the deterministic multistep solver has no counterpart for, with the value that means "not used"
-    _NOT_IN_DPM = dict(mask=None, x0=None, eta=0., temperature=1., noise_dropout=0.)
 
     def make_dpm_schedule(self, S, order=2, skip_type="time_uniform", solver_type="dpmsolver", lower_order_final=True,
                           t_grid=None) -> dpm_solver.DPMSchedule:
@@ -1109,27 +1092,12 @@ class DPMSolverSampler(DDIMSampler):
         ``conditioning``.  Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then x and the data prediction m of every step i with
         ``(S - i - 1) % log_every_t == 0`` or i = 0 (DDIM's rule).  Every argument is checked before any GPU work (ValueError; TypeError
         for missing or unknown ones); inpainting (mask / x0), eta, temperature and noise dropout are refused.  Without callbacks the
-        steps run from mugd_sample_dpm calls, one per stretch between two recorded intermediates; with ``callback`` / ``img_callback``
-        they run one by one through mugd_dpm_update."""
-        for name, off in self._NOT_IN_DPM.items():
-            v = kwargs.pop(name, off)
-            if off is None:
-                bad = v is not None
-            else:
-                bad = isinstance(v, bool) or not isinstance(v, (int, float)) or v != off
-            if bad:
-                raise ValueError(f"{name}={v!r}: DPM-Solver++ multistep is a deterministic solver without {name}")
-        if kwargs:
-            raise TypeError(f"DPMSolverSampler.sample got unexpected arguments {sorted(kwargs)}")
-        if conditioning is not None:
-            if c is not None:
-                raise TypeError("give the conditioning as c or as conditioning, not both")
-            c = conditioning
+        steps run from mugd_sample_dpm calls, with them one by one through mugd_dpm_update."""
+        _refuse_ddim_only(kwargs, "DPMSolverSampler", "DPM-Solver++ multistep is a deterministic solver without {}")
+        c = _conditioning(c, conditioning)
         if c is None or w is None:
             raise TypeError("DPMSolverSampler.sample needs the conditioning c and the audio features w")
-        scale = unconditional_guidance_scale
-        if isinstance(scale, bool) or not isinstance(scale, (int, float, np.floating)) or not np.isfinite(scale):
-            raise ValueError(f"unconditional_guidance_scale={scale!r} must be a finite number")
+        scale = _finite_scale(unconditional_guidance_scale)
         sched = self.make_dpm_schedule(S, order, skip_type, solver_type, lower_order_final)
         size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
         if verbose:
@@ -1156,57 +1124,19 @@ class DPMSolverSampler(DDIMSampler):
             pred = torch.empty(B * Lz, Cz, device=dev)
             dpm = sess.dpm(B, total, cfg_on, scale, _ptr(pred), ring, coef)
 
-            intermediates = {'x_inter': [x], 'pred_x0': [x]}
-            iterator = time_range
-            if progress:
-                cls = tqdm_class if tqdm_class is not None else _tqdm
-                if cls is not None:
-                    iterator = cls(time_range, desc='Charting, using DPM-Solver++ Sampler', total=total)
+            def launch(first, n):
+                # the ring and the step counter stay on the device, so a call may start inside the warm-up
+                sess.plan.launch_dpm(dpm, first, n)
 
-            def current_x():
-                return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+            # the per-step loop runs the same kernel: the referee of the device loop
+            advance = _step_ops(sess)
+            stream = torch.cuda.current_stream().cuda_stream
 
-            def current_pred():
-                return eng.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
+            def step(i, t):
+                sess.eval(graph=True)
+                L_.check(eng.lib.mugd_dpm_update(C.byref(dpm), stream), "mugd_dpm_update")
+                eng.run_ops(advance)
 
-            def logged(i):
-                index = total - i - 1
-                return index % log_every_t == 0 or index == total - 1              # DDIM's rule, ddim.py:154
-
-            if callback is None and img_callback is None:
-                # one mugd_sample_dpm call per stretch between two recorded intermediates: the ring and the step counter stay on the
-                # device, so a call may start inside the warm-up
-                it = iter(iterator)
-                i = 0
-                while i < total:
-                    j = i
-                    while not logged(j):
-                        j += 1
-                    sess.plan.launch_dpm(dpm, i, j - i + 1)
-                    for _ in range(j - i + 1):
-                        next(it, None)                                          # keeps a progress bar (tqdm_class) moving
-                    intermediates['x_inter'].append(current_x())
-                    intermediates['pred_x0'].append(current_pred())
-                    i = j + 1
-                for _ in it:
-                    pass
-            else:
-                # one step at a time from the same kernel: the referee of the device loop
-                adv = L_.StepAdvance()
-                adv.step = _ptr(sess.step)
-                advance = OpList()
-                advance.add(L_.OP_STEP_ADVANCE, adv)
-                stream = torch.cuda.current_stream().cuda_stream
-                for i, _ in enumerate(iterator):
-                    sess.eval(graph=True)
-                    L_.check(eng.lib.mugd_dpm_update(C.byref(dpm), stream), "mugd_dpm_update")
-                    eng.run_ops(advance)
-                    if callback:
-                        callback(i)
-                    if img_callback:
-                        img_callback(current_pred(), i)
-                    if logged(i):
-                        intermediates['x_inter'].append(current_x())
-                        intermediates['pred_x0'].append(current_pred())
-            self.last_launches_per_step = sess.plan.launches + 2
-            return current_x(), intermediates
+            return self._run_request(sess, x, shape, pred, time_range, total, log_every_t, 'Charting, using DPM-Solver++ Sampler',
+                                     tqdm_class, progress, callback, img_callback, callback is None and img_callback is None, launch,
+                                     step, 2)
