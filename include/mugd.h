@@ -359,6 +359,32 @@ int  mugd_sample_dpm(mugd_plan* eval_plan, const mugd_dpm* d, int32_t first_step
 /* the update kernel alone (the counter not advanced), for a host that runs the DPM-Solver++ steps one by one */
 int  mugd_dpm_update(const mugd_dpm* d, void* stream);
 
+/* ---- DPM-Solver++ from an existing chart: inpainting and per-chart-strength remix ---------------------------------------------
+ * mugd_dpm_ex extends a mugd_dpm request by one of:
+ *   stage  inpainting: step k of a mugd_sample_dpm_ex call first runs the mugd_sample_staged stage kernel for row k of the stage's
+ *          tables (x <- (alpha_i * x0 + sigma_i * q_noise[k]) * mask + (1 - mask) * x with q_coef[k] = (alpha_i, sigma_i) of the step);
+ *          the stage must blend the update's x / x_dup over n = B*C*L elements and stage no step noise.
+ *   start  remix: chart b (elements b * n/B .. (b+1) * n/B - 1 of the dense rows) runs from step start[b] on; before that it is left
+ *          untouched (x, x_dup, ring and pred_x0), so its rows keep the latent they were loaded with.  From step start[b] on chart b
+ *          takes order k = min(coef row i's order, i - start[b] + 1) and applies row (i, k - 1) = order_coef[8 (3i + k - 1) ..] of the
+ *          per-order table [S][3][8] (same layout as coef; row (i, order_i - 1) equals coef row i), reading only the ring slots of its
+ *          own steps.  Everything else is the mugd_dpm update, bit for bit.
+ * Neither (both NULL) is mugd_sample_dpm.  stage and start are exclusive; start and order_coef go together. */
+typedef struct mugd_dpm_ex {
+    mugd_dpm dpm;                          /* the update (coef [S][8], ring, step counter, ...)                                 */
+    const mugd_stage* stage;               /* inpainting blend in front of each step, or NULL                                  */
+    const int32_t* start;                  /* [B] device: the first step of each chart, or NULL                                */
+    const float* order_coef;               /* [S][3][8] device per-order rows, given exactly with start                         */
+    int32_t B, reserved_;                  /* charts (with start)                                                              */
+} mugd_dpm_ex;
+/* steps first_step .. first_step + n_steps - 1 of the S-step request (the counter holding first_step), no host synchronisation:
+ * n_steps x { stage kernel (with stage) ; graph replay ; update ; *step += 1 }: with a stage the launches per step of
+ * mugd_sample_staged, otherwise those of mugd_sample_dpm.  Every argument is checked before the first launch (first_step + n_steps <=
+ * S, the stage's q_coef rows finite).  A standalone entry point: the ABI version is unchanged. */
+int  mugd_sample_dpm_ex(mugd_plan* eval_plan, const mugd_dpm_ex* e, int32_t first_step, int32_t n_steps, void* stream);
+/* the update alone for the counter's step (per chart with start; the stage is not run), for a host that runs the steps one by one */
+int  mugd_dpm_ex_update(const mugd_dpm_ex* e, void* stream);
+
 /* ---- remixing an existing chart (SDEdit / img2img): DDIMSampler.stochastic_encode and decode with a per-chart start ---------------
  * mugd_stochastic_encode: out[b] = sqrt_a[t[b]] * x0[b] + sqrt_1ma[t[b]] * noise[b], each product and the sum one IEEE
  * round-to-nearest (no contraction), bit-identical to torch's extract_into_tensor expressions.  x0, noise and out are device NCL

@@ -324,6 +324,27 @@ int mugd_sample_dpm(mugd_plan* eval_plan, const mugd_dpm* d, int32_t first_step,
     return MUGD_OK;
 }
 
+int mugd_sample_dpm_ex(mugd_plan* eval_plan, const mugd_dpm_ex* e, int32_t first_step, int32_t n_steps, void* stream) {
+    // the descriptor is checked before the plan, so a host can test its arguments without a device
+    MUGD_REQUIRE(e, "mugd_sample_dpm_ex: null descriptor");
+    int rc = check_dpm_ex(*e, n_steps);
+    if (rc != MUGD_OK) return rc;
+    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= e->dpm.S,
+                 "mugd_sample_dpm_ex: first_step=%d, n_steps=%d outside the S=%d steps of the request", first_step, n_steps, e->dpm.S);
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_dpm_ex: the evaluation plan must be captured (mugd_plan_capture)");
+    const DeviceInfo& dev = eval_plan->h->dev;
+    cudaStream_t st = (cudaStream_t)stream;
+    mugd_step_advance adv;
+    adv.step = e->dpm.step;
+    for (int32_t k = 0; k < n_steps; ++k) {
+        if (e->stage && (rc = launch_stage(*e->stage, k, st)) != MUGD_OK) return rc;
+        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
+        if ((rc = launch_dpm_ex_update(*e, st)) != MUGD_OK) return rc;
+        if ((rc = launch_step_advance(dev, adv, st, nullptr)) != MUGD_OK) return rc;
+    }
+    return MUGD_OK;
+}
+
 int mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
                      int32_t n_steps, void* stream) {
     MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_join: the evaluation plan must be captured (mugd_plan_capture)");

@@ -75,6 +75,10 @@ int launch_ddpm_update(const mugd_ddpm& d, int32_t k, cudaStream_t st);
 // mugd_sample_dpm / mugd_dpm_update: check_dpm validates the descriptor; launch_dpm_update runs the update of the counter's step
 int check_dpm(const mugd_dpm& d);
 int launch_dpm_update(const mugd_dpm& d, cudaStream_t st);
+// mugd_sample_dpm_ex / mugd_dpm_ex_update: check_dpm_ex validates the descriptor for a call of n_steps (the stage's host table
+// included); launch_dpm_ex_update runs the update of the counter's step, per-chart when starts are given
+int check_dpm_ex(const mugd_dpm_ex& e, int32_t n_steps);
+int launch_dpm_ex_update(const mugd_dpm_ex& e, cudaStream_t st);
 // mugd_sample_join: check_join validates the descriptor; launch_join runs the join kernel against the device step counter
 int check_join(const mugd_join& j);
 int launch_join(const mugd_join& j, const int32_t* step, cudaStream_t st);

@@ -1,26 +1,19 @@
 // DPM-Solver++ multistep sampler (data prediction, Lu et al. 2022; Stable Diffusion 2's DPM_Solver(predict_x0=True) "multistep"):
-// the update of one step.  The host (mug_diffusion_b200/dpm_solver.py) expands each step into one coefficient row; the loop
-// mugd_sample_dpm lives in api.cu beside mugd_sample; mugd_dpm_update runs the update alone.
+// the update of one step.  The host (mug_diffusion_b200/dpm_solver.py) expands each step into one coefficient row; the loops
+// mugd_sample_dpm / mugd_sample_dpm_ex live in api.cu beside mugd_sample; mugd_dpm_update / mugd_dpm_ex_update run the update alone.
 #include "common.cuh"
 
 namespace mugd {
 
-// One thread per element of the dense [B*L, C] rows.  Step i = *step reads coefficient row i = (alpha, sigma, A, c0, c1, c2, order):
+// The update of element i at step `step` with coefficient row `row` of order `order` (1..3):
 //   e  = eps rows (CFG: e_u + scale * (e_c - e_u), uncond half first, as the DDIM update)
 //   m0 = (x - sigma * e) / alpha                                    the data prediction at t_i
 //   x  = ((A * x + c0 * m0) + c1 * m1) + c2 * m2                      m1 / m2: the predictions of steps i-1 / i-2 (ring slots)
-// in this order, every product, sum and the quotient one IEEE round-to-nearest, no contraction.  Terms past the row's order are not
+// in this order, every product, sum and the quotient one IEEE round-to-nearest, no contraction.  Terms past the order are not
 // formed: their ring slots may not have been written yet (and 0 * NaN is NaN).  x goes to x and x_dup, m0 to pred_x0 and to ring
-// slot i mod 3.  A counter outside [0, S) leaves everything unchanged.
-__global__ void __launch_bounds__(256)
-dpm_update_kernel(const mugd_dpm d) {
-    pdl_wait();
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int step = *d.step;
-    if (i >= d.n || (unsigned)step >= (unsigned)d.S) return;
-    const float* row = d.coef + 8 * (int64_t)step;
+// slot step mod 3.  Both update kernels run this, so a chart computes the same bits in either.
+__device__ __forceinline__ void dpm_element(const mugd_dpm& d, const float* row, int order, int step, int i) {
     const float alpha = row[0], sigma = row[1], A = row[2], c0 = row[3];
-    const int order = (int)row[6];
     const int64_t N = d.n;
     float e;
     if (d.cfg) {
@@ -40,6 +33,34 @@ dpm_update_kernel(const mugd_dpm d) {
     if (d.pred_x0) d.pred_x0[i] = m0;
 }
 
+// One thread per element of the dense [B*L, C] rows.  Step i = *step applies coefficient row i = (alpha, sigma, A, c0, c1, c2,
+// order) with its own order.  A counter outside [0, S) leaves everything unchanged.
+__global__ void __launch_bounds__(256)
+dpm_update_kernel(const mugd_dpm d) {
+    pdl_wait();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int step = *d.step;
+    if (i >= d.n || (unsigned)step >= (unsigned)d.S) return;
+    const float* row = d.coef + 8 * (int64_t)step;
+    dpm_element(d, row, (int)row[6], step, i);
+}
+
+// The same update with one start per chart (the B charts own consecutive blocks of n / B elements): chart b runs from step start[b]
+// on.  Before that it is left untouched (x, x_dup, its ring slots and pred_x0 are neither read nor written), so its rows keep the
+// latent they were loaded with.  From its start on it takes the order min(order of row i, i - start[b] + 1), warming up like a fresh
+// request, and applies row (i, order - 1) of the per-order table [S][3][8]; it reads only the ring slots of its own steps.
+__global__ void __launch_bounds__(256)
+dpm_update_starts_kernel(const mugd_dpm d, const int32_t* __restrict__ start, const float* __restrict__ order_coef, int per_chart) {
+    pdl_wait();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int step = *d.step;
+    if (i >= d.n || (unsigned)step >= (unsigned)d.S) return;
+    const int first = start[i / per_chart];
+    if (step < first) return;
+    const int order = max(1, min(min((int)d.coef[8 * (int64_t)step + 6], step - first + 1), 3));
+    dpm_element(d, order_coef + 8 * (3 * (int64_t)step + order - 1), order, step, i);
+}
+
 int check_dpm(const mugd_dpm& d) {
     MUGD_REQUIRE(d.x && d.eps && d.ring && d.coef && d.step, "dpm: x, eps, ring, coef and step must be given");
     MUGD_REQUIRE(d.n > 0, "dpm: n=%d", d.n);
@@ -55,6 +76,33 @@ int launch_dpm_update(const mugd_dpm& d, cudaStream_t st) {
     return MUGD_OK;
 }
 
+int check_dpm_ex(const mugd_dpm_ex& e, int32_t n_steps) {
+    int rc = check_dpm(e.dpm);
+    if (rc != MUGD_OK) return rc;
+    MUGD_REQUIRE(!e.stage || !e.start, "dpm_ex: a stage (inpainting) and per-chart starts cannot be combined");
+    MUGD_REQUIRE(!e.start == !e.order_coef, "dpm_ex: start and order_coef go together");
+    if (e.start) {
+        MUGD_REQUIRE(e.B > 0 && e.dpm.n % e.B == 0, "dpm_ex: B=%d does not divide n=%d", e.B, e.dpm.n);
+    }
+    if (e.stage) {
+        const mugd_stage& s = *e.stage;
+        if ((rc = check_stage(s, n_steps)) != MUGD_OK) return rc;
+        MUGD_REQUIRE(s.x0, "dpm_ex: the stage has no x0 (a DPM-Solver++ stage is the inpainting blend)");
+        MUGD_REQUIRE(!s.noise, "dpm_ex: the stage stages step noise; DPM-Solver++ draws none");
+        MUGD_REQUIRE(s.x == e.dpm.x && s.x_dup == e.dpm.x_dup, "dpm_ex: the stage blends other rows than the update's x / x_dup");
+        MUGD_REQUIRE((int64_t)s.B * s.C * s.L == e.dpm.n, "dpm_ex: the stage's B*C*L=%lld, the update's n=%d",
+                     (long long)s.B * s.C * s.L, e.dpm.n);
+    }
+    return MUGD_OK;
+}
+
+int launch_dpm_ex_update(const mugd_dpm_ex& e, cudaStream_t st) {
+    if (!e.start) return launch_dpm_update(e.dpm, st);
+    MUGD_CHECK_CUDA(launch_k(dpm_update_starts_kernel, dim3((e.dpm.n + 255) / 256), dim3(256), 0, st, e.dpm, e.start, e.order_coef,
+                             e.dpm.n / e.B));
+    return MUGD_OK;
+}
+
 }  // namespace mugd
 
 using namespace mugd;
@@ -64,4 +112,11 @@ extern "C" int mugd_dpm_update(const mugd_dpm* d, void* stream) {
     int rc = check_dpm(*d);
     if (rc != MUGD_OK) return rc;
     return launch_dpm_update(*d, (cudaStream_t)stream);
+}
+
+extern "C" int mugd_dpm_ex_update(const mugd_dpm_ex* e, void* stream) {
+    MUGD_REQUIRE(e, "mugd_dpm_ex_update: null argument");
+    int rc = check_dpm_ex(*e, 0);
+    if (rc != MUGD_OK) return rc;
+    return launch_dpm_ex_update(*e, (cudaStream_t)stream);
 }

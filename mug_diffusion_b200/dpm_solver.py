@@ -103,6 +103,7 @@ class DPMSchedule:
     model_times: np.ndarray
     rows: np.ndarray
     orders: np.ndarray
+    order_rows: Optional[np.ndarray] = None
 
     @property
     def S(self) -> int:
@@ -111,6 +112,60 @@ class DPMSchedule:
     def rows_f32(self) -> np.ndarray:
         """the rows rounded once to float32, as the kernel reads them"""
         return np.ascontiguousarray(self.rows, dtype=np.float32)
+
+    def order_rows_f32(self) -> np.ndarray:
+        """``order_rows`` [S, 3, 8] rounded once to float32: row (i, k - 1) is the order-k update from t_i to t_i+1 (NaN where
+        k > i + 1, an update no chart can take), as the per-chart update kernel reads them"""
+        return np.ascontiguousarray(self.order_rows, dtype=np.float32)
+
+    def q_coef_f32(self) -> np.ndarray:
+        """the inpainting blend's [S, 2] table (alpha_i, sigma_i) of t_i, the rows' first two columns in float32"""
+        return np.ascontiguousarray(self.rows_f32()[:, :2])
+
+    def encode_tables_f32(self):
+        """the noising tables of a chart that is to be denoised over its last s steps, indexed by s in [0, S]: (alpha, sigma) of
+        t_S-s for s >= 1, and (1, 0) at s = 0 so that such a chart comes back exactly"""
+        a, s = np.ones(self.S + 1, np.float32), np.zeros(self.S + 1, np.float32)
+        r = self.rows_f32()
+        a[1:], s[1:] = r[::-1, ROW_ALPHA], r[::-1, ROW_SIGMA]
+        return a, s
+
+
+def chart_orders(sched: DPMSchedule, starts) -> np.ndarray:
+    """[B, S] the order each chart takes at each step when chart b runs steps S - starts[b] .. S - 1 (starts[b] = its number of
+    steps): min(sched.orders[i], i - (S - starts[b]) + 1), so it warms up like a fresh request and keeps lower_order_final; 0 while
+    the chart is held"""
+    S = sched.S
+    i = np.arange(S)[None, :]
+    first = S - np.asarray(starts, dtype=np.int64)[:, None]
+    return np.where(i >= first, np.minimum(sched.orders[None, :], i - first + 1), 0)
+
+
+def expand_row(i: int, k: int, alpha, sigma, lam, solver_type: str) -> np.ndarray:
+    """The coefficient row (alpha_i, sigma_i, A, c0, c1, c2, k, 0) of the order-k update from t_i to t_i+1 on a grid with these
+    alpha, sigma and lambda (float64, k <= i + 1): the D-form of ``multistep_schedule`` expanded into x = A x + c0 m0 + c1 m1 + c2 m2.
+    The per-step rows of a request and the per-order rows of a remix both come from here."""
+    h = lam[i + 1] - lam[i]
+    phi = np.expm1(-h)
+    a_t = alpha[i + 1]
+    A = sigma[i + 1] / sigma[i]
+    c0, c1, c2 = -a_t * phi, 0., 0.
+    if k == 2:
+        r0 = (lam[i] - lam[i - 1]) / h
+        g = -0.5 * a_t * phi if solver_type == "dpmsolver" else a_t * (phi / h + 1.)      # coefficient of D1
+        c0 += g / r0
+        c1 -= g / r0
+    elif k == 3:
+        r0 = (lam[i] - lam[i - 1]) / h
+        r1 = (lam[i - 1] - lam[i - 2]) / h
+        p = a_t * (phi / h + 1.)                                                        # coefficient of D1
+        q = -a_t * ((phi + h) / h ** 2 - 0.5)                                            # coefficient of D2
+        a0 = p * (1. + r0 / (r0 + r1)) + q / (r0 + r1)                                  # of D1_0 = (m0 - m1) / r0
+        a1 = -p * r0 / (r0 + r1) - q / (r0 + r1)                                       # of D1_1 = (m1 - m2) / r1
+        c0 += a0 / r0
+        c1 += -a0 / r0 + a1 / r1
+        c2 += -a1 / r1
+    return np.array([alpha[i], sigma[i], A, c0, c1, c2, k, 0.])
 
 
 def multistep_schedule(alphas_cumprod, S: int, order: int = 2, skip_type: str = "time_uniform", solver_type: str = "dpmsolver",
@@ -123,7 +178,9 @@ def multistep_schedule(alphas_cumprod, S: int, order: int = 2, skip_type: str = 
                   x = (s_t/s_0) x - a_t phi m0 + a_t (phi/h + 1) D1       ("taylor")           D1 = (m0 - m1) / r0
         order 3   x = (s_t/s_0) x - a_t phi m0 + a_t (phi/h + 1) D1 - a_t ((phi + h)/h^2 - 1/2) D2,
                   D1_0 = (m0 - m1)/r0, D1_1 = (m1 - m2)/r1, D1 = D1_0 + r0/(r0 + r1) (D1_0 - D1_1), D2 = (D1_0 - D1_1)/(r0 + r1)
-    expanded into x = A x + c0 m0 + c1 m1 + c2 m2 in float64."""
+    expanded into x = A x + c0 m0 + c1 m1 + c2 m2 in float64 (``expand_row``).  ``order_rows`` [S, 3, 8] holds row (i, k - 1) =
+    the order-k update of step i for every k <= min(i + 1, 3), NaN elsewhere: a chart that joins the request late takes lower orders
+    (``chart_orders``), and row (i, orders[i]) is rows[i] itself."""
     if isinstance(order, bool) or order not in ORDERS:
         raise ValueError(f"order={order!r}: one of {ORDERS}")
     if solver_type not in SOLVER_TYPES:
@@ -140,28 +197,9 @@ def multistep_schedule(alphas_cumprod, S: int, order: int = 2, skip_type: str = 
     S = int(S)
     alpha, sigma, lam = ns.marginal_alpha(t), ns.marginal_std(t), ns.marginal_lambda(t)
     orders = step_orders(S, order, lower_order_final)
-    rows = np.zeros((S, ROW_WIDTH), dtype=np.float64)
+    rows = np.stack([expand_row(i, int(orders[i]), alpha, sigma, lam, solver_type) for i in range(S)])
+    by_order = np.full((S, 3, ROW_WIDTH), np.nan)
     for i in range(S):
-        k = int(orders[i])
-        h = lam[i + 1] - lam[i]
-        phi = np.expm1(-h)
-        a_t = alpha[i + 1]
-        A = sigma[i + 1] / sigma[i]
-        c0, c1, c2 = -a_t * phi, 0., 0.
-        if k == 2:
-            r0 = (lam[i] - lam[i - 1]) / h
-            g = -0.5 * a_t * phi if solver_type == "dpmsolver" else a_t * (phi / h + 1.)      # coefficient of D1
-            c0 += g / r0
-            c1 -= g / r0
-        elif k == 3:
-            r0 = (lam[i] - lam[i - 1]) / h
-            r1 = (lam[i - 1] - lam[i - 2]) / h
-            p = a_t * (phi / h + 1.)                                                        # coefficient of D1
-            q = -a_t * ((phi + h) / h ** 2 - 0.5)                                            # coefficient of D2
-            a0 = p * (1. + r0 / (r0 + r1)) + q / (r0 + r1)                                  # of D1_0 = (m0 - m1) / r0
-            a1 = -p * r0 / (r0 + r1) - q / (r0 + r1)                                       # of D1_1 = (m1 - m2) / r1
-            c0 += a0 / r0
-            c1 += -a0 / r0 + a1 / r1
-            c2 += -a1 / r1
-        rows[i] = (alpha[i], sigma[i], A, c0, c1, c2, k, 0.)
-    return DPMSchedule(t=t, model_times=model_time(ns, t[:-1]), rows=rows, orders=orders)
+        for k in range(1, min(i + 1, 3) + 1):
+            by_order[i, k - 1] = expand_row(i, k, alpha, sigma, lam, solver_type)
+    return DPMSchedule(t=t, model_times=model_time(ns, t[:-1]), rows=rows, orders=orders, order_rows=by_order)

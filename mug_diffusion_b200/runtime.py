@@ -73,6 +73,11 @@ class Plan:
         """steps first_step .. first_step + steps - 1 of a DPM-Solver++ request from one C call (mugd_sample_dpm)"""
         self._launch_steps("mugd_sample_dpm", dpm, first_step, steps)
 
+    def launch_dpm_ex(self, ex: L_.DpmEx, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a DPM-Solver++ inpainting or per-chart-start request from one C call
+        (mugd_sample_dpm_ex)"""
+        self._launch_steps("mugd_sample_dpm_ex", ex, first_step, steps)
+
     def launch_join(self, join: L_.Join, tail: OpList, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a decode request whose charts join at different iterations, from one C call
         (mugd_sample_join: the join kernel, the graph replay and the tail per step)"""
@@ -546,6 +551,20 @@ class Session:
         d.eps, d.pred_x0, d.ring, d.coef, d.step = self.eps.ptr, pred_x0 or None, _ptr(ring), _ptr(coef), _ptr(self.step)
         d.n, d.S, d.cfg, d.scale = n, S, int(cfg_on), float(scale)
         return d
+
+    def dpm_ex(self, dpm: L_.Dpm, stage: Optional[L_.Stage] = None, B: int = 0, start: Optional[torch.Tensor] = None,
+               order_coef: Optional[torch.Tensor] = None) -> L_.DpmEx:
+        """the mugd_sample_dpm_ex descriptor around ``dpm``: with ``stage`` (ddim_stage's, x0 / mask / q_noise / q_coef filled in) the
+        inpainting blend runs in front of each step; with ``start`` ([B] int32, the first step of each chart) and ``order_coef``
+        (the [S, 3, 8] per-order rows) every chart runs from its own step.  The caller keeps the stage and both tensors alive."""
+        e = L_.DpmEx()
+        e.dpm = dpm
+        e.stage = C.addressof(stage) if stage is not None else None
+        if start is not None:
+            assert start.shape == (B,) and start.dtype == torch.int32 and start.is_contiguous()
+            assert order_coef.shape == (dpm.S, 3, 8) and order_coef.dtype == torch.float32 and order_coef.is_contiguous()
+            e.start, e.order_coef, e.B = _ptr(start), _ptr(order_coef), B
+        return e
 
     def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:
         """the ops that follow each evaluation of an S-step request for B samples: the DDIM update of the xin rows (both halves

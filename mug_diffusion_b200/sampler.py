@@ -571,6 +571,24 @@ def _finite_scale(scale):
     return scale
 
 
+def per_chart_steps(B: int, value, n: int, name: str, where: str = "") -> list:
+    """``value`` (one integer, or one integer per chart) as B integers in [0, n]; ValueError for malformed ones"""
+    if isinstance(value, (int, np.integer)) and not isinstance(value, bool):
+        out = [int(value)] * B
+    elif isinstance(value, (list, tuple, np.ndarray, torch.Tensor)):
+        out = list(value.tolist() if isinstance(value, (np.ndarray, torch.Tensor)) else value)
+        if len(out) != B:
+            raise ValueError(f"{name} has {len(out)} entries for {B} charts")
+        if any(isinstance(v, bool) or not isinstance(v, (int, np.integer)) for v in out):
+            raise ValueError(f"{name}={out!r}: the starts must be integers")
+        out = [int(v) for v in out]
+    else:
+        raise ValueError(f"{name}={value!r} must be an integer or one integer per chart")
+    if any(v < 0 or v > n for v in out):
+        raise ValueError(f"{name}={out}: every start must lie in [0, {n}]{where}")
+    return out
+
+
 # --------------------------------------------------------------------------------------------------
 # DDIM sampler
 # --------------------------------------------------------------------------------------------------
@@ -760,22 +778,7 @@ class DDIMSampler(_DeviceLoopSampler):
 
     def _decode_starts(self, x_latent, t_start):
         """the per-chart start indices of a decode request; ValueError for malformed ones"""
-        n = self.ddim_timesteps.shape[0]
-        B = x_latent.shape[0]
-        if isinstance(t_start, (int, np.integer)) and not isinstance(t_start, bool):
-            starts = [int(t_start)] * B
-        elif isinstance(t_start, (list, tuple, np.ndarray, torch.Tensor)):
-            starts = list(t_start.tolist() if isinstance(t_start, (np.ndarray, torch.Tensor)) else t_start)
-            if len(starts) != B:
-                raise ValueError(f"t_start has {len(starts)} entries for {B} charts")
-            if any(isinstance(s, bool) or not isinstance(s, (int, np.integer)) for s in starts):
-                raise ValueError(f"t_start={starts!r}: the starts must be integers")
-            starts = [int(s) for s in starts]
-        else:
-            raise ValueError(f"t_start={t_start!r} must be an integer or one integer per chart")
-        if any(s < 0 or s > n for s in starts):
-            raise ValueError(f"t_start={starts}: every start must lie in [0, {n}] (n = len(ddim_timesteps))")
-        return starts
+        return per_chart_steps(x_latent.shape[0], t_start, self.ddim_timesteps.shape[0], "t_start", " (n = len(ddim_timesteps))")
 
     @torch.no_grad()
     def decode(self, x_latent, c, w, t_start, unconditional_guidance_scale=1., unconditional_conditioning=None,
@@ -1083,6 +1086,16 @@ class DPMSolverSampler(_DeviceLoopSampler):
         return dpm_solver.multistep_schedule(alphas_cumprod_f64(self.model.cfg), int(S), int(order), skip_type, solver_type,
                                              bool(lower_order_final), t_grid)
 
+    def _check_request(self, S, c, w, batch_size, shape, x_T, mask, x0, order, skip_type, solver_type, lower_order_final, log_every_t,
+                       scale, uc):
+        """the checks sample() and inpaint() share, before any GPU work: returns (guidance scale, schedule, [B, C, L] shape)"""
+        if c is None or w is None:
+            raise TypeError("DPMSolverSampler.sample needs the conditioning c and the audio features w")
+        scale = _finite_scale(scale)
+        sched = self.make_dpm_schedule(S, order, skip_type, solver_type, lower_order_final)
+        size = request_size(self.model, c, batch_size, shape, x_T, mask, x0, scale, uc, log_every_t)
+        return scale, sched, size
+
     @torch.no_grad()
     def sample(self, S, c=None, w=None, batch_size=None, shape=None, x_T=None, order=2, skip_type="time_uniform",
                solver_type="dpmsolver", lower_order_final=True, callback=None, img_callback=None, log_every_t=100,
@@ -1091,15 +1104,12 @@ class DPMSolverSampler(_DeviceLoopSampler):
         """S steps of DPM-Solver++ multistep of ``order`` from x_T (drawn when not given) to t = 1/N; ``c`` may also be given as
         ``conditioning``.  Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then x and the data prediction m of every step i with
         ``(S - i - 1) % log_every_t == 0`` or i = 0 (DDIM's rule).  Every argument is checked before any GPU work (ValueError; TypeError
-        for missing or unknown ones); inpainting (mask / x0), eta, temperature and noise dropout are refused.  Without callbacks the
-        steps run from mugd_sample_dpm calls, with them one by one through mugd_dpm_update."""
+        for missing or unknown ones); inpainting (mask / x0: see ``inpaint``), eta, temperature and noise dropout are refused.  Without
+        callbacks the steps run from mugd_sample_dpm calls, with them one by one through mugd_dpm_update."""
         _refuse_ddim_only(kwargs, "DPMSolverSampler", "DPM-Solver++ multistep is a deterministic solver without {}")
         c = _conditioning(c, conditioning)
-        if c is None or w is None:
-            raise TypeError("DPMSolverSampler.sample needs the conditioning c and the audio features w")
-        scale = _finite_scale(unconditional_guidance_scale)
-        sched = self.make_dpm_schedule(S, order, skip_type, solver_type, lower_order_final)
-        size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
+        scale, sched, size = self._check_request(S, c, w, batch_size, shape, x_T, None, None, order, skip_type, solver_type,
+                                                 lower_order_final, log_every_t, unconditional_guidance_scale, unconditional_conditioning)
         if verbose:
             print(f'Data shape for DPM-Solver++ sampling is {size}, {S} steps of order {order} ({skip_type}, {solver_type})')
         return self.dpm_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
@@ -1107,15 +1117,39 @@ class DPMSolverSampler(_DeviceLoopSampler):
                                  tqdm_class=tqdm_class)
 
     @torch.no_grad()
+    def inpaint(self, S, c=None, w=None, batch_size=None, mask=None, x0=None, shape=None, x_T=None, order=2, skip_type="time_uniform", solver_type="dpmsolver",
+                lower_order_final=True, callback=None, img_callback=None, log_every_t=100, unconditional_guidance_scale=1.,
+                unconditional_conditioning=None, tqdm_class=None, verbose=True, conditioning=None):
+        """Regenerate the part of the chart ``x0`` [B, C, L] where ``mask`` (broadcast to [B, C, L]) is 0, keeping the rest: ``sample``
+        in which, before the evaluation of step i, x <- (alpha_i * x0 + sigma_i * eps_i) * mask + (1 - mask) * x with the schedule's
+        alpha_i / sigma_i of t_i (DDIM inpainting's blend, ddim.py:140-144) and eps_i = randn_like(x0) drawn per step from the device's
+        generator, as DDIM inpainting at eta = 0 draws it.  Returns ``(z, {'x_inter', 'pred_x0'})`` logged as by ``sample``.  Every
+        argument is checked before any GPU work (those of ``sample``; x0 of the request's shape, a mask that broadcasts to it).  Without
+        callbacks, and with float32 mask / x0 on the model's device (``takes_device_loop``), the steps run from mugd_sample_dpm_ex calls
+        with the blend staged in front of each step (the noise of a call drawn up front, at most STAGE_TABLE_BYTES per table); otherwise
+        one by one."""
+        c = _conditioning(c, conditioning)
+        if not isinstance(mask, torch.Tensor) or not isinstance(x0, torch.Tensor):
+            raise ValueError("inpainting needs the mask and x0 as tensors")
+        scale, sched, size = self._check_request(S, c, w, batch_size, shape, x_T, mask, x0, order, skip_type, solver_type,
+                                                 lower_order_final, log_every_t, unconditional_guidance_scale, unconditional_conditioning)
+        if verbose:
+            print(f'Data shape for DPM-Solver++ inpainting is {size}, {S} steps of order {order} ({skip_type}, {solver_type})')
+        return self.dpm_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
+                                 unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
+                                 tqdm_class=tqdm_class, mask=mask, x0=x0)
+
+    @torch.no_grad()
     def dpm_sampling(self, w, c, shape, sched: dpm_solver.DPMSchedule, x_T=None, callback=None, img_callback=None, log_every_t=100,
-                     unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True):
-        """the request of ``sched`` (make_dpm_schedule) on the GPU"""
+                     unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, mask=None, x0=None):
+        """the request of ``sched`` (make_dpm_schedule) on the GPU; with ``mask`` / ``x0`` the inpainting of ``inpaint``"""
         model = self.model
         eng = model.engine
         dev = self.device
         B, Cz, Lz = shape
         total = sched.S
         scale = unconditional_guidance_scale
+        blend = mask is not None
         self.last_schedule = sched
         with eng.lock:
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times)
@@ -1123,20 +1157,144 @@ class DPMSolverSampler(_DeviceLoopSampler):
             ring = torch.empty(3, B * Lz * Cz, device=dev)                     # the data predictions of the last three steps
             pred = torch.empty(B * Lz, Cz, device=dev)
             dpm = sess.dpm(B, total, cfg_on, scale, _ptr(pred), ring, coef)
+            device_loop = takes_device_loop(shape, x.device, mask, x0, callback, img_callback)
+            qcoef = sched.q_coef_f32() if blend else None                       # (alpha_i, sigma_i) of the blend before step i
+            per_call = max(1, STAGE_TABLE_BYTES // (4 * B * Cz * Lz))
+            stage = None
+            if device_loop and blend:
+                # the blend runs in front of every step (mugd_sample_dpm_ex); a call's q_sample noise is drawn up front, in the per-step
+                # loop's order
+                stage = sess.ddim_stage(B, cfg_on)
+                x0c = x0.contiguous()
+                mask_e = mask.expand(shape).contiguous()                        # the blend's mask, expanded once per request
+                q_tab = torch.empty((min(per_call, total),) + tuple(shape), device=dev)
+                stage.x0, stage.mask, stage.q_noise = _ptr(x0c), _ptr(mask_e), _ptr(q_tab)
+                ex = sess.dpm_ex(dpm, stage)
 
             def launch(first, n):
                 # the ring and the step counter stay on the device, so a call may start inside the warm-up
-                sess.plan.launch_dpm(dpm, first, n)
+                if stage is None:
+                    sess.plan.launch_dpm(dpm, first, n)
+                else:
+                    draw_step_noise(n, shape, x0, q_tab, False, None, 0., dev)
+                    stage.q_coef = qcoef[first:].ctypes.data
+                    sess.plan.launch_dpm_ex(ex, first, n)
 
-            # the per-step loop runs the same kernel: the referee of the device loop
+            # the per-step loop runs the same kernels: the referee of the device loop
             advance = _step_ops(sess)
             stream = torch.cuda.current_stream().cuda_stream
+            q_dev = torch.from_numpy(qcoef).to(dev) if blend else None
 
             def step(i, t):
+                if blend:
+                    x0d = x0.to(dev)
+                    x_orig = q_dev[i, 0] * x0d + q_dev[i, 1] * torch.randn_like(x0d)
+                    sess.load_x(x_orig * mask + (1. - mask) * self._read_x(sess, shape), dup=cfg_on)
                 sess.eval(graph=True)
                 L_.check(eng.lib.mugd_dpm_update(C.byref(dpm), stream), "mugd_dpm_update")
                 eng.run_ops(advance)
 
             return self._run_request(sess, x, shape, pred, time_range, total, log_every_t, 'Charting, using DPM-Solver++ Sampler',
-                                     tqdm_class, progress, callback, img_callback, callback is None and img_callback is None, launch,
-                                     step, 2)
+                                     tqdm_class, progress, callback, img_callback, device_loop, launch, step,
+                                     3 if stage is not None else 2, chunk=per_call if stage is not None else None)
+
+    # ---- remixing an existing chart: stochastic_encode + decode on the DPM-Solver++ grid --------------------------------------------
+    @staticmethod
+    def _require_schedule(sched):
+        if not isinstance(sched, dpm_solver.DPMSchedule) or sched.order_rows is None:
+            raise ValueError("sched must be a DPMSchedule from make_dpm_schedule")
+
+    @torch.no_grad()
+    def stochastic_encode(self, x0, t_enc, sched: dpm_solver.DPMSchedule, noise=None):
+        """Noise the latent ``x0`` [B, C, L] for a remix over the last ``t_enc[b]`` steps of ``sched`` (an integer in [0, S], or one per
+        chart): alpha(t_S-s) * x0 + sigma(t_S-s) * noise with s = t_enc[b], the marginal at the time where ``decode`` with t_start = s
+        starts (no off-by-one, unlike DDIM's stochastic_encode / decode pair); s = 0 returns x0 exactly.  noise = torch.randn_like(x0)
+        when not given.  One kernel (mugd_stochastic_encode over the schedule's float32 tables of S + 1 rows).  ValueError, before any
+        GPU work, for malformed arguments."""
+        model = self.model
+        dev = self.device
+        self._require_schedule(sched)
+        if not isinstance(x0, torch.Tensor) or x0.dim() != 3 or x0.dtype != torch.float32 or x0.device != torch.device(dev):
+            raise ValueError(f"x0 must be a float32 [B, C, L] tensor on {dev}")
+        B = x0.shape[0]
+        steps = per_chart_steps(B, t_enc, sched.S, "t_enc", " (S = sched.S)")
+        if noise is not None and (not isinstance(noise, torch.Tensor) or noise.shape != x0.shape or noise.dtype != torch.float32
+                                  or noise.device != x0.device):
+            raise ValueError(f"noise must be a float32 tensor of x0's shape {tuple(x0.shape)} on {dev}")
+        if noise is None:
+            noise = torch.randn_like(x0)
+        out = torch.empty(x0.shape, device=dev)
+        if out.numel() == 0:
+            return out
+        a, s = (torch.from_numpy(v).to(dev) for v in sched.encode_tables_f32())
+        x0c, nc = x0.contiguous(), noise.contiguous()
+        td = torch.tensor(steps, dtype=torch.int64, device=dev)
+        d = L_.QEncode()
+        d.x0, d.noise, d.t, d.sqrt_a, d.sqrt_1ma, d.out = _ptr(x0c), _ptr(nc), _ptr(td), _ptr(a), _ptr(s), _ptr(out)
+        d.B, d.C, d.L, d.n = B, x0.shape[1], x0.shape[2], sched.S + 1
+        with model.engine.lock:
+            L_.check(model.engine.lib.mugd_stochastic_encode(C.byref(d), torch.cuda.current_stream().cuda_stream), "mugd_stochastic_encode")
+        return out
+
+    @torch.no_grad()
+    def decode(self, x_latent, c, w, t_start, sched: dpm_solver.DPMSchedule, unconditional_guidance_scale=1.,
+               unconditional_conditioning=None, tqdm_class=None):
+        """Denoise ``x_latent`` [B, C, L] (e.g. from ``stochastic_encode``) under (c, w) over the last ``t_start`` steps of ``sched``:
+        chart b runs steps S - t_start[b] .. S - 1 from x_latent[b] (``t_start``: an integer in [0, S], or one per chart) and returns
+        the final latent.  A chart's first step is order 1 and its order at step i is min(sched.orders[i], i - (S - t_start[b]) + 1)
+        (``dpm_solver.chart_orders``): it warms up like a fresh request and keeps lower_order_final.  All charts run in one device loop
+        of m = max(t_start) iterations from step S - m (mugd_sample_dpm_ex, the launches per step of mugd_sample_dpm); a chart is left
+        untouched until its start, and one with t_start[b] = 0 comes back as x_latent[b].  With every t_start = S this is
+        dpm_sampling(x_T=x_latent) bit for bit.  Charts with a smaller start still occupy their batch rows for all m iterations: group
+        charts by strength into separate calls to avoid the idle rows.  Every argument is checked before any GPU work (ValueError)."""
+        model = self.model
+        self._require_schedule(sched)
+        if not isinstance(x_latent, torch.Tensor) or x_latent.dim() != 3 or x_latent.shape[0] < 1 or x_latent.shape[1] != model.z_channels:
+            raise ValueError(f"x_latent must be a [B, {model.z_channels}, L] tensor"
+                             + (f", got {tuple(x_latent.shape)}" if isinstance(x_latent, torch.Tensor) else ""))
+        starts = per_chart_steps(x_latent.shape[0], t_start, sched.S, "t_start", " (S = sched.S)")
+        scale = _finite_scale(unconditional_guidance_scale)
+        B, Cz, Lz = (int(v) for v in x_latent.shape)
+        request_size(model, c, B, (Cz, Lz), x_latent, None, None, scale, unconditional_conditioning, 1)
+        if c is None or w is None:
+            raise ValueError("decode needs the conditioning c and the audio features w")
+        if max(starts) == 0:
+            return x_latent
+        return self.dpm_decoding(w, c, x_latent, starts, sched, scale, unconditional_conditioning, tqdm_class)
+
+    @torch.no_grad()
+    def dpm_decoding(self, w, c, x_latent, starts, sched: dpm_solver.DPMSchedule, unconditional_guidance_scale=1.,
+                     unconditional_conditioning=None, tqdm_class=None, per_step=False):
+        """``decode`` of checked arguments (``starts``: t_start per chart, max(starts) >= 1) on the GPU.  ``per_step``: the steps run
+        one by one through mugd_dpm_ex_update, the referee of the device loop."""
+        model = self.model
+        eng = model.engine
+        dev = self.device
+        B, Cz, Lz = (int(v) for v in x_latent.shape)
+        shape = (B, Cz, Lz)
+        S, m = sched.S, max(starts)
+        with eng.lock:
+            # the timestep table holds all S model times and the counter starts at S - m, so step i reads row i of every table
+            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_latent, unconditional_guidance_scale,
+                                                             unconditional_conditioning, sched.model_times)
+            sess.set_step(S - m)
+            coef = torch.from_numpy(sched.rows_f32()).to(dev)
+            order_coef = torch.from_numpy(sched.order_rows_f32()).to(dev)
+            first = torch.tensor([S - s for s in starts], dtype=torch.int32, device=dev)
+            ring = torch.empty(3, B * Lz * Cz, device=dev)
+            dpm = sess.dpm(B, S, cfg_on, unconditional_guidance_scale, 0, ring, coef)
+            ex = sess.dpm_ex(dpm, B=B, start=first, order_coef=order_coef)
+            bar = self._progress(time_range[S - m:], 'Decoding image', m, tqdm_class)
+            if per_step:
+                advance = _step_ops(sess)
+                stream = torch.cuda.current_stream().cuda_stream
+                for _ in bar:
+                    sess.eval(graph=True)
+                    L_.check(eng.lib.mugd_dpm_ex_update(C.byref(ex), stream), "mugd_dpm_ex_update")
+                    eng.run_ops(advance)
+            else:
+                sess.plan.launch_dpm_ex(ex, S - m, m)
+                for _ in bar:                                                   # keeps a progress bar moving
+                    pass
+            self.last_launches_per_step = sess.plan.launches + 2
+            return self._read_x(sess, shape)
