@@ -139,7 +139,7 @@ typedef struct mugd_s4conv {
     const float* u; int64_t ldu;           /* [B*L, H]                                                     */
     const float* Kt;                       /* [L][H] kernel taps, tap-major (from mugd_s4_kernel_gen)      */
     const float* D;                        /* [H]                                                          */
-    float* y; int64_t ldy;                 /* gelu(conv + D*u)                                             */
+    float* y; int64_t ldy;                 /* gelu(conv + D*u); must not overlap u                         */
     int32_t B, L, H;
 } mugd_s4conv;
 
@@ -517,6 +517,12 @@ int  mugd_set_tc_single_pass_tf32(mugd_handle* h, int enabled);
 /* attention kernel: 1 (default) = QK^T and PV on the wgmma tensor cores (3xTF32, fp32 accuracy); 0 = exact-fp32 FFMA kernel
  * (the referee of the parity tests).  Replaces the einsum/softmax body of CrossAttention.forward, attention.py:99-121 */
 int  mugd_set_attention_impl(mugd_handle* h, int impl);
+
+/* causal S4 convolution kernel: 0 (default) = automatic: the resident kernel, which holds all of u and K of its 16 channels in
+ * shared memory, wherever that fits (L <= 1584 on an H100), the streamed kernel beyond; 1 = resident (refuses a longer L);
+ * 2 = streamed at any length.  The two agree bit for bit; the switch lets tests and benchmarks run both at one length.  Read when
+ * the op is launched, like the attention switch. */
+int  mugd_set_s4conv_impl(mugd_handle* h, int impl);
 
 /* ---- measurement aids (process-wide, not needed in production) -------------------------------------
  * planner cost constants of the tensor-core GEMM (relative cost of a 32-deep k-step of a 128-column tile, unused, of a

@@ -123,6 +123,27 @@ def z_length_for(frames: int, per_latent: int = 64) -> int:
     return (int(frames / per_latent / 32) + 1) * 32
 
 
+# The longest latent a request may have.  The U-Net's S4 layers generate their convolution kernels with a one-shot DFT of length
+# L_internal, which a trained checkpoint's L buffers (512 / 256 / 128 / 64) reach by doubling: at z_length 8192 every layer runs at
+# L_internal 8192, the next doubling would need 16384, past what that DFT holds in shared memory.
+MAX_Z_LENGTH = 8192
+
+
+def max_samples(per_latent: int = 64, hop_length: int = MelConfig.hop_length) -> int:
+    """the most samples an audio may have so that ``z_length_for`` stays within MAX_Z_LENGTH: 67,108,735 for the shipped model"""
+    return (MAX_Z_LENGTH * per_latent - 1) * hop_length - 1
+
+
+def check_z_length(z_length: int, per_latent: int = 64, cfg: MelConfig = MelConfig()) -> None:
+    """Refuses a latent longer than MAX_Z_LENGTH with the audio length it corresponds to.  Host only: runs before any GPU work."""
+    if int(z_length) > MAX_Z_LENGTH:
+        n = max_samples(per_latent, cfg.hop_length)
+        secs = (n + 1) / cfg.sr
+        raise L_.MugdError(
+            f"z_length {int(z_length)} is longer than the supported maximum {MAX_Z_LENGTH}: audio of at most {n:,} samples at "
+            f"{cfg.sr:,} Hz ({secs:.1f} s, {int(secs) // 60} min {secs % 60:.0f} s) can be charted")
+
+
 # ---- device -------------------------------------------------------------------------------------------------------------
 class MelFrontEnd:
     """The kernel's tables on one engine's device, and the calls that run it."""
@@ -183,6 +204,7 @@ class MelFrontEnd:
             raise L_.MugdError(f"the audio encoder reads {wcfg.n_freq} mel bands, the front-end makes {self.cfg.n_mels}")
         per = frames_per_latent(len(wcfg.channel_mult), unet_levels)
         zl = z_length_for(n_frames(y.shape[1], self.cfg.hop_length), per)
+        check_z_length(zl, per, self.cfg)
         sess = self.engine.wave_session(1, per * zl)
         self.write_rows(y, sess.mel, per * zl)
         hs = sess.run()

@@ -133,6 +133,13 @@ int mugd_set_attention_impl(mugd_handle* h, int impl) {
     return MUGD_OK;
 }
 
+int mugd_set_s4conv_impl(mugd_handle* h, int impl) {
+    MUGD_REQUIRE(h, "null handle");
+    MUGD_REQUIRE(impl >= 0 && impl <= 2, "set_s4conv_impl: %d (0 = automatic, 1 = resident, 2 = streamed)", impl);
+    h->dev.s4conv_impl = impl;
+    return MUGD_OK;
+}
+
 int mugd_set_pdl(int enabled) {
     g_use_pdl = enabled != 0;
     return MUGD_OK;

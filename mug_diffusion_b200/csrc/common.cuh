@@ -43,6 +43,7 @@ struct DeviceInfo {
     // per-handle switches
     int tc_single_pass = 0;     // opt-in plain-TF32 tensor-core products (NOT fp32-accurate; never used by parity tests / bench)
     int attention_impl = 1;     // 1 = wgmma attention, 0 = exact-fp32 FFMA referee
+    int s4conv_impl = 0;        // 0 = automatic, 1 = resident kernel, 2 = streamed kernel (mugd_set_s4conv_impl)
 };
 
 // per-family launchers (each validates its descriptor and enqueues kernels on `st`);

@@ -123,11 +123,169 @@ s4conv_kernel(const mugd_s4conv s, int nsplit, int Lpad) {
     }
 }
 
+// -----------------------------------------------------------------------------------------------------
+// Streamed form, for lengths whose u and K do not fit in shared memory (L > 1584 on an H100).  A CTA still owns 16 channels of one
+// sample, but walks the outputs in windows of S4S_W = 256 (one super block per warp, as above) and, per window [o0, o0 + W), the
+// taps in tiles [j0, j0 + T): the tile needs u rows [o0 - j0 - T + 1, o0 + W - j0) and K taps [j0, j0 + T), zero below row 0 and
+// beyond L.  Tiles go through two shared-memory stages with cp.async (zero-fill for the padding), so the next tile lands while this
+// one is computed; the accumulators stay in registers across a window's tiles.  The causal cost of window w is w + 1 tiles, so a
+// CTA takes windows in pairs (nwin - 1 - p, p) like the super-block pairs above.
+//
+// Per output the FMAs are the resident kernel's: taps in ascending chunks of 8 (tile by tile, then chunk by chunk), the same
+// software-pipelined register window, the same trailing zero chunk of the lower half, the same epilogue expression -- the two
+// kernels agree bit for bit wherever both run.
+// -----------------------------------------------------------------------------------------------------
+constexpr int S4S_W = S4_WARPS * 2 * S4_R;                      // outputs per window (256)
+constexpr int S4S_T = 256;                                      // taps per tile
+constexpr int S4S_UROWS = S4S_W + S4S_T + S4_R;                 // u rows of a tile: [o0 - j0 - T - 8, o0 + W - j0) (8 for the prefetch)
+constexpr int S4S_KROWS = S4S_T + S4_R;                         // taps of a tile: [j0, j0 + T + 8)
+constexpr int S4S_STAGE = (S4S_UROWS + S4S_KROWS) * S4_PITCH;   // floats per stage
+constexpr size_t S4S_SMEM = 2 * S4S_STAGE * sizeof(float);      // 112,896 B
+
+__device__ __forceinline__ void cp_async4(float* dst, const float* src, bool valid) {
+    // src-size 0 writes a zero and reads nothing
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src),
+                 "r"(valid ? 4 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait1() { asm volatile("cp.async.wait_group 1;\n" ::: "memory"); }
+
+__device__ __forceinline__ int s4s_tiles(int win) { return (win * S4S_W + S4S_W + S4S_T - 1) / S4S_T; }
+
+// this CTA's walk: pairs p = blockIdx.z, + nsplit, ...; per pair window nwin - 1 - p, then window p (once when they coincide); per
+// window its tiles t = 0, 1, ...
+struct S4Walk {
+    int p, which, t;
+    __device__ int win(int nwin) const { return which == 0 ? nwin - 1 - p : p; }
+    __device__ void next(int nwin, int nsplit) {
+        if (++t < s4s_tiles(win(nwin))) return;
+        t = 0;
+        if (which == 0 && p != nwin - 1 - p) which = 1;
+        else { which = 0; p += nsplit; }
+    }
+};
+
+__device__ __forceinline__ void s4s_load(float* stage, const mugd_s4conv& s, const float* ub, const float* Kc, int o0, int j0) {
+    float* us = stage;
+    float* ks = stage + S4S_UROWS * S4_PITCH;
+    const int r0 = o0 - j0 - S4S_T - S4_R;
+    for (int i = threadIdx.x; i < S4S_UROWS * S4_CH; i += 32 * S4_WARPS) {
+        const int row = i / S4_CH, c = i % S4_CH, l = r0 + row;
+        const bool ok = l >= 0 && l < s.L;
+        cp_async4(us + row * S4_PITCH + c, ub + (int64_t)(ok ? l : 0) * s.ldu + c, ok);
+    }
+    for (int i = threadIdx.x; i < S4S_KROWS * S4_CH; i += 32 * S4_WARPS) {
+        const int row = i / S4_CH, c = i % S4_CH, j = j0 + row;
+        const bool ok = j < s.L;
+        cp_async4(ks + row * S4_PITCH + c, Kc + (int64_t)(ok ? j : 0) * s.H + c, ok);
+    }
+}
+
+__global__ void __launch_bounds__(32 * S4_WARPS)
+s4conv_stream_kernel(const mugd_s4conv s, int nsplit) {
+    extern __shared__ float smem_s4[];                          // [2][S4S_STAGE]: u rows, then K taps, pitch S4_PITCH
+    const int L = s.L;
+    const int nwin = (L + S4S_W - 1) / S4S_W, npairs = (nwin + 1) / 2;
+    S4Walk cur = {(int)blockIdx.z, 0, 0};
+    if (cur.p >= npairs) return;
+    pdl_wait();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int ch = lane & (S4_CH - 1), half = lane >> 4;
+    const int c0 = blockIdx.x * S4_CH;
+    const int b = blockIdx.y;
+    const float* ub = s.u + (int64_t)b * L * s.ldu + c0;
+    const float* Kc = s.Kt + c0;
+    const int h = c0 + ch;
+    const float Dh = s.D[h];
+    float* yb = s.y + (int64_t)b * L * s.ldy + h;
+
+    s4s_load(smem_s4, s, ub, Kc, cur.win(nwin) * S4S_W, 0);
+    cp_async_commit();
+    S4Walk nxt = cur;
+    nxt.next(nwin, nsplit);
+    float acc[S4_R];
+#pragma unroll 1
+    for (int k = 0;; ++k) {
+        const bool more = nxt.p < npairs;
+        if (more) s4s_load(smem_s4 + ((k + 1) & 1) * S4S_STAGE, s, ub, Kc, nxt.win(nwin) * S4S_W, nxt.t * S4S_T);
+        cp_async_commit();                                      // (an empty group on the last tile)
+        cp_async_wait1();                                       // this tile has landed
+        __syncthreads();
+
+        const int o0 = cur.win(nwin) * S4S_W, j0 = cur.t * S4S_T;
+        const int sb = o0 / (2 * S4_R) + warp;                  // this warp's super block
+        const int l0 = sb * 2 * S4_R + half * S4_R;             // this lane's first output
+        const int jend = min(j0 + S4S_T, (sb + 1) * 2 * S4_R);  // the super block's taps end at sb*16 + 16
+        if (cur.t == 0) {
+#pragma unroll
+            for (int r = 0; r < S4_R; ++r) acc[r] = 0.f;
+        }
+        if (sb * 2 * S4_R < L && jend > j0) {
+            const float* stage = smem_s4 + (k & 1) * S4S_STAGE;
+            // hi[x * PITCH] = u[l0 - j0 + x] (tile row l0 - o0 + T + 8 + x),  kp[i * PITCH] = K[j0 + i]
+            const float* hi = stage + (l0 - o0 + S4S_T + S4_R) * S4_PITCH + ch;
+            const float* kp = stage + S4S_UROWS * S4_PITCH + ch;
+            const float* up = hi - S4_R * S4_PITCH;             // window rows l0 - jc - 8 + r
+            const int nchunks = (jend - j0) / S4_R;             // even: both ends are multiples of 16
+            float wa[S4_R], wb[S4_R], wc[S4_R], ka[S4_R], kb[S4_R];
+#pragma unroll
+            for (int r = 0; r < S4_R; ++r) { wb[r] = hi[r * S4_PITCH]; wa[r] = up[r * S4_PITCH]; ka[r] = kp[r * S4_PITCH]; }
+#pragma unroll 1
+            for (int c = 0; c < nchunks; c += 2) {
+                up -= S4_R * S4_PITCH; kp += S4_R * S4_PITCH;
+#pragma unroll
+                for (int r = 0; r < S4_R; ++r) { wc[r] = up[r * S4_PITCH]; kb[r] = kp[r * S4_PITCH]; }
+                s4_chunk(acc, wa, wb, ka);                      // lo = wa, hi = wb
+                up -= S4_R * S4_PITCH; kp += S4_R * S4_PITCH;
+#pragma unroll
+                for (int r = 0; r < S4_R; ++r) { wb[r] = up[r * S4_PITCH]; ka[r] = kp[r * S4_PITCH]; }
+                s4_chunk(acc, wc, wa, kb);                      // lo = wc, hi = wa
+#pragma unroll
+                for (int r = 0; r < S4_R; ++r) { wa[r] = wb[r]; wb[r] = wc[r]; }
+            }
+        }
+        if (cur.t == s4s_tiles(cur.win(nwin)) - 1 && sb * 2 * S4_R < L) {
+#pragma unroll
+            for (int r = 0; r < S4_R; ++r) {
+                const int li = l0 + r;
+                if (li < L) yb[(int64_t)li * s.ldy] = gelu_f(acc[r] + Dh * ub[(int64_t)li * s.ldu + ch]);
+            }
+        }
+        __syncthreads();                                        // the stage is refilled by the next iteration's load
+        if (!more) break;
+        cur = nxt;
+        nxt.next(nwin, nsplit);
+    }
+}
+
+static int launch_s4conv_stream(const DeviceInfo& dev, const mugd_s4conv& s, cudaStream_t st) {
+    MUGD_REQUIRE((int)S4S_SMEM <= dev.max_smem_optin, "s4conv: the streamed kernel needs %zu B of shared memory (max %d)", S4S_SMEM,
+                 dev.max_smem_optin);
+    // windows read u rows other CTAs have already written outputs for: y must not overlap u
+    const char *u0 = (const char*)s.u, *u1 = (const char*)(s.u + ((int64_t)s.B * s.L - 1) * s.ldu + s.H);
+    const char *y0 = (const char*)s.y, *y1 = (const char*)(s.y + ((int64_t)s.B * s.L - 1) * s.ldy + s.H);
+    MUGD_REQUIRE(y1 <= u0 || u1 <= y0, "s4conv: y overlaps u (the streamed kernel cannot run in place)");
+    const int base = (s.H / S4_CH) * s.B;
+    const int nwin = (s.L + S4S_W - 1) / S4S_W, npairs = (nwin + 1) / 2;
+    // every pair of windows costs nwin + 1 tiles: split the pairs over more CTAs until the grid covers the SMs, two CTAs each
+    // (2 x 112,896 B of shared memory and 512 threads at <= 64 registers fit one SM)
+    int nsplit = 1;
+    while (nsplit < npairs && base * nsplit < 2 * dev.sm_count) ++nsplit;
+    MUGD_CHECK_CUDA(launch_k(s4conv_stream_kernel, dim3(s.H / S4_CH, s.B, nsplit), dim3(32 * S4_WARPS), S4S_SMEM, st, s, nsplit));
+    return MUGD_OK;
+}
+
 int launch_s4conv(const DeviceInfo& dev, const mugd_s4conv& s, cudaStream_t st, int* launches) {
     MUGD_REQUIRE(s.B > 0 && s.L > 0 && s.H > 0 && s.H % S4_CH == 0, "s4conv: H=%d must be a positive multiple of %d", s.H, S4_CH);
     MUGD_REQUIRE(s.ldu >= s.H && s.ldy >= s.H, "s4conv: ld < H");
     const int Lpad = (s.L + 2 * S4_R - 1) / (2 * S4_R) * (2 * S4_R);
     const size_t smem = ((size_t)(S4_PAD + Lpad) + (size_t)(Lpad + 3 * S4_R)) * S4_PITCH * sizeof(float);
+    // automatic: the resident kernel wherever its u and K fit in shared memory, the streamed one beyond
+    if (dev.s4conv_impl == 2 || (dev.s4conv_impl == 0 && (int)smem > dev.max_smem_optin)) {
+        const int rc = launch_s4conv_stream(dev, s, st);
+        if (rc == MUGD_OK && launches) *launches += 1;
+        return rc;
+    }
     MUGD_REQUIRE((int)smem <= dev.max_smem_optin, "s4conv: L=%d needs %zu B of shared memory (max %d)", s.L, smem, dev.max_smem_optin);
     const int base = (s.H / S4_CH) * s.B;
     const int npairs = (Lpad / (2 * S4_R) + 1) / 2;
@@ -239,7 +397,9 @@ __global__ void s4_irfft_kernel(const double2* __restrict__ kf, int H, int Lint,
     }
 }
 
-cudaError_t s4_allow_smem(int bytes) { return allow_dynamic_smem(bytes, s4conv_kernel<true>, s4conv_kernel<false>, s4_irfft_kernel); }
+cudaError_t s4_allow_smem(int bytes) {
+    return allow_dynamic_smem(bytes, s4conv_kernel<true>, s4conv_kernel<false>, s4conv_stream_kernel, s4_irfft_kernel);
+}
 
 }  // namespace mugd
 

@@ -230,6 +230,7 @@ def load() -> C.CDLL:
     lib.mugd_plan_load.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(Region), C.c_int32, C.POINTER(C.c_void_p)]
     lib.mugd_set_tc_single_pass_tf32.argtypes = [C.c_void_p, C.c_int]
     lib.mugd_set_attention_impl.argtypes = [C.c_void_p, C.c_int]
+    lib.mugd_set_s4conv_impl.argtypes = [C.c_void_p, C.c_int]
     lib.mugd_debug_set_tc_tile_n.argtypes = [C.c_int]
     lib.mugd_debug_set_tc_cost.argtypes = [C.c_float, C.c_float, C.c_float, C.c_float]
     # measurement switches for tuning sweeps (tools/); none of them changes results
@@ -258,7 +259,7 @@ EXPORTED_SYMBOLS = [
     "mugd_abi_version", "mugd_last_error", "mugd_create", "mugd_destroy", "mugd_device_info", "mugd_set_gemm_impl",
     "mugd_op_run", "mugd_plan_create", "mugd_plan_run", "mugd_plan_capture", "mugd_plan_replay",
     "mugd_plan_launch_count", "mugd_plan_destroy", "mugd_s4_kernel_gen", "mugd_fill_i32", "mugd_abi_sizes", "mugd_gemm_tc_query",
-    "mugd_set_pdl", "mugd_set_tc_single_pass_tf32", "mugd_set_attention_impl", "mugd_debug_set_tc_tile_n", "mugd_debug_set_tc_cost", "mugd_gemm_tc_variant",
+    "mugd_set_pdl", "mugd_set_tc_single_pass_tf32", "mugd_set_attention_impl", "mugd_set_s4conv_impl", "mugd_debug_set_tc_tile_n", "mugd_debug_set_tc_cost", "mugd_gemm_tc_variant",
     "mugd_debug_set_attention_dump", "mugd_debug_set_tc_timing", "mugd_sample", "mugd_plan_save", "mugd_plan_load", "mugd_plan_regions", "mugd_plan_ops",
     "mugd_melspec", "mugd_grid_scan", "mugd_chart_snap", "mugd_remove_mini_jacks",
     "mugd_sample_staged", "mugd_sample_plms", "mugd_plms_combine",

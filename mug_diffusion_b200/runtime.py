@@ -11,6 +11,7 @@ import torch
 from torch.utils.weak import WeakIdKeyDictionary
 
 from . import lib as L_
+from .audio import check_z_length
 from .config import EncoderConfig, ModelConfig
 from .engine import (Arena, CTX_TOKENS_MAX, DecoderCompiler, EncoderCompiler, MAX_STEPS, OpList, UNetCompiler, View, tc_weight_map)
 from .packer import WeightBlob, pack_model
@@ -249,6 +250,7 @@ class MugEngine:
         return s
 
     def session(self, Beff: int, Lz: int, per_sample_t: bool = False) -> "Session":
+        check_z_length(Lz)
         return self._lru_get(self.sessions, (Beff, Lz, per_sample_t), lambda: Session(self, Beff, Lz, per_sample_t))
 
     def wave_session(self, B: int, T: int):
@@ -259,6 +261,7 @@ class MugEngine:
         return self._lru_get(self.dec_sessions, ("wave", B, T), lambda: WaveSession(self, B, T))
 
     def decoder_session(self, B: int, Lz: int) -> "DecoderSession":
+        check_z_length(Lz)
         return self._lru_get(self.dec_sessions, (B, Lz), lambda: DecoderSession(self, B, Lz))
 
     @property
