@@ -235,9 +235,11 @@ int  mugd_plan_launch_count(mugd_plan* p);                 /* kernels launched b
 void mugd_plan_destroy(mugd_plan* p);
 
 /* ---- the sampler loop from ONE call: DDIMSampler.ddim_sampling's for-loop (ddim.py:136-157) -------------------------------
- * n_steps x { replay the captured evaluation plan (one CUDA graph = Beff U-Net evaluations) ; run the `tail` ops eagerly on the same
- * stream: MUGD_OP_DDIM_UPDATE (CFG combine + x_{t-1}) and MUGD_OP_STEP_ADVANCE (device step counter) }.  Nothing synchronises; the
- * step-dependent rows (time embedding, DDIM coefficients) are selected on the device by the counter.  `eval_plan` must be captured. */
+ * Every mugd_sample* call runs the same loop, n_steps x { pre-step kernels ; replay of the captured evaluation plan (one CUDA graph =
+ * Beff U-Net evaluations) ; the step's kernels ; *step += 1 on the device step counter }, on one stream with nothing synchronising:
+ * the step-dependent rows (time embedding, sampler coefficients) are selected on the device by the counter.  `eval_plan` must be
+ * captured, and every argument is checked before the first launch.  Here the step's kernels are the `tail` ops, run eagerly:
+ * MUGD_OP_DDIM_UPDATE (CFG combine + x_{t-1}) and MUGD_OP_STEP_ADVANCE (the counter advance). */
 int  mugd_sample(mugd_plan* eval_plan, const mugd_op* tail, int32_t n_tail, int32_t n_steps, void* stream);
 
 /* ---- the same loop for inpainting and eta > 0 requests: what the host stages in front of each step ---------------------------
@@ -260,9 +262,8 @@ typedef struct mugd_stage {
     float* noise_rows;                     /* [B*L, C] the DDIM op's noise rows                                */
     int32_t B, C, L, reserved_;
 } mugd_stage;
-/* n_steps x { stage kernel for step i ; replay of the captured evaluation plan ; the tail ops }.  Every argument is checked before the
- * first launch: each MUGD_OP_DDIM_UPDATE of the tail must update the same rows (x, x_dup, n = B*C*L) and, with noise, read noise_rows.
- * A standalone entry point: the ABI version is unchanged. */
+/* n_steps x { stage kernel for step i ; replay of the captured evaluation plan ; the tail ops }.  Each MUGD_OP_DDIM_UPDATE of the tail
+ * must update the same rows (x, x_dup, n = B*C*L) and, with noise, read noise_rows. */
 int  mugd_sample_staged(mugd_plan* eval_plan, const mugd_stage* stage, const mugd_op* tail, int32_t n_tail, int32_t n_steps,
                         void* stream);
 
@@ -289,9 +290,8 @@ typedef struct mugd_plms {
     float* x_stash;                        /* [n] x across step 0's second evaluation                                           */
     int32_t cfg; float scale;              /* classifier-free guidance: cfg = 1 and its scale                                  */
 } mugd_plms;
-/* steps first_step .. first_step + n_steps - 1 of the update's S-step request, no host synchronisation.  Every argument is checked before
- * the first launch.  Launches per step: the plan's graph, the combine kernel, the update and the advance (step 0: one more graph replay,
- * combine and update, two counter fills and two copies).  A standalone entry point: the ABI version is unchanged. */
+/* steps first_step .. first_step + n_steps - 1 of the update's S-step request.  Launches per step: the plan's graph, the combine
+ * kernel, the update and the advance (step 0: one more graph replay, combine and update, two counter fills and two copies). */
 int  mugd_sample_plms(mugd_plan* eval_plan, const mugd_plms* p, int32_t first_step, int32_t n_steps, void* stream);
 /* the combine kernel alone for step `step` (heun = 1: step 0's second combine), for a host that runs the PLMS steps one by one */
 int  mugd_plms_combine(const mugd_plms* p, int32_t step, int32_t heun, void* stream);
@@ -323,9 +323,8 @@ typedef struct mugd_ddpm {
     int32_t clip;                          /* 1 = clip_denoised                                                                 */
     int32_t reserved_;
 } mugd_ddpm;
-/* steps first_step .. first_step + n_steps - 1 of the T-step request, no host synchronisation: n_steps x { graph replay, update with
- * noise row k, *step += 1 }, the same launches per step as mugd_sample.  Every argument is checked before the first launch
- * (first_step + n_steps <= T <= MUGD_MAX_STEPS).  A standalone entry point: the ABI version is unchanged. */
+/* steps first_step .. first_step + n_steps - 1 of the T-step request: n_steps x { graph replay, update with noise row k, *step += 1 },
+ * the same launches per step as mugd_sample (first_step + n_steps <= T <= MUGD_MAX_STEPS). */
 int  mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_step, int32_t n_steps, void* stream);
 /* the update kernel alone (noise row 0, the counter not advanced), for a host that runs the DDPM steps one by one */
 int  mugd_ddpm_update(const mugd_ddpm* d, void* stream);
@@ -352,9 +351,8 @@ typedef struct mugd_dpm {
     int32_t n, S;                          /* elements of x; steps of the request (S <= MUGD_MAX_STEPS)                         */
     int32_t cfg; float scale;              /* classifier-free guidance: cfg = 1 and its scale                                  */
 } mugd_dpm;
-/* steps first_step .. first_step + n_steps - 1 of the S-step request, no host synchronisation: n_steps x { graph replay, update,
- * *step += 1 }, the same launches per step as mugd_sample.  Every argument is checked before the first launch
- * (first_step + n_steps <= S <= MUGD_MAX_STEPS).  A standalone entry point: the ABI version is unchanged. */
+/* steps first_step .. first_step + n_steps - 1 of the S-step request: n_steps x { graph replay, update, *step += 1 }, the same
+ * launches per step as mugd_sample (first_step + n_steps <= S <= MUGD_MAX_STEPS). */
 int  mugd_sample_dpm(mugd_plan* eval_plan, const mugd_dpm* d, int32_t first_step, int32_t n_steps, void* stream);
 /* the update kernel alone (the counter not advanced), for a host that runs the DPM-Solver++ steps one by one */
 int  mugd_dpm_update(const mugd_dpm* d, void* stream);
@@ -377,10 +375,10 @@ typedef struct mugd_dpm_ex {
     const float* order_coef;               /* [S][3][8] device per-order rows, given exactly with start                         */
     int32_t B, reserved_;                  /* charts (with start)                                                              */
 } mugd_dpm_ex;
-/* steps first_step .. first_step + n_steps - 1 of the S-step request (the counter holding first_step), no host synchronisation:
- * n_steps x { stage kernel (with stage) ; graph replay ; update ; *step += 1 }: with a stage the launches per step of
- * mugd_sample_staged, otherwise those of mugd_sample_dpm.  Every argument is checked before the first launch (first_step + n_steps <=
- * S, the stage's q_coef rows finite).  A standalone entry point: the ABI version is unchanged. */
+/* steps first_step .. first_step + n_steps - 1 of the S-step request (the counter holding first_step): n_steps x { stage kernel (with
+ * stage) ; graph replay ; update ; *step += 1 }: with a stage the launches per step of mugd_sample_staged, otherwise those of
+ * mugd_sample_dpm (first_step + n_steps <= S, the stage's q_coef rows finite).  Unlike the other loops it checks the descriptor before
+ * the plan, so a host can test its arguments without a device. */
 int  mugd_sample_dpm_ex(mugd_plan* eval_plan, const mugd_dpm_ex* e, int32_t first_step, int32_t n_steps, void* stream);
 /* the update alone for the counter's step (per chart with start; the stage is not run), for a host that runs the steps one by one */
 int  mugd_dpm_ex_update(const mugd_dpm_ex* e, void* stream);
@@ -412,9 +410,8 @@ typedef struct mugd_join {
     int32_t B, C, L, reserved_;
 } mugd_join;
 /* steps first_step .. first_step + n_steps - 1 (the counter holding first_step): n_steps x { join kernel ; replay of the captured
- * evaluation plan ; the tail ops }, no host synchronisation: one launch per step more than mugd_sample.  Every argument is checked
- * before the first launch: the tail holds exactly one MUGD_OP_DDIM_UPDATE, on the join's x / x_dup with n = B*C*L, and
- * first_step + n_steps <= its S.  A standalone entry point: the ABI version is unchanged. */
+ * evaluation plan ; the tail ops }: one launch per step more than mugd_sample.  The tail holds exactly one MUGD_OP_DDIM_UPDATE, on the
+ * join's x / x_dup with n = B*C*L, and first_step + n_steps <= its S. */
 int  mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
                       int32_t n_steps, void* stream);
 

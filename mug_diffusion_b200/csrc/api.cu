@@ -62,6 +62,60 @@ static int dispatch(mugd_handle* h, const mugd_op& op, cudaStream_t st, int* lau
     }
 }
 
+// ---- the sampler loops -----------------------------------------------------------------------------------------------------
+// Step k of every mugd_sample* call: before(k) (pre-step kernels), one replay of the captured evaluation plan, after(k) (the
+// step's update kernels) and, given a device step counter, *step += 1.  The first failing call ends the loop with its code.
+template <typename Before, typename After>
+static int run_steps(const mugd_plan* eval_plan, int32_t n_steps, int32_t* step, cudaStream_t st, Before before, After after) {
+    mugd_step_advance adv;
+    adv.step = step;
+    for (int32_t k = 0; k < n_steps; ++k) {
+        int rc = before(k);
+        if (rc != MUGD_OK) return rc;
+        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
+        if ((rc = after(k)) != MUGD_OK) return rc;
+        if (step && (rc = launch_step_advance(eval_plan->h->dev, adv, st, nullptr)) != MUGD_OK) return rc;
+    }
+    return MUGD_OK;
+}
+
+static int no_kernels(int32_t) { return MUGD_OK; }
+
+// The DDIM loops: the tail ops (MUGD_OP_DDIM_UPDATE, MUGD_OP_STEP_ADVANCE, ...) after each replay; they advance the counter.
+template <typename Before>
+static int run_tail_steps(const mugd_plan* eval_plan, const mugd_op* tail, int32_t n_tail, int32_t n_steps, cudaStream_t st,
+                          Before before) {
+    return run_steps(eval_plan, n_steps, nullptr, st, before, [&](int32_t) {
+        for (int32_t k = 0; k < n_tail; ++k) {
+            int rc = dispatch(eval_plan->h, tail[k], st, nullptr);
+            if (rc != MUGD_OK) return rc;
+        }
+        return (int)MUGD_OK;
+    });
+}
+
+// DPM-Solver++: the stage kernel in front of each step (inpainting), then the update, per chart with starts.
+static int run_dpm_steps(const mugd_plan* eval_plan, const mugd_dpm_ex& e, int32_t n_steps, cudaStream_t st) {
+    return run_steps(
+        eval_plan, n_steps, e.dpm.step, st, [&](int32_t k) { return e.stage ? launch_stage(*e.stage, k, st) : MUGD_OK; },
+        [&](int32_t) { return launch_dpm_ex_update(e, st); });
+}
+
+static int check_step_range(const char* fn, int32_t first_step, int32_t n_steps, const char* total_name, int32_t total) {
+    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= total,
+                 "%s: first_step=%d, n_steps=%d outside the %s=%d steps of the request", fn, first_step, n_steps, total_name, total);
+    return MUGD_OK;
+}
+
+// A DDIM update in the tail of a staged or join loop must update the rows the pre-step kernel (`what`) writes.
+static int check_tail_rows(const char* fn, const char* what, int k, const mugd_ddim_update& d, const float* x, const float* x_dup,
+                           int32_t B, int32_t C, int32_t L) {
+    const int64_t n = (int64_t)B * C * L;
+    MUGD_REQUIRE(d.x == x && d.x_dup == x_dup, "%s: tail op %d updates other rows than the %s's x / x_dup", fn, k, what);
+    MUGD_REQUIRE(d.n == n, "%s: tail op %d updates n=%d elements, the %s B*C*L=%lld", fn, k, d.n, what, (long long)n);
+    return MUGD_OK;
+}
+
 }  // namespace mugd
 
 using namespace mugd;
@@ -214,15 +268,7 @@ int mugd_plan_replay(mugd_plan* p, int32_t times, void* stream) {
 int mugd_sample(mugd_plan* eval_plan, const mugd_op* tail, int32_t n_tail, int32_t n_steps, void* stream) {
     MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample: the evaluation plan must be captured (mugd_plan_capture)");
     MUGD_REQUIRE(n_steps >= 0 && n_tail >= 0 && (n_tail == 0 || tail), "mugd_sample: bad arguments");
-    cudaStream_t st = (cudaStream_t)stream;
-    for (int i = 0; i < n_steps; ++i) {
-        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
-        for (int k = 0; k < n_tail; ++k) {
-            int rc = dispatch(eval_plan->h, tail[k], st, nullptr);
-            if (rc != MUGD_OK) return rc;
-        }
-    }
-    return MUGD_OK;
+    return run_tail_steps(eval_plan, tail, n_tail, n_steps, (cudaStream_t)stream, no_kernels);
 }
 
 int mugd_sample_staged(mugd_plan* eval_plan, const mugd_stage* stage, const mugd_op* tail, int32_t n_tail, int32_t n_steps,
@@ -234,29 +280,16 @@ int mugd_sample_staged(mugd_plan* eval_plan, const mugd_stage* stage, const mugd
     const mugd_stage& s = *stage;
     int rc = check_stage(s, n_steps);
     if (rc != MUGD_OK) return rc;
-    const int64_t n = (int64_t)s.B * s.C * s.L;
     for (int k = 0; k < n_tail; ++k) {
         if (tail[k].kind != MUGD_OP_DDIM_UPDATE) continue;
         const mugd_ddim_update& d = tail[k].u.ddim;
-        MUGD_REQUIRE(d.x == s.x && d.x_dup == s.x_dup, "mugd_sample_staged: tail op %d updates other rows than the stage's x / x_dup", k);
-        MUGD_REQUIRE(d.n == n, "mugd_sample_staged: tail op %d updates n=%d elements, the stage B*C*L=%lld", k, d.n, (long long)n);
+        if ((rc = check_tail_rows("mugd_sample_staged", "stage", k, d, s.x, s.x_dup, s.B, s.C, s.L)) != MUGD_OK) return rc;
         MUGD_REQUIRE(!s.noise || d.noise == s.noise_rows, "mugd_sample_staged: tail op %d reads its noise from other rows than noise_rows",
                      k);
     }
     const bool staged = s.x0 || s.noise;
     cudaStream_t st = (cudaStream_t)stream;
-    for (int i = 0; i < n_steps; ++i) {
-        if (staged) {
-            rc = launch_stage(s, i, st);
-            if (rc != MUGD_OK) return rc;
-        }
-        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
-        for (int k = 0; k < n_tail; ++k) {
-            rc = dispatch(eval_plan->h, tail[k], st, nullptr);
-            if (rc != MUGD_OK) return rc;
-        }
-    }
-    return MUGD_OK;
+    return run_tail_steps(eval_plan, tail, n_tail, n_steps, st, [&](int32_t i) { return staged ? launch_stage(s, i, st) : MUGD_OK; });
 }
 
 int mugd_sample_plms(mugd_plan* eval_plan, const mugd_plms* p, int32_t first_step, int32_t n_steps, void* stream) {
@@ -265,17 +298,15 @@ int mugd_sample_plms(mugd_plan* eval_plan, const mugd_plms* p, int32_t first_ste
     int rc = check_plms(*p);
     if (rc != MUGD_OK) return rc;
     const mugd_ddim_update& u = p->update;
-    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= u.S,
-                 "mugd_sample_plms: first_step=%d, n_steps=%d outside the S=%d steps of the request", first_step, n_steps, u.S);
+    if ((rc = check_step_range("mugd_sample_plms", first_step, n_steps, "S", u.S)) != MUGD_OK) return rc;
     const DeviceInfo& dev = eval_plan->h->dev;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t xbytes = sizeof(float) * (size_t)u.n;
     int32_t* const step = const_cast<int32_t*>(u.step);      // the update reads the counter this loop sets and advances
-    mugd_step_advance adv;
-    adv.step = step;
-    for (int32_t i = first_step; i < first_step + n_steps; ++i) {
-        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
-        if ((rc = launch_plms_combine(*p, i, 0, st)) != MUGD_OK) return rc;
+    return run_steps(eval_plan, n_steps, step, st, no_kernels, [&](int32_t k) -> int {
+        const int32_t i = first_step + k;
+        int rc = launch_plms_combine(*p, i, 0, st);
+        if (rc != MUGD_OK) return rc;
         if (i == 0) {
             // pseudo improved Euler (plms.py:219-223): the Euler x_prev of e_t goes into both CFG halves of the input rows, the plan
             // evaluates it at t_next = time_range[min(1, S - 1)] (:145), then x is restored and e' = (e_t + e_t_next) / 2
@@ -287,10 +318,8 @@ int mugd_sample_plms(mugd_plan* eval_plan, const mugd_plms* p, int32_t first_ste
             if ((rc = launch_plms_combine(*p, 0, 1, st)) != MUGD_OK) return rc;
             if ((rc = mugd_fill_i32(step, 0, stream)) != MUGD_OK) return rc;
         }
-        if ((rc = launch_ddim_update(dev, u, st, nullptr)) != MUGD_OK) return rc;
-        if ((rc = launch_step_advance(dev, adv, st, nullptr)) != MUGD_OK) return rc;
-    }
-    return MUGD_OK;
+        return launch_ddim_update(dev, u, st, nullptr);
+    });
 }
 
 int mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_step, int32_t n_steps, void* stream) {
@@ -298,18 +327,9 @@ int mugd_sample_ddpm(mugd_plan* eval_plan, const mugd_ddpm* d, int32_t first_ste
     MUGD_REQUIRE(d, "mugd_sample_ddpm: null ddpm");
     int rc = check_ddpm(*d);
     if (rc != MUGD_OK) return rc;
-    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= d->T,
-                 "mugd_sample_ddpm: first_step=%d, n_steps=%d outside the T=%d steps of the request", first_step, n_steps, d->T);
-    const DeviceInfo& dev = eval_plan->h->dev;
+    if ((rc = check_step_range("mugd_sample_ddpm", first_step, n_steps, "T", d->T)) != MUGD_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    mugd_step_advance adv;
-    adv.step = d->step;
-    for (int32_t k = 0; k < n_steps; ++k) {
-        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
-        if ((rc = launch_ddpm_update(*d, k, st)) != MUGD_OK) return rc;
-        if ((rc = launch_step_advance(dev, adv, st, nullptr)) != MUGD_OK) return rc;
-    }
-    return MUGD_OK;
+    return run_steps(eval_plan, n_steps, d->step, st, no_kernels, [&](int32_t k) { return launch_ddpm_update(*d, k, st); });
 }
 
 int mugd_sample_dpm(mugd_plan* eval_plan, const mugd_dpm* d, int32_t first_step, int32_t n_steps, void* stream) {
@@ -317,18 +337,10 @@ int mugd_sample_dpm(mugd_plan* eval_plan, const mugd_dpm* d, int32_t first_step,
     MUGD_REQUIRE(d, "mugd_sample_dpm: null dpm");
     int rc = check_dpm(*d);
     if (rc != MUGD_OK) return rc;
-    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= d->S,
-                 "mugd_sample_dpm: first_step=%d, n_steps=%d outside the S=%d steps of the request", first_step, n_steps, d->S);
-    const DeviceInfo& dev = eval_plan->h->dev;
-    cudaStream_t st = (cudaStream_t)stream;
-    mugd_step_advance adv;
-    adv.step = d->step;
-    for (int32_t k = 0; k < n_steps; ++k) {
-        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
-        if ((rc = launch_dpm_update(*d, st)) != MUGD_OK) return rc;
-        if ((rc = launch_step_advance(dev, adv, st, nullptr)) != MUGD_OK) return rc;
-    }
-    return MUGD_OK;
+    if ((rc = check_step_range("mugd_sample_dpm", first_step, n_steps, "S", d->S)) != MUGD_OK) return rc;
+    mugd_dpm_ex e = {};
+    e.dpm = *d;
+    return run_dpm_steps(eval_plan, e, n_steps, (cudaStream_t)stream);
 }
 
 int mugd_sample_dpm_ex(mugd_plan* eval_plan, const mugd_dpm_ex* e, int32_t first_step, int32_t n_steps, void* stream) {
@@ -336,20 +348,9 @@ int mugd_sample_dpm_ex(mugd_plan* eval_plan, const mugd_dpm_ex* e, int32_t first
     MUGD_REQUIRE(e, "mugd_sample_dpm_ex: null descriptor");
     int rc = check_dpm_ex(*e, n_steps);
     if (rc != MUGD_OK) return rc;
-    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= e->dpm.S,
-                 "mugd_sample_dpm_ex: first_step=%d, n_steps=%d outside the S=%d steps of the request", first_step, n_steps, e->dpm.S);
+    if ((rc = check_step_range("mugd_sample_dpm_ex", first_step, n_steps, "S", e->dpm.S)) != MUGD_OK) return rc;
     MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_dpm_ex: the evaluation plan must be captured (mugd_plan_capture)");
-    const DeviceInfo& dev = eval_plan->h->dev;
-    cudaStream_t st = (cudaStream_t)stream;
-    mugd_step_advance adv;
-    adv.step = e->dpm.step;
-    for (int32_t k = 0; k < n_steps; ++k) {
-        if (e->stage && (rc = launch_stage(*e->stage, k, st)) != MUGD_OK) return rc;
-        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
-        if ((rc = launch_dpm_ex_update(*e, st)) != MUGD_OK) return rc;
-        if ((rc = launch_step_advance(dev, adv, st, nullptr)) != MUGD_OK) return rc;
-    }
-    return MUGD_OK;
+    return run_dpm_steps(eval_plan, *e, n_steps, (cudaStream_t)stream);
 }
 
 int mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
@@ -360,29 +361,18 @@ int mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op*
     const mugd_join& j = *join;
     int rc = check_join(j);
     if (rc != MUGD_OK) return rc;
-    const int64_t n = (int64_t)j.B * j.C * j.L;
     const mugd_ddim_update* upd = nullptr;
     for (int k = 0; k < n_tail; ++k) {
         if (tail[k].kind != MUGD_OP_DDIM_UPDATE) continue;
         MUGD_REQUIRE(!upd, "mugd_sample_join: the tail holds more than one DDIM update (op %d)", k);
         upd = &tail[k].u.ddim;
-        MUGD_REQUIRE(upd->x == j.x && upd->x_dup == j.x_dup, "mugd_sample_join: tail op %d updates other rows than the join's x / x_dup", k);
-        MUGD_REQUIRE(upd->n == n, "mugd_sample_join: tail op %d updates n=%d elements, the join B*C*L=%lld", k, upd->n, (long long)n);
+        if ((rc = check_tail_rows("mugd_sample_join", "join", k, *upd, j.x, j.x_dup, j.B, j.C, j.L)) != MUGD_OK) return rc;
         MUGD_REQUIRE(upd->step, "mugd_sample_join: tail op %d has no device step counter", k);
     }
     MUGD_REQUIRE(upd, "mugd_sample_join: the tail holds no DDIM update");
-    MUGD_REQUIRE(first_step >= 0 && n_steps >= 0 && (int64_t)first_step + n_steps <= upd->S,
-                 "mugd_sample_join: first_step=%d, n_steps=%d outside the S=%d steps of the request", first_step, n_steps, upd->S);
+    if ((rc = check_step_range("mugd_sample_join", first_step, n_steps, "S", upd->S)) != MUGD_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    for (int i = 0; i < n_steps; ++i) {
-        if ((rc = launch_join(j, upd->step, st)) != MUGD_OK) return rc;
-        MUGD_CHECK_CUDA(cudaGraphLaunch(eval_plan->exec, st));
-        for (int k = 0; k < n_tail; ++k) {
-            rc = dispatch(eval_plan->h, tail[k], st, nullptr);
-            if (rc != MUGD_OK) return rc;
-        }
-    }
-    return MUGD_OK;
+    return run_tail_steps(eval_plan, tail, n_tail, n_steps, st, [&](int32_t) { return launch_join(j, upd->step, st); });
 }
 
 int mugd_abi_sizes(int32_t* out, int32_t n) {

@@ -86,6 +86,28 @@ int launch_join(const mugd_join& j, const int32_t* step, cudaStream_t st);
 int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, cudaStream_t st, int* launches);
 bool gemm_tc_supported(const mugd_gemm& g);
 
+// Descriptor checks shared by the sampler kernels; `who` prefixes the message ("ddpm", "dpm", ...).
+// cfg selects classifier-free guidance: 0 or 1.
+inline int check_cfg(const char* who, int cfg) {
+    MUGD_REQUIRE(cfg == 0 || cfg == 1, "%s: cfg=%d", who, cfg);
+    return MUGD_OK;
+}
+inline int check_scale(const char* who, float scale) {
+    MUGD_REQUIRE(isfinite(scale), "%s: scale is not finite", who);
+    return MUGD_OK;
+}
+// The evaluation reads x in both CFG halves, so an update that writes x writes its CFG copy exactly when cfg = 1.
+inline int check_x_dup(const char* who, const float* x_dup, int cfg) {
+    MUGD_REQUIRE(!x_dup == !cfg, "%s: x_dup must be given exactly when cfg = 1 (the evaluation reads x in both halves)", who);
+    return MUGD_OK;
+}
+// A kernel over 32x32 (channel, position) tiles of B samples [C, L]: int32 element indices, grid (L/32, C/32, B).
+inline int check_tile_grid(const char* who, int32_t B, int32_t C, int32_t L) {
+    MUGD_REQUIRE(B > 0 && C > 0 && L > 0 && (int64_t)B * C * L <= INT32_MAX, "%s: bad shape B=%d C=%d L=%d", who, B, C, L);
+    MUGD_REQUIRE(B <= 65535 && (C + 31) / 32 <= 65535, "%s: B=%d / C=%d too large for one launch", who, B, C);
+    return MUGD_OK;
+}
+
 // Kernels that need more than 48 KB of dynamic shared memory are allowed the device's opt-in maximum (`bytes`) by mugd_create, after
 // its cudaSetDevice: the attribute belongs to the current device's context, so it is set once for every device a handle is created
 // on.  A launch still asks for only its own byte count, so occupancy and the shared-memory carve-out do not change.  Each kernel
@@ -127,6 +149,27 @@ inline cudaError_t allow_dynamic_smem(int bytes, Kernels... kernels) {
 // launch with this grid's memory flush.  Explicit triggers
 // (at entry, in the short kernels only, after the GEMM main loop) were tried and not kept.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+// The noise prediction of element i of the sampler's eps rows: with cfg, the guidance combine e_u + scale * (e_c - e_u) of the
+// uncond half [0, n) and the cond half [n, 2n) (ddim.py:175), each operation one IEEE round-to-nearest in torch's eager order, no
+// contraction.  Every update kernel forms e here, so all of them match torch bit for bit.
+__device__ __forceinline__ float cfg_eps(const float* eps, int64_t i, int64_t n, int cfg, float scale) {
+    if (!cfg) return eps[i];
+    const float eu = eps[i], ec = eps[n + i];
+    return __fadd_rn(eu, __fmul_rn(scale, __fsub_rn(ec, eu)));
+}
+
+// Loads the 32x32 tile at (c0, l0) of one sample's NCL rows `in` [C, L] into tile[c - c0][l - l0], coalesced along L by a CTA of
+// 32 x 8 threads; entries past C or L are left unwritten.  The [32][33] padding keeps the transposed reads tile[tx][r] free of bank
+// conflicts.
+__device__ __forceinline__ void load_ncl_tile(float (&tile)[32][33], const float* in, int c0, int l0, int C, int L) {
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+#pragma unroll
+    for (int r = ty; r < 32; r += 8) {
+        const int c = c0 + r, l = l0 + tx;
+        if (c < C && l < L) tile[r][tx] = in[(int64_t)c * L + l];
+    }
+}
 
 // ---- device helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }

@@ -21,12 +21,7 @@ ddpm_update_kernel(const mugd_ddpm d, const float* __restrict__ nz) {
     const int c0 = blockIdx.y * 32, l0 = blockIdx.x * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;   // 32 x 8
     const int C = d.C, L = d.L;
-    const int64_t base = (int64_t)bb * C * L;
-#pragma unroll
-    for (int r = ty; r < 32; r += 8) {
-        const int c = c0 + r, l = l0 + tx;
-        if (c < C && l < L) t_n[r][tx] = nz[base + (int64_t)c * L + l];
-    }
+    load_ncl_tile(t_n, nz + (int64_t)bb * C * L, c0, l0, C, L);
     __syncthreads();
     const int t = d.T - 1 - *d.step;
     if ((unsigned)t >= (unsigned)d.T) return;
@@ -38,13 +33,7 @@ ddpm_update_kernel(const mugd_ddpm d, const float* __restrict__ nz) {
         const int l = l0 + r, c = c0 + tx;
         if (c >= C || l >= L) continue;
         const int64_t row = ((int64_t)bb * L + l) * C + c;
-        float e;
-        if (d.cfg) {
-            const float eu = d.eps[row], ec = d.eps[n + row];
-            e = __fadd_rn(eu, __fmul_rn(d.scale, __fsub_rn(ec, eu)));
-        } else {
-            e = d.eps[row];
-        }
+        const float e = cfg_eps(d.eps, row, n, d.cfg, d.scale);
         const float x = d.x[row];
         float xr = __fsub_rn(__fmul_rn(sra, x), __fmul_rn(srm1, e));
         if (d.clip && !isnan(xr)) xr = fminf(fmaxf(xr, -10.0f), 10.0f);
@@ -58,15 +47,13 @@ ddpm_update_kernel(const mugd_ddpm d, const float* __restrict__ nz) {
 
 int check_ddpm(const mugd_ddpm& d) {
     MUGD_REQUIRE(d.x && d.eps && d.noise && d.coef && d.step, "ddpm: x, eps, noise, coef and step must be given");
-    MUGD_REQUIRE(d.B > 0 && d.C > 0 && d.L > 0 && (int64_t)d.B * d.C * d.L <= INT32_MAX, "ddpm: bad shape B=%d C=%d L=%d", d.B, d.C,
-                 d.L);
-    MUGD_REQUIRE(d.B <= 65535 && (d.C + 31) / 32 <= 65535, "ddpm: B=%d / C=%d too large for one launch", d.B, d.C);
+    int rc = check_tile_grid("ddpm", d.B, d.C, d.L);
+    if (rc != MUGD_OK) return rc;
     MUGD_REQUIRE(d.T > 0 && d.T <= MUGD_MAX_STEPS, "ddpm: T=%d outside [1, %d]", d.T, MUGD_MAX_STEPS);
-    MUGD_REQUIRE(d.cfg == 0 || d.cfg == 1, "ddpm: cfg=%d", d.cfg);
+    if ((rc = check_cfg("ddpm", d.cfg)) != MUGD_OK) return rc;
     MUGD_REQUIRE(d.clip == 0 || d.clip == 1, "ddpm: clip=%d", d.clip);
-    MUGD_REQUIRE(isfinite(d.scale), "ddpm: scale is not finite");
-    MUGD_REQUIRE(!d.x_dup == !d.cfg, "ddpm: x_dup must be given exactly when cfg = 1 (the evaluation reads x in both halves)");
-    return MUGD_OK;
+    if ((rc = check_scale("ddpm", d.scale)) != MUGD_OK) return rc;
+    return check_x_dup("ddpm", d.x_dup, d.cfg);
 }
 
 int launch_ddpm_update(const mugd_ddpm& d, int32_t k, cudaStream_t st) {

@@ -15,13 +15,7 @@ namespace mugd {
 __device__ __forceinline__ void dpm_element(const mugd_dpm& d, const float* row, int order, int step, int i) {
     const float alpha = row[0], sigma = row[1], A = row[2], c0 = row[3];
     const int64_t N = d.n;
-    float e;
-    if (d.cfg) {
-        const float eu = d.eps[i], ec = d.eps[N + i];
-        e = __fadd_rn(eu, __fmul_rn(d.scale, __fsub_rn(ec, eu)));
-    } else {
-        e = d.eps[i];
-    }
+    const float e = cfg_eps(d.eps, i, N, d.cfg, d.scale);
     const float x = d.x[i];
     const float m0 = __fdiv_rn(__fsub_rn(x, __fmul_rn(sigma, e)), alpha);
     float xn = __fadd_rn(__fmul_rn(A, x), __fmul_rn(c0, m0));
@@ -65,10 +59,10 @@ int check_dpm(const mugd_dpm& d) {
     MUGD_REQUIRE(d.x && d.eps && d.ring && d.coef && d.step, "dpm: x, eps, ring, coef and step must be given");
     MUGD_REQUIRE(d.n > 0, "dpm: n=%d", d.n);
     MUGD_REQUIRE(d.S > 0 && d.S <= MUGD_MAX_STEPS, "dpm: S=%d outside [1, %d]", d.S, MUGD_MAX_STEPS);
-    MUGD_REQUIRE(d.cfg == 0 || d.cfg == 1, "dpm: cfg=%d", d.cfg);
-    MUGD_REQUIRE(isfinite(d.scale), "dpm: scale is not finite");
-    MUGD_REQUIRE(!d.x_dup == !d.cfg, "dpm: x_dup must be given exactly when cfg = 1 (the evaluation reads x in both halves)");
-    return MUGD_OK;
+    int rc = check_cfg("dpm", d.cfg);
+    if (rc != MUGD_OK) return rc;
+    if ((rc = check_scale("dpm", d.scale)) != MUGD_OK) return rc;
+    return check_x_dup("dpm", d.x_dup, d.cfg);
 }
 
 int launch_dpm_update(const mugd_dpm& d, cudaStream_t st) {

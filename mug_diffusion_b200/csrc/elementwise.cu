@@ -22,13 +22,7 @@ ddim_update_kernel(const mugd_ddim_update d) {
     const int index = d.S - 1 - step;                     // ddim.py:138
     const float* cf = d.coef + 4 * index;
     const float a_t = cf[0], a_prev = cf[1], sigma = cf[2], s1m = cf[3];
-    float e;
-    if (d.cfg) {
-        const float eu = d.eps[i], ec = d.eps[(int64_t)d.n + i];
-        e = __fadd_rn(eu, __fmul_rn(d.scale, __fsub_rn(ec, eu)));   // ddim.py:175
-    } else {
-        e = d.eps[i];
-    }
+    const float e = cfg_eps(d.eps, i, d.n, d.cfg, d.scale);   // ddim.py:175
     const float x = d.x[i];
     const float pred = __fdiv_rn(__fsub_rn(x, __fmul_rn(s1m, e)), __fsqrt_rn(a_t));            // :189
     const float dir = __fmul_rn(__fsqrt_rn(__fsub_rn(__fsub_rn(1.0f, a_prev), __fmul_rn(sigma, sigma))), e);  // :191
@@ -59,6 +53,7 @@ stage_kernel(const mugd_stage s, const float* __restrict__ qn, const float* __re
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;   // 32 x 8
     const int C = s.C, L = s.L;
     const int64_t base = (int64_t)bb * C * L;
+    // load_ncl_tile's loop, once for all four tiles: four calls would load the tiles one after another instead of interleaved
 #pragma unroll
     for (int r = ty; r < 32; r += 8) {
         const int c = c0 + r, l = l0 + tx;
@@ -91,9 +86,8 @@ stage_kernel(const mugd_stage s, const float* __restrict__ qn, const float* __re
 
 int check_stage(const mugd_stage& s, int32_t n_steps) {
     MUGD_REQUIRE(s.x, "sample_staged: stage.x is NULL");
-    MUGD_REQUIRE(s.B > 0 && s.C > 0 && s.L > 0 && (int64_t)s.B * s.C * s.L <= INT32_MAX, "sample_staged: bad shape B=%d C=%d L=%d",
-                 s.B, s.C, s.L);
-    MUGD_REQUIRE(s.B <= 65535 && (s.C + 31) / 32 <= 65535, "sample_staged: B=%d / C=%d too large for one launch", s.B, s.C);
+    int rc = check_tile_grid("sample_staged", s.B, s.C, s.L);
+    if (rc != MUGD_OK) return rc;
     MUGD_REQUIRE(!s.q_coef || s.q_noise, "sample_staged: q_coef given without a q-noise table");
     MUGD_REQUIRE(!s.q_noise || s.x0, "sample_staged: q-noise table given without x0");
     MUGD_REQUIRE(!s.mask || s.x0, "sample_staged: mask given without x0");

@@ -17,13 +17,7 @@ plms_combine_kernel(const float* __restrict__ eps, float* __restrict__ hist, flo
     pdl_wait();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    float e;
-    if (cfg) {
-        const float eu = eps[i], ec = eps[(int64_t)n + i];
-        e = __fadd_rn(eu, __fmul_rn(scale, __fsub_rn(ec, eu)));                                   // plms.py:186
-    } else {
-        e = eps[i];
-    }
+    const float e = cfg_eps(eps, i, n, cfg, scale);                                                // plms.py:186
     const int64_t N = n;
     float ep;
     if (heun) {
@@ -56,9 +50,9 @@ int check_plms(const mugd_plms& p) {
     MUGD_REQUIRE(u.eps == p.e_prime, "plms: update.eps must be e_prime (the update runs on e')");
     MUGD_REQUIRE(u.cfg == 0, "plms: update.cfg must be 0 (the combine kernel applies the guidance)");
     MUGD_REQUIRE(u.noise == nullptr, "plms: update.noise must be NULL (PLMS runs at eta = 0)");
-    MUGD_REQUIRE(p.cfg == 0 || p.cfg == 1, "plms: cfg=%d", p.cfg);
-    MUGD_REQUIRE(isfinite(p.scale), "plms: scale is not finite");
-    return MUGD_OK;
+    int rc = check_cfg("plms", p.cfg);
+    if (rc != MUGD_OK) return rc;
+    return check_scale("plms", p.scale);
 }
 
 int launch_plms_combine(const mugd_plms& p, int32_t step, int heun, cudaStream_t st) {

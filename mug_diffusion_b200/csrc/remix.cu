@@ -42,12 +42,7 @@ join_kernel(const mugd_join j, const int32_t* __restrict__ step) {
     const int c0 = blockIdx.y * 32, l0 = blockIdx.x * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;   // 32 x 8
     const int C = j.C, L = j.L;
-    const float* in = j.x_latent + (int64_t)bb * C * L;
-#pragma unroll
-    for (int r = ty; r < 32; r += 8) {
-        const int c = c0 + r, l = l0 + tx;
-        if (c < C && l < L) tile[r][tx] = in[(int64_t)c * L + l];
-    }
+    load_ncl_tile(tile, j.x_latent + (int64_t)bb * C * L, c0, l0, C, L);
     __syncthreads();
 #pragma unroll
     for (int r = ty; r < 32; r += 8) {
@@ -61,10 +56,7 @@ join_kernel(const mugd_join j, const int32_t* __restrict__ step) {
 
 int check_join(const mugd_join& j) {
     MUGD_REQUIRE(j.x && j.x_latent && j.join, "sample_join: x, x_latent and join must be given");
-    MUGD_REQUIRE(j.B > 0 && j.C > 0 && j.L > 0 && (int64_t)j.B * j.C * j.L <= INT32_MAX, "sample_join: bad shape B=%d C=%d L=%d", j.B,
-                 j.C, j.L);
-    MUGD_REQUIRE(j.B <= 65535 && (j.C + 31) / 32 <= 65535, "sample_join: B=%d / C=%d too large for one launch", j.B, j.C);
-    return MUGD_OK;
+    return check_tile_grid("sample_join", j.B, j.C, j.L);
 }
 
 int launch_join(const mugd_join& j, const int32_t* step, cudaStream_t st) {

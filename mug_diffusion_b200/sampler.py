@@ -429,7 +429,8 @@ class MugDiffusionB200:
 # what every sampler shares: the request's session and the request loop
 # --------------------------------------------------------------------------------------------------
 class _DeviceLoopSampler:
-    """The constructor, the per-request session load and the request loop (``_run_request``) of every sampler here."""
+    """The constructor, the per-request session load and the request loop (``_run_request``) of every sampler here, and the
+    encode launch and latent check of the samplers that remix a chart."""
 
     def __init__(self, model, schedule="linear", **kwargs):
         if not isinstance(model, MugDiffusionB200):
@@ -524,6 +525,39 @@ class _DeviceLoopSampler:
                     record()
         self.last_launches_per_step = sess.plan.launches + tail_launches
         return self._read_x(sess, shape), intermediates
+
+    def _stochastic_encode(self, x0, noise, indices, tables, n):
+        """``stochastic_encode``'s kernel: out[b] = sqrt_a[t[b]] * x0[b] + sqrt_1ma[t[b]] * noise[b] (noise = randn_like(x0) when not
+        given), t = ``indices(B)`` (which checks them), (sqrt_a, sqrt_1ma) = ``tables()`` of n rows.  ValueError before any GPU work."""
+        dev = self.device
+        if not isinstance(x0, torch.Tensor) or x0.dim() != 3 or x0.dtype != torch.float32 or x0.device != torch.device(dev):
+            raise ValueError(f"x0 must be a float32 [B, C, L] tensor on {dev}")
+        t = indices(x0.shape[0])
+        if noise is not None and (not isinstance(noise, torch.Tensor) or noise.shape != x0.shape or noise.dtype != torch.float32
+                                  or noise.device != x0.device):
+            raise ValueError(f"noise must be a float32 tensor of x0's shape {tuple(x0.shape)} on {dev}")
+        if noise is None:
+            noise = torch.randn_like(x0)
+        out = torch.empty(x0.shape, device=dev)
+        if out.numel() == 0:
+            return out
+        sa, s1m = tables()
+        x0c, nc = x0.contiguous(), noise.contiguous()
+        td = torch.as_tensor(t, dtype=torch.int64).to(dev)
+        d = L_.QEncode()
+        d.x0, d.noise, d.t, d.sqrt_a, d.sqrt_1ma, d.out = _ptr(x0c), _ptr(nc), _ptr(td), _ptr(sa), _ptr(s1m), _ptr(out)
+        d.B, d.C, d.L, d.n = x0.shape[0], x0.shape[1], x0.shape[2], n
+        eng = self.model.engine
+        with eng.lock:
+            L_.check(eng.lib.mugd_stochastic_encode(C.byref(d), torch.cuda.current_stream().cuda_stream), "mugd_stochastic_encode")
+        return out
+
+    def _check_latent(self, x_latent):
+        """ValueError unless ``x_latent`` is a [B, z_channels, L] tensor with B >= 1 (what ``decode`` starts from)"""
+        z = self.model.z_channels
+        if not isinstance(x_latent, torch.Tensor) or x_latent.dim() != 3 or x_latent.shape[0] < 1 or x_latent.shape[1] != z:
+            raise ValueError(f"x_latent must be a [B, {z}, L] tensor"
+                             + (f", got {tuple(x_latent.shape)}" if isinstance(x_latent, torch.Tensor) else ""))
 
 
 def _step_ops(sess: Session, update: Optional[L_.DdimUpdate] = None) -> OpList:
@@ -745,36 +779,23 @@ class DDIMSampler(_DeviceLoopSampler):
         if not use_original_steps:
             self._require_schedule("stochastic_encode")
         n = int(model.sqrt_alphas_cumprod.shape[0] if use_original_steps else len(self.ddim_alphas))
-        if not isinstance(x0, torch.Tensor) or x0.dim() != 3 or x0.dtype != torch.float32 or x0.device != torch.device(dev):
-            raise ValueError(f"x0 must be a float32 [B, C, L] tensor on {dev}")
-        B = x0.shape[0]
-        tt = torch.as_tensor(t)
-        if tt.dtype in (torch.bool,) or tt.is_floating_point() or tt.is_complex() or tuple(tt.shape) != (B,):
-            raise ValueError(f"t must be {B} integer table indices, one per chart (got dtype {tt.dtype}, shape {tuple(tt.shape)})")
-        th = tt.cpu()
-        if B and (int(th.min()) < 0 or int(th.max()) > n - 1):
-            raise ValueError(f"t={th.tolist()}: indices must lie in [0, {n - 1}]")
-        if noise is not None and (not isinstance(noise, torch.Tensor) or noise.shape != x0.shape or noise.dtype != torch.float32
-                                  or noise.device != x0.device):
-            raise ValueError(f"noise must be a float32 tensor of x0's shape {tuple(x0.shape)} on {dev}")
-        if noise is None:
-            noise = torch.randn_like(x0)
-        if use_original_steps:
-            sa, s1m = model.sqrt_alphas_cumprod, model.sqrt_one_minus_alphas_cumprod
-        else:
-            sa = torch.sqrt(torch.as_tensor(self.ddim_alphas).to(dev, torch.float32))
-            s1m = torch.as_tensor(self.ddim_sqrt_one_minus_alphas).to(dev, torch.float32)
-        out = torch.empty(x0.shape, device=dev)
-        if out.numel() == 0:
-            return out
-        x0c, nc = x0.contiguous(), noise.contiguous()
-        td = th.to(dev, torch.int64)
-        d = L_.QEncode()
-        d.x0, d.noise, d.t, d.sqrt_a, d.sqrt_1ma, d.out = _ptr(x0c), _ptr(nc), _ptr(td), _ptr(sa), _ptr(s1m), _ptr(out)
-        d.B, d.C, d.L, d.n = B, x0.shape[1], x0.shape[2], n
-        with model.engine.lock:
-            L_.check(model.engine.lib.mugd_stochastic_encode(C.byref(d), torch.cuda.current_stream().cuda_stream), "mugd_stochastic_encode")
-        return out
+
+        def indices(B):
+            tt = torch.as_tensor(t)
+            if tt.dtype in (torch.bool,) or tt.is_floating_point() or tt.is_complex() or tuple(tt.shape) != (B,):
+                raise ValueError(f"t must be {B} integer table indices, one per chart (got dtype {tt.dtype}, shape {tuple(tt.shape)})")
+            th = tt.cpu()
+            if B and (int(th.min()) < 0 or int(th.max()) > n - 1):
+                raise ValueError(f"t={th.tolist()}: indices must lie in [0, {n - 1}]")
+            return th
+
+        def tables():
+            if use_original_steps:
+                return model.sqrt_alphas_cumprod, model.sqrt_one_minus_alphas_cumprod
+            return (torch.sqrt(torch.as_tensor(self.ddim_alphas).to(dev, torch.float32)),
+                    torch.as_tensor(self.ddim_sqrt_one_minus_alphas).to(dev, torch.float32))
+
+        return self._stochastic_encode(x0, noise, indices, tables, n)
 
     def _decode_starts(self, x_latent, t_start):
         """the per-chart start indices of a decode request; ValueError for malformed ones"""
@@ -799,9 +820,7 @@ class DDIMSampler(_DeviceLoopSampler):
         self._require_schedule("decode")
         if np.any(np.asarray(self.ddim_sigmas) != 0):
             raise ValueError("decode runs at eta = 0: call make_schedule(S, ddim_eta=0.)")
-        if not isinstance(x_latent, torch.Tensor) or x_latent.dim() != 3 or x_latent.shape[0] < 1 or x_latent.shape[1] != model.z_channels:
-            raise ValueError(f"x_latent must be a [B, {model.z_channels}, L] tensor"
-                             + (f", got {tuple(x_latent.shape)}" if isinstance(x_latent, torch.Tensor) else ""))
+        self._check_latent(x_latent)
         starts = self._decode_starts(x_latent, t_start)
         scale, uc = unconditional_guidance_scale, unconditional_conditioning
         B, Cz, Lz = (int(v) for v in x_latent.shape)
@@ -1211,30 +1230,9 @@ class DPMSolverSampler(_DeviceLoopSampler):
         starts (no off-by-one, unlike DDIM's stochastic_encode / decode pair); s = 0 returns x0 exactly.  noise = torch.randn_like(x0)
         when not given.  One kernel (mugd_stochastic_encode over the schedule's float32 tables of S + 1 rows).  ValueError, before any
         GPU work, for malformed arguments."""
-        model = self.model
-        dev = self.device
         self._require_schedule(sched)
-        if not isinstance(x0, torch.Tensor) or x0.dim() != 3 or x0.dtype != torch.float32 or x0.device != torch.device(dev):
-            raise ValueError(f"x0 must be a float32 [B, C, L] tensor on {dev}")
-        B = x0.shape[0]
-        steps = per_chart_steps(B, t_enc, sched.S, "t_enc", " (S = sched.S)")
-        if noise is not None and (not isinstance(noise, torch.Tensor) or noise.shape != x0.shape or noise.dtype != torch.float32
-                                  or noise.device != x0.device):
-            raise ValueError(f"noise must be a float32 tensor of x0's shape {tuple(x0.shape)} on {dev}")
-        if noise is None:
-            noise = torch.randn_like(x0)
-        out = torch.empty(x0.shape, device=dev)
-        if out.numel() == 0:
-            return out
-        a, s = (torch.from_numpy(v).to(dev) for v in sched.encode_tables_f32())
-        x0c, nc = x0.contiguous(), noise.contiguous()
-        td = torch.tensor(steps, dtype=torch.int64, device=dev)
-        d = L_.QEncode()
-        d.x0, d.noise, d.t, d.sqrt_a, d.sqrt_1ma, d.out = _ptr(x0c), _ptr(nc), _ptr(td), _ptr(a), _ptr(s), _ptr(out)
-        d.B, d.C, d.L, d.n = B, x0.shape[1], x0.shape[2], sched.S + 1
-        with model.engine.lock:
-            L_.check(model.engine.lib.mugd_stochastic_encode(C.byref(d), torch.cuda.current_stream().cuda_stream), "mugd_stochastic_encode")
-        return out
+        return self._stochastic_encode(x0, noise, lambda B: per_chart_steps(B, t_enc, sched.S, "t_enc", " (S = sched.S)"),
+                                       lambda: [torch.from_numpy(v).to(self.device) for v in sched.encode_tables_f32()], sched.S + 1)
 
     @torch.no_grad()
     def decode(self, x_latent, c, w, t_start, sched: dpm_solver.DPMSchedule, unconditional_guidance_scale=1.,
@@ -1249,9 +1247,7 @@ class DPMSolverSampler(_DeviceLoopSampler):
         charts by strength into separate calls to avoid the idle rows.  Every argument is checked before any GPU work (ValueError)."""
         model = self.model
         self._require_schedule(sched)
-        if not isinstance(x_latent, torch.Tensor) or x_latent.dim() != 3 or x_latent.shape[0] < 1 or x_latent.shape[1] != model.z_channels:
-            raise ValueError(f"x_latent must be a [B, {model.z_channels}, L] tensor"
-                             + (f", got {tuple(x_latent.shape)}" if isinstance(x_latent, torch.Tensor) else ""))
+        self._check_latent(x_latent)
         starts = per_chart_steps(x_latent.shape[0], t_start, sched.S, "t_start", " (S = sched.S)")
         scale = _finite_scale(unconditional_guidance_scale)
         B, Cz, Lz = (int(v) for v in x_latent.shape)
