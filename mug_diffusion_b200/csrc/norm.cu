@@ -224,6 +224,7 @@ int launch_layernorm(const DeviceInfo&, const mugd_layernorm& g, cudaStream_t st
     MUGD_REQUIRE(g.C % 4 == 0 && g.C <= LN_MAXQ * 128, "layernorm: C=%d must be a multiple of 4 and <= %d", g.C, LN_MAXQ * 128);
     MUGD_REQUIRE(g.ldx % 4 == 0 && g.ldy % 4 == 0 && aligned16(g.x) && aligned16(g.y) && aligned16(g.gamma) && aligned16(g.beta),
                  "layernorm: operands must be 16-byte aligned with ld %% 4 == 0");
+    MUGD_REQUIRE(g.ldx >= g.C && g.ldy >= g.C, "layernorm: leading dimension smaller than C");
     const int blocks = (g.rows + LN_WARPS - 1) / LN_WARPS;
     MUGD_CHECK_CUDA(launch_k(layernorm_kernel, dim3(blocks), dim3(LN_WARPS * 32), 0, st, g.x, g.ldx, g.y, g.ldy, g.gamma, g.beta, g.rows,
                              g.C, g.eps));
