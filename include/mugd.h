@@ -383,6 +383,26 @@ int  mugd_sample_dpm_ex(mugd_plan* eval_plan, const mugd_dpm_ex* e, int32_t firs
 /* the update alone for the counter's step (per chart with start; the stage is not run), for a host that runs the steps one by one */
 int  mugd_dpm_ex_update(const mugd_dpm_ex* e, void* stream);
 
+/* ---- DPM-Solver++ inversion: an existing chart run backwards to its noise, with one stop per chart -------------------------------
+ * mugd_dpm_stop runs a mugd_dpm request whose coefficient rows are an inversion schedule's (the grid reversed, from t = 1/N up): chart
+ * b (elements b * n/B .. (b+1) * n/B - 1 of the dense rows) runs steps 0 .. stop[b] - 1 and is left untouched from step stop[b] on
+ * (x, x_dup, ring and pred_x0 neither read nor written), so after the loop it sits at the node of its own stop.  A running chart
+ * applies coefficient row i as the mugd_dpm update does, bit for bit, except a row whose column 7 is nonzero: an order-1 step in
+ * DDIM's form, m0 as above, then x = coef[8i+4] * m0 + coef[8i+5] * e (alpha and sigma of the step's target time), each product and
+ * the sum one IEEE round-to-nearest.  That form avoids the cancellation of A * x + c0 * m0 when A = sigma_i+1 / sigma_i is large,
+ * as it is on the first steps away from t = 1/N.  All stops equal to S runs every chart through every row. */
+typedef struct mugd_dpm_stop {
+    mugd_dpm dpm;                          /* the update (coef [S][8], ring, step counter, ...)                                 */
+    const int32_t* stop;                   /* [B] device: the number of steps each chart runs                                  */
+    int32_t B, reserved_;                  /* charts (B divides n); reserved_ = 0                                              */
+} mugd_dpm_stop;
+/* steps first_step .. first_step + n_steps - 1 (the counter holding first_step): n_steps x { graph replay ; stop-aware update ;
+ * *step += 1 }, the launches per step of mugd_sample_dpm (first_step + n_steps <= S).  It checks the descriptor before the plan, so a
+ * host can test its arguments without a device. */
+int  mugd_sample_dpm_stop(mugd_plan* eval_plan, const mugd_dpm_stop* e, int32_t first_step, int32_t n_steps, void* stream);
+/* the stop-aware update alone for the counter's step, for a host that runs the steps one by one */
+int  mugd_dpm_stop_update(const mugd_dpm_stop* e, void* stream);
+
 /* ---- remixing an existing chart (SDEdit / img2img): DDIMSampler.stochastic_encode and decode with a per-chart start ---------------
  * mugd_stochastic_encode: out[b] = sqrt_a[t[b]] * x0[b] + sqrt_1ma[t[b]] * noise[b], each product and the sum one IEEE
  * round-to-nearest (no contraction), bit-identical to torch's extract_into_tensor expressions.  x0, noise and out are device NCL

@@ -353,6 +353,17 @@ int mugd_sample_dpm_ex(mugd_plan* eval_plan, const mugd_dpm_ex* e, int32_t first
     return run_dpm_steps(eval_plan, *e, n_steps, (cudaStream_t)stream);
 }
 
+int mugd_sample_dpm_stop(mugd_plan* eval_plan, const mugd_dpm_stop* e, int32_t first_step, int32_t n_steps, void* stream) {
+    // the descriptor is checked before the plan, so a host can test its arguments without a device
+    MUGD_REQUIRE(e, "mugd_sample_dpm_stop: null descriptor");
+    int rc = check_dpm_stop(*e);
+    if (rc != MUGD_OK) return rc;
+    if ((rc = check_step_range("mugd_sample_dpm_stop", first_step, n_steps, "S", e->dpm.S)) != MUGD_OK) return rc;
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_dpm_stop: the evaluation plan must be captured (mugd_plan_capture)");
+    cudaStream_t st = (cudaStream_t)stream;
+    return run_steps(eval_plan, n_steps, e->dpm.step, st, no_kernels, [&](int32_t) { return launch_dpm_stop_update(*e, st); });
+}
+
 int mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
                      int32_t n_steps, void* stream) {
     MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_join: the evaluation plan must be captured (mugd_plan_capture)");

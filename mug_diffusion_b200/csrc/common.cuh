@@ -80,6 +80,10 @@ int launch_dpm_update(const mugd_dpm& d, cudaStream_t st);
 // included); launch_dpm_ex_update runs the update of the counter's step, per-chart when starts are given
 int check_dpm_ex(const mugd_dpm_ex& e, int32_t n_steps);
 int launch_dpm_ex_update(const mugd_dpm_ex& e, cudaStream_t st);
+// mugd_sample_dpm_stop / mugd_dpm_stop_update: check_dpm_stop validates the descriptor; launch_dpm_stop_update runs the inversion
+// update of the counter's step for the charts that have not reached their stop
+int check_dpm_stop(const mugd_dpm_stop& e);
+int launch_dpm_stop_update(const mugd_dpm_stop& e, cudaStream_t st);
 // mugd_sample_join: check_join validates the descriptor; launch_join runs the join kernel against the device step counter
 int check_join(const mugd_join& j);
 int launch_join(const mugd_join& j, const int32_t* step, cudaStream_t st);

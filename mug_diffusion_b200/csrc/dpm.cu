@@ -1,6 +1,7 @@
 // DPM-Solver++ multistep sampler (data prediction, Lu et al. 2022; Stable Diffusion 2's DPM_Solver(predict_x0=True) "multistep"):
 // the update of one step.  The host (mug_diffusion_b200/dpm_solver.py) expands each step into one coefficient row; the loops
-// mugd_sample_dpm / mugd_sample_dpm_ex live in api.cu beside mugd_sample; mugd_dpm_update / mugd_dpm_ex_update run the update alone.
+// mugd_sample_dpm / mugd_sample_dpm_ex / mugd_sample_dpm_stop live in api.cu beside mugd_sample; mugd_dpm_update /
+// mugd_dpm_ex_update / mugd_dpm_stop_update run the update alone.
 #include "common.cuh"
 
 namespace mugd {
@@ -55,6 +56,34 @@ dpm_update_starts_kernel(const mugd_dpm d, const int32_t* __restrict__ start, co
     dpm_element(d, order_coef + 8 * (3 * (int64_t)step + order - 1), order, step, i);
 }
 
+// An inversion row in DDIM's form (ROW_FORM = 1, order 1): m0 as above, then x = alpha_next * m0 + sigma_next * e with
+// (alpha_next, sigma_next) = (row[4], row[5]), each product and the sum one IEEE round-to-nearest.  Same outputs as dpm_element.
+__device__ __forceinline__ void dpm_eps_form_element(const mugd_dpm& d, const float* row, int step, int i) {
+    const int64_t N = d.n;
+    const float e = cfg_eps(d.eps, i, N, d.cfg, d.scale);
+    const float m0 = __fdiv_rn(__fsub_rn(d.x[i], __fmul_rn(row[1], e)), row[0]);
+    const float xn = __fadd_rn(__fmul_rn(row[4], m0), __fmul_rn(row[5], e));
+    d.ring[(step % 3) * N + i] = m0;
+    d.x[i] = xn;
+    if (d.x_dup) d.x_dup[i] = xn;
+    if (d.pred_x0) d.pred_x0[i] = m0;
+}
+
+// Inversion with one stop per chart (the mirror of dpm_update_starts_kernel): chart b runs steps 0 .. stop[b] - 1.  From its stop on
+// it is left untouched (x, x_dup, its ring slots and pred_x0 are neither read nor written).  A running chart applies coefficient row
+// i: through dpm_element, as dpm_update_kernel does, or, for a row with ROW_FORM = 1, in DDIM's form.
+__global__ void __launch_bounds__(256)
+dpm_update_stops_kernel(const mugd_dpm d, const int32_t* __restrict__ stop, int per_chart) {
+    pdl_wait();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int step = *d.step;
+    if (i >= d.n || (unsigned)step >= (unsigned)d.S) return;
+    if (step >= stop[i / per_chart]) return;
+    const float* row = d.coef + 8 * (int64_t)step;
+    if (row[7] != 0.f) dpm_eps_form_element(d, row, step, i);
+    else dpm_element(d, row, (int)row[6], step, i);
+}
+
 int check_dpm(const mugd_dpm& d) {
     MUGD_REQUIRE(d.x && d.eps && d.ring && d.coef && d.step, "dpm: x, eps, ring, coef and step must be given");
     MUGD_REQUIRE(d.n > 0, "dpm: n=%d", d.n);
@@ -97,6 +126,20 @@ int launch_dpm_ex_update(const mugd_dpm_ex& e, cudaStream_t st) {
     return MUGD_OK;
 }
 
+int check_dpm_stop(const mugd_dpm_stop& e) {
+    int rc = check_dpm(e.dpm);
+    if (rc != MUGD_OK) return rc;
+    MUGD_REQUIRE(e.stop, "dpm_stop: stop must be given");
+    MUGD_REQUIRE(e.B > 0 && e.dpm.n % e.B == 0, "dpm_stop: B=%d does not divide n=%d", e.B, e.dpm.n);
+    MUGD_REQUIRE(e.reserved_ == 0, "dpm_stop: reserved_=%d must be 0", e.reserved_);
+    return MUGD_OK;
+}
+
+int launch_dpm_stop_update(const mugd_dpm_stop& e, cudaStream_t st) {
+    MUGD_CHECK_CUDA(launch_k(dpm_update_stops_kernel, dim3((e.dpm.n + 255) / 256), dim3(256), 0, st, e.dpm, e.stop, e.dpm.n / e.B));
+    return MUGD_OK;
+}
+
 }  // namespace mugd
 
 using namespace mugd;
@@ -113,4 +156,11 @@ extern "C" int mugd_dpm_ex_update(const mugd_dpm_ex* e, void* stream) {
     int rc = check_dpm_ex(*e, 0);
     if (rc != MUGD_OK) return rc;
     return launch_dpm_ex_update(*e, (cudaStream_t)stream);
+}
+
+extern "C" int mugd_dpm_stop_update(const mugd_dpm_stop* e, void* stream) {
+    MUGD_REQUIRE(e, "mugd_dpm_stop_update: null argument");
+    int rc = check_dpm_stop(*e);
+    if (rc != MUGD_OK) return rc;
+    return launch_dpm_stop_update(*e, (cudaStream_t)stream);
 }

@@ -21,9 +21,12 @@ import numpy as np
 SKIP_TYPES = ("time_uniform", "logSNR", "time_quadratic")
 SOLVER_TYPES = ("dpmsolver", "taylor")
 ORDERS = (1, 2, 3)
-# columns of a coefficient row (the kernel's [S][8] table; column 7 is padding)
-ROW_ALPHA, ROW_SIGMA, ROW_A, ROW_C0, ROW_C1, ROW_C2, ROW_ORDER = range(7)
+# columns of a coefficient row (the kernel's [S][8] table; column 7 is padding, except in inversion rows: ROW_FORM)
+ROW_ALPHA, ROW_SIGMA, ROW_A, ROW_C0, ROW_C1, ROW_C2, ROW_ORDER, ROW_FORM = range(8)
 ROW_WIDTH = 8
+# an inversion row with ROW_FORM = FORM_EPS is an order-1 step that the stop-aware update kernel takes in DDIM's form
+# x = alpha_j+1 * m0 + sigma_j+1 * e, with (alpha_j+1, sigma_j+1) in the c1 / c2 columns, which order 1 never reads
+FORM_EXPANDED, FORM_EPS = 0., 1.
 
 
 class NoiseScheduleVP:
@@ -104,6 +107,9 @@ class DPMSchedule:
     rows: np.ndarray
     orders: np.ndarray
     order_rows: Optional[np.ndarray] = None
+    order: int = 0                                   # the requested order and solver type, and the noise schedule the grid lives on
+    solver_type: str = ""
+    ns: Optional[NoiseScheduleVP] = None
 
     @property
     def S(self) -> int:
@@ -202,4 +208,27 @@ def multistep_schedule(alphas_cumprod, S: int, order: int = 2, skip_type: str = 
     for i in range(S):
         for k in range(1, min(i + 1, 3) + 1):
             by_order[i, k - 1] = expand_row(i, k, alpha, sigma, lam, solver_type)
-    return DPMSchedule(t=t, model_times=model_time(ns, t[:-1]), rows=rows, orders=orders, order_rows=by_order)
+    return DPMSchedule(t=t, model_times=model_time(ns, t[:-1]), rows=rows, orders=orders, order_rows=by_order, order=order,
+                       solver_type=solver_type, ns=ns)
+
+
+def inversion_schedule(sched: DPMSchedule) -> DPMSchedule:
+    """The tables of the inversion of ``sched`` (a ``multistep_schedule``): the probability-flow ODE run backwards on the reversed grid
+    u_j = t_S-j, j = 0 .. S.  Step j goes from u_j to u_j+1, evaluates the U-Net at model_time(u_j) and has order min(j + 1, order)
+    (no lower_order_final: charts stop at different steps); its row is ``expand_row`` on the reversed grid's alpha / sigma / lambda,
+    where h < 0.  After s steps a chart sits at t_S-s, where a remix over the last s steps of ``sched`` starts.
+    Every order-1 row also carries DDIM's form (ROW_FORM = FORM_EPS, alpha_j+1 / sigma_j+1 in the c1 / c2 columns): leaving u_0 = 1/N,
+    where sigma is about 0.01, A = sigma_j+1 / sigma_j reaches 17 (time_uniform, S = 10), and A x + c0 m0 then cancels terms of that
+    size in float32 (up to 1.9e-6 of max |x| per step against 1e-7 for the other steps); alpha_j+1 m0 + sigma_j+1 e cancels nothing.
+    ``order_rows`` is None: every chart starts at step 0, so its orders are the rows'."""
+    if not isinstance(sched, DPMSchedule) or sched.ns is None or sched.order not in ORDERS:
+        raise ValueError("sched must be a DPMSchedule from multistep_schedule")
+    ns, S = sched.ns, sched.S
+    u = np.ascontiguousarray(sched.t[::-1], dtype=np.float64)
+    alpha, sigma, lam = ns.marginal_alpha(u), ns.marginal_std(u), ns.marginal_lambda(u)
+    orders = np.minimum(np.arange(S) + 1, sched.order).astype(np.int64)
+    rows = np.stack([expand_row(j, int(orders[j]), alpha, sigma, lam, sched.solver_type) for j in range(S)])
+    one = orders == 1
+    rows[one, ROW_C1], rows[one, ROW_C2], rows[one, ROW_FORM] = alpha[1:][one], sigma[1:][one], FORM_EPS
+    return DPMSchedule(t=u, model_times=model_time(ns, u[:-1]), rows=rows, orders=orders, order=sched.order,
+                       solver_type=sched.solver_type, ns=ns)

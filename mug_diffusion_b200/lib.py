@@ -124,6 +124,10 @@ class DpmEx(C.Structure):
     _fields_ = [("dpm", Dpm), ("stage", _f), ("start", _f), ("order_coef", _f), ("B", C.c_int32), ("reserved_", C.c_int32)]
 
 
+class DpmStop(C.Structure):
+    _fields_ = [("dpm", Dpm), ("stop", _f), ("B", C.c_int32), ("reserved_", C.c_int32)]
+
+
 class QEncode(C.Structure):
     _fields_ = [("x0", _f), ("noise", _f), ("t", _f), ("sqrt_a", _f), ("sqrt_1ma", _f), ("out", _f),
                 ("B", C.c_int32), ("C", C.c_int32), ("L", C.c_int32), ("n", C.c_int32)]
@@ -224,6 +228,8 @@ def load() -> C.CDLL:
     lib.mugd_dpm_update.argtypes = [C.POINTER(Dpm), C.c_void_p]
     lib.mugd_sample_dpm_ex.argtypes = [C.c_void_p, C.POINTER(DpmEx), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_dpm_ex_update.argtypes = [C.POINTER(DpmEx), C.c_void_p]
+    lib.mugd_sample_dpm_stop.argtypes = [C.c_void_p, C.POINTER(DpmStop), C.c_int32, C.c_int32, C.c_void_p]
+    lib.mugd_dpm_stop_update.argtypes = [C.POINTER(DpmStop), C.c_void_p]
     lib.mugd_stochastic_encode.argtypes = [C.POINTER(QEncode), C.c_void_p]
     lib.mugd_sample_join.argtypes = [C.c_void_p, C.POINTER(Join), C.POINTER(Op), C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_plan_save.argtypes = [C.c_void_p, C.POINTER(Region), C.c_int32, C.c_char_p]
@@ -265,4 +271,5 @@ EXPORTED_SYMBOLS = [
     "mugd_sample_staged", "mugd_sample_plms", "mugd_plms_combine",
     "mugd_sample_ddpm", "mugd_ddpm_update", "mugd_stochastic_encode", "mugd_sample_join",
     "mugd_sample_dpm", "mugd_dpm_update", "mugd_sample_dpm_ex", "mugd_dpm_ex_update",
+    "mugd_sample_dpm_stop", "mugd_dpm_stop_update",
 ]

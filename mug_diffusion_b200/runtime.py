@@ -79,6 +79,11 @@ class Plan:
         (mugd_sample_dpm_ex)"""
         self._launch_steps("mugd_sample_dpm_ex", ex, first_step, steps)
 
+    def launch_dpm_stop(self, e: L_.DpmStop, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a DPM-Solver++ inversion with one stop per chart from one C call
+        (mugd_sample_dpm_stop)"""
+        self._launch_steps("mugd_sample_dpm_stop", e, first_step, steps)
+
     def launch_join(self, join: L_.Join, tail: OpList, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a decode request whose charts join at different iterations, from one C call
         (mugd_sample_join: the join kernel, the graph replay and the tail per step)"""
@@ -567,6 +572,14 @@ class Session:
             assert start.shape == (B,) and start.dtype == torch.int32 and start.is_contiguous()
             assert order_coef.shape == (dpm.S, 3, 8) and order_coef.dtype == torch.float32 and order_coef.is_contiguous()
             e.start, e.order_coef, e.B = _ptr(start), _ptr(order_coef), B
+        return e
+
+    def dpm_stop(self, dpm: L_.Dpm, B: int, stop: torch.Tensor) -> L_.DpmStop:
+        """the mugd_sample_dpm_stop descriptor around ``dpm`` (an inversion schedule's rows): chart b runs steps 0 .. stop[b] - 1
+        (``stop``: [B] int32 on the device).  The caller keeps the tensor alive."""
+        assert stop.shape == (B,) and stop.dtype == torch.int32 and stop.is_contiguous()
+        e = L_.DpmStop()
+        e.dpm, e.stop, e.B = dpm, _ptr(stop), B
         return e
 
     def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:
