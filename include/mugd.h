@@ -403,6 +403,28 @@ int  mugd_sample_dpm_stop(mugd_plan* eval_plan, const mugd_dpm_stop* e, int32_t 
 /* the stop-aware update alone for the counter's step, for a host that runs the steps one by one */
 int  mugd_dpm_stop_update(const mugd_dpm_stop* e, void* stream);
 
+/* ---- UniPC multistep predictor-corrector (Zhao et al. 2023; data prediction, B(h) = bh1 / bh2) ----------------------------------
+ * mugd_unipc runs an S-step request whose predictor rows are dpm.coef ([S][8], the mugd_dpm row layout) and whose corrector rows are
+ * corr ([S][8]: A', dn, d0, d1, d2, order k, on, unused).  Iteration i (the device counter holding i): replay the evaluation plan on the
+ * predicted latent x~_i (x, x_dup), then one update kernel: m_i = (x~_i - sigma_i * e) / alpha_i as mugd_dpm computes m0; if corrector
+ * row i is on (column 6 nonzero)
+ *   x_i = (((A' * xc + dn * m_i) + d0 * m_i-1) + d1 * m_i-2) + d2 * m_i-3   (the d1 term only for k >= 2, d2 only for k = 3)
+ * with xc = x_i-1, else x_i = x~_i; then predictor row i on (x_i, m_i) exactly as the mugd_dpm update: x~_i+1 = ((A * x_i + c0 * m_i)
+ * + c1 * m_i-1) + c2 * m_i-2.  xc <- x_i, x and x_dup <- x~_i+1, pred_x0 <- m_i and ring slot i mod 3 <- m_i (after m_i-3 has been
+ * read from it); then *step += 1.  Every intermediate is one IEEE round-to-nearest in this order, no contraction.  The rows come from
+ * the host (mug_diffusion_b200/unipc.py).  Corrector row 0 is off; the last latent x~_S is the request's result. */
+typedef struct mugd_unipc {
+    mugd_dpm dpm;                          /* the predictor (coef [S][8], ring, step counter, x / x_dup, eps, pred_x0, ...)     */
+    float* xc;                             /* [n] the corrected latent x_i-1 of the previous iteration (overlaps no other rows) */
+    const float* corr;                     /* [S][8] corrector rows                                                             */
+} mugd_unipc;
+/* steps first_step .. first_step + n_steps - 1 (the counter holding first_step): n_steps x { graph replay ; update ; *step += 1 }, the
+ * launches per step of mugd_sample_dpm (first_step + n_steps <= S).  It checks the descriptor before the plan, so a host can test its
+ * arguments without a device. */
+int  mugd_sample_unipc(mugd_plan* eval_plan, const mugd_unipc* u, int32_t first_step, int32_t n_steps, void* stream);
+/* the update alone for the counter's step (the counter not advanced), for a host that runs the steps one by one */
+int  mugd_unipc_update(const mugd_unipc* u, void* stream);
+
 /* ---- remixing an existing chart (SDEdit / img2img): DDIMSampler.stochastic_encode and decode with a per-chart start ---------------
  * mugd_stochastic_encode: out[b] = sqrt_a[t[b]] * x0[b] + sqrt_1ma[t[b]] * noise[b], each product and the sum one IEEE
  * round-to-nearest (no contraction), bit-identical to torch's extract_into_tensor expressions.  x0, noise and out are device NCL

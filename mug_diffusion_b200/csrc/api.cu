@@ -364,6 +364,17 @@ int mugd_sample_dpm_stop(mugd_plan* eval_plan, const mugd_dpm_stop* e, int32_t f
     return run_steps(eval_plan, n_steps, e->dpm.step, st, no_kernels, [&](int32_t) { return launch_dpm_stop_update(*e, st); });
 }
 
+int mugd_sample_unipc(mugd_plan* eval_plan, const mugd_unipc* u, int32_t first_step, int32_t n_steps, void* stream) {
+    // the descriptor is checked before the plan, so a host can test its arguments without a device
+    MUGD_REQUIRE(u, "mugd_sample_unipc: null descriptor");
+    int rc = check_unipc(*u);
+    if (rc != MUGD_OK) return rc;
+    if ((rc = check_step_range("mugd_sample_unipc", first_step, n_steps, "S", u->dpm.S)) != MUGD_OK) return rc;
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_unipc: the evaluation plan must be captured (mugd_plan_capture)");
+    cudaStream_t st = (cudaStream_t)stream;
+    return run_steps(eval_plan, n_steps, u->dpm.step, st, no_kernels, [&](int32_t) { return launch_unipc_update(*u, st); });
+}
+
 int mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
                      int32_t n_steps, void* stream) {
     MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_join: the evaluation plan must be captured (mugd_plan_capture)");

@@ -84,6 +84,10 @@ int launch_dpm_ex_update(const mugd_dpm_ex& e, cudaStream_t st);
 // update of the counter's step for the charts that have not reached their stop
 int check_dpm_stop(const mugd_dpm_stop& e);
 int launch_dpm_stop_update(const mugd_dpm_stop& e, cudaStream_t st);
+// mugd_sample_unipc / mugd_unipc_update: check_unipc validates the descriptor; launch_unipc_update runs the UniPC update of the
+// counter's step
+int check_unipc(const mugd_unipc& u);
+int launch_unipc_update(const mugd_unipc& u, cudaStream_t st);
 // mugd_sample_join: check_join validates the descriptor; launch_join runs the join kernel against the device step counter
 int check_join(const mugd_join& j);
 int launch_join(const mugd_join& j, const int32_t* step, cudaStream_t st);

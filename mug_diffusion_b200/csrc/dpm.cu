@@ -1,7 +1,8 @@
 // DPM-Solver++ multistep sampler (data prediction, Lu et al. 2022; Stable Diffusion 2's DPM_Solver(predict_x0=True) "multistep"):
 // the update of one step.  The host (mug_diffusion_b200/dpm_solver.py) expands each step into one coefficient row; the loops
 // mugd_sample_dpm / mugd_sample_dpm_ex / mugd_sample_dpm_stop live in api.cu beside mugd_sample; mugd_dpm_update /
-// mugd_dpm_ex_update / mugd_dpm_stop_update run the update alone.
+// mugd_dpm_ex_update / mugd_dpm_stop_update run the update alone.  The UniPC predictor-corrector update (mugd_sample_unipc /
+// mugd_unipc_update; rows from mug_diffusion_b200/unipc.py) shares the DPM-Solver++ arithmetic.
 #include "common.cuh"
 
 namespace mugd {
@@ -12,16 +13,29 @@ namespace mugd {
 //   x  = ((A * x + c0 * m0) + c1 * m1) + c2 * m2                      m1 / m2: the predictions of steps i-1 / i-2 (ring slots)
 // in this order, every product, sum and the quotient one IEEE round-to-nearest, no contraction.  Terms past the order are not
 // formed: their ring slots may not have been written yet (and 0 * NaN is NaN).  x goes to x and x_dup, m0 to pred_x0 and to ring
-// slot step mod 3.  Both update kernels run this, so a chart computes the same bits in either.
-__device__ __forceinline__ void dpm_element(const mugd_dpm& d, const float* row, int order, int step, int i) {
-    const float alpha = row[0], sigma = row[1], A = row[2], c0 = row[3];
+// slot step mod 3.  Every DPM-Solver++ update kernel and the UniPC update run these functions, so a chart computes the same bits in
+// each.
+__device__ __forceinline__ float dpm_data_prediction(const mugd_dpm& d, float alpha, float sigma, int i, float x) {
+    const float e = cfg_eps(d.eps, i, d.n, d.cfg, d.scale);
+    return __fdiv_rn(__fsub_rn(x, __fmul_rn(sigma, e)), alpha);
+}
+
+// the multistep update ((A * x + c0 * m0) + c1 * m1) + c2 * m2 of row `row` (A = row[2], c0 = row[3]), terms up to `order`
+__device__ __forceinline__ float dpm_predict(const mugd_dpm& d, const float* row, float A, float c0, int order, int step, int i, float x,
+                                             float m0) {
     const int64_t N = d.n;
-    const float e = cfg_eps(d.eps, i, N, d.cfg, d.scale);
-    const float x = d.x[i];
-    const float m0 = __fdiv_rn(__fsub_rn(x, __fmul_rn(sigma, e)), alpha);
     float xn = __fadd_rn(__fmul_rn(A, x), __fmul_rn(c0, m0));
     if (order >= 2) xn = __fadd_rn(xn, __fmul_rn(row[4], d.ring[((step + 2) % 3) * N + i]));
     if (order >= 3) xn = __fadd_rn(xn, __fmul_rn(row[5], d.ring[((step + 1) % 3) * N + i]));
+    return xn;
+}
+
+__device__ __forceinline__ void dpm_element(const mugd_dpm& d, const float* row, int order, int step, int i) {
+    const float alpha = row[0], sigma = row[1], A = row[2], c0 = row[3];
+    const int64_t N = d.n;
+    const float x = d.x[i];
+    const float m0 = dpm_data_prediction(d, alpha, sigma, i, x);
+    const float xn = dpm_predict(d, row, A, c0, order, step, i, x, m0);
     d.ring[(step % 3) * N + i] = m0;
     d.x[i] = xn;
     if (d.x_dup) d.x_dup[i] = xn;
@@ -84,6 +98,41 @@ dpm_update_stops_kernel(const mugd_dpm d, const int32_t* __restrict__ stop, int 
     else dpm_element(d, row, (int)row[6], step, i);
 }
 
+// UniPC (mug_diffusion_b200/unipc.py): iteration i evaluated the U-Net at the predicted x~_i (x, x_dup).  With m_i its data prediction as in
+// dpm_element, corrector row i = (A', dn, d0, d1, d2, k, on) gives the corrected latent of step i from xc = x_i-1:
+//   x_i = (((A' * xc + dn * m_i) + d0 * m_i-1) + d1 * m_i-2) + d2 * m_i-3     (the d1 term for k >= 2, d2 for k = 3)
+// or x_i = x~_i when the row is off.  Then the predictor row i (dpm_predict on x_i and m_i) gives x~_i+1.  xc <- x_i, x and x_dup <-
+// x~_i+1, pred_x0 <- m_i, and ring slot i mod 3 <- m_i after its m_i-3 has been read.  Each product and sum one IEEE round-to-nearest,
+// no contraction.  A counter outside [0, S) leaves everything unchanged.
+__global__ void __launch_bounds__(256)
+unipc_update_kernel(const mugd_unipc u) {
+    pdl_wait();
+    const mugd_dpm& d = u.dpm;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int step = *d.step;
+    if (i >= d.n || (unsigned)step >= (unsigned)d.S) return;
+    const int64_t N = d.n;
+    const float* row = d.coef + 8 * (int64_t)step;
+    const float* corr = u.corr + 8 * (int64_t)step;
+    const float alpha = row[0], sigma = row[1], A = row[2], c0 = row[3];
+    const float xt = d.x[i];
+    const float m0 = dpm_data_prediction(d, alpha, sigma, i, xt);
+    float x = xt;
+    if (corr[6] != 0.f) {
+        const int k = (int)corr[5];
+        x = __fadd_rn(__fmul_rn(corr[0], u.xc[i]), __fmul_rn(corr[1], m0));
+        x = __fadd_rn(x, __fmul_rn(corr[2], d.ring[((step + 2) % 3) * N + i]));
+        if (k >= 2) x = __fadd_rn(x, __fmul_rn(corr[3], d.ring[((step + 1) % 3) * N + i]));
+        if (k >= 3) x = __fadd_rn(x, __fmul_rn(corr[4], d.ring[(step % 3) * N + i]));
+    }
+    const float xn = dpm_predict(d, row, A, c0, (int)row[6], step, i, x, m0);
+    u.xc[i] = x;
+    d.ring[(step % 3) * N + i] = m0;
+    d.x[i] = xn;
+    if (d.x_dup) d.x_dup[i] = xn;
+    if (d.pred_x0) d.pred_x0[i] = m0;
+}
+
 int check_dpm(const mugd_dpm& d) {
     MUGD_REQUIRE(d.x && d.eps && d.ring && d.coef && d.step, "dpm: x, eps, ring, coef and step must be given");
     MUGD_REQUIRE(d.n > 0, "dpm: n=%d", d.n);
@@ -140,6 +189,25 @@ int launch_dpm_stop_update(const mugd_dpm_stop& e, cudaStream_t st) {
     return MUGD_OK;
 }
 
+static bool overlaps(const float* a, int64_t na, const float* b, int64_t nb) {
+    return a && b && a < b + nb && b < a + na;
+}
+
+int check_unipc(const mugd_unipc& u) {
+    int rc = check_dpm(u.dpm);
+    if (rc != MUGD_OK) return rc;
+    const mugd_dpm& d = u.dpm;
+    MUGD_REQUIRE(u.xc && u.corr, "unipc: xc and corr must be given");
+    MUGD_REQUIRE(!overlaps(u.xc, d.n, d.x, d.n) && !overlaps(u.xc, d.n, d.x_dup, d.n) && !overlaps(u.xc, d.n, d.ring, 3 * (int64_t)d.n),
+                 "unipc: xc overlaps x, x_dup or the ring");
+    return MUGD_OK;
+}
+
+int launch_unipc_update(const mugd_unipc& u, cudaStream_t st) {
+    MUGD_CHECK_CUDA(launch_k(unipc_update_kernel, dim3((u.dpm.n + 255) / 256), dim3(256), 0, st, u));
+    return MUGD_OK;
+}
+
 }  // namespace mugd
 
 using namespace mugd;
@@ -163,4 +231,11 @@ extern "C" int mugd_dpm_stop_update(const mugd_dpm_stop* e, void* stream) {
     int rc = check_dpm_stop(*e);
     if (rc != MUGD_OK) return rc;
     return launch_dpm_stop_update(*e, (cudaStream_t)stream);
+}
+
+extern "C" int mugd_unipc_update(const mugd_unipc* u, void* stream) {
+    MUGD_REQUIRE(u, "mugd_unipc_update: null argument");
+    int rc = check_unipc(*u);
+    if (rc != MUGD_OK) return rc;
+    return launch_unipc_update(*u, (cudaStream_t)stream);
 }

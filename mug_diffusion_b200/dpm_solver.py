@@ -18,6 +18,8 @@ from typing import Optional
 
 import numpy as np
 
+# the most steps a request may take: rows of the time-embedding table a sampling session holds (MUGD_MAX_STEPS in mugd.h)
+MAX_STEPS = 1000
 SKIP_TYPES = ("time_uniform", "logSNR", "time_quadratic")
 SOLVER_TYPES = ("dpmsolver", "taylor")
 ORDERS = (1, 2, 3)
@@ -73,6 +75,17 @@ def time_steps(ns: NoiseScheduleVP, skip_type: str, S: int) -> np.ndarray:
     if skip_type == "time_quadratic":
         return np.linspace(t_T ** 0.5, t_0 ** 0.5, S + 1) ** 2
     raise ValueError(f"skip_type={skip_type!r}: one of {SKIP_TYPES}")
+
+
+def request_grid(ns: NoiseScheduleVP, skip_type: str, S: int, t_grid: Optional[np.ndarray] = None) -> np.ndarray:
+    """the S + 1 points of a request's grid: ``t_grid`` when given (S + 1 decreasing times in [1/N, 1], else ValueError), otherwise
+    ``time_steps(ns, skip_type, S)``"""
+    if t_grid is None:
+        return time_steps(ns, skip_type, S)
+    t = np.asarray(t_grid, dtype=np.float64)
+    if t.shape != (S + 1,) or not np.all(np.diff(t) < 0) or t[-1] < ns.eps or t[0] > ns.T:
+        raise ValueError(f"t_grid must hold S + 1 = {S + 1} decreasing times in [1/N, 1]")
+    return t
 
 
 def ddim_grid(ns: NoiseScheduleVP, ddim_timesteps) -> np.ndarray:
@@ -194,12 +207,7 @@ def multistep_schedule(alphas_cumprod, S: int, order: int = 2, skip_type: str = 
     if isinstance(S, bool) or not isinstance(S, (int, np.integer)) or S < order:
         raise ValueError(f"S={S!r}: a multistep request of order {order} needs at least {order} steps")
     ns = NoiseScheduleVP(alphas_cumprod)
-    if t_grid is None:
-        t = time_steps(ns, skip_type, int(S))
-    else:
-        t = np.asarray(t_grid, dtype=np.float64)
-        if t.shape != (S + 1,) or not np.all(np.diff(t) < 0) or t[-1] < ns.eps or t[0] > ns.T:
-            raise ValueError(f"t_grid must hold S + 1 = {S + 1} decreasing times in [1/N, 1]")
+    t = request_grid(ns, skip_type, int(S), t_grid)
     S = int(S)
     alpha, sigma, lam = ns.marginal_alpha(t), ns.marginal_std(t), ns.marginal_lambda(t)
     orders = step_orders(S, order, lower_order_final)

@@ -21,12 +21,12 @@ import torch
 
 from . import lib as L_
 from .config import DecoderConfig, EncoderConfig, ModelConfig, UNetConfig
+from .dpm_solver import MAX_STEPS
 from .netspec import RES_LAYERS, Block, decoder_layout, encoder_layout, unet_layout
 from .packer import WeightBlob, pack_model
 
 GN_EPS = 1e-6     # models.py:11
 LN_EPS = 1e-5     # nn.LayerNorm default, attention.py:136-138
-MAX_STEPS = 1000
 CTX_TOKENS_MAX = 64
 
 

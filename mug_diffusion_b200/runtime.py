@@ -84,6 +84,10 @@ class Plan:
         (mugd_sample_dpm_stop)"""
         self._launch_steps("mugd_sample_dpm_stop", e, first_step, steps)
 
+    def launch_unipc(self, u: L_.Unipc, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a UniPC request from one C call (mugd_sample_unipc)"""
+        self._launch_steps("mugd_sample_unipc", u, first_step, steps)
+
     def launch_join(self, join: L_.Join, tail: OpList, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a decode request whose charts join at different iterations, from one C call
         (mugd_sample_join: the join kernel, the graph replay and the tail per step)"""
@@ -581,6 +585,17 @@ class Session:
         e = L_.DpmStop()
         e.dpm, e.stop, e.B = dpm, _ptr(stop), B
         return e
+
+    def unipc(self, B: int, S: int, cfg_on: bool, scale: float, pred_x0: int, ring: torch.Tensor, coef: torch.Tensor, xc: torch.Tensor,
+              corr: torch.Tensor) -> L_.Unipc:
+        """the mugd_sample_unipc descriptor of an S-step request for B samples: ``dpm``'s with the predictor rows ``coef`` ([S, 8]), plus
+        the corrector rows ``corr`` ([S, 8]) and the corrected latent ``xc`` ([B*Lz*C]).  The caller keeps the tensors alive."""
+        assert corr.shape == (S, 8) and corr.dtype == torch.float32 and corr.is_contiguous()
+        u = L_.Unipc()
+        u.dpm = self.dpm(B, S, cfg_on, scale, pred_x0, ring, coef)
+        assert xc.numel() == u.dpm.n and xc.dtype == torch.float32 and xc.is_contiguous()
+        u.xc, u.corr = _ptr(xc), _ptr(corr)
+        return u
 
     def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:
         """the ops that follow each evaluation of an S-step request for B samples: the DDIM update of the xin rows (both halves

@@ -5,6 +5,7 @@ Reference surface kept (SURVEY §8b):
     sampler = PLMSSampler(model)                                  mug/diffusion/plms.py:11 (scripts/mapping.py --plms)
     sampler = DDPMSampler(model)                                  DDPM.log_beatmap's loop, mug/diffusion/diffusion.py:255-282
     sampler = DPMSolverSampler(model)                             DPM-Solver++ multistep (Stable Diffusion 2's DPMSolverSampler)
+    sampler = UniPCSampler(model)                                 UniPC multistep predictor-corrector (Zhao et al., 2023)
     samples, inter = sampler.sample(S, c, w, batch_size, ...)     mug/diffusion/ddim.py:56-107
     eps    = model.model.forward(x, t, c, w)                      mug/diffusion/diffusion.py:52-54
     logits = model.model.decode(z)                                mug/diffusion/diffusion.py:49-50
@@ -21,7 +22,7 @@ from typing import Dict, Optional, Sequence
 import numpy as np
 import torch
 
-from . import dpm_solver
+from . import dpm_solver, unipc
 from . import lib as L_
 from .config import DecoderConfig, EncoderConfig, ModelConfig, UNetConfig
 from .engine import MAX_STEPS, OpList, View
@@ -1396,3 +1397,83 @@ class DPMSolverSampler(_DeviceLoopSampler):
                     pass
             self.last_launches_per_step = sess.plan.launches + 2
             return self._read_x(sess, shape)
+
+
+# --------------------------------------------------------------------------------------------------
+# UniPC sampler
+# --------------------------------------------------------------------------------------------------
+class UniPCSampler(_DeviceLoopSampler):
+    """UniPC multistep (Zhao et al., 2023): a 1st- to 3rd-order multistep predictor (UniP) with a corrector (UniC) in data-prediction
+    form, with the ``sample(S, ...)`` shape of DDIMSampler and DPMSolverSampler.  The corrector reuses the evaluation the next step needs
+    anyway, so a step still costs one batched U-Net evaluation and one update kernel (csrc/dpm.cu, rows from ``unipc``), and raises
+    the solver's order by one; 5-10 steps of order 2 or 3 are its usual use.  Same constructor as DDIMSampler.  Deterministic (no noise
+    is drawn apart from x_T when it is not given)."""
+
+    def make_unipc_schedule(self, S, order=2, skip_type="time_uniform", variant="bh2", lower_order_final=True, use_corrector=True,
+                            disable_corrector=(), t_grid=None) -> unipc.UniPCSchedule:
+        """the predictor and corrector rows and model times of an S-step request (``unipc.multistep_schedule``; ``t_grid``: an
+        explicit continuous-time grid of S + 1 points from 1 down to 1/N instead of ``skip_type``'s).  ValueError for malformed
+        arguments."""
+        return unipc.multistep_schedule(alphas_cumprod_f64(self.model.cfg), S, order, skip_type, variant, lower_order_final,
+                                        use_corrector, disable_corrector, t_grid)
+
+    @torch.no_grad()
+    def sample(self, S, c=None, w=None, batch_size=None, shape=None, x_T=None, order=2, skip_type="time_uniform", variant="bh2",
+               lower_order_final=True, use_corrector=True, disable_corrector=(), t_grid=None, callback=None, img_callback=None,
+               log_every_t=100, unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True,
+               conditioning=None, **kwargs):
+        """S steps of UniPC of ``order`` from x_T (drawn when not given) to t = 1/N; ``c`` may also be given as ``conditioning``.
+        Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then, after every iteration i with ``(S - i - 1) % log_every_t == 0`` or
+        i = 0 (DDIM's rule), the latent the next evaluation sees (the predicted x~_i+1; the last one is z) and the data prediction m_i.
+        Every argument is checked before any GPU work (ValueError; TypeError for missing or unknown ones); mask / x0, eta, temperature
+        and noise dropout are refused.  Without callbacks the steps run from mugd_sample_unipc calls, with them one by one through
+        mugd_unipc_update."""
+        _refuse_ddim_only(kwargs, "UniPCSampler", "UniPC is a deterministic solver without {}")
+        c = _conditioning(c, conditioning)
+        if c is None or w is None:
+            raise TypeError("UniPCSampler.sample needs the conditioning c and the audio features w")
+        scale = _finite_scale(unconditional_guidance_scale)
+        sched = self.make_unipc_schedule(S, order, skip_type, variant, lower_order_final, use_corrector, disable_corrector, t_grid)
+        size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
+        if verbose:
+            print(f'Data shape for UniPC sampling is {size}, {S} steps of order {order} ({skip_type}, {variant})')
+        return self.unipc_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
+                                   unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
+                                   tqdm_class=tqdm_class)
+
+    @torch.no_grad()
+    def unipc_sampling(self, w, c, shape, sched: unipc.UniPCSchedule, x_T=None, callback=None, img_callback=None, log_every_t=100,
+                       unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True):
+        """the request of ``sched`` (make_unipc_schedule) on the GPU, from checked arguments"""
+        model = self.model
+        eng = model.engine
+        dev = self.device
+        B, Cz, Lz = shape
+        total = sched.S
+        scale = unconditional_guidance_scale
+        self.last_schedule = sched
+        with eng.lock:
+            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times)
+            coef = torch.from_numpy(sched.rows_f32()).to(dev)
+            corr = torch.from_numpy(sched.corr_rows_f32()).to(dev)
+            ring = torch.empty(3, B * Lz * Cz, device=dev)                     # the data predictions of the last three steps
+            xc = torch.empty(B * Lz * Cz, device=dev)                          # the corrected latent of the previous step
+            pred = torch.empty(B * Lz, Cz, device=dev)
+            u = sess.unipc(B, total, cfg_on, scale, _ptr(pred), ring, coef, xc, corr)
+
+            def launch(first, n):
+                # the ring, xc and the step counter stay on the device, so a call may start anywhere in the request
+                sess.plan.launch_unipc(u, first, n)
+
+            # the per-step loop runs the same kernel: the referee of the device loop
+            advance = _step_ops(sess)
+            stream = torch.cuda.current_stream().cuda_stream
+
+            def step(i, t):
+                sess.eval(graph=True)
+                L_.check(eng.lib.mugd_unipc_update(C.byref(u), stream), "mugd_unipc_update")
+                eng.run_ops(advance)
+
+            return self._run_request(sess, x, shape, pred, time_range, total, log_every_t, 'Charting, using UniPC Sampler',
+                                     tqdm_class, progress, callback, img_callback, callback is None and img_callback is None, launch,
+                                     step, 2)
