@@ -425,6 +425,56 @@ int  mugd_sample_unipc(mugd_plan* eval_plan, const mugd_unipc* u, int32_t first_
 /* the update alone for the counter's step (the counter not advanced), for a host that runs the steps one by one */
 int  mugd_unipc_update(const mugd_unipc* u, void* stream);
 
+/* ---- UniPC from an existing chart: inpainting and per-chart-strength remix -----------------------------------------------------
+ * mugd_unipc_ex extends a mugd_unipc request by one of:
+ *   stage  inpainting: step k of a mugd_sample_unipc_ex call first runs the mugd_sample_staged stage kernel for row k of the stage's
+ *          tables (x <- (alpha_i * x0 + sigma_i * q_noise[k]) * mask + (1 - mask) * x), as mugd_dpm_ex does.  It blends the latent
+ *          the U-Net sees (x, x_dup) only; xc, the solver's own state, is not blended.  The stage must blend the update's x / x_dup
+ *          over n = B*C*L elements and stage no step noise.
+ *   start  remix: chart b (elements b * n/B .. (b+1) * n/B - 1 of the dense rows) runs from step f = start[b] on; before that it is
+ *          left untouched (x, x_dup, xc, ring and pred_x0), so its rows keep the latent they were loaded with.  At step i >= f its
+ *          predictor takes order kp = min(coef row i's order, i - f + 1) from row (i, kp - 1) of order_coef [S][3][8], and its
+ *          corrector runs only if corr row i is on and i > f (there is no earlier evaluation at f), at order kc = min(corr row i's
+ *          order, i - f) from row (i, kc - 1) of order_corr [S][3][8] (the corr row layout).  It reads only the ring slots of its own
+ *          steps.  Everything else is the mugd_unipc update, bit for bit.
+ * Neither (both NULL) is mugd_sample_unipc.  stage and start are exclusive; start, order_coef and order_corr go together. */
+typedef struct mugd_unipc_ex {
+    mugd_unipc unipc;                      /* the update (coef, corr, xc, ring, step counter, ...)                              */
+    const mugd_stage* stage;               /* inpainting blend in front of each step, or NULL                                  */
+    const int32_t* start;                  /* [B] device: the first step of each chart, or NULL                                */
+    const float* order_coef;               /* [S][3][8] device per-order predictor rows, given exactly with start               */
+    const float* order_corr;               /* [S][3][8] device per-order corrector rows, given exactly with start               */
+    int32_t B, reserved_;                  /* charts (with start); reserved_ = 0                                               */
+} mugd_unipc_ex;
+/* steps first_step .. first_step + n_steps - 1 (the counter holding first_step): n_steps x { stage kernel (with stage) ; graph replay ;
+ * update ; *step += 1 }: with a stage the launches per step of mugd_sample_staged, otherwise those of mugd_sample_unipc.  It checks
+ * the descriptor before the plan, so a host can test its arguments without a device. */
+int  mugd_sample_unipc_ex(mugd_plan* eval_plan, const mugd_unipc_ex* e, int32_t first_step, int32_t n_steps, void* stream);
+/* the update alone for the counter's step (per chart with start; the stage is not run), for a host that runs the steps one by one */
+int  mugd_unipc_ex_update(const mugd_unipc_ex* e, void* stream);
+
+/* ---- UniPC inversion: an existing chart run backwards to its noise, with one stop per chart ------------------------------------
+ * mugd_unipc_stop runs a mugd_unipc request whose rows are an inversion schedule's (the grid reversed, from t = 1/N up): chart b runs
+ * iterations 0 .. stop[b] - 1 and is left untouched from iteration stop[b] on (x, x_dup, xc, ring and pred_x0 neither read nor
+ * written).  A running chart applies corrector row i and predictor row i as the mugd_unipc update does, bit for bit, except in two
+ * row forms that avoid multiplying a latent by sigma_i+1 / sigma_i, which reaches 17 on the first steps away from t = 1/N:
+ *   corrector row with column 7 nonzero (correction form): c = ((d_n * (m_i - m_i-1) + d1 * (m_i-2 - m_i-1)) + d2 * (m_i-3 - m_i-1))
+ *     (d1 for k >= 2, d2 for k = 3; d_n = corr[8i+1], d1 = corr[8i+3], d2 = corr[8i+4]) and x_i = x~_i + c, which holds because an
+ *     inversion never blends x~_i;
+ *   predictor row with column 7 nonzero (order 1 in DDIM's form): x~_i+1 = coef[8i+4] * m_i + coef[8i+5] * e, then + A * c when a
+ *     correction-form corrector ran in this iteration (a DDIM-form row needs the corrector, if any, in the correction form).
+ * Each difference, product and sum one IEEE round-to-nearest.  All stops equal to S runs every chart through every row. */
+typedef struct mugd_unipc_stop {
+    mugd_unipc unipc;                      /* the update (coef, corr, xc, ring, step counter, ...)                              */
+    const int32_t* stop;                   /* [B] device: the number of iterations each chart runs                             */
+    int32_t B, reserved_;                  /* charts (B divides n); reserved_ = 0                                              */
+} mugd_unipc_stop;
+/* steps first_step .. first_step + n_steps - 1 (the counter holding first_step): n_steps x { graph replay ; stop-aware update ;
+ * *step += 1 }, the launches per step of mugd_sample_unipc.  It checks the descriptor before the plan. */
+int  mugd_sample_unipc_stop(mugd_plan* eval_plan, const mugd_unipc_stop* e, int32_t first_step, int32_t n_steps, void* stream);
+/* the stop-aware update alone for the counter's step, for a host that runs the steps one by one */
+int  mugd_unipc_stop_update(const mugd_unipc_stop* e, void* stream);
+
 /* ---- remixing an existing chart (SDEdit / img2img): DDIMSampler.stochastic_encode and decode with a per-chart start ---------------
  * mugd_stochastic_encode: out[b] = sqrt_a[t[b]] * x0[b] + sqrt_1ma[t[b]] * noise[b], each product and the sum one IEEE
  * round-to-nearest (no contraction), bit-identical to torch's extract_into_tensor expressions.  x0, noise and out are device NCL

@@ -375,6 +375,30 @@ int mugd_sample_unipc(mugd_plan* eval_plan, const mugd_unipc* u, int32_t first_s
     return run_steps(eval_plan, n_steps, u->dpm.step, st, no_kernels, [&](int32_t) { return launch_unipc_update(*u, st); });
 }
 
+int mugd_sample_unipc_ex(mugd_plan* eval_plan, const mugd_unipc_ex* e, int32_t first_step, int32_t n_steps, void* stream) {
+    // the descriptor is checked before the plan, so a host can test its arguments without a device
+    MUGD_REQUIRE(e, "mugd_sample_unipc_ex: null descriptor");
+    int rc = check_unipc_ex(*e, n_steps);
+    if (rc != MUGD_OK) return rc;
+    if ((rc = check_step_range("mugd_sample_unipc_ex", first_step, n_steps, "S", e->unipc.dpm.S)) != MUGD_OK) return rc;
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_unipc_ex: the evaluation plan must be captured (mugd_plan_capture)");
+    cudaStream_t st = (cudaStream_t)stream;
+    return run_steps(
+        eval_plan, n_steps, e->unipc.dpm.step, st, [&](int32_t k) { return e->stage ? launch_stage(*e->stage, k, st) : MUGD_OK; },
+        [&](int32_t) { return launch_unipc_ex_update(*e, st); });
+}
+
+int mugd_sample_unipc_stop(mugd_plan* eval_plan, const mugd_unipc_stop* e, int32_t first_step, int32_t n_steps, void* stream) {
+    // the descriptor is checked before the plan, so a host can test its arguments without a device
+    MUGD_REQUIRE(e, "mugd_sample_unipc_stop: null descriptor");
+    int rc = check_unipc_stop(*e);
+    if (rc != MUGD_OK) return rc;
+    if ((rc = check_step_range("mugd_sample_unipc_stop", first_step, n_steps, "S", e->unipc.dpm.S)) != MUGD_OK) return rc;
+    MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_unipc_stop: the evaluation plan must be captured (mugd_plan_capture)");
+    cudaStream_t st = (cudaStream_t)stream;
+    return run_steps(eval_plan, n_steps, e->unipc.dpm.step, st, no_kernels, [&](int32_t) { return launch_unipc_stop_update(*e, st); });
+}
+
 int mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
                      int32_t n_steps, void* stream) {
     MUGD_REQUIRE(eval_plan && eval_plan->exec, "mugd_sample_join: the evaluation plan must be captured (mugd_plan_capture)");

@@ -88,6 +88,12 @@ int launch_dpm_stop_update(const mugd_dpm_stop& e, cudaStream_t st);
 // counter's step
 int check_unipc(const mugd_unipc& u);
 int launch_unipc_update(const mugd_unipc& u, cudaStream_t st);
+// mugd_sample_unipc_ex / mugd_unipc_ex_update and mugd_sample_unipc_stop / mugd_unipc_stop_update: the UniPC counterparts of the
+// DPM-Solver++ ex and stop pairs above
+int check_unipc_ex(const mugd_unipc_ex& e, int32_t n_steps);
+int launch_unipc_ex_update(const mugd_unipc_ex& e, cudaStream_t st);
+int check_unipc_stop(const mugd_unipc_stop& e);
+int launch_unipc_stop_update(const mugd_unipc_stop& e, cudaStream_t st);
 // mugd_sample_join: check_join validates the descriptor; launch_join runs the join kernel against the device step counter
 int check_join(const mugd_join& j);
 int launch_join(const mugd_join& j, const int32_t* step, cudaStream_t st);

@@ -111,8 +111,25 @@ def step_orders(S: int, order: int, lower_order_final: bool) -> np.ndarray:
     return np.asarray(out, dtype=np.int64)
 
 
+class GridTables:
+    """The tables a schedule whose rows begin with (alpha_i, sigma_i) of t_i (``rows_f32``) gives the inpainting blend and the remix
+    encoder; DPMSchedule and unipc.UniPCSchedule share them."""
+
+    def q_coef_f32(self) -> np.ndarray:
+        """the inpainting blend's [S, 2] table (alpha_i, sigma_i) of t_i, the rows' first two columns in float32"""
+        return np.ascontiguousarray(self.rows_f32()[:, :2])
+
+    def encode_tables_f32(self):
+        """the noising tables of a chart that is to be denoised over its last s steps, indexed by s in [0, S]: (alpha, sigma) of
+        t_S-s for s >= 1, and (1, 0) at s = 0 so that such a chart comes back exactly"""
+        a, s = np.ones(self.S + 1, np.float32), np.zeros(self.S + 1, np.float32)
+        r = self.rows_f32()
+        a[1:], s[1:] = r[::-1, ROW_ALPHA], r[::-1, ROW_SIGMA]
+        return a, s
+
+
 @dataclass
-class DPMSchedule:
+class DPMSchedule(GridTables):
     """One request's tables: ``model_times`` [S] float32 (evaluation i runs at model_times[i]), ``rows`` [S, 8] float64
     (alpha_i, sigma_i, A, c0, c1, c2, order, 0), the continuous grid ``t`` [S + 1] and each step's ``orders``."""
     t: np.ndarray
@@ -136,18 +153,6 @@ class DPMSchedule:
         """``order_rows`` [S, 3, 8] rounded once to float32: row (i, k - 1) is the order-k update from t_i to t_i+1 (NaN where
         k > i + 1, an update no chart can take), as the per-chart update kernel reads them"""
         return np.ascontiguousarray(self.order_rows, dtype=np.float32)
-
-    def q_coef_f32(self) -> np.ndarray:
-        """the inpainting blend's [S, 2] table (alpha_i, sigma_i) of t_i, the rows' first two columns in float32"""
-        return np.ascontiguousarray(self.rows_f32()[:, :2])
-
-    def encode_tables_f32(self):
-        """the noising tables of a chart that is to be denoised over its last s steps, indexed by s in [0, S]: (alpha, sigma) of
-        t_S-s for s >= 1, and (1, 0) at s = 0 so that such a chart comes back exactly"""
-        a, s = np.ones(self.S + 1, np.float32), np.zeros(self.S + 1, np.float32)
-        r = self.rows_f32()
-        a[1:], s[1:] = r[::-1, ROW_ALPHA], r[::-1, ROW_SIGMA]
-        return a, s
 
 
 def chart_orders(sched: DPMSchedule, starts) -> np.ndarray:

@@ -132,6 +132,15 @@ class Unipc(C.Structure):
     _fields_ = [("dpm", Dpm), ("xc", _f), ("corr", _f)]
 
 
+class UnipcEx(C.Structure):
+    _fields_ = [("unipc", Unipc), ("stage", _f), ("start", _f), ("order_coef", _f), ("order_corr", _f), ("B", C.c_int32),
+                ("reserved_", C.c_int32)]
+
+
+class UnipcStop(C.Structure):
+    _fields_ = [("unipc", Unipc), ("stop", _f), ("B", C.c_int32), ("reserved_", C.c_int32)]
+
+
 class QEncode(C.Structure):
     _fields_ = [("x0", _f), ("noise", _f), ("t", _f), ("sqrt_a", _f), ("sqrt_1ma", _f), ("out", _f),
                 ("B", C.c_int32), ("C", C.c_int32), ("L", C.c_int32), ("n", C.c_int32)]
@@ -236,6 +245,10 @@ def load() -> C.CDLL:
     lib.mugd_dpm_stop_update.argtypes = [C.POINTER(DpmStop), C.c_void_p]
     lib.mugd_sample_unipc.argtypes = [C.c_void_p, C.POINTER(Unipc), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_unipc_update.argtypes = [C.POINTER(Unipc), C.c_void_p]
+    lib.mugd_sample_unipc_ex.argtypes = [C.c_void_p, C.POINTER(UnipcEx), C.c_int32, C.c_int32, C.c_void_p]
+    lib.mugd_unipc_ex_update.argtypes = [C.POINTER(UnipcEx), C.c_void_p]
+    lib.mugd_sample_unipc_stop.argtypes = [C.c_void_p, C.POINTER(UnipcStop), C.c_int32, C.c_int32, C.c_void_p]
+    lib.mugd_unipc_stop_update.argtypes = [C.POINTER(UnipcStop), C.c_void_p]
     lib.mugd_stochastic_encode.argtypes = [C.POINTER(QEncode), C.c_void_p]
     lib.mugd_sample_join.argtypes = [C.c_void_p, C.POINTER(Join), C.POINTER(Op), C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_plan_save.argtypes = [C.c_void_p, C.POINTER(Region), C.c_int32, C.c_char_p]
@@ -278,5 +291,6 @@ EXPORTED_SYMBOLS = [
     "mugd_sample_ddpm", "mugd_ddpm_update", "mugd_stochastic_encode", "mugd_sample_join",
     "mugd_sample_dpm", "mugd_dpm_update", "mugd_sample_dpm_ex", "mugd_dpm_ex_update",
     "mugd_sample_dpm_stop", "mugd_dpm_stop_update",
-    "mugd_sample_unipc", "mugd_unipc_update",
+    "mugd_sample_unipc", "mugd_unipc_update", "mugd_sample_unipc_ex", "mugd_unipc_ex_update",
+    "mugd_sample_unipc_stop", "mugd_unipc_stop_update",
 ]

@@ -88,6 +88,16 @@ class Plan:
         """steps first_step .. first_step + steps - 1 of a UniPC request from one C call (mugd_sample_unipc)"""
         self._launch_steps("mugd_sample_unipc", u, first_step, steps)
 
+    def launch_unipc_ex(self, ex: L_.UnipcEx, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a UniPC inpainting or per-chart-start request from one C call
+        (mugd_sample_unipc_ex)"""
+        self._launch_steps("mugd_sample_unipc_ex", ex, first_step, steps)
+
+    def launch_unipc_stop(self, e: L_.UnipcStop, first_step: int, steps: int):
+        """steps first_step .. first_step + steps - 1 of a UniPC inversion with one stop per chart from one C call
+        (mugd_sample_unipc_stop)"""
+        self._launch_steps("mugd_sample_unipc_stop", e, first_step, steps)
+
     def launch_join(self, join: L_.Join, tail: OpList, first_step: int, steps: int):
         """steps first_step .. first_step + steps - 1 of a decode request whose charts join at different iterations, from one C call
         (mugd_sample_join: the join kernel, the graph replay and the tail per step)"""
@@ -596,6 +606,31 @@ class Session:
         assert xc.numel() == u.dpm.n and xc.dtype == torch.float32 and xc.is_contiguous()
         u.xc, u.corr = _ptr(xc), _ptr(corr)
         return u
+
+    def unipc_ex(self, u: L_.Unipc, stage: Optional[L_.Stage] = None, B: int = 0, start: Optional[torch.Tensor] = None,
+                 order_coef: Optional[torch.Tensor] = None, order_corr: Optional[torch.Tensor] = None) -> L_.UnipcEx:
+        """the mugd_sample_unipc_ex descriptor around ``u``: with ``stage`` (ddim_stage's, x0 / mask / q_noise / q_coef filled in) the
+        inpainting blend runs in front of each step; with ``start`` ([B] int32, the first step of each chart) and ``order_coef`` /
+        ``order_corr`` (the [S, 3, 8] per-order predictor and corrector rows) every chart runs from its own step.  The caller keeps
+        the stage and the tensors alive."""
+        e = L_.UnipcEx()
+        e.unipc = u
+        e.stage = C.addressof(stage) if stage is not None else None
+        if start is not None:
+            S = u.dpm.S
+            assert start.shape == (B,) and start.dtype == torch.int32 and start.is_contiguous()
+            for t in (order_coef, order_corr):
+                assert t.shape == (S, 3, 8) and t.dtype == torch.float32 and t.is_contiguous()
+            e.start, e.order_coef, e.order_corr, e.B = _ptr(start), _ptr(order_coef), _ptr(order_corr), B
+        return e
+
+    def unipc_stop(self, u: L_.Unipc, B: int, stop: torch.Tensor) -> L_.UnipcStop:
+        """the mugd_sample_unipc_stop descriptor around ``u`` (an inversion schedule's rows): chart b runs iterations 0 .. stop[b] - 1
+        (``stop``: [B] int32 on the device).  The caller keeps the tensor alive."""
+        assert stop.shape == (B,) and stop.dtype == torch.int32 and stop.is_contiguous()
+        e = L_.UnipcStop()
+        e.unipc, e.stop, e.B = u, _ptr(stop), B
+        return e
 
     def ddim_tail(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> OpList:
         """the ops that follow each evaluation of an S-step request for B samples: the DDIM update of the xin rows (both halves

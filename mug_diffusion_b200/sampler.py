@@ -29,7 +29,7 @@ from .engine import MAX_STEPS, OpList, View
 from .lib import MugdError
 from .postprocess import objects_to_array
 from .prompt import PromptEmbedder
-from .runtime import DiagonalGaussianDistribution, MugEngine, Session, _ptr
+from .runtime import DiagonalGaussianDistribution, MugEngine, Plan, Session, _ptr
 
 try:  # the reference falls back to tqdm when no tqdm_class is given (ddim.py:133-135)
     from tqdm import tqdm as _tqdm
@@ -553,10 +553,11 @@ class _DeviceLoopSampler:
             L_.check(eng.lib.mugd_stochastic_encode(C.byref(d), torch.cuda.current_stream().cuda_stream), "mugd_stochastic_encode")
         return out
 
-    def _invert(self, who, x0, c, w, t_enc, inv: dpm_solver.DPMSchedule, scale, uc, callback, img_callback, log_every_t, tqdm_class,
-                verbose, kwargs):
-        """``invert`` of both samplers: the checks, before any GPU work, then the inversion over the rows of ``inv`` (an
-        ``inversion_schedule``) in which chart b runs steps 0 .. t_enc[b] - 1.  Returns z; ``last_intermediates`` holds the logged
+    def _invert(self, who, x0, c, w, t_enc, inv, scale, uc, callback, img_callback, log_every_t, tqdm_class, verbose, kwargs,
+                solver=None):
+        """``invert`` of every sampler: the checks, before any GPU work, then the inversion over the rows of ``inv`` (an
+        ``inversion_schedule``) in which chart b runs steps 0 .. t_enc[b] - 1.  ``solver``: (descriptor, launch, update) of
+        ``_inversion``, DPM-Solver++'s stop-aware update when not given.  Returns z; ``last_intermediates`` holds the logged
         intermediates."""
         _refuse_ddim_only(kwargs, who, "inversion is deterministic and has no {}", "invert")
         model = self.model
@@ -577,12 +578,15 @@ class _DeviceLoopSampler:
             return x0
         if verbose:
             print(f'Inverting {B} charts of shape {tuple(x0.shape[1:])} over t_enc = {stops} of {inv.S} steps')
-        return self._inversion(x0, c, w, stops, inv, scale, uc, callback, img_callback, log_every_t, tqdm_class)
+        return self._inversion(x0, c, w, stops, inv, scale, uc, callback, img_callback, log_every_t, tqdm_class,
+                               *(solver or _dpm_stop_solver(inv)))
 
-    def _inversion(self, x0, c, w, stops, inv: dpm_solver.DPMSchedule, scale, uc, callback, img_callback, log_every_t, tqdm_class):
+    def _inversion(self, x0, c, w, stops, inv, scale, uc, callback, img_callback, log_every_t, tqdm_class, descriptor, launch, update):
         """the inversion of checked arguments on the GPU: one loop of m = max(stops) iterations over rows 0 .. m - 1 of ``inv``.
-        Without callbacks it runs from mugd_sample_dpm_stop calls (one per stretch between logged steps), with them one by one
-        through mugd_dpm_stop_update; both launch the same kernels."""
+        ``descriptor(sess, B, m, cfg_on, scale, pred, ring, stop)`` gives the solver's stop-aware descriptor and the tensors it
+        points to; ``launch`` is the Plan method that runs steps from one C call and ``update`` the libmugd entry point of one step.
+        Without callbacks the steps run from ``launch`` calls (one per stretch between logged steps), with them one by one through
+        ``update``; both launch the same kernels."""
         model = self.model
         eng = model.engine
         dev = self.device
@@ -591,14 +595,13 @@ class _DeviceLoopSampler:
         m = max(stops)
         with eng.lock:
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x0, scale, uc, inv.model_times[:m])
-            coef = torch.from_numpy(inv.rows_f32()[:m].copy()).to(dev)
             ring = torch.empty(3, B * Lz * Cz, device=dev)                     # the data predictions of the last three steps
             pred = torch.zeros(B * Lz, Cz, device=dev)                          # a stopped chart keeps its last prediction
             stop = torch.tensor(stops, dtype=torch.int32, device=dev)
-            e = sess.dpm_stop(sess.dpm(B, m, cfg_on, scale, _ptr(pred), ring, coef), B, stop)
+            e, alive = descriptor(sess, B, m, cfg_on, scale, pred, ring, stop)  # alive: the tensors e points to, held until the end
 
-            def launch(first, n):
-                sess.plan.launch_dpm_stop(e, first, n)
+            def run(first, n):
+                launch(sess.plan, e, first, n)
 
             # the per-step loop runs the same kernel: the referee of the device loop
             advance = _step_ops(sess)
@@ -606,12 +609,12 @@ class _DeviceLoopSampler:
 
             def step(i, t):
                 sess.eval(graph=True)
-                L_.check(eng.lib.mugd_dpm_stop_update(C.byref(e), stream), "mugd_dpm_stop_update")
+                L_.check(getattr(eng.lib, update)(C.byref(e), stream), update)
                 eng.run_ops(advance)
 
             z, self.last_intermediates = self._run_request(sess, x, shape, pred, time_range, m, log_every_t, 'Inverting a chart',
                                                            tqdm_class, True, callback, img_callback,
-                                                           callback is None and img_callback is None, launch, step, 2)
+                                                           callback is None and img_callback is None, run, step, 2)
             return z
 
     def _check_latent(self, x_latent):
@@ -620,6 +623,24 @@ class _DeviceLoopSampler:
         if not isinstance(x_latent, torch.Tensor) or x_latent.dim() != 3 or x_latent.shape[0] < 1 or x_latent.shape[1] != z:
             raise ValueError(f"x_latent must be a [B, {z}, L] tensor"
                              + (f", got {tuple(x_latent.shape)}" if isinstance(x_latent, torch.Tensor) else ""))
+
+
+def _dpm_stop_solver(inv: dpm_solver.DPMSchedule):
+    """``_inversion``'s (descriptor, launch, update) for DPM-Solver++ (and DDIM) rows: mugd_dpm_stop over rows 0 .. m - 1 of ``inv``"""
+    def descriptor(sess, B, m, cfg_on, scale, pred, ring, stop):
+        coef = torch.from_numpy(inv.rows_f32()[:m].copy()).to(ring.device)
+        return sess.dpm_stop(sess.dpm(B, m, cfg_on, scale, _ptr(pred), ring, coef), B, stop), (coef,)
+    return descriptor, Plan.launch_dpm_stop, "mugd_dpm_stop_update"
+
+
+def _unipc_stop_solver(inv: unipc.UniPCSchedule):
+    """``_inversion``'s (descriptor, launch, update) for UniPC rows: mugd_unipc_stop over rows 0 .. m - 1 of ``inv``"""
+    def descriptor(sess, B, m, cfg_on, scale, pred, ring, stop):
+        coef = torch.from_numpy(inv.rows_f32()[:m].copy()).to(ring.device)
+        corr = torch.from_numpy(inv.corr_rows_f32()[:m].copy()).to(ring.device)
+        xc = torch.empty(ring.shape[1], device=ring.device)                  # the corrected latent of the previous step
+        return sess.unipc_stop(sess.unipc(B, m, cfg_on, scale, _ptr(pred), ring, coef, xc, corr), B, stop), (coef, corr, xc)
+    return descriptor, Plan.launch_unipc_stop, "mugd_unipc_stop_update"
 
 
 def _step_ops(sess: Session, update: Optional[L_.DdimUpdate] = None) -> OpList:
@@ -1442,15 +1463,46 @@ class UniPCSampler(_DeviceLoopSampler):
                                    tqdm_class=tqdm_class)
 
     @torch.no_grad()
+    def inpaint(self, S, c=None, w=None, batch_size=None, mask=None, x0=None, shape=None, x_T=None, order=2, skip_type="time_uniform",
+                variant="bh2", lower_order_final=True, use_corrector=True, disable_corrector=(), t_grid=None, callback=None,
+                img_callback=None, log_every_t=100, unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None,
+                verbose=True, conditioning=None):
+        """Regenerate the part of the chart ``x0`` [B, C, L] where ``mask`` (broadcast to [B, C, L]) is 0, keeping the rest: ``sample``
+        in which, before the evaluation of iteration i, x~_i <- (alpha_i * x0 + sigma_i * eps_i) * mask + (1 - mask) * x~_i with the
+        schedule's alpha_i / sigma_i of t_i and eps_i = randn_like(x0) drawn per step from the device's generator (the draw order of
+        DDIM inpainting at eta = 0 and of DPMSolverSampler.inpaint).  The blend touches only the latent the U-Net sees; xc, the
+        corrector's previous corrected latent, is the solver's own state and is not blended.  Returns ``(z, {'x_inter', 'pred_x0'})``
+        logged as by ``sample``.  Every argument is checked before any GPU work (those of ``sample``; x0 of the request's shape, a mask
+        that broadcasts to it).  Without callbacks, and with float32 mask / x0 on the model's device (``takes_device_loop``), the
+        steps run from mugd_sample_unipc_ex calls with the blend staged in front of each step (the noise of a call drawn up front, at
+        most STAGE_TABLE_BYTES per table); otherwise one by one."""
+        c = _conditioning(c, conditioning)
+        if not isinstance(mask, torch.Tensor) or not isinstance(x0, torch.Tensor):
+            raise ValueError("inpainting needs the mask and x0 as tensors")
+        if c is None or w is None:
+            raise TypeError("UniPCSampler.inpaint needs the conditioning c and the audio features w")
+        scale = _finite_scale(unconditional_guidance_scale)
+        sched = self.make_unipc_schedule(S, order, skip_type, variant, lower_order_final, use_corrector, disable_corrector, t_grid)
+        size = request_size(self.model, c, batch_size, shape, x_T, mask, x0, scale, unconditional_conditioning, log_every_t)
+        if verbose:
+            print(f'Data shape for UniPC inpainting is {size}, {S} steps of order {order} ({skip_type}, {variant})')
+        return self.unipc_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
+                                   unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
+                                   tqdm_class=tqdm_class, mask=mask, x0=x0)
+
+    @torch.no_grad()
     def unipc_sampling(self, w, c, shape, sched: unipc.UniPCSchedule, x_T=None, callback=None, img_callback=None, log_every_t=100,
-                       unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True):
-        """the request of ``sched`` (make_unipc_schedule) on the GPU, from checked arguments"""
+                       unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, mask=None,
+                       x0=None):
+        """the request of ``sched`` (make_unipc_schedule) on the GPU, from checked arguments; with ``mask`` / ``x0`` the inpainting of
+        ``inpaint``"""
         model = self.model
         eng = model.engine
         dev = self.device
         B, Cz, Lz = shape
         total = sched.S
         scale = unconditional_guidance_scale
+        blend = mask is not None
         self.last_schedule = sched
         with eng.lock:
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times)
@@ -1460,20 +1512,140 @@ class UniPCSampler(_DeviceLoopSampler):
             xc = torch.empty(B * Lz * Cz, device=dev)                          # the corrected latent of the previous step
             pred = torch.empty(B * Lz, Cz, device=dev)
             u = sess.unipc(B, total, cfg_on, scale, _ptr(pred), ring, coef, xc, corr)
+            device_loop = takes_device_loop(shape, x.device, mask, x0, callback, img_callback)
+            qcoef = sched.q_coef_f32() if blend else None                       # (alpha_i, sigma_i) of the blend before iteration i
+            per_call = max(1, STAGE_TABLE_BYTES // (4 * B * Cz * Lz))
+            stage = None
+            if device_loop and blend:
+                # the blend runs in front of every step (mugd_sample_unipc_ex); a call's q_sample noise is drawn up front, in the
+                # per-step loop's order
+                stage = sess.ddim_stage(B, cfg_on)
+                x0c = x0.contiguous()
+                mask_e = mask.expand(shape).contiguous()                        # the blend's mask, expanded once per request
+                q_tab = torch.empty((min(per_call, total),) + tuple(shape), device=dev)
+                stage.x0, stage.mask, stage.q_noise = _ptr(x0c), _ptr(mask_e), _ptr(q_tab)
+                ex = sess.unipc_ex(u, stage)
 
             def launch(first, n):
                 # the ring, xc and the step counter stay on the device, so a call may start anywhere in the request
-                sess.plan.launch_unipc(u, first, n)
+                if stage is None:
+                    sess.plan.launch_unipc(u, first, n)
+                else:
+                    draw_step_noise(n, shape, x0, q_tab, False, None, 0., dev)
+                    stage.q_coef = qcoef[first:].ctypes.data
+                    sess.plan.launch_unipc_ex(ex, first, n)
 
-            # the per-step loop runs the same kernel: the referee of the device loop
+            # the per-step loop runs the same kernels: the referee of the device loop
             advance = _step_ops(sess)
             stream = torch.cuda.current_stream().cuda_stream
+            q_dev = torch.from_numpy(qcoef).to(dev) if blend else None
 
             def step(i, t):
+                if blend:
+                    x0d = x0.to(dev)
+                    x_orig = q_dev[i, 0] * x0d + q_dev[i, 1] * torch.randn_like(x0d)
+                    sess.load_x(x_orig * mask + (1. - mask) * self._read_x(sess, shape), dup=cfg_on)
                 sess.eval(graph=True)
                 L_.check(eng.lib.mugd_unipc_update(C.byref(u), stream), "mugd_unipc_update")
                 eng.run_ops(advance)
 
             return self._run_request(sess, x, shape, pred, time_range, total, log_every_t, 'Charting, using UniPC Sampler',
-                                     tqdm_class, progress, callback, img_callback, callback is None and img_callback is None, launch,
-                                     step, 2)
+                                     tqdm_class, progress, callback, img_callback, device_loop, launch, step,
+                                     3 if stage is not None else 2, chunk=per_call if stage is not None else None)
+
+    # ---- remixing and inverting an existing chart on the UniPC grid ---------------------------------------------------------------
+    @staticmethod
+    def _require_schedule(sched):
+        if not isinstance(sched, unipc.UniPCSchedule) or sched.order_rows is None or sched.order_corr is None:
+            raise ValueError("sched must be a UniPCSchedule from make_unipc_schedule")
+
+    @torch.no_grad()
+    def stochastic_encode(self, x0, t_enc, sched: unipc.UniPCSchedule, noise=None):
+        """Noise the latent ``x0`` [B, C, L] for a remix over the last ``t_enc[b]`` steps of ``sched`` (an integer in [0, S], or one per
+        chart): alpha(t_S-s) * x0 + sigma(t_S-s) * noise with s = t_enc[b], the marginal at the time where ``decode`` with t_start = s
+        starts; s = 0 returns x0 exactly.  noise = torch.randn_like(x0) when not given.  DPMSolverSampler.stochastic_encode's kernel
+        and contract.  ValueError, before any GPU work, for malformed arguments."""
+        self._require_schedule(sched)
+        return self._stochastic_encode(x0, noise, lambda B: per_chart_steps(B, t_enc, sched.S, "t_enc", " (S = sched.S)"),
+                                       lambda: [torch.from_numpy(v).to(self.device) for v in sched.encode_tables_f32()], sched.S + 1)
+
+    @torch.no_grad()
+    def decode(self, x_latent, c, w, t_start, sched: unipc.UniPCSchedule, unconditional_guidance_scale=1.,
+               unconditional_conditioning=None, tqdm_class=None):
+        """Denoise ``x_latent`` [B, C, L] (e.g. from ``stochastic_encode``) under (c, w) over the last ``t_start`` steps of ``sched``:
+        chart b runs iterations f_b = S - t_start[b] .. S - 1 from x_latent[b] (``t_start``: an integer in [0, S], or one per chart)
+        and returns the final latent.  It warms up like a fresh request (``unipc.chart_orders``): its predictor at iteration i has
+        order min(sched.orders[i], i - f_b + 1), and its corrector runs only where sched.corrector[i] is set and i > f_b (there is
+        no earlier evaluation at f_b), at order min(sched.orders[i - 1], i - f_b).  All charts run in one device loop of
+        m = max(t_start) iterations from iteration S - m (mugd_sample_unipc_ex, the launches per step of mugd_sample_unipc); a chart
+        is left untouched until its start, and one with t_start[b] = 0 comes back as x_latent[b].  With every t_start = S this is
+        unipc_sampling(x_T=x_latent) bit for bit.  Every argument is checked before any GPU work (ValueError)."""
+        model = self.model
+        self._require_schedule(sched)
+        self._check_latent(x_latent)
+        starts = per_chart_steps(x_latent.shape[0], t_start, sched.S, "t_start", " (S = sched.S)")
+        scale = _finite_scale(unconditional_guidance_scale)
+        B, Cz, Lz = (int(v) for v in x_latent.shape)
+        request_size(model, c, B, (Cz, Lz), x_latent, None, None, scale, unconditional_conditioning, 1)
+        if c is None or w is None:
+            raise ValueError("decode needs the conditioning c and the audio features w")
+        if max(starts) == 0:
+            return x_latent
+        return self.unipc_decoding(w, c, x_latent, starts, sched, scale, unconditional_conditioning, tqdm_class)
+
+    @torch.no_grad()
+    def unipc_decoding(self, w, c, x_latent, starts, sched: unipc.UniPCSchedule, unconditional_guidance_scale=1.,
+                       unconditional_conditioning=None, tqdm_class=None, per_step=False):
+        """``decode`` of checked arguments (``starts``: t_start per chart, max(starts) >= 1) on the GPU.  ``per_step``: the steps run
+        one by one through mugd_unipc_ex_update, the referee of the device loop."""
+        model = self.model
+        eng = model.engine
+        dev = self.device
+        B, Cz, Lz = (int(v) for v in x_latent.shape)
+        shape = (B, Cz, Lz)
+        S, m = sched.S, max(starts)
+        with eng.lock:
+            # the timestep table holds all S model times and the counter starts at S - m, so step i reads row i of every table
+            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_latent, unconditional_guidance_scale,
+                                                             unconditional_conditioning, sched.model_times)
+            sess.set_step(S - m)
+            coef = torch.from_numpy(sched.rows_f32()).to(dev)
+            corr = torch.from_numpy(sched.corr_rows_f32()).to(dev)
+            order_coef = torch.from_numpy(sched.order_rows_f32()).to(dev)
+            order_corr = torch.from_numpy(sched.order_corr_f32()).to(dev)
+            first = torch.tensor([S - s for s in starts], dtype=torch.int32, device=dev)
+            ring = torch.empty(3, B * Lz * Cz, device=dev)
+            xc = torch.empty(B * Lz * Cz, device=dev)
+            u = sess.unipc(B, S, cfg_on, unconditional_guidance_scale, 0, ring, coef, xc, corr)
+            ex = sess.unipc_ex(u, B=B, start=first, order_coef=order_coef, order_corr=order_corr)
+            bar = self._progress(time_range[S - m:], 'Decoding image', m, tqdm_class)
+            if per_step:
+                advance = _step_ops(sess)
+                stream = torch.cuda.current_stream().cuda_stream
+                for _ in bar:
+                    sess.eval(graph=True)
+                    L_.check(eng.lib.mugd_unipc_ex_update(C.byref(ex), stream), "mugd_unipc_ex_update")
+                    eng.run_ops(advance)
+            else:
+                sess.plan.launch_unipc_ex(ex, S - m, m)
+                for _ in bar:                                                   # keeps a progress bar moving
+                    pass
+            self.last_launches_per_step = sess.plan.launches + 2
+            return self._read_x(sess, shape)
+
+    @torch.no_grad()
+    def invert(self, x0, c, w, t_enc, sched: unipc.UniPCSchedule, unconditional_guidance_scale=1., unconditional_conditioning=None,
+               callback=None, img_callback=None, log_every_t=100, tqdm_class=None, verbose=True, **kwargs):
+        """Deterministic inversion: run the latent ``x0`` [B, C, z_length] of a chart backwards along UniPC's ODE solution of ``sched``
+        (make_unipc_schedule), with the U-Net in the loop, t_enc[b] iterations for chart b (an integer in [0, S], or one per chart),
+        on ``unipc.inversion_schedule(sched)``: the reversed grid, predictor orders min(j + 1, order), and the corrector on every
+        iteration j >= 1 when ``sched`` has one (its disable_corrector steps do not carry over).  Chart b ends at t_S-t_enc[b], where
+        ``decode(z, c, w, t_start=t_enc, sched)`` starts it: same t_enc, no off-by-one.  t_enc[b] = 0 returns x0[b] bit for bit.  All
+        charts run in one loop of max(t_enc) iterations; a chart is left untouched once it has run its steps.  Draws no random
+        numbers.  Returns z; ``last_intermediates`` holds {'x_inter', 'pred_x0'} logged as by ``sample``.  Without callbacks the steps
+        run from mugd_sample_unipc_stop calls, with them one by one through mugd_unipc_stop_update.  Every argument is checked before
+        any GPU work (ValueError); mask, eta, temperature and noise dropout are refused."""
+        self._require_schedule(sched)
+        inv = unipc.inversion_schedule(sched)
+        return self._invert("UniPCSampler", x0, c, w, t_enc, inv, unconditional_guidance_scale, unconditional_conditioning, callback,
+                            img_callback, log_every_t, tqdm_class, verbose, kwargs, _unipc_stop_solver(inv))
