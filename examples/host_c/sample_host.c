@@ -2,11 +2,14 @@
  * from a bundle written by `python -m mug_diffusion_b200.bundle`, through the C ABI of libmugd.so only.
  *
  *   make -C examples/host_c            (gcc + the CUDA runtime; no torch, no Python)
- *   examples/host_c/sample_host <bundle dir>
+ *   examples/host_c/sample_host <bundle dir>             (reproduce the bundle's request, compare with its expected outputs)
+ *   examples/host_c/sample_host <bundle dir> --seed N    (a seeded bundle: draw charts N, N + 1, ... instead; no comparison)
  *
  * manifest.txt lines:  region <name> <bytes> zero|file <file>   |  plan <file> run|graph  |  sample <eval> <tail> <steps>
  *                      stage <field> <region> <offset>          (one pointer of the mugd_stage of the next `staged` line)
  *                      staged <eval> <tail> <steps> <q_coef file>|- <B> <C> <L>   (inpainting / eta > 0: mugd_sample_staged)
+ *                      seeds <file> <B>                         (a seeded bundle: the charts' uint64 seeds, uploaded once)
+ *                      randn <region> <purpose> <first_draw> <n_draws> <draw_stride> <B> <n>   (fill a region with mugd_randn)
  *                      expect <region> <bytes> <file>           (outputs to compare; exit status 1 on mismatch)
  * This mirrors what DDIMSampler.sample + model.decode do in the reference (mug/diffusion/ddim.py:56-196, diffusion.py:49-50). */
 #include <cuda_runtime.h>
@@ -44,8 +47,10 @@ static mugd_region* find_region(const char* name) {
 }
 
 int main(int argc, char** argv) {
-    if (argc < 2) { fprintf(stderr, "usage: %s <bundle dir>\n", argv[0]); return 2; }
+    if (argc != 2 && !(argc == 4 && strcmp(argv[2], "--seed") == 0)) { fprintf(stderr, "usage: %s <bundle dir> [--seed N]\n", argv[0]); return 2; }
     const char* dir = argv[1];
+    const int own_seed = argc == 4;
+    const unsigned long long seed0 = own_seed ? strtoull(argv[3], NULL, 10) : 0;
     char path[1024], line[2048];
     snprintf(path, sizeof(path), "%s/manifest.txt", dir);
     FILE* mf = fopen(path, "r");
@@ -63,6 +68,8 @@ int main(int argc, char** argv) {
     float sample_ms = 0.f;
     mugd_stage stage;
     memset(&stage, 0, sizeof(stage));
+    uint64_t* seeds = NULL;                /* device [B]: the charts' seeds of a seeded bundle */
+    int n_seeds = 0;
 
     while (fgets(line, sizeof(line), mf)) {
         char a[64], b[256], c[256], d[256];
@@ -153,7 +160,35 @@ int main(int argc, char** argv) {
             free(q_coef);
             mugd_plan_destroy(pe);
             mugd_plan_destroy(pt);
+        } else if (strcmp(a, "seeds") == 0) {
+            if (sscanf(line, "%*s %255s %d", b, &n_seeds) != 2 || n_seeds < 1 || seeds) { fprintf(stderr, "bad line: %s", line); return 2; }
+            uint64_t* host = (uint64_t*)read_file(dir, b, 8LL * n_seeds);
+            for (int i = 0; own_seed && i < n_seeds; ++i) host[i] = seed0 + (unsigned long long)i;   /* chart i = seed + i (mod 2^64) */
+            CK(cudaMalloc((void**)&seeds, 8 * (size_t)n_seeds));
+            CK(cudaMemcpy(seeds, host, 8 * (size_t)n_seeds, cudaMemcpyHostToDevice));
+            free(host);
+        } else if (strcmp(a, "randn") == 0) {
+            mugd_normal nd;
+            memset(&nd, 0, sizeof(nd));
+            long long n = 0;
+            if (sscanf(line, "%*s %63s %d %d %d %d %d %lld", d, &nd.purpose, &nd.first_draw, &nd.n_draws, &nd.draw_stride, &nd.B, &n) != 7 ||
+                !seeds || nd.B != n_seeds) {
+                fprintf(stderr, "bad line (or no seeds line before it): %s", line);
+                return 2;
+            }
+            mugd_region* r = find_region(d);
+            if (4LL * n * nd.B * nd.n_draws > r->bytes) { fprintf(stderr, "randn table larger than region %s: %s", d, line); return 2; }
+            nd.out = (float*)r->base;
+            nd.seeds = seeds;
+            nd.n = n;
+            MK(mugd_randn(&nd, st));
+            CK(cudaStreamSynchronize(st));
+            printf("drew %-12s purpose %d, draws %d x %d from %d, %d charts\n", d, nd.purpose, nd.n_draws, nd.draw_stride, nd.first_draw, nd.B);
         } else if (strcmp(a, "expect") == 0) {
+            if (own_seed) {
+                if (sscanf(line, "%*s %63s", d) == 1) printf("%-12s not compared: charts drawn from --seed %llu\n", d, seed0);
+                continue;
+            }
             if (sscanf(line, "%*s %63s %lld %255s", d, &nbytes, b) != 3) { fprintf(stderr, "bad line: %s", line); return 2; }
             mugd_region* r = find_region(d);
             float* got = (float*)malloc((size_t)nbytes);
@@ -176,6 +211,8 @@ int main(int argc, char** argv) {
         }
     }
     fclose(mf);
+    if (own_seed && !seeds) { fprintf(stderr, "--seed needs a seeded bundle (python -m mug_diffusion_b200.bundle ... --seeds ...)\n"); return 2; }
+    if (seeds) CK(cudaFree(seeds));
     mugd_destroy(h);
     return bad;
 }

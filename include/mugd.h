@@ -507,6 +507,26 @@ typedef struct mugd_join {
 int  mugd_sample_join(mugd_plan* eval_plan, const mugd_join* join, const mugd_op* tail, int32_t n_tail, int32_t first_step,
                       int32_t n_steps, void* stream);
 
+/* ---- per-chart seeds: standard normals that depend only on (seed, purpose, draw, element) ------------------------------------------
+ * out[k][b][e] (k < n_draws, b < B, e < n) is element e of chart b for draw first_draw + draw_stride * k, with chart b's 64-bit seed
+ * seeds[b] (a device array).  For q = e >> 2:
+ *   (x0, x1, x2, x3) = Philox4x32-10(counter = (q, draw, purpose, 0), key = (lo32(seeds[b]), hi32(seeds[b])))
+ * and Box-Muller turns (x0, x1) into elements 4q, 4q + 1 and (x2, x3) into 4q + 2, 4q + 3:
+ *   u1 = ((xa >> 8) + 1) * 2^-24,  u2 = (xb >> 8) * 2^-24,  r = sqrtf(-2 logf(u1)),  z_even = r cospi(2 u2),  z_odd = r sinpi(2 u2).
+ * The values do not depend on B, on a chart's position in the batch, on the launch configuration or on the device, so one launch
+ * fills a whole [n_draws][B, C, L] noise table of mugd_sample_staged, mugd_sample_ddpm or the DPM-Solver++ / UniPC stages (n = C * L,
+ * NCL order), and a chart drawn alone gets the same bits.  draw_stride = -1 fills a table whose steps walk the schedule's rows
+ * downwards (DDIM, DDPM).  The descriptor is checked before any device call: MUGD_ERR_INVALID for a null pointer, B, n or n_draws
+ * below 1, a negative first_draw or purpose, draw_stride other than +-1, a draw outside [0, 2^31) or n / 4 past 2^32.  One launch. */
+typedef struct mugd_normal {
+    float* out;                            /* [n_draws][B][n]                                                  */
+    const uint64_t* seeds;                 /* [B] device: one seed per chart                                   */
+    int64_t n;                             /* elements per chart                                               */
+    int32_t B, purpose, first_draw, n_draws;
+    int32_t draw_stride, reserved_;        /* +1 or -1: row k holds draw first_draw + draw_stride * k          */
+} mugd_normal;
+int  mugd_randn(const mugd_normal* d, void* stream);
+
 /* ---- plans on disk: a host without Python (examples/host_c) loads what the Python plan compiler produced ---------------------
  * Every pointer of a plan lies in one of a few device allocations ("regions": weight blob, activation arena, side tables, the
  * caller's staging buffers).  mugd_plan_save stores each pointer as (region, offset); mugd_plan_load resolves them against the

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmugd.so")
 STAMP = os.path.join(HERE, "build", "libmugd.stamp")
-SOURCES = ["api.cu", "norm.cu", "gemm_simt.cu", "gemm_tc.cu", "attention.cu", "attention_tc.cu", "s4.cu", "elementwise.cu", "plan_io.cu", "melspec.cu", "gridscan.cu", "chartpost.cu", "plms.cu", "ddpm.cu", "remix.cu", "dpm.cu"]
+SOURCES = ["api.cu", "norm.cu", "gemm_simt.cu", "gemm_tc.cu", "attention.cu", "attention_tc.cu", "s4.cu", "elementwise.cu", "plan_io.cu", "melspec.cu", "gridscan.cu", "chartpost.cu", "plms.cu", "ddpm.cu", "remix.cu", "dpm.cu", "randn.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default", "--use_fast_math=false",

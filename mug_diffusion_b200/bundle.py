@@ -15,6 +15,9 @@ Request flow = DDIMSampler.sample + model.decode (ddim.py:56-196, diffusion.py:4
 An inpainting or eta > 0 request stages x0, the mask and the random numbers of every step (drawn up front from torch's CUDA generator in
 the sampler's order) as input regions, with the q_sample coefficients in stage_coef.bin, and runs its loop as one mugd_sample_staged
 call: `stage <field> <region> <offset>` lines describe the mugd_stage, `staged eval.plan tail.plan <steps> <coef file> <B> <C> <L>` runs it.
+A seeded bundle (--seeds 7,8) carries no random numbers: `seeds <file> <B>` gives the charts' 64-bit seeds and each
+`randn <region> <purpose> <first_draw> <n_draws> <draw_stride> <B> <n>` line fills x_T or a noise table with one mugd_randn call
+(seeding.py's convention), so the host can also draw new charts from seeds of its own.
 """
 from __future__ import annotations
 
@@ -27,6 +30,7 @@ import numpy as np
 import torch
 
 from . import lib as L_
+from . import seeding
 from .engine import OpList
 from .runtime import Plan, _ptr
 from .sampler import draw_step_noise, q_coef_table
@@ -40,10 +44,13 @@ def _save_plan(eng, ops: OpList, regions: List[L_.Region], path: str) -> Plan:
 
 
 def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out_dir: str, eta: float = 0.0, temperature: float = 1.0,
-                  noise_dropout: float = 0.0, inpaint: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
+                  noise_dropout: float = 0.0, inpaint: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                  seeds=None) -> Dict[str, torch.Tensor]:
     """Compile the request (inp: x_T, c, uc, w[4] on the host; inpaint: (x0, mask) of DDIMSampler.sample), write the bundle, run it
     once through the very same plans and return the results (z, logits) that the C host must reproduce.  The random numbers of an
-    eta > 0 or inpainting request are drawn here from the CUDA generator as DDIMSampler.sample draws them."""
+    eta > 0 or inpainting request are drawn here from the CUDA generator as DDIMSampler.sample draws them.  With ``seeds``
+    (seeding.chart_seeds) x_T and every noise table are the charts' seeded draws, DDIMSampler.sample(seeds=...)'s, and the bundle
+    holds the seeds and `randn` lines instead of their contents; inp's x_T is not used."""
     from .sampler import DDIMSampler
 
     os.makedirs(out_dir, exist_ok=True)
@@ -51,6 +58,10 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
     dev = eng.device
     cfg = eng.cfg
     B, Cz, Lz = inp["x_T"].shape
+    if seeds is not None:
+        if noise_dropout > 0.:
+            raise ValueError("a seeded bundle draws no dropout mask")
+        seeds = seeding.chart_seeds(seeds, B)
     cfg_on = scale != 1.0
     Beff = 2 * B if cfg_on else B
     sampler = DDIMSampler(model)
@@ -64,7 +75,9 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
         T = inp["c"].shape[2]
         sess.set_ctx_tokens(T)
         # ---- staging buffers of the caller (inputs / outputs in the reference's NCL layout) ----
-        st = dict(in_x=inp["x_T"].to(dev).contiguous(), in_c=inp["c"].to(dev).contiguous(), in_uc=inp["uc"].to(dev).contiguous(),
+        seeded = None if seeds is None else seeding.ChartNoise(seeds, (B, Cz, Lz), dev)
+        x_T = inp["x_T"] if seeded is None else seeded.draw(seeding.X_T, 0)
+        st = dict(in_x=x_T.to(dev).contiguous(), in_c=inp["c"].to(dev).contiguous(), in_uc=inp["uc"].to(dev).contiguous(),
                   pred=torch.zeros(B * Lz * Cz, device=dev), out_z=torch.zeros(B, Cz, Lz, device=dev),
                   out_logits=torch.zeros(B, cfg.decoder.x_channels, dec.Lout, device=dev))
         w4 = [w.to(dev).contiguous() for w in list(inp["w"])[-cfg.unet.levels:]]
@@ -83,7 +96,14 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
             st["in_qnoise"] = torch.empty((total,) + shape, device=dev)
             qcoef = q_coef_table(model, ts)
             qcoef.tofile(os.path.join(out_dir, "stage_coef.bin"))
-        draw_step_noise(total, shape, st.get("in_x0"), st.get("in_qnoise"), has_noise, st.get("in_noise"), noise_dropout, dev)
+        # step i reads the DDIM coefficient row total - 1 - i, so a seeded table walks the draws downwards from total - 1
+        randn_rows = {} if seeded is None else dict(seeded=seeded, first_draw=total - 1, draw_stride=-1)
+        draw_step_noise(total, shape, st.get("in_x0"), st.get("in_qnoise"), has_noise, st.get("in_noise"), noise_dropout, dev,
+                        **randn_rows)
+        # what a seeded bundle draws on the host instead of loading: region -> (purpose, first_draw, n_draws, draw_stride)
+        drawn = {} if seeded is None else {"in_x": (seeding.X_T, 0, 1, 1)}
+        if seeded is not None:
+            drawn.update({k: (p, total - 1, total, -1) for k, p in (("in_noise", seeding.STEP), ("in_qnoise", seeding.Q)) if k in st})
         # per-request host tables for this S
         sess.set_timestep_table(ts.copy())
         sess.set_ddim_schedule(sampler.ddim_alphas, sampler.ddim_alphas_prev, sampler.ddim_sigmas, sampler.ddim_sqrt_one_minus_alphas)
@@ -130,11 +150,16 @@ def export_bundle(model, inp: Dict[str, torch.Tensor], S: int, scale: float, out
         for n in names:
             t = tensors[n]
             nbytes = t.numel() * t.element_size()
-            if n in contents or n in inputs:
+            if (n in contents or n in inputs) and n not in drawn:
                 t.detach().cpu().contiguous().numpy().tofile(os.path.join(out_dir, n + ".bin"))
                 lines.append(f"region {n} {nbytes} file {n}.bin")
             else:
                 lines.append(f"region {n} {nbytes} zero -")
+        if seeded is not None:
+            seeding.seed_array(seeds).tofile(os.path.join(out_dir, "seeds.bin"))
+            lines.append(f"seeds seeds.bin {B}")
+            for n, (purpose, first, count, stride) in drawn.items():
+                lines.append(f"randn {n} {purpose} {first} {count} {stride} {B} {Cz * Lz}")
         for name, ops, mode in seq:
             path = os.path.join(out_dir, name + ".plan")
             if ops is None:
@@ -190,12 +215,17 @@ def main():
     ap.add_argument("--noise-dropout", type=float, default=0.0)
     ap.add_argument("--inpaint", action="store_true", help="keep the first half of a synthetic chart latent, regenerate the rest")
     ap.add_argument("--seed", type=int, default=0, help="torch CUDA generator seed of the staged random numbers")
+    ap.add_argument("--seeds", default=None, help="per-chart seeds, e.g. 7,8 (or one int s for charts s, s + 1, ...): the bundle "
+                                                  "draws x_T and its noise tables with mugd_randn instead of carrying them")
     a = ap.parse_args()
+    seeds = None if a.seeds is None else [int(v) for v in a.seeds.split(",")]
+    if seeds is not None and len(seeds) == 1:
+        seeds = seeds[0]
     model = MugDiffusionB200.from_state_dict(synth.synthetic_state_dict(a.L), z_length=a.L)
     inp = synth.synthetic_inputs(a.B, a.L)
     torch.cuda.manual_seed(a.seed)
     res = export_bundle(model, inp, a.S, a.scale, a.out, eta=a.eta, temperature=a.temperature, noise_dropout=a.noise_dropout,
-                        inpaint=synth.synthetic_inpainting(a.B, a.L) if a.inpaint else None)
+                        inpaint=synth.synthetic_inpainting(a.B, a.L) if a.inpaint else None, seeds=seeds)
     print("bundle written to", a.out, "| z", tuple(res["z"].shape), "logits", tuple(res["logits"].shape))
 
 

@@ -151,6 +151,11 @@ class Join(C.Structure):
                 ("B", C.c_int32), ("C", C.c_int32), ("L", C.c_int32), ("reserved_", C.c_int32)]
 
 
+class Normal(C.Structure):
+    _fields_ = [("out", _f), ("seeds", _f), ("n", C.c_int64), ("B", C.c_int32), ("purpose", C.c_int32), ("first_draw", C.c_int32),
+                ("n_draws", C.c_int32), ("draw_stride", C.c_int32), ("reserved_", C.c_int32)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", Gemm), ("gn", GroupNorm), ("ln", LayerNorm), ("attn", Attention), ("s4", S4Conv),
                 ("ddim", DdimUpdate), ("tr", Transpose), ("cp", Copy2D), ("adv", StepAdvance), ("notes", Notes), ("embed", Embed),
@@ -250,6 +255,7 @@ def load() -> C.CDLL:
     lib.mugd_sample_unipc_stop.argtypes = [C.c_void_p, C.POINTER(UnipcStop), C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_unipc_stop_update.argtypes = [C.POINTER(UnipcStop), C.c_void_p]
     lib.mugd_stochastic_encode.argtypes = [C.POINTER(QEncode), C.c_void_p]
+    lib.mugd_randn.argtypes = [C.POINTER(Normal), C.c_void_p]
     lib.mugd_sample_join.argtypes = [C.c_void_p, C.POINTER(Join), C.POINTER(Op), C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.mugd_plan_save.argtypes = [C.c_void_p, C.POINTER(Region), C.c_int32, C.c_char_p]
     lib.mugd_plan_load.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(Region), C.c_int32, C.POINTER(C.c_void_p)]
@@ -292,5 +298,5 @@ EXPORTED_SYMBOLS = [
     "mugd_sample_dpm", "mugd_dpm_update", "mugd_sample_dpm_ex", "mugd_dpm_ex_update",
     "mugd_sample_dpm_stop", "mugd_dpm_stop_update",
     "mugd_sample_unipc", "mugd_unipc_update", "mugd_sample_unipc_ex", "mugd_unipc_ex_update",
-    "mugd_sample_unipc_stop", "mugd_unipc_stop_update",
+    "mugd_sample_unipc_stop", "mugd_unipc_stop_update", "mugd_randn",
 ]

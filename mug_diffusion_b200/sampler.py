@@ -22,7 +22,7 @@ from typing import Dict, Optional, Sequence
 import numpy as np
 import torch
 
-from . import dpm_solver, unipc
+from . import dpm_solver, seeding, unipc
 from . import lib as L_
 from .config import DecoderConfig, EncoderConfig, ModelConfig, UNetConfig
 from .engine import MAX_STEPS, OpList, View
@@ -103,10 +103,19 @@ STAGE_TABLE_BYTES = 64 << 20
 
 
 def draw_step_noise(steps: int, shape, x0: Optional[torch.Tensor], q_table: Optional[torch.Tensor], draw_noise: bool,
-                    noise_table: Optional[torch.Tensor], noise_dropout: float, device):
+                    noise_table: Optional[torch.Tensor], noise_dropout: float, device, seeded: Optional[seeding.ChartNoise] = None,
+                    first_draw: int = 0, draw_stride: int = 1):
     """The random numbers of ``steps`` DDIM steps, drawn in the per-step loop's order from the device's default generator: per step
     q_sample's randn_like(x0) into q_table[k] (when q_table is given, ddim.py:142), then randn(shape) [+ dropout] (when draw_noise,
-    ddim.py:192-194) into noise_table[k], or discarded when noise_table is None.  Same values, same generator state afterwards."""
+    ddim.py:192-194) into noise_table[k], or discarded when noise_table is None.  Same values, same generator state afterwards.
+    A seeded request (``seeded``) fills each given table with one mugd_randn launch instead, row k from draw first_draw +
+    draw_stride * k of the schedule (seeding.Q for q_table, seeding.STEP for noise_table), and leaves the generator untouched."""
+    if seeded is not None:
+        if q_table is not None:
+            seeded.fill(q_table, seeding.Q, first_draw, steps, draw_stride)
+        if draw_noise and noise_table is not None:
+            seeded.fill(noise_table, seeding.STEP, first_draw, steps, draw_stride)
+        return
     for k in range(steps):
         if q_table is not None:
             q_table[k].copy_(torch.randn_like(x0))
@@ -116,6 +125,12 @@ def draw_step_noise(steps: int, shape, x0: Optional[torch.Tensor], q_table: Opti
                 nz = torch.nn.functional.dropout(nz, p=noise_dropout)
             if noise_table is not None:
                 noise_table[k].copy_(nz)
+
+
+def _seeded_rows(seeded: Optional[seeding.ChartNoise], first_draw: int, draw_stride: int = 1) -> dict:
+    """draw_step_noise's keyword arguments for a table whose row k is draw first_draw + draw_stride * k of a seeded request; none for
+    a request without seeds"""
+    return {} if seeded is None else dict(seeded=seeded, first_draw=first_draw, draw_stride=draw_stride)
 
 
 def q_coef_table(model, time_range: np.ndarray) -> np.ndarray:
@@ -395,6 +410,18 @@ class MugDiffusionB200:
                           parameterization=parameterization)
         return sd_all, cfg
 
+    @torch.no_grad()
+    def chart_noise(self, seeds, shape=None) -> torch.Tensor:
+        """The x_T a seeded request starts from: chart b's seeding.X_T draw with seed s_b (``seeds``: an int s for charts s, s + 1,
+        ..., or one per chart).  ``shape``: the request's [B, C, L] or (C, L), default (z_channels, z_length); an int seed without a
+        batch size in ``shape`` gives one chart.  ValueError for malformed seeds."""
+        if shape is not None and len(shape) == 3:
+            B, Cz, Lz = (int(v) for v in shape)
+        else:
+            Cz, Lz = (self.z_channels, self.z_length) if shape is None else (int(v) for v in shape)
+            B = 1 if isinstance(seeds, (int, np.integer)) else len(seeds)
+        return seeding.ChartNoise(seeding.chart_seeds(seeds, B), (B, Cz, Lz), self.device).draw(seeding.X_T, 0)
+
     # the reference's q_sample, used only by the inpainting (mask) branch of ddim_sampling (ddim.py:141-144)
     def q_sample(self, x_start, t, noise=None):
         noise = torch.randn_like(x_start) if noise is None else noise
@@ -445,6 +472,15 @@ class _DeviceLoopSampler:
     def _x_T(self, shape, x_T):
         """the request's start latent: x_T on the device, or drawn from its generator when not given"""
         return torch.randn(shape, device=self.device) if x_T is None else x_T.to(self.device, torch.float32)
+
+    def _seeded(self, seeds, shape) -> Optional[seeding.ChartNoise]:
+        """the request's ChartNoise (its seeds on the device), None when it is not seeded"""
+        return None if seeds is None else seeding.ChartNoise(seeding.chart_seeds(seeds, shape[0]), shape, self.device)
+
+    def _seeded_start(self, seeds, shape, x_T):
+        """(ChartNoise or None, x_T): a seeded request without x_T starts from its charts' seeding.X_T draw"""
+        seeded = self._seeded(seeds, shape)
+        return seeded, (seeded.draw(seeding.X_T, 0) if seeded is not None and x_T is None else x_T)
 
     def _load_session(self, w, c, shape, x_T, scale, uc, time_range):
         """x_T (drawn when not given), whether classifier-free guidance is on, and the session of this shape with the timestep table
@@ -527,9 +563,10 @@ class _DeviceLoopSampler:
         self.last_launches_per_step = sess.plan.launches + tail_launches
         return self._read_x(sess, shape), intermediates
 
-    def _stochastic_encode(self, x0, noise, indices, tables, n):
+    def _stochastic_encode(self, x0, noise, indices, tables, n, seeds=None):
         """``stochastic_encode``'s kernel: out[b] = sqrt_a[t[b]] * x0[b] + sqrt_1ma[t[b]] * noise[b] (noise = randn_like(x0) when not
-        given), t = ``indices(B)`` (which checks them), (sqrt_a, sqrt_1ma) = ``tables()`` of n rows.  ValueError before any GPU work."""
+        given, chart b's seeding.ENCODE draw 0 with ``seeds``), t = ``indices(B)`` (which checks them), (sqrt_a, sqrt_1ma) =
+        ``tables()`` of n rows.  ValueError before any GPU work."""
         dev = self.device
         if not isinstance(x0, torch.Tensor) or x0.dim() != 3 or x0.dtype != torch.float32 or x0.device != torch.device(dev):
             raise ValueError(f"x0 must be a float32 [B, C, L] tensor on {dev}")
@@ -537,7 +574,12 @@ class _DeviceLoopSampler:
         if noise is not None and (not isinstance(noise, torch.Tensor) or noise.shape != x0.shape or noise.dtype != torch.float32
                                   or noise.device != x0.device):
             raise ValueError(f"noise must be a float32 tensor of x0's shape {tuple(x0.shape)} on {dev}")
-        if noise is None:
+        if seeds is not None:
+            if noise is not None:
+                raise ValueError("give the noise or the seeds, not both")
+            seeds = seeding.chart_seeds(seeds, x0.shape[0])
+            noise = self._seeded(seeds, x0.shape).draw(seeding.ENCODE, 0) if x0.numel() else torch.empty_like(x0)
+        elif noise is None:
             noise = torch.randn_like(x0)
         out = torch.empty(x0.shape, device=dev)
         if out.numel() == 0:
@@ -673,6 +715,18 @@ def _refuse_ddim_only(kwargs: dict, sampler: str, why: str, method: str = "sampl
         raise TypeError(f"{sampler}.{method} got unexpected arguments {sorted(kwargs)}")
 
 
+def _request_seeds(seeds, B: int, noise_dropout=0., match_reference_rng=False) -> Optional[list]:
+    """the checked per-chart seeds of a request of B charts (seeding.chart_seeds), None when it is not seeded.  ValueError for
+    malformed seeds, and for noise_dropout > 0 or match_reference_rng=True together with seeds."""
+    if seeds is None:
+        return None
+    if noise_dropout > 0.:
+        raise ValueError(f"noise_dropout={noise_dropout!r}: a seeded request draws no dropout mask; give seeds or noise_dropout")
+    if match_reference_rng:
+        raise ValueError("match_reference_rng=True consumes torch's generator, which a seeded request leaves untouched")
+    return seeding.chart_seeds(seeds, B)
+
+
 def _conditioning(c, conditioning):
     """``c``, which may also be given as the reference's ``conditioning``"""
     if conditioning is None:
@@ -725,7 +779,7 @@ class DDIMSampler(_DeviceLoopSampler):
     @torch.no_grad()
     def sample(self, S, c, w, batch_size, shape=None, callback=None, img_callback=None, eta=0., mask=None, x0=None,
                temperature=1., noise_dropout=0., verbose=True, x_T=None, log_every_t=100,
-               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, **kwargs):
+               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, seeds=None, **kwargs):
         if c is not None and not isinstance(c, dict) and c.shape[0] != batch_size:
             print(f"Warning: Got {c.shape[0]} conditionings but batch-size is {batch_size}")
         self.make_schedule(ddim_num_steps=S, ddim_eta=eta, verbose=verbose)
@@ -739,7 +793,7 @@ class DDIMSampler(_DeviceLoopSampler):
                                   noise_dropout=noise_dropout, temperature=temperature, x_T=x_T, log_every_t=log_every_t,
                                   unconditional_guidance_scale=unconditional_guidance_scale,
                                   unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class,
-                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)))
+                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)), seeds=seeds)
 
     def _schedule_subset(self, timesteps, ddim_use_original_steps) -> np.ndarray:
         """the DDIM timesteps a request runs: all of make_schedule's, or ddim_timesteps[:ddim_subset_end(k, n)] for timesteps=k
@@ -771,22 +825,27 @@ class DDIMSampler(_DeviceLoopSampler):
     @torch.no_grad()
     def ddim_sampling(self, w, c, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None, mask=None, x0=None,
                       img_callback=None, log_every_t=100, temperature=1., noise_dropout=0., unconditional_guidance_scale=1.,
-                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False):
+                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False, seeds=None):
         """ddim.py:110-159 on the GPU.  ``timesteps=k`` runs the reference's truncated schedule, the last, low-noise
         ddim_timesteps[:ddim_subset_end(k, n)] from x_T; when that is empty, x_T comes back with both intermediate lists [x_T].
-        ``ddim_use_original_steps=True`` raises ValueError before any GPU work (see ORIGINAL_STEPS)."""
+        ``ddim_use_original_steps=True`` raises ValueError before any GPU work (see ORIGINAL_STEPS).
+        ``seeds`` (seeding.chart_seeds: an int s for charts s, s + 1, ..., or one per chart): every random number comes from the
+        charts' seeds, x_T (unless given), the step noise and the inpainting noise of schedule row r from draw r, and torch's
+        generator is left untouched; noise_dropout and match_reference_rng are refused with it."""
+        B, Cz, Lz = shape
+        seeds = _request_seeds(seeds, B, noise_dropout, match_reference_rng)
         model = self.model
         eng = model.engine
         dev = self.device
-        B, Cz, Lz = shape
         ts = self._schedule_subset(timesteps, ddim_use_original_steps)
         if ts.shape[0] == 0:
-            return self._empty_request(shape, x_T)
+            return self._empty_request(shape, self._seeded_start(seeds, shape, x_T)[1])
         # the reference draws (and, with noise_dropout, masks) noise every step even when sigma == 0 (ddim.py:192-194); the
         # draw is skipped here unless it can change the result or the caller asks for the same global-RNG consumption
         has_noise = bool(np.any(np.asarray(self.ddim_sigmas) != 0))
         blend, draw = mask is not None, has_noise or bool(match_reference_rng)
         with eng.lock:
+            seeded, x_T = self._seeded_start(seeds, shape, x_T)
             x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, unconditional_guidance_scale, unconditional_conditioning,
                                                              ts)
             total = time_range.shape[0]
@@ -815,8 +874,10 @@ class DDIMSampler(_DeviceLoopSampler):
                     stage.noise = _ptr(n_tab)
 
             def launch(first, n):
+                # step i reads the DDIM coefficient row total - 1 - i: the seeded draws walk the rows downwards
                 if blend or draw:
-                    draw_step_noise(n, shape, x0, q_tab, draw, n_tab, noise_dropout, dev)
+                    draw_step_noise(n, shape, x0, q_tab, draw, n_tab, noise_dropout, dev,
+                                    **_seeded_rows(seeded, total - 1 - first, -1))
                 if stage is None:
                     sess.plan.launch(n, tail)
                 else:
@@ -828,9 +889,15 @@ class DDIMSampler(_DeviceLoopSampler):
                 if blend:
                     assert x0 is not None
                     tsb = torch.full((B,), int(t), device=dev, dtype=torch.long)
-                    x_orig = model.q_sample(x0.to(dev), tsb)
+                    x0d = x0.to(dev)
+                    if seeded is None:
+                        x_orig = model.q_sample(x0d, tsb)
+                    else:
+                        x_orig = model.q_sample(x0d, tsb, seeded.draw(seeding.Q, total - 1 - i))
                     sess.load_x(x_orig * mask + (1. - mask) * self._read_x(sess, shape), dup=cfg_on)
-                if draw:
+                if draw and seeded is not None:
+                    nz = seeded.draw(seeding.STEP, total - 1 - i)
+                elif draw:
                     nz = torch.randn(shape, device=dev)                          # ddim.py:192
                     if noise_dropout > 0.:
                         # dropout(sigma * n * T) == sigma * T * dropout(n): same Bernoulli draw, same 1/(1-p) scale (:193-194)
@@ -850,10 +917,11 @@ class DDIMSampler(_DeviceLoopSampler):
             raise ValueError(f"{what} needs the DDIM schedule: call make_schedule(S) first")
 
     @torch.no_grad()
-    def stochastic_encode(self, x0, t, use_original_steps=False, noise=None):
+    def stochastic_encode(self, x0, t, use_original_steps=False, noise=None, seeds=None):
         """Noise the latent ``x0`` [B, C, L] to DDIM index ``t[b]`` per chart: sqrt(ddim_alphas)[t] * x0 + ddim_sqrt_one_minus_alphas[t]
         * noise (Stable Diffusion's formulation), with noise = torch.randn_like(x0) when not given (the generator ends where randn_like
-        leaves it).  ``t``: a [B] integer tensor (or sequence) of indices into make_schedule's tables; ``use_original_steps=True``
+        leaves it), or chart b's seeding.ENCODE draw with ``seeds`` (one int for charts s, s + 1, ..., or one per chart).  ``t``: a [B]
+        integer tensor (or sequence) of indices into make_schedule's tables; ``use_original_steps=True``
         indexes the model's sqrt_alphas_cumprod / sqrt_one_minus_alphas_cumprod instead.  One kernel, bit-identical to those torch
         expressions on CUDA (the square root is torch's).  ValueError, before any GPU work, for malformed arguments and indices
         outside the table."""
@@ -878,7 +946,7 @@ class DDIMSampler(_DeviceLoopSampler):
             return (torch.sqrt(torch.as_tensor(self.ddim_alphas).to(dev, torch.float32)),
                     torch.as_tensor(self.ddim_sqrt_one_minus_alphas).to(dev, torch.float32))
 
-        return self._stochastic_encode(x0, noise, indices, tables, n)
+        return self._stochastic_encode(x0, noise, indices, tables, n, seeds)
 
     def _decode_starts(self, x_latent, t_start):
         """the per-chart start indices of a decode request; ValueError for malformed ones"""
@@ -1005,13 +1073,14 @@ class PLMSSampler(DDIMSampler):
     @torch.no_grad()
     def sample(self, S, c=None, w=None, batch_size=None, shape=None, callback=None, img_callback=None, eta=0., mask=None, x0=None,
                temperature=1., noise_dropout=0., verbose=True, x_T=None, log_every_t=100, unconditional_guidance_scale=1.,
-               unconditional_conditioning=None, tqdm_class=None, conditioning=None, **kwargs):
+               unconditional_conditioning=None, tqdm_class=None, conditioning=None, seeds=None, **kwargs):
         """The call scripts/mapping.py:476-483 makes (``c`` may also be given as the reference's ``conditioning``).  Returns
         ``(samples, {'x_inter', 'pred_x0'})`` with plms.py:134,166-168's logging rule.  Every argument is checked before any GPU
         work.  Requests without callback / img_callback / mask run from mugd_sample_plms calls, one per stretch between two recorded
         intermediates; the others run the steps one by one.  ``match_reference_rng=True``: the CUDA generator consumes what the
         reference's discarded step noise consumes (randn(shape) [+ dropout], twice at step 0 and once per later step; for B > 1 the
-        reference's noise_like receives a [B, B, C, L] shape from its [b, 1, 1, 1] coefficients, this draws [B, C, L])."""
+        reference's noise_like receives a [B, B, C, L] shape from its [b, 1, 1, 1] coefficients, this draws [B, C, L]).
+        ``seeds``: x_T (unless given) and the inpainting noise come from the charts' seeds, as in DDIMSampler.ddim_sampling."""
         if eta != 0:
             raise ValueError('ddim_eta must be 0 for PLMS')
         c = _conditioning(c, conditioning)
@@ -1024,7 +1093,7 @@ class PLMSSampler(DDIMSampler):
                                   log_every_t=log_every_t, noise_dropout=noise_dropout,
                                   unconditional_guidance_scale=unconditional_guidance_scale,
                                   unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class,
-                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)))
+                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)), seeds=seeds)
 
     def _check_request(self, S, c, w, batch_size, shape, x_T, mask, x0, scale, uc, log_every_t):
         """the request's [B, C, L] shape; ValueError / TypeError for what the device path cannot take"""
@@ -1041,16 +1110,17 @@ class PLMSSampler(DDIMSampler):
     @torch.no_grad()
     def plms_sampling(self, w, c, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None, mask=None, x0=None,
                       img_callback=None, log_every_t=100, noise_dropout=0., unconditional_guidance_scale=1.,
-                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False):
+                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False, seeds=None):
         """plms.py:115-170 (and p_sample_plms, :172-236) on the GPU.  ``timesteps=k`` runs the truncated schedule of plms.py:128-136
         (t_next and the warm-up follow it); ``ddim_use_original_steps=True`` raises as in ddim_sampling."""
+        B, Cz, Lz = shape
+        seeds = _request_seeds(seeds, B, noise_dropout, match_reference_rng)
         model = self.model
         eng = model.engine
         dev = self.device
-        B, Cz, Lz = shape
         ts = self._schedule_subset(timesteps, ddim_use_original_steps)
         if ts.shape[0] == 0:
-            return self._empty_request(shape, x_T)
+            return self._empty_request(shape, self._seeded_start(seeds, shape, x_T)[1])
         match_rng = bool(match_reference_rng)
         scale = unconditional_guidance_scale
 
@@ -1060,6 +1130,7 @@ class PLMSSampler(DDIMSampler):
                 draw_step_noise(k, shape, None, None, True, None, noise_dropout, dev)
 
         with eng.lock:
+            seeded, x_T = self._seeded_start(seeds, shape, x_T)
             x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, scale, unconditional_conditioning, ts)
             total = time_range.shape[0]
             pred = torch.empty(B * Lz, Cz, device=dev)
@@ -1081,7 +1152,11 @@ class PLMSSampler(DDIMSampler):
                 if mask is not None:
                     assert x0 is not None
                     tsb = torch.full((B,), int(t), device=dev, dtype=torch.long)
-                    x_orig = model.q_sample(x0.to(dev), tsb)                    # plms.py:147-150
+                    x0d = x0.to(dev)                                           # plms.py:147-150
+                    if seeded is None:
+                        x_orig = model.q_sample(x0d, tsb)
+                    else:
+                        x_orig = model.q_sample(x0d, tsb, seeded.draw(seeding.Q, total - 1 - i))
                     sess.load_x(x_orig * mask + (1. - mask) * self._read_x(sess, shape), dup=cfg_on)
                 sess.eval(graph=True)
                 L_.check(eng.lib.mugd_plms_combine(C.byref(plms), i, 0, stream), "mugd_plms_combine")
@@ -1113,14 +1188,15 @@ class DDPMSampler(_DeviceLoopSampler):
 
     @torch.no_grad()
     def sample(self, c, w, batch_size, shape=None, x_T=None, callback=None, img_callback=None, log_every_t=100, clip_denoised=None,
-               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True, **kwargs):
+               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True, seeds=None, **kwargs):
         """``T = model.num_timesteps`` ancestral steps for ``batch_size`` latents of ``shape`` = (channels, length) (default the
         model's).  ``clip_denoised=None`` takes the model's.  Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then the x and
         x_recon of every step whose timestep i has ``i % log_every_t == 0 or i == T - 1`` (diffusion.py:279).  Every argument is
         checked before any GPU work; ``S`` (if given) must be T, and inpainting, eta, temperature and noise dropout are refused.
         Without callbacks the steps run from mugd_sample_ddpm calls (each call's noise table at most STAGE_TABLE_BYTES), with them
         one by one.  Both draw one randn(shape) per step from the device's generator (and x_T first when it is not given), as the
-        reference does."""
+        reference does; with ``seeds`` (seeding.chart_seeds) the noise of timestep t is the charts' seeding.STEP draw t instead, one
+        mugd_randn launch per noise table, and the generator is left untouched."""
         T = self.ddpm_num_timesteps
         S = kwargs.pop("S", None)
         if S is not None and (isinstance(S, bool) or S != T):
@@ -1133,16 +1209,17 @@ class DDPMSampler(_DeviceLoopSampler):
             raise ValueError(f"clip_denoised={clip_denoised!r} must be True, False or None")
         scale = _finite_scale(unconditional_guidance_scale)
         size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
+        seeds = _request_seeds(seeds, size[0])
         if verbose:
             print(f'Data shape for DDPM sampling is {size}, {T} steps')
         return self.ddpm_sampling(w, c, size, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
                                   clip_denoised=bool(clip), unconditional_guidance_scale=scale,
-                                  unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class)
+                                  unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class, seeds=seeds)
 
     @torch.no_grad()
     def ddpm_sampling(self, w, c, shape, x_T=None, callback=None, img_callback=None, log_every_t=100, clip_denoised=True,
-                      unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True):
-        """diffusion.py:234-282 on the GPU."""
+                      unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, seeds=None):
+        """diffusion.py:234-282 on the GPU; ``seeds``: checked per-chart seeds (step i draws timestep T - 1 - i)."""
         model = self.model
         eng = model.engine
         dev = self.device
@@ -1150,6 +1227,7 @@ class DDPMSampler(_DeviceLoopSampler):
         T = self.ddpm_num_timesteps
         scale = unconditional_guidance_scale
         with eng.lock:
+            seeded, x_T = self._seeded_start(seeds, shape, x_T)
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, np.arange(T)[::-1])
             coef = model.ddpm_coef_table()
             pred = torch.empty(B * Lz, Cz, device=dev)
@@ -1159,7 +1237,7 @@ class DDPMSampler(_DeviceLoopSampler):
 
             def launch(first, n):
                 # the noise of a call is drawn up front, in the per-step loop's order
-                draw_step_noise(n, shape, None, None, True, table, 0., dev)
+                draw_step_noise(n, shape, None, None, True, table, 0., dev, **_seeded_rows(seeded, T - 1 - first, -1))
                 sess.plan.launch_ddpm(ddpm, first, n)
 
             # the per-step loop runs the same kernel: the referee of the device loop
@@ -1168,7 +1246,7 @@ class DDPMSampler(_DeviceLoopSampler):
 
             def step(i, t):
                 sess.eval(graph=True)
-                draw_step_noise(1, shape, None, None, True, table, 0., dev)       # noise_like, diffusion.py:274
+                draw_step_noise(1, shape, None, None, True, table, 0., dev, **_seeded_rows(seeded, int(t)))  # noise_like, :274
                 L_.check(eng.lib.mugd_ddpm_update(C.byref(ddpm), stream), "mugd_ddpm_update")
                 eng.run_ops(advance)
 
@@ -1225,26 +1303,28 @@ class DPMSolverSampler(_DeviceLoopSampler):
     def sample(self, S, c=None, w=None, batch_size=None, shape=None, x_T=None, order=2, skip_type="time_uniform",
                solver_type="dpmsolver", lower_order_final=True, callback=None, img_callback=None, log_every_t=100,
                unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True, conditioning=None,
-               **kwargs):
+               seeds=None, **kwargs):
         """S steps of DPM-Solver++ multistep of ``order`` from x_T (drawn when not given) to t = 1/N; ``c`` may also be given as
         ``conditioning``.  Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then x and the data prediction m of every step i with
         ``(S - i - 1) % log_every_t == 0`` or i = 0 (DDIM's rule).  Every argument is checked before any GPU work (ValueError; TypeError
         for missing or unknown ones); inpainting (mask / x0: see ``inpaint``), eta, temperature and noise dropout are refused.  Without
-        callbacks the steps run from mugd_sample_dpm calls, with them one by one through mugd_dpm_update."""
+        callbacks the steps run from mugd_sample_dpm calls, with them one by one through mugd_dpm_update.  ``seeds``
+        (seeding.chart_seeds): x_T, when not given, is the charts' seeding.X_T draw."""
         _refuse_ddim_only(kwargs, "DPMSolverSampler", "DPM-Solver++ multistep is a deterministic solver without {}")
         c = _conditioning(c, conditioning)
         scale, sched, size = self._check_request(S, c, w, batch_size, shape, x_T, None, None, order, skip_type, solver_type,
                                                  lower_order_final, log_every_t, unconditional_guidance_scale, unconditional_conditioning)
+        seeds = _request_seeds(seeds, size[0])
         if verbose:
             print(f'Data shape for DPM-Solver++ sampling is {size}, {S} steps of order {order} ({skip_type}, {solver_type})')
         return self.dpm_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
                                  unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
-                                 tqdm_class=tqdm_class)
+                                 tqdm_class=tqdm_class, seeds=seeds)
 
     @torch.no_grad()
     def inpaint(self, S, c=None, w=None, batch_size=None, mask=None, x0=None, shape=None, x_T=None, order=2, skip_type="time_uniform", solver_type="dpmsolver",
                 lower_order_final=True, callback=None, img_callback=None, log_every_t=100, unconditional_guidance_scale=1.,
-                unconditional_conditioning=None, tqdm_class=None, verbose=True, conditioning=None):
+                unconditional_conditioning=None, tqdm_class=None, verbose=True, conditioning=None, seeds=None):
         """Regenerate the part of the chart ``x0`` [B, C, L] where ``mask`` (broadcast to [B, C, L]) is 0, keeping the rest: ``sample``
         in which, before the evaluation of step i, x <- (alpha_i * x0 + sigma_i * eps_i) * mask + (1 - mask) * x with the schedule's
         alpha_i / sigma_i of t_i (DDIM inpainting's blend, ddim.py:140-144) and eps_i = randn_like(x0) drawn per step from the device's
@@ -1252,22 +1332,26 @@ class DPMSolverSampler(_DeviceLoopSampler):
         argument is checked before any GPU work (those of ``sample``; x0 of the request's shape, a mask that broadcasts to it).  Without
         callbacks, and with float32 mask / x0 on the model's device (``takes_device_loop``), the steps run from mugd_sample_dpm_ex calls
         with the blend staged in front of each step (the noise of a call drawn up front, at most STAGE_TABLE_BYTES per table); otherwise
-        one by one."""
+        one by one.  ``seeds`` (seeding.chart_seeds): x_T (unless given) and eps_i, the charts' seeding.Q draw i, come from the
+        charts' seeds, and torch's generator is left untouched."""
         c = _conditioning(c, conditioning)
         if not isinstance(mask, torch.Tensor) or not isinstance(x0, torch.Tensor):
             raise ValueError("inpainting needs the mask and x0 as tensors")
         scale, sched, size = self._check_request(S, c, w, batch_size, shape, x_T, mask, x0, order, skip_type, solver_type,
                                                  lower_order_final, log_every_t, unconditional_guidance_scale, unconditional_conditioning)
+        seeds = _request_seeds(seeds, size[0])
         if verbose:
             print(f'Data shape for DPM-Solver++ inpainting is {size}, {S} steps of order {order} ({skip_type}, {solver_type})')
         return self.dpm_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
                                  unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
-                                 tqdm_class=tqdm_class, mask=mask, x0=x0)
+                                 tqdm_class=tqdm_class, mask=mask, x0=x0, seeds=seeds)
 
     @torch.no_grad()
     def dpm_sampling(self, w, c, shape, sched: dpm_solver.DPMSchedule, x_T=None, callback=None, img_callback=None, log_every_t=100,
-                     unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, mask=None, x0=None):
-        """the request of ``sched`` (make_dpm_schedule) on the GPU; with ``mask`` / ``x0`` the inpainting of ``inpaint``"""
+                     unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, mask=None, x0=None,
+                     seeds=None):
+        """the request of ``sched`` (make_dpm_schedule) on the GPU; with ``mask`` / ``x0`` the inpainting of ``inpaint``; ``seeds``:
+        checked per-chart seeds"""
         model = self.model
         eng = model.engine
         dev = self.device
@@ -1277,6 +1361,7 @@ class DPMSolverSampler(_DeviceLoopSampler):
         blend = mask is not None
         self.last_schedule = sched
         with eng.lock:
+            seeded, x_T = self._seeded_start(seeds, shape, x_T)
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times)
             coef = torch.from_numpy(sched.rows_f32()).to(dev)
             ring = torch.empty(3, B * Lz * Cz, device=dev)                     # the data predictions of the last three steps
@@ -1301,7 +1386,7 @@ class DPMSolverSampler(_DeviceLoopSampler):
                 if stage is None:
                     sess.plan.launch_dpm(dpm, first, n)
                 else:
-                    draw_step_noise(n, shape, x0, q_tab, False, None, 0., dev)
+                    draw_step_noise(n, shape, x0, q_tab, False, None, 0., dev, **_seeded_rows(seeded, first))
                     stage.q_coef = qcoef[first:].ctypes.data
                     sess.plan.launch_dpm_ex(ex, first, n)
 
@@ -1313,7 +1398,8 @@ class DPMSolverSampler(_DeviceLoopSampler):
             def step(i, t):
                 if blend:
                     x0d = x0.to(dev)
-                    x_orig = q_dev[i, 0] * x0d + q_dev[i, 1] * torch.randn_like(x0d)
+                    eps = torch.randn_like(x0d) if seeded is None else seeded.draw(seeding.Q, i)
+                    x_orig = q_dev[i, 0] * x0d + q_dev[i, 1] * eps
                     sess.load_x(x_orig * mask + (1. - mask) * self._read_x(sess, shape), dup=cfg_on)
                 sess.eval(graph=True)
                 L_.check(eng.lib.mugd_dpm_update(C.byref(dpm), stream), "mugd_dpm_update")
@@ -1330,15 +1416,17 @@ class DPMSolverSampler(_DeviceLoopSampler):
             raise ValueError("sched must be a DPMSchedule from make_dpm_schedule")
 
     @torch.no_grad()
-    def stochastic_encode(self, x0, t_enc, sched: dpm_solver.DPMSchedule, noise=None):
+    def stochastic_encode(self, x0, t_enc, sched: dpm_solver.DPMSchedule, noise=None, seeds=None):
         """Noise the latent ``x0`` [B, C, L] for a remix over the last ``t_enc[b]`` steps of ``sched`` (an integer in [0, S], or one per
         chart): alpha(t_S-s) * x0 + sigma(t_S-s) * noise with s = t_enc[b], the marginal at the time where ``decode`` with t_start = s
         starts (no off-by-one, unlike DDIM's stochastic_encode / decode pair); s = 0 returns x0 exactly.  noise = torch.randn_like(x0)
-        when not given.  One kernel (mugd_stochastic_encode over the schedule's float32 tables of S + 1 rows).  ValueError, before any
+        when not given, chart b's seeding.ENCODE draw with ``seeds``.  One kernel (mugd_stochastic_encode over the schedule's float32
+        tables of S + 1 rows).  ValueError, before any
         GPU work, for malformed arguments."""
         self._require_schedule(sched)
         return self._stochastic_encode(x0, noise, lambda B: per_chart_steps(B, t_enc, sched.S, "t_enc", " (S = sched.S)"),
-                                       lambda: [torch.from_numpy(v).to(self.device) for v in sched.encode_tables_f32()], sched.S + 1)
+                                       lambda: [torch.from_numpy(v).to(self.device) for v in sched.encode_tables_f32()], sched.S + 1,
+                                       seeds)
 
     @torch.no_grad()
     def invert(self, x0, c, w, t_enc, sched: dpm_solver.DPMSchedule, unconditional_guidance_scale=1., unconditional_conditioning=None,
@@ -1442,13 +1530,13 @@ class UniPCSampler(_DeviceLoopSampler):
     def sample(self, S, c=None, w=None, batch_size=None, shape=None, x_T=None, order=2, skip_type="time_uniform", variant="bh2",
                lower_order_final=True, use_corrector=True, disable_corrector=(), t_grid=None, callback=None, img_callback=None,
                log_every_t=100, unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True,
-               conditioning=None, **kwargs):
+               conditioning=None, seeds=None, **kwargs):
         """S steps of UniPC of ``order`` from x_T (drawn when not given) to t = 1/N; ``c`` may also be given as ``conditioning``.
         Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then, after every iteration i with ``(S - i - 1) % log_every_t == 0`` or
         i = 0 (DDIM's rule), the latent the next evaluation sees (the predicted x~_i+1; the last one is z) and the data prediction m_i.
         Every argument is checked before any GPU work (ValueError; TypeError for missing or unknown ones); mask / x0, eta, temperature
         and noise dropout are refused.  Without callbacks the steps run from mugd_sample_unipc calls, with them one by one through
-        mugd_unipc_update."""
+        mugd_unipc_update.  ``seeds`` (seeding.chart_seeds): x_T, when not given, is the charts' seeding.X_T draw."""
         _refuse_ddim_only(kwargs, "UniPCSampler", "UniPC is a deterministic solver without {}")
         c = _conditioning(c, conditioning)
         if c is None or w is None:
@@ -1456,17 +1544,18 @@ class UniPCSampler(_DeviceLoopSampler):
         scale = _finite_scale(unconditional_guidance_scale)
         sched = self.make_unipc_schedule(S, order, skip_type, variant, lower_order_final, use_corrector, disable_corrector, t_grid)
         size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
+        seeds = _request_seeds(seeds, size[0])
         if verbose:
             print(f'Data shape for UniPC sampling is {size}, {S} steps of order {order} ({skip_type}, {variant})')
         return self.unipc_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
                                    unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
-                                   tqdm_class=tqdm_class)
+                                   tqdm_class=tqdm_class, seeds=seeds)
 
     @torch.no_grad()
     def inpaint(self, S, c=None, w=None, batch_size=None, mask=None, x0=None, shape=None, x_T=None, order=2, skip_type="time_uniform",
                 variant="bh2", lower_order_final=True, use_corrector=True, disable_corrector=(), t_grid=None, callback=None,
                 img_callback=None, log_every_t=100, unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None,
-                verbose=True, conditioning=None):
+                verbose=True, conditioning=None, seeds=None):
         """Regenerate the part of the chart ``x0`` [B, C, L] where ``mask`` (broadcast to [B, C, L]) is 0, keeping the rest: ``sample``
         in which, before the evaluation of iteration i, x~_i <- (alpha_i * x0 + sigma_i * eps_i) * mask + (1 - mask) * x~_i with the
         schedule's alpha_i / sigma_i of t_i and eps_i = randn_like(x0) drawn per step from the device's generator (the draw order of
@@ -1475,7 +1564,8 @@ class UniPCSampler(_DeviceLoopSampler):
         logged as by ``sample``.  Every argument is checked before any GPU work (those of ``sample``; x0 of the request's shape, a mask
         that broadcasts to it).  Without callbacks, and with float32 mask / x0 on the model's device (``takes_device_loop``), the
         steps run from mugd_sample_unipc_ex calls with the blend staged in front of each step (the noise of a call drawn up front, at
-        most STAGE_TABLE_BYTES per table); otherwise one by one."""
+        most STAGE_TABLE_BYTES per table); otherwise one by one.  ``seeds`` (seeding.chart_seeds): x_T (unless given) and eps_i, the
+        charts' seeding.Q draw i, come from the charts' seeds, and torch's generator is left untouched."""
         c = _conditioning(c, conditioning)
         if not isinstance(mask, torch.Tensor) or not isinstance(x0, torch.Tensor):
             raise ValueError("inpainting needs the mask and x0 as tensors")
@@ -1484,18 +1574,19 @@ class UniPCSampler(_DeviceLoopSampler):
         scale = _finite_scale(unconditional_guidance_scale)
         sched = self.make_unipc_schedule(S, order, skip_type, variant, lower_order_final, use_corrector, disable_corrector, t_grid)
         size = request_size(self.model, c, batch_size, shape, x_T, mask, x0, scale, unconditional_conditioning, log_every_t)
+        seeds = _request_seeds(seeds, size[0])
         if verbose:
             print(f'Data shape for UniPC inpainting is {size}, {S} steps of order {order} ({skip_type}, {variant})')
         return self.unipc_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
                                    unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
-                                   tqdm_class=tqdm_class, mask=mask, x0=x0)
+                                   tqdm_class=tqdm_class, mask=mask, x0=x0, seeds=seeds)
 
     @torch.no_grad()
     def unipc_sampling(self, w, c, shape, sched: unipc.UniPCSchedule, x_T=None, callback=None, img_callback=None, log_every_t=100,
                        unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, mask=None,
-                       x0=None):
-        """the request of ``sched`` (make_unipc_schedule) on the GPU, from checked arguments; with ``mask`` / ``x0`` the inpainting of
-        ``inpaint``"""
+                       x0=None, seeds=None):
+        """the request of ``sched`` (make_unipc_schedule) on the GPU, from checked arguments (``seeds``: per-chart seeds); with
+        ``mask`` / ``x0`` the inpainting of ``inpaint``"""
         model = self.model
         eng = model.engine
         dev = self.device
@@ -1505,6 +1596,7 @@ class UniPCSampler(_DeviceLoopSampler):
         blend = mask is not None
         self.last_schedule = sched
         with eng.lock:
+            seeded, x_T = self._seeded_start(seeds, shape, x_T)
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times)
             coef = torch.from_numpy(sched.rows_f32()).to(dev)
             corr = torch.from_numpy(sched.corr_rows_f32()).to(dev)
@@ -1531,7 +1623,7 @@ class UniPCSampler(_DeviceLoopSampler):
                 if stage is None:
                     sess.plan.launch_unipc(u, first, n)
                 else:
-                    draw_step_noise(n, shape, x0, q_tab, False, None, 0., dev)
+                    draw_step_noise(n, shape, x0, q_tab, False, None, 0., dev, **_seeded_rows(seeded, first))
                     stage.q_coef = qcoef[first:].ctypes.data
                     sess.plan.launch_unipc_ex(ex, first, n)
 
@@ -1543,7 +1635,8 @@ class UniPCSampler(_DeviceLoopSampler):
             def step(i, t):
                 if blend:
                     x0d = x0.to(dev)
-                    x_orig = q_dev[i, 0] * x0d + q_dev[i, 1] * torch.randn_like(x0d)
+                    eps = torch.randn_like(x0d) if seeded is None else seeded.draw(seeding.Q, i)
+                    x_orig = q_dev[i, 0] * x0d + q_dev[i, 1] * eps
                     sess.load_x(x_orig * mask + (1. - mask) * self._read_x(sess, shape), dup=cfg_on)
                 sess.eval(graph=True)
                 L_.check(eng.lib.mugd_unipc_update(C.byref(u), stream), "mugd_unipc_update")
@@ -1560,14 +1653,16 @@ class UniPCSampler(_DeviceLoopSampler):
             raise ValueError("sched must be a UniPCSchedule from make_unipc_schedule")
 
     @torch.no_grad()
-    def stochastic_encode(self, x0, t_enc, sched: unipc.UniPCSchedule, noise=None):
+    def stochastic_encode(self, x0, t_enc, sched: unipc.UniPCSchedule, noise=None, seeds=None):
         """Noise the latent ``x0`` [B, C, L] for a remix over the last ``t_enc[b]`` steps of ``sched`` (an integer in [0, S], or one per
         chart): alpha(t_S-s) * x0 + sigma(t_S-s) * noise with s = t_enc[b], the marginal at the time where ``decode`` with t_start = s
-        starts; s = 0 returns x0 exactly.  noise = torch.randn_like(x0) when not given.  DPMSolverSampler.stochastic_encode's kernel
+        starts; s = 0 returns x0 exactly.  noise = torch.randn_like(x0) when not given, chart b's seeding.ENCODE draw with ``seeds``.
+        DPMSolverSampler.stochastic_encode's kernel
         and contract.  ValueError, before any GPU work, for malformed arguments."""
         self._require_schedule(sched)
         return self._stochastic_encode(x0, noise, lambda B: per_chart_steps(B, t_enc, sched.S, "t_enc", " (S = sched.S)"),
-                                       lambda: [torch.from_numpy(v).to(self.device) for v in sched.encode_tables_f32()], sched.S + 1)
+                                       lambda: [torch.from_numpy(v).to(self.device) for v in sched.encode_tables_f32()], sched.S + 1,
+                                       seeds)
 
     @torch.no_grad()
     def decode(self, x_latent, c, w, t_start, sched: unipc.UniPCSchedule, unconditional_guidance_scale=1.,
