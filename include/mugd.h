@@ -54,7 +54,12 @@ enum mugd_op_kind {
     MUGD_OP_NOTES = 10,        /* decoder logits -> ordered note list (OsuManiaConvertor.array_to_objects)   */
     MUGD_OP_EMBED = 11,        /* prompt ids -> [B, H, F] embedding (BeatmapFeatureEmbedder.forward)         */
     MUGD_OP_TF32_SPLIT = 12,   /* weight preprocessing: w -> (hi in place, lo) for the 3xTF32 tensor-core GEMM */
-    MUGD_OP_POSTERIOR = 13     /* first-stage encoder moments -> mean / logvar / std / z (DiagonalGaussianDistribution)  */
+    MUGD_OP_POSTERIOR = 13,    /* first-stage encoder moments -> mean / logvar / std / z (DiagonalGaussianDistribution)  */
+    /* ragged batches (samples of different valid lengths padded to one L): each takes its base op's descriptor plus a device
+     * int32 `valid[B]` of rows per sample at the op's resolution, clamped to [0, L] by the kernel.  Rows l >= valid[b] are padding. */
+    MUGD_OP_GROUPNORM_VAR = 14,/* GroupNorm(+SiLU) over the valid rows only; padded rows are never read and are written as 0   */
+    MUGD_OP_ATTENTION_VAR = 15,/* self-attention with keys j < valid[b] only (rows past it never read); padded queries -> 0    */
+    MUGD_OP_ROW_MASK = 16      /* x[b*L + l][0..cols) = 0 for l >= valid[b] (a store, never a multiply)                        */
 };
 
 /* A-operand row addressing of MUGD_OP_GEMM (rows are tokens of B samples, Lout output rows each) */
@@ -204,6 +209,27 @@ typedef struct mugd_posterior {
     int32_t B, Z, L;
 } mugd_posterior;
 
+/* Ragged batches: the three op kinds below let one plan of B samples padded to L rows serve samples of different lengths.  The
+ * valid lengths are data (a device array the host rewrites between requests), so one captured graph serves any mix.  An op that
+ * mixes rows must keep padded rows out of valid ones: GroupNorm sums over valid rows only, self-attention bounds its keys, and a k = 3
+ * conv must find exact zeros in row valid[b] of its input (written by MUGD_OP_GROUPNORM_VAR or MUGD_OP_ROW_MASK).  Padded rows may
+ * hold anything, NaN included: no kernel here reads them into a valid result. */
+typedef struct mugd_groupnorm_var {
+    mugd_groupnorm gn;                     /* B, L (rows per sample, padded), C, G, ...                      */
+    const int32_t* valid;                  /* [B] device: valid rows of each sample                          */
+} mugd_groupnorm_var;
+
+typedef struct mugd_attention_var {
+    mugd_attention attn;                   /* self-attention: Lq == Lk                                       */
+    const int32_t* valid;                  /* [B] device: valid rows (queries and keys) of each sample       */
+} mugd_attention_var;
+
+typedef struct mugd_row_mask {
+    float* x; int64_t ld;                  /* [B*L, ld], columns 0 .. cols - 1 masked                        */
+    const int32_t* valid;                  /* [B] device                                                     */
+    int32_t B, L, cols, reserved_;
+} mugd_row_mask;
+
 typedef struct mugd_op {
     int32_t kind;
     int32_t tag;                           /* free for the host (profiling labels)                          */
@@ -211,6 +237,7 @@ typedef struct mugd_op {
         mugd_gemm gemm; mugd_groupnorm gn; mugd_layernorm ln; mugd_attention attn; mugd_s4conv s4;
         mugd_ddim_update ddim; mugd_transpose tr; mugd_copy2d cp; mugd_step_advance adv; mugd_notes notes;
         mugd_embed embed; mugd_tf32_split split; mugd_posterior post;
+        mugd_groupnorm_var gnv; mugd_attention_var attnv; mugd_row_mask mask;   /* ragged batches (same union size) */
     } u;
 } mugd_op;
 
@@ -652,7 +679,8 @@ int  mugd_debug_set_tc_timing(long long* device_buf);
 /* ---- utility ---------------------------------------------------------------------------------- */
 int  mugd_fill_i32(int32_t* dst, int32_t value, void* stream);
 /* sizeof() of {mugd_op, mugd_gemm, mugd_groupnorm, mugd_layernorm, mugd_attention, mugd_s4conv, mugd_ddim_update, mugd_transpose,
- * mugd_copy2d, mugd_notes, mugd_embed, mugd_tf32_split, mugd_posterior} so a foreign-language mirror can verify its layout */
+ * mugd_copy2d, mugd_notes, mugd_embed, mugd_tf32_split, mugd_posterior} so a foreign-language mirror can verify its layout; with
+ * n >= 16 also {mugd_groupnorm_var, mugd_attention_var, mugd_row_mask} in entries 13..15 (n >= 13 is enough for the first 13) */
 int  mugd_abi_sizes(int32_t* out, int32_t n);
 
 #ifdef __cplusplus

@@ -16,7 +16,7 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import List, Optional, Tuple, Union
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -209,3 +209,41 @@ class MelFrontEnd:
         self.write_rows(y, sess.mel, per * zl)
         hs = sess.run()
         return [None if h is None else h.expand(count, -1, -1) for h in hs], zl
+
+
+def pad_features(per_song_features: Sequence[Sequence[Optional[torch.Tensor]]]) -> Tuple[List[Optional[torch.Tensor]], List[int]]:
+    """One ragged batch from several songs: ``per_song_features[k]`` is the audio-encoder list of song k (``audio_features``'s first
+    result, or the wave encoder's 10-entry list), whose level-l maps are [b_k, C_l, L_k >> l] at the song's own z_length L_k.
+    Returns (w, z_lengths): w holds, per entry, the songs' maps concatenated along the batch and zero-padded to Lmax >> l
+    (Lmax = max L_k; entries that are None for every song stay None), and z_lengths one L_k per chart (b_k charts of song k), for
+    ``sample(..., shape=(C, Lmax), z_lengths=z_lengths)``.  ValueError for songs whose lists do not line up."""
+    songs = [list(f) for f in per_song_features]
+    if not songs:
+        raise ValueError("pad_features needs at least one song")
+    n = len(songs[0])
+    if any(len(f) != n for f in songs):
+        raise ValueError("every song's feature list must have the same number of entries")
+    used = [i for i in range(n) if any(f[i] is not None for f in songs)]
+    if not used or any(f[i] is None for f in songs for i in used):
+        raise ValueError("every song must carry the same feature entries")
+    top = max(used, key=lambda i: songs[0][i].shape[-1])      # the full-resolution entry: its length is the song's z_length
+    lens, counts = [], []
+    for f in songs:
+        b, Lk = int(f[top].shape[0]), int(f[top].shape[-1])
+        for i in used:
+            if f[i].dim() != 3 or f[i].shape[0] != b or Lk % f[i].shape[-1] or f[i].shape[1] != songs[0][i].shape[1]:
+                raise ValueError(f"entry {i}: shape {tuple(f[i].shape)} does not line up with the song's {tuple(f[top].shape)}")
+        lens.append(Lk)
+        counts.append(b)
+    Lmax = max(lens)
+    w: List[Optional[torch.Tensor]] = [None] * n
+    for i in used:
+        ds = lens[0] // int(songs[0][i].shape[-1])
+        ref = songs[0][i]
+        out = torch.zeros(sum(counts), int(ref.shape[1]), Lmax // ds, dtype=ref.dtype, device=ref.device)
+        row = 0
+        for f, b in zip(songs, counts):
+            out[row:row + b, :, :f[i].shape[-1]] = f[i]
+            row += b
+        w[i] = out
+    return w, [Lk for Lk, b in zip(lens, counts) for _ in range(b)]

@@ -56,6 +56,9 @@ static int dispatch(mugd_handle* h, const mugd_op& op, cudaStream_t st, int* lau
         case MUGD_OP_EMBED: return launch_embed(h->dev, op.u.embed, st, launches);
         case MUGD_OP_TF32_SPLIT: return launch_tf32_split(h->dev, op.u.split, st, launches);
         case MUGD_OP_POSTERIOR: return launch_posterior(h->dev, op.u.post, st, launches);
+        case MUGD_OP_GROUPNORM_VAR: return launch_groupnorm_var(h->dev, op.u.gnv, st, launches);
+        case MUGD_OP_ATTENTION_VAR: return launch_attention_var(h->dev, op.u.attnv, st, launches);
+        case MUGD_OP_ROW_MASK: return launch_row_mask(h->dev, op.u.mask, st, launches);
         default:
             set_error("unknown op kind %d", op.kind);
             return MUGD_ERR_INVALID;
@@ -428,6 +431,7 @@ int mugd_abi_sizes(int32_t* out, int32_t n) {
     out[6] = sizeof(mugd_ddim_update); out[7] = sizeof(mugd_transpose); out[8] = sizeof(mugd_copy2d);
     out[9] = sizeof(mugd_notes); out[10] = sizeof(mugd_embed); out[11] = sizeof(mugd_tf32_split);
     out[12] = sizeof(mugd_posterior);
+    if (n >= 16) { out[13] = sizeof(mugd_groupnorm_var); out[14] = sizeof(mugd_attention_var); out[15] = sizeof(mugd_row_mask); }
     return MUGD_OK;
 }
 

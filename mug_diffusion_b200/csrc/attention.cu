@@ -32,9 +32,12 @@ struct AttSmem {
     static constexpr int FLOATS = QT + KT + VS + PT;
 };
 
-template <int D>
+// Padded rows of a ragged batch (Desc = mugd_attention_var): keys j >= lk are neither read nor scored, query rows i >= lq are
+// written as zeros, and a CTA whose rows are all padding only writes its zeros.
+template <int D, typename Desc = mugd_attention>
 __global__ void __launch_bounds__(AT_THREADS)
-attention_kernel(const mugd_attention a) {
+attention_kernel(const Desc d) {
+    const mugd_attention& a = attn_desc(d);
     constexpr int DC = D / 16;                 // output columns per thread
     constexpr int SQ = AT_BQ + AT_PAD, SK = AT_BK + AT_PAD;
     extern __shared__ __align__(16) float sm[];
@@ -50,6 +53,16 @@ attention_kernel(const mugd_attention a) {
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
     const int b = blockIdx.z, h = blockIdx.y;
     const int q0 = blockIdx.x * AT_BQ;
+    const int lq = attn_rows(d, b, a.Lq), lk = attn_rows(d, b, a.Lk);
+    if constexpr (attn_is_var<Desc>) {
+        if (q0 >= lq) {
+            for (int t = tid; t < AT_BQ * D; t += AT_THREADS) {
+                const int r = t / D, c = t - r * D;
+                if (q0 + r < a.Lq) a.o[((int64_t)b * a.Lq + q0 + r) * a.ldo + h * D + c] = 0.f;
+            }
+            return;
+        }
+    }
     for (int t = tid; t < NT; t += AT_THREADS) {
         rel[t] = a.relpos[t * a.H + h];
         cg[t] = a.cgain[t * a.H + h];
@@ -60,7 +73,7 @@ attention_kernel(const mugd_attention a) {
         for (int t = tid; t < AT_BQ * QD; t += AT_THREADS) {
             const int r = t / QD, c = (t - r * QD) * 4;
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (q0 + r < a.Lq) v = ld_f4(qb + (int64_t)(q0 + r) * a.ldq + c);
+            if (q0 + r < lq) v = ld_f4(qb + (int64_t)(q0 + r) * a.ldq + c);
             Qt[(c + 0) * SQ + r] = v.x; Qt[(c + 1) * SQ + r] = v.y; Qt[(c + 2) * SQ + r] = v.z; Qt[(c + 3) * SQ + r] = v.w;
         }
     }
@@ -74,12 +87,12 @@ attention_kernel(const mugd_attention a) {
     const float* kb = a.k + (int64_t)b * a.Lk * a.ldk + h * D;
     const float* vb = a.v + (int64_t)b * a.Lk * a.ldv + h * D;
 
-    for (int j0 = 0; j0 < a.Lk; j0 += AT_BK) {
+    for (int j0 = 0; j0 < lk; j0 += AT_BK) {
         __syncthreads();                       // previous tile consumed (first pass: Qt / tables written)
         for (int t = tid; t < AT_BK * QD; t += AT_THREADS) {
             const int r = t / QD, c = (t - r * QD) * 4;
             float4 kv = make_float4(0.f, 0.f, 0.f, 0.f), vv = kv;
-            if (j0 + r < a.Lk) {
+            if (j0 + r < lk) {
                 kv = ld_f4(kb + (int64_t)(j0 + r) * a.ldk + c);
                 vv = ld_f4(vb + (int64_t)(j0 + r) * a.ldv + c);
             }
@@ -114,7 +127,7 @@ attention_kernel(const mugd_attention a) {
             for (int j = 0; j < 4; ++j) {
                 const int kj = j0 + tx * 4 + j;
                 idx[j] = max(-P, min(P, kj - qi)) + P;
-                s[i][j] = (kj < a.Lk) ? (s[i][j] + rel[idx[j]]) * a.scale : -INFINITY;
+                s[i][j] = (kj < lk) ? (s[i][j] + rel[idx[j]]) * a.scale : -INFINITY;
                 mx = fmaxf(mx, s[i][j]);
             }
 #pragma unroll
@@ -140,7 +153,7 @@ attention_kernel(const mugd_attention a) {
             *reinterpret_cast<float4*>(&Pt[(tx * 4 + j) * SQ + ty * 4]) = make_float4(pc[0][j], pc[1][j], pc[2][j], pc[3][j]);
         __syncthreads();
         // ---- O += P V ----------------------------------------------------------------------------------------
-        const int nk = min(AT_BK, a.Lk - j0);
+        const int nk = min(AT_BK, lk - j0);
 #pragma unroll 4
         for (int kk = 0; kk < nk; ++kk) {
             const float4 pa = *reinterpret_cast<const float4*>(&Pt[kk * SQ + ty * 4]);
@@ -161,20 +174,17 @@ attention_kernel(const mugd_attention a) {
             const float inv = 1.0f / l_i[i];
             float* op = a.o + ((int64_t)b * a.Lq + qi) * a.ldo + h * D + tx * DC;
 #pragma unroll
-            for (int c = 0; c < DC; ++c) op[c] = o[i][c] * inv;
+            for (int c = 0; c < DC; ++c) op[c] = qi < lq ? o[i][c] * inv : 0.f;
         }
     }
 }
 
-cudaError_t attention_allow_smem(int bytes) {
-    return allow_dynamic_smem(bytes, attention_kernel<32>, attention_kernel<48>, attention_kernel<64>);
-}
-
-template <int D>
-static int attention_launch(const mugd_attention& a, cudaStream_t st) {
+template <int D, typename Desc>
+static int attention_launch(const Desc& d, cudaStream_t st) {
+    const mugd_attention& a = attn_desc(d);
     const size_t bytes = sizeof(float) * (AttSmem<D>::FLOATS + 2 * (2 * a.pos_max + 1));
     dim3 grid((a.Lq + AT_BQ - 1) / AT_BQ, a.H, a.B);
-    MUGD_CHECK_CUDA(launch_k(attention_kernel<D>, grid, dim3(AT_THREADS), bytes, st, a));
+    MUGD_CHECK_CUDA(launch_k(attention_kernel<D, Desc>, grid, dim3(AT_THREADS), bytes, st, d));
     return MUGD_OK;
 }
 
@@ -189,9 +199,10 @@ constexpr int ASK_WARPS = 8;
 constexpr int ASK_RW = 4;         // query rows a warp carries together
 constexpr int ASK_ROWS = ASK_WARPS * ASK_RW;      // query rows per CTA
 
-template <int D>
+template <int D, typename Desc = mugd_attention>
 __global__ void __launch_bounds__(ASK_WARPS * 32)
-attention_smallk_kernel(const mugd_attention a) {
+attention_smallk_kernel(const Desc d) {
+    const mugd_attention& a = attn_desc(d);
     constexpr int DV = (D + 31) / 32;                 // output channels per lane
     constexpr int KP = D + 1;                         // K row pitch: lane j reads row j, the odd pitch keeps the lanes on distinct banks
     constexpr int QD = D / 4;
@@ -204,7 +215,17 @@ attention_smallk_kernel(const mugd_attention a) {
     const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * ASK_ROWS;
     const int P = a.pos_max;
     const int qbase = q0 + warp * ASK_RW;             // the warp's ASK_RW query rows go through the kernel together
-    const bool key_ok = lane < a.Lk;
+    const int lq = attn_rows(d, b, a.Lq), lk = attn_rows(d, b, a.Lk);
+    if constexpr (attn_is_var<Desc>) {              // a CTA of padded rows only: zeros (uniform over the CTA, before any barrier)
+        if (q0 >= lq) {
+            for (int t = tid; t < ASK_ROWS * D; t += ASK_WARPS * 32) {
+                const int r = t / D, c = t - r * D;
+                if (q0 + r < a.Lq) a.o[((int64_t)b * a.Lq + q0 + r) * a.ldo + h * D + c] = 0.f;
+            }
+            return;
+        }
+    }
+    const bool key_ok = lane < lk;
     // everything this thread needs from global memory is requested up front, in one round trip with the K / V fill: its slice of
     // the warp's query rows and the bias / gain of (its key, each row) -- 2 x ASK_RW table entries, not the whole 2P+1 table
     float qpre[ASK_RW][DV], relv[ASK_RW], cgv[ASK_RW];
@@ -223,7 +244,7 @@ attention_smallk_kernel(const mugd_attention a) {
     for (int t = tid; t < 32 * QD; t += ASK_WARPS * 32) {
         const int r = t / QD, c = (t - r * QD) * 4;
         float4 kv = make_float4(0.f, 0.f, 0.f, 0.f), vv = kv;
-        if (r < a.Lk) {
+        if (r < lk) {
             kv = ld_f4(kb + (int64_t)r * a.ldk + c);
             vv = ld_f4(vb + (int64_t)r * a.ldv + c);
         }
@@ -274,7 +295,7 @@ attention_smallk_kernel(const mugd_attention a) {
     for (int i = 0; i < ASK_RW; ++i)
 #pragma unroll
         for (int c = 0; c < DV; ++c) o[i][c] = 0.f;
-    for (int j = 0; j < a.Lk; ++j) {
+    for (int j = 0; j < lk; ++j) {
         float vj[DV];
 #pragma unroll
         for (int c = 0; c < DV; ++c) vj[c] = (lane + c * 32 < D) ? Vs[j * D + lane + c * 32] : 0.f;
@@ -293,23 +314,30 @@ attention_smallk_kernel(const mugd_attention a) {
             float* op = a.o + ((int64_t)b * a.Lq + qi) * a.ldo + h * D;
 #pragma unroll
             for (int c = 0; c < DV; ++c)
-                if (lane + c * 32 < D) op[lane + c * 32] = o[i][c] * inv;
+                if (lane + c * 32 < D) op[lane + c * 32] = qi < lq ? o[i][c] * inv : 0.f;
         }
     }
 }
 
-template <int D>
-static int attention_smallk_launch(const mugd_attention& a, cudaStream_t st) {
+template <int D, typename Desc>
+static int attention_smallk_launch(const Desc& d, cudaStream_t st) {
+    const mugd_attention& a = attn_desc(d);
     const size_t bytes = sizeof(float) * (32 * (D + 1) + 32 * D + ASK_ROWS * D + 4);
     dim3 grid((a.Lq + ASK_ROWS - 1) / ASK_ROWS, a.H, a.B);      // (more rows per CTA -- fewer re-reads of K / V -- measured slower)
-    MUGD_CHECK_CUDA(launch_k(attention_smallk_kernel<D>, grid, dim3(ASK_WARPS * 32), bytes, st, a));
+    MUGD_CHECK_CUDA(launch_k(attention_smallk_kernel<D, Desc>, grid, dim3(ASK_WARPS * 32), bytes, st, d));
     return MUGD_OK;
 }
 
-int launch_attention_tc(const DeviceInfo& dev, const mugd_attention& a, cudaStream_t st);   // attention_tc.cu
-// 1 (default): both contractions on the wgmma tensor cores (attention_tc.cu), a lane-per-key kernel when there are at most 32 keys;
-// 0: the tiled FFMA kernel above for everything (referee)
-int launch_attention(const DeviceInfo& dev, const mugd_attention& a, cudaStream_t st, int* launches) {
+cudaError_t attention_allow_smem(int bytes) {
+    return allow_dynamic_smem(bytes, attention_kernel<32>, attention_kernel<48>, attention_kernel<64>,
+                              attention_kernel<32, mugd_attention_var>, attention_kernel<48, mugd_attention_var>,
+                              attention_kernel<64, mugd_attention_var>);
+}
+
+int launch_attention_tc(const DeviceInfo& dev, const mugd_attention& a, cudaStream_t st);       // attention_tc.cu
+int launch_attention_tc(const DeviceInfo& dev, const mugd_attention_var& a, cudaStream_t st);
+
+static int check_attention(const mugd_attention& a) {
     MUGD_REQUIRE(a.B > 0 && a.H > 0 && a.Lq > 0 && a.Lk > 0, "attention: empty shape");
     MUGD_REQUIRE(a.D == 32 || a.D == 48 || a.D == 64, "attention: head dim %d not in {32,48,64}", a.D);
     MUGD_REQUIRE(a.pos_max >= 0 && a.pos_max <= 1024, "attention: pos_max %d", a.pos_max);
@@ -317,16 +345,35 @@ int launch_attention(const DeviceInfo& dev, const mugd_attention& a, cudaStream_
                      a.ldv % 4 == 0 && a.ldo % 4 == 0, "attention: alignment");
     MUGD_REQUIRE(a.ldq >= a.H * a.D && a.ldk >= a.H * a.D && a.ldv >= a.H * a.D && a.ldo >= a.H * a.D, "attention: ld < H*D");
     MUGD_REQUIRE(a.relpos && a.cgain, "attention: tables missing");
-    int rc;
+    return MUGD_OK;
+}
+
+// 1 (default): both contractions on the wgmma tensor cores (attention_tc.cu), a lane-per-key kernel when there are at most 32 keys;
+// 0: the tiled FFMA kernel above for everything (referee).  A ragged op takes the same kernel as the plain op of its shape.
+template <typename Desc>
+static int dispatch_attention(const DeviceInfo& dev, const Desc& d, cudaStream_t st, int* launches) {
+    const mugd_attention& a = attn_desc(d);
+    int rc = check_attention(a);
+    if (rc != MUGD_OK) return rc;
     // per shape (tools/profile_ops.py --only attention): with head dim 32 (Lq = 256 at the default length) the rows are many
     // and short and the FFMA lanes saturate; with head dim 48 / 64 the lane-per-key kernel wins
     if (dev.attention_impl == 1 && a.Lk <= 32 && a.D >= 48)
-        rc = (a.D == 48) ? attention_smallk_launch<48>(a, st) : attention_smallk_launch<64>(a, st);
-    else if (dev.attention_impl == 1) rc = launch_attention_tc(dev, a, st);
-    else rc = (a.D == 32) ? attention_launch<32>(a, st) : (a.D == 48) ? attention_launch<48>(a, st) : attention_launch<64>(a, st);
+        rc = (a.D == 48) ? attention_smallk_launch<48>(d, st) : attention_smallk_launch<64>(d, st);
+    else if (dev.attention_impl == 1) rc = launch_attention_tc(dev, d, st);
+    else rc = (a.D == 32) ? attention_launch<32>(d, st) : (a.D == 48) ? attention_launch<48>(d, st) : attention_launch<64>(d, st);
     if (rc != MUGD_OK) return rc;
     if (launches) *launches += 1;
     return MUGD_OK;
+}
+
+int launch_attention(const DeviceInfo& dev, const mugd_attention& a, cudaStream_t st, int* launches) {
+    return dispatch_attention(dev, a, st, launches);
+}
+
+int launch_attention_var(const DeviceInfo& dev, const mugd_attention_var& a, cudaStream_t st, int* launches) {
+    MUGD_REQUIRE(a.valid, "attention_var: valid lengths missing");
+    MUGD_REQUIRE(a.attn.Lq == a.attn.Lk, "attention_var: self-attention only (Lq=%d, Lk=%d)", a.attn.Lq, a.attn.Lk);
+    return dispatch_attention(dev, a, st, launches);
 }
 
 }  // namespace mugd

@@ -48,9 +48,13 @@ struct Smem {
     static size_t total(int pos_max) { return TILE_BYTES + AUX_BYTES + 2 * (2 * pos_max + 1) * 4 + 1024; }
 };
 
-template <int D>
+// Ragged batches (Desc = mugd_attention_var): only the lk valid keys of the sample are scored.  Key tiles fully past lk are never
+// loaded; in the last one the rows past lk (which the TMA box still brings in, NaN or not) are replaced by zeros before any MMA,
+// exactly as the plain kernel zeroes keys past Lk.  Query rows past lq are written as zeros; a CTA of padded rows only writes its zeros.
+template <int D, typename Desc = mugd_attention>
 __global__ void __launch_bounds__(THREADS, 1)
-attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const mugd_attention a, float* dbg) {
+attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const Desc d, float* dbg) {
+    const mugd_attention& a = attn_desc(d);
     using S = Smem<D>;
     constexpr int STAGES = S::STAGES;
     constexpr int KD = D / 8;                               // k8 steps of S = Q K^T
@@ -72,7 +76,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * BQ;
     const int rq = (warp >> 2) * 64 + (warp & 3) * 16 + g8;  // this thread's query rows: rq, rq + 8 (tile-relative)
     const int qa = q0 + rq, qb = qa + 8;
-    const int ntiles = (a.Lk + BKV - 1) / BKV;
+    const int ntiles_all = (a.Lk + BKV - 1) / BKV;
 
     if (tid == 0) {
         for (int s = 0; s < STAGES; ++s) mbar_init(bar_full(s), 1);
@@ -80,6 +84,17 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     }
     __syncthreads();
     pdl_wait();
+    const int lq = attn_rows(d, b, a.Lq), lk = attn_rows(d, b, a.Lk);
+    const int ntiles = attn_is_var<Desc> ? (lk + BKV - 1) / BKV : ntiles_all;
+    if constexpr (attn_is_var<Desc>) {
+        if (q0 >= lq) {                                     // uniform over the CTA; no copy has been issued yet
+            for (int t = tid; t < BQ * D; t += THREADS) {
+                const int r = t / D, c = t - r * D;
+                if (q0 + r < a.Lq) a.o[((int64_t)b * a.Lq + q0 + r) * a.ldo + h * D + c] = 0.f;
+            }
+            return;
+        }
+    }
 
     // raw K / V head slices of key tile t -> stage t % STAGES (keys >= Lk and channels >= H*D arrive as zeros)
     auto issue_tile = [&](int t) {
@@ -114,7 +129,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
                 const int c = kk * 8 + t4 + (e >> 1) * 4;
                 const bool rb = e & 1;
                 float x = 0.f;
-                if ((rb ? qb : qa) < a.Lq) x = (rb ? qpb : qpa)[c];
+                if ((rb ? qb : qa) < lq) x = (rb ? qpb : qpa)[c];
                 const float hi = to_tf32(x);
                 qhi[kk][e] = __float_as_uint(hi);
                 qlo[kk][e] = __float_as_uint(to_tf32(x - hi));
@@ -128,7 +143,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     for (int t = 0; t < ntiles; ++t) {
         const int s = t % STAGES;
         const int j0 = t * BKV;
-        const int nk = min(BKV, a.Lk - j0);
+        const int nk = min(BKV, lk - j0);
         mbar_wait(bar_full(s), (uint32_t)(t / STAGES) & 1u);
         // ---- key tile: raw -> k_hi in place, k_lo beside it (elementwise, so swizzle-agnostic); keys past Lk -> 0 -------------
         for (int f = tid; f < S::KSLABS * 1024; f += THREADS) {
@@ -193,7 +208,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
                 const int kj = j0 + j * 8 + 2 * t4 + (e & 1);
                 const int qi = (e & 2) ? qb : qa;
                 const int idx = max(-P, min(P, kj - qi)) + P;
-                const float sc = (kj < a.Lk) ? fmaf(sacc[4 * j + e], a.scale, rel[idx]) : -INFINITY;
+                const float sc = (kj < lk) ? fmaf(sacc[4 * j + e], a.scale, rel[idx]) : -INFINITY;
                 sacc[4 * j + e] = sc;
                 if (e & 2) mxb = fmaxf(mxb, sc); else mxa = fmaxf(mxa, sc);
             }
@@ -260,8 +275,8 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 #pragma unroll
     for (int j = 0; j < NO / 4; ++j) {
         const int c = j * 8 + 2 * t4;
-        if (qa < a.Lq) *reinterpret_cast<float2*>(opa + c) = make_float2(o[4 * j] * ia, o[4 * j + 1] * ia);
-        if (qb < a.Lq) *reinterpret_cast<float2*>(opb + c) = make_float2(o[4 * j + 2] * ib, o[4 * j + 3] * ib);
+        if (qa < a.Lq) *reinterpret_cast<float2*>(opa + c) = qa < lq ? make_float2(o[4 * j] * ia, o[4 * j + 1] * ia) : make_float2(0.f, 0.f);
+        if (qb < a.Lq) *reinterpret_cast<float2*>(opb + c) = qb < lq ? make_float2(o[4 * j + 2] * ib, o[4 * j + 3] * ib) : make_float2(0.f, 0.f);
     }
 }
 
@@ -275,8 +290,9 @@ static int encode_kv(CUtensorMap* tm, const float* p, int64_t ld, int cols, int 
 
 static float* g_dbg = nullptr;      // debugging aid: CTA (0,0,0) dumps the raw logits of its first key tile (16 of each row's 40 floats)
 
-template <int D>
-static int launch(const mugd_attention& a, cudaStream_t st) {
+template <int D, typename Desc>
+static int launch(const Desc& d, cudaStream_t st) {
+    const mugd_attention& a = attn_desc(d);
     CUtensorMap tmK, tmV;
     int rc = encode_kv(&tmK, a.k, a.ldk, a.H * D, a.Lk, a.B);
     if (rc != MUGD_OK) return rc;
@@ -284,18 +300,25 @@ static int launch(const mugd_attention& a, cudaStream_t st) {
     if (rc != MUGD_OK) return rc;
     const size_t bytes = Smem<D>::total(a.pos_max);
     dim3 grid((a.Lq + BQ - 1) / BQ, a.H, a.B);
-    MUGD_CHECK_CUDA(launch_k(attention_tc_kernel<D>, grid, dim3(THREADS), bytes, st, tmK, tmV, a, g_dbg));
+    MUGD_CHECK_CUDA(launch_k(attention_tc_kernel<D, Desc>, grid, dim3(THREADS), bytes, st, tmK, tmV, d, g_dbg));
     return MUGD_OK;
 }
 
 }  // namespace atc
 
 cudaError_t attention_tc_allow_smem(int bytes) {
-    return allow_dynamic_smem(bytes, atc::attention_tc_kernel<32>, atc::attention_tc_kernel<48>, atc::attention_tc_kernel<64>);
+    return allow_dynamic_smem(bytes, atc::attention_tc_kernel<32>, atc::attention_tc_kernel<48>, atc::attention_tc_kernel<64>,
+                              atc::attention_tc_kernel<32, mugd_attention_var>, atc::attention_tc_kernel<48, mugd_attention_var>,
+                              atc::attention_tc_kernel<64, mugd_attention_var>);
 }
 
 int launch_attention_tc(const DeviceInfo&, const mugd_attention& a, cudaStream_t st) {
     return (a.D == 32) ? atc::launch<32>(a, st) : (a.D == 48) ? atc::launch<48>(a, st) : atc::launch<64>(a, st);
+}
+
+int launch_attention_tc(const DeviceInfo&, const mugd_attention_var& v, cudaStream_t st) {
+    const int D = v.attn.D;
+    return (D == 32) ? atc::launch<32>(v, st) : (D == 48) ? atc::launch<48>(v, st) : atc::launch<64>(v, st);
 }
 
 }  // namespace mugd

@@ -63,6 +63,10 @@ int launch_notes(const DeviceInfo& dev, const mugd_notes& n, cudaStream_t st, in
 int launch_embed(const DeviceInfo& dev, const mugd_embed& e, cudaStream_t st, int* launches);
 int launch_tf32_split(const DeviceInfo& dev, const mugd_tf32_split& s, cudaStream_t st, int* launches);
 int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_t st, int* launches);
+// ragged batches: valid[b] rows per sample (norm.cu, attention.cu, elementwise.cu)
+int launch_groupnorm_var(const DeviceInfo& dev, const mugd_groupnorm_var& g, cudaStream_t st, int* launches);
+int launch_attention_var(const DeviceInfo& dev, const mugd_attention_var& a, cudaStream_t st, int* launches);
+int launch_row_mask(const DeviceInfo& dev, const mugd_row_mask& m, cudaStream_t st, int* launches);
 // mugd_sample_staged: check_stage validates a stage for n_steps (host arrays included); launch_stage runs step i of it
 int check_stage(const mugd_stage& s, int32_t n_steps);
 int launch_stage(const mugd_stage& s, int32_t i, cudaStream_t st);
@@ -190,6 +194,15 @@ __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x));
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
 // exact-erf GELU (nn.GELU() default; attention.py:45, s4.py:187-188)
 __device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+
+// Attention kernels are instantiated for both descriptors: mugd_attention (every row valid) and mugd_attention_var (ragged batches,
+// sample b's first clamp(valid[b], 0, n) rows valid).  With the plain descriptor attn_rows() is n, so those instances compile to the
+// code they had before ragged batches existed.
+__host__ __device__ __forceinline__ const mugd_attention& attn_desc(const mugd_attention& a) { return a; }
+__host__ __device__ __forceinline__ const mugd_attention& attn_desc(const mugd_attention_var& a) { return a.attn; }
+__device__ __forceinline__ int attn_rows(const mugd_attention&, int, int n) { return n; }
+__device__ __forceinline__ int attn_rows(const mugd_attention_var& a, int b, int n) { return min(max(a.valid[b], 0), n); }
+template <typename Desc> constexpr bool attn_is_var = sizeof(Desc) != sizeof(mugd_attention);
 
 __device__ __forceinline__ float4 ld_f4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ void st_f4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }

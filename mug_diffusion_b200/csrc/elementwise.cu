@@ -182,6 +182,32 @@ int launch_copy2d(const DeviceInfo& dev, const mugd_copy2d& c, cudaStream_t st, 
     return MUGD_OK;
 }
 
+// ragged batches: rows l >= clamp(valid[b], 0, L) of sample b, columns 0 .. cols - 1, set to 0 by a store (padded rows may hold NaN,
+// which a multiply by 0 would keep).  Grid (x, B): the CTAs of one sample stride over its padded elements only.
+__global__ void __launch_bounds__(256)
+row_mask_kernel(const mugd_row_mask m) {
+    pdl_wait();
+    const int b = blockIdx.y;
+    const int Lv = min(max(m.valid[b], 0), m.L);
+    const int64_t total = (int64_t)(m.L - Lv) * m.cols;
+    float* xb = m.x + ((int64_t)b * m.L + Lv) * m.ld;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / m.cols;
+        xb[r * m.ld + (i - r * m.cols)] = 0.f;
+    }
+}
+
+int launch_row_mask(const DeviceInfo& dev, const mugd_row_mask& m, cudaStream_t st, int* launches) {
+    MUGD_REQUIRE(m.x && m.valid && m.B > 0 && m.B <= 65535 && m.L > 0 && m.cols > 0 && m.ld >= m.cols,
+                 "row_mask: bad descriptor B=%d L=%d cols=%d ld=%lld", m.B, m.L, m.cols, (long long)m.ld);
+    const int64_t per_sample = (int64_t)m.L * m.cols;
+    int blocks = (int)((per_sample + 255) / 256);
+    if (blocks > 64) blocks = 64;
+    MUGD_CHECK_CUDA(launch_k(row_mask_kernel, dim3(blocks, m.B), dim3(256), 0, st, m));
+    if (launches) *launches += 1;
+    return MUGD_OK;
+}
+
 // weight preprocessing for the 3xTF32 GEMM: hi over w, lo beside it (same roundings as the converter warps apply to activations)
 __global__ void __launch_bounds__(256)
 tf32_split_kernel(float* __restrict__ w_hi, float* __restrict__ lo, int64_t n4) {

@@ -39,17 +39,17 @@ __device__ __forceinline__ void gn_block_stats(double s, double ss, double inv_n
     rstd = r;
 }
 
+// The bodies take the sample's row stride L and the rows they normalise, Lv <= L: the plain kernels pass Lv = L, the ragged ones
+// (MUGD_OP_GROUPNORM_VAR) the sample's valid count, so rows past it are neither read nor written here.
 template <int NV>
-__global__ void __launch_bounds__(GN_THREADS)
-groupnorm_silu_reg_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy,
-                          const float* __restrict__ gamma, const float* __restrict__ beta,
-                          int L, int C, int G, float eps, int silu) {
-    pdl_wait();
+__device__ __forceinline__ void gn_reg_body(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy,
+                                            const float* __restrict__ gamma, const float* __restrict__ beta,
+                                            int L, int Lv, int C, int G, float eps, int silu) {
     const int g = blockIdx.x, b = blockIdx.y;
     const int cg = C / G;
     const int q = cg >> 2;                 // float4 per row of this group
-    const int total = L * q;
-    const double inv_n = 1.0 / ((double)L * cg);       // requested before the loads: off the chain behind the block reduction
+    const int total = Lv * q;
+    const double inv_n = 1.0 / ((double)Lv * cg);      // requested before the loads: off the chain behind the block reduction
     const float* xb = x + (int64_t)b * L * ldx + (int64_t)g * cg;
     float* yb = y + (int64_t)b * L * ldy + (int64_t)g * cg;
     float4 v[NV];
@@ -103,17 +103,24 @@ groupnorm_silu_reg_kernel(const float* __restrict__ x, int64_t ldx, float* __res
     }
 }
 
-// two-pass form for slabs that do not fit the registers: moments, then apply (the second read is served by L1/L2)
+template <int NV>
 __global__ void __launch_bounds__(GN_THREADS)
-groupnorm_silu_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy,
-                      const float* __restrict__ gamma, const float* __restrict__ beta,
-                      int L, int C, int G, float eps, int silu) {
+groupnorm_silu_reg_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy,
+                          const float* __restrict__ gamma, const float* __restrict__ beta,
+                          int L, int C, int G, float eps, int silu) {
     pdl_wait();
+    gn_reg_body<NV>(x, ldx, y, ldy, gamma, beta, L, L, C, G, eps, silu);
+}
+
+// two-pass form for slabs that do not fit the registers: moments, then apply (the second read is served by L1/L2)
+__device__ __forceinline__ void gn_body(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy,
+                                        const float* __restrict__ gamma, const float* __restrict__ beta,
+                                        int L, int Lv, int C, int G, float eps, int silu) {
     const int g = blockIdx.x, b = blockIdx.y;
     const int cg = C / G;
     const int q = cg >> 2;
-    const int total = L * q;
-    const double inv_n = 1.0 / ((double)L * cg);       // requested before the loads: off the chain behind the block reduction
+    const int total = Lv * q;
+    const double inv_n = 1.0 / ((double)Lv * cg);      // requested before the loads: off the chain behind the block reduction
     const float* xb = x + (int64_t)b * L * ldx + (int64_t)g * cg;
     float* yb = y + (int64_t)b * L * ldy + (int64_t)g * cg;
 
@@ -143,16 +150,67 @@ groupnorm_silu_kernel(const float* __restrict__ x, int64_t ldx, float* __restric
     }
 }
 
+__global__ void __launch_bounds__(GN_THREADS)
+groupnorm_silu_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy,
+                      const float* __restrict__ gamma, const float* __restrict__ beta,
+                      int L, int C, int G, float eps, int silu) {
+    pdl_wait();
+    gn_body(x, ldx, y, ldy, gamma, beta, L, L, C, G, eps, silu);
+}
+
+// ---- ragged batches (MUGD_OP_GROUPNORM_VAR): sample b normalises its first Lv = clamp(valid[b], 0, L) rows with moments over those
+// rows alone and writes exact zeros (a store) to rows Lv .. L-1, which it never reads -- padded rows may hold NaN.  Lv = 0 writes
+// zeros only (its moments are never applied).  The bodies are the plain kernels' with Lv in place of L where rows are counted.
+__device__ __forceinline__ int gn_valid_rows(const int32_t* valid, int L) { return min(max(valid[blockIdx.y], 0), L); }
+
+__device__ __forceinline__ void gn_zero_tail(float* y, int64_t ldy, int L, int Lv, int C, int G) {
+    const int g = blockIdx.x, b = blockIdx.y;
+    const int q = (C / G) >> 2;
+    float* yb = y + ((int64_t)b * L + Lv) * ldy + (int64_t)g * (C / G);
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = threadIdx.x; i < (L - Lv) * q; i += GN_THREADS) {
+        const int row = i / q, qq = i - row * q;
+        st_f4(yb + (int64_t)row * ldy + qq * 4, z);
+    }
+}
+
+template <int NV>
+__global__ void __launch_bounds__(GN_THREADS)
+groupnorm_silu_reg_var_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy,
+                              const float* __restrict__ gamma, const float* __restrict__ beta,
+                              int L, int C, int G, float eps, int silu, const int32_t* __restrict__ valid) {
+    pdl_wait();
+    const int Lv = gn_valid_rows(valid, L);
+    gn_reg_body<NV>(x, ldx, y, ldy, gamma, beta, L, Lv, C, G, eps, silu);
+    gn_zero_tail(y, ldy, L, Lv, C, G);
+}
+
+__global__ void __launch_bounds__(GN_THREADS)
+groupnorm_silu_var_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy,
+                          const float* __restrict__ gamma, const float* __restrict__ beta,
+                          int L, int C, int G, float eps, int silu, const int32_t* __restrict__ valid) {
+    pdl_wait();
+    const int Lv = gn_valid_rows(valid, L);
+    gn_body(x, ldx, y, ldy, gamma, beta, L, Lv, C, G, eps, silu);
+    gn_zero_tail(y, ldy, L, Lv, C, G);
+}
+
 // A second form -- one thread-block CLUSTER per sample, CTAs owning bands of whole rows (fully coalesced, gamma / beta per thread,
 // band moments exchanged through distributed shared memory) -- was built, measured and lost almost everywhere: inside the
 // graph the slabs come out of L2, where the 16..48-byte pieces of this kernel cost little, while two cluster barriers + the DSMEM
 // exchange sit on every launch's critical path.  Removed.
-int launch_groupnorm(const DeviceInfo&, const mugd_groupnorm& g, cudaStream_t st, int* launches) {
+static int check_groupnorm(const mugd_groupnorm& g) {
     MUGD_REQUIRE(g.B > 0 && g.L > 0 && g.C > 0 && g.G > 0, "groupnorm: empty shape B=%d L=%d C=%d G=%d", g.B, g.L, g.C, g.G);
     MUGD_REQUIRE(g.C % g.G == 0 && (g.C / g.G) % 4 == 0, "groupnorm: C/G must be a multiple of 4 (C=%d G=%d)", g.C, g.G);
     MUGD_REQUIRE(g.ldx % 4 == 0 && g.ldy % 4 == 0 && aligned16(g.x) && aligned16(g.y) && aligned16(g.gamma) && aligned16(g.beta),
                  "groupnorm: operands must be 16-byte aligned with ld %% 4 == 0");
     MUGD_REQUIRE(g.ldx >= g.C && g.ldy >= g.C, "groupnorm: leading dimension smaller than C");
+    return MUGD_OK;
+}
+
+int launch_groupnorm(const DeviceInfo&, const mugd_groupnorm& g, cudaStream_t st, int* launches) {
+    const int rc = check_groupnorm(g);
+    if (rc != MUGD_OK) return rc;
     dim3 grid(g.G, g.B);
     const int per_thread = (g.L * (g.C / g.G / 4) + GN_THREADS - 1) / GN_THREADS;     // float4 per thread
 #define GN_GO(K) MUGD_CHECK_CUDA(launch_k(K, grid, dim3(GN_THREADS), 0, st, g.x, g.ldx, g.y, g.ldy, g.gamma, g.beta, g.L, g.C, g.G, g.eps, g.silu))
@@ -162,6 +220,26 @@ int launch_groupnorm(const DeviceInfo&, const mugd_groupnorm& g, cudaStream_t st
     else if (per_thread <= 16) GN_GO(groupnorm_silu_reg_kernel<16>);
     else if (per_thread <= GN_MAXV) GN_GO(groupnorm_silu_reg_kernel<GN_MAXV>);
     else GN_GO(groupnorm_silu_kernel);
+#undef GN_GO
+    if (launches) *launches += 1;
+    return MUGD_OK;
+}
+
+// the same variant choice as launch_groupnorm, by the padded length L
+int launch_groupnorm_var(const DeviceInfo&, const mugd_groupnorm_var& v, cudaStream_t st, int* launches) {
+    const mugd_groupnorm& g = v.gn;
+    int rc = check_groupnorm(g);
+    if (rc != MUGD_OK) return rc;
+    MUGD_REQUIRE(v.valid, "groupnorm_var: valid lengths missing");
+    dim3 grid(g.G, g.B);
+    const int per_thread = (g.L * (g.C / g.G / 4) + GN_THREADS - 1) / GN_THREADS;
+#define GN_GO(K) MUGD_CHECK_CUDA(launch_k(K, grid, dim3(GN_THREADS), 0, st, g.x, g.ldx, g.y, g.ldy, g.gamma, g.beta, g.L, g.C, g.G, g.eps, g.silu, v.valid))
+    if (per_thread <= 2) GN_GO(groupnorm_silu_reg_var_kernel<2>);
+    else if (per_thread <= 4) GN_GO(groupnorm_silu_reg_var_kernel<4>);
+    else if (per_thread <= 8) GN_GO(groupnorm_silu_reg_var_kernel<8>);
+    else if (per_thread <= 16) GN_GO(groupnorm_silu_reg_var_kernel<16>);
+    else if (per_thread <= GN_MAXV) GN_GO(groupnorm_silu_reg_var_kernel<GN_MAXV>);
+    else GN_GO(groupnorm_silu_var_kernel);
 #undef GN_GO
     if (launches) *launches += 1;
     return MUGD_OK;

@@ -39,6 +39,12 @@ static const PtrField k_ptr_fields[] = {
     PF(MUGD_OP_TF32_SPLIT, split.w_hi), PF(MUGD_OP_TF32_SPLIT, split.lo),
     PF(MUGD_OP_POSTERIOR, post.params), PF(MUGD_OP_POSTERIOR, post.noise), PF(MUGD_OP_POSTERIOR, post.mean), PF(MUGD_OP_POSTERIOR, post.logvar),
     PF(MUGD_OP_POSTERIOR, post.std), PF(MUGD_OP_POSTERIOR, post.z),
+    PF(MUGD_OP_GROUPNORM_VAR, gnv.gn.x), PF(MUGD_OP_GROUPNORM_VAR, gnv.gn.y), PF(MUGD_OP_GROUPNORM_VAR, gnv.gn.gamma),
+    PF(MUGD_OP_GROUPNORM_VAR, gnv.gn.beta), PF(MUGD_OP_GROUPNORM_VAR, gnv.valid),
+    PF(MUGD_OP_ATTENTION_VAR, attnv.attn.q), PF(MUGD_OP_ATTENTION_VAR, attnv.attn.k), PF(MUGD_OP_ATTENTION_VAR, attnv.attn.v),
+    PF(MUGD_OP_ATTENTION_VAR, attnv.attn.o), PF(MUGD_OP_ATTENTION_VAR, attnv.attn.relpos), PF(MUGD_OP_ATTENTION_VAR, attnv.attn.cgain),
+    PF(MUGD_OP_ATTENTION_VAR, attnv.valid),
+    PF(MUGD_OP_ROW_MASK, mask.x), PF(MUGD_OP_ROW_MASK, mask.valid),
 };
 #undef PF
 

@@ -96,12 +96,16 @@ def scatter_batch(tensors: Optional[Sequence[torch.Tensor]], shapes: Sequence[Se
     return out
 
 
-def sample_sharded(sample_fn, request: Optional[Dict[str, object]], shapes: Dict[str, Sequence[int]], device: torch.device, src: int = 0):
+def sample_sharded(sample_fn, request: Optional[Dict[str, object]], shapes: Dict[str, Sequence[int]], device: torch.device, src: int = 0,
+                   z_lengths=None):
     """One sampling request over all ranks (BASELINE config 4: 256 charts on 8 GPUs): rank ``src`` holds the request
     (x_T [B,16,L], c / uc [B,128,T], w = the four audio feature maps), every rank receives its contiguous slice of the batch, runs
     ``sample_fn(x_T, c, uc, w) -> result [b, ...]`` on it -- the samples are independent through the whole DDIM loop and the decode, so
     there is no collective per step -- and the results are gathered on ``src`` in batch order (None elsewhere).
     ``shapes``: the whole-batch shapes of ``x_T``, ``c``, ``uc`` and ``w0..w3`` (known to every rank, e.g. from the request header)."""
+    if z_lengths is not None:
+        from .lib import MugdError
+        raise MugdError("z_lengths: sharding a request of charts of different lengths is not supported; run it on one GPU")
     keys = ["x_T", "c", "uc", "w0", "w1", "w2", "w3"]
     rank, world = dist.get_rank(), dist.get_world_size()
     tensors = None

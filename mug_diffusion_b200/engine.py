@@ -74,9 +74,12 @@ class Arena:
 
 
 class OpList:
-    def __init__(self, tc_map: Optional[Dict[int, Tuple[int, int]]] = None):
+    def __init__(self, tc_map: Optional[Dict[int, Tuple[int, int]]] = None, valid: Optional[Dict[int, int]] = None):
         self.ops: List[L_.Op] = []
         self.tc_map = tc_map or {}         # W pointer -> (W_hi, W_lo) pointers of the TF32 split
+        # ragged batches: rows per sample of a resolution -> device address of its int32 valid-row counts, one per sample.  A GroupNorm
+        # or self-attention at a resolution listed here becomes its _VAR op; without it every op is the plain one.
+        self.valid = valid or {}
 
     def add(self, kind: int, desc, tag: int = 0):
         self.ops.append(L_.make_op(kind, desc, tag))
@@ -138,8 +141,21 @@ class OpList:
         d.B, d.L, d.C, d.G = B, Lrows, x.cols, G
         d.eps, d.silu = GN_EPS, int(silu)
         assert x.rows == B * Lrows and y.cols == x.cols
-        self.add(L_.OP_GROUPNORM, d, tag)
+        if Lrows in self.valid:
+            v = L_.GroupNormVar()
+            v.gn, v.valid = d, self.valid[Lrows]
+            self.add(L_.OP_GROUPNORM_VAR, v, tag)
+        else:
+            self.add(L_.OP_GROUPNORM, d, tag)
         return len(self.ops) - 1
+
+    def row_mask(self, x: View, B: int, Lrows: int, tag: int = 0):
+        """rows l >= valid[b] of x ([B * Lrows, cols]) set to 0, at the resolution of Lrows rows per sample (ragged plans only)"""
+        assert x.rows == B * Lrows
+        d = L_.RowMask()
+        d.x, d.ld, d.valid = x.ptr, x.ld, self.valid[Lrows]
+        d.B, d.L, d.cols = B, Lrows, x.cols
+        self.add(L_.OP_ROW_MASK, d, tag)
 
     def layernorm(self, x: View, y: View, gamma: int, beta: int, tag: int = 0):
         d = L_.LayerNorm()
@@ -150,14 +166,19 @@ class OpList:
         return len(self.ops) - 1
 
     def attention(self, q: View, k: View, v: View, o: View, relpos: int, cgain: int, B: int, H: int, Lq: int,
-                  Lk: int, pos_max: int, tag: int = 0):
+                  Lk: int, pos_max: int, tag: int = 0, self_attn: bool = False):
         d = L_.Attention()
         D = q.cols // H
         d.q, d.ldq, d.k, d.ldk, d.v, d.ldv, d.o, d.ldo = q.ptr, q.ld, k.ptr, k.ld, v.ptr, v.ld, o.ptr, o.ld
         d.relpos, d.cgain = relpos, cgain
         d.B, d.H, d.D, d.Lq, d.Lk, d.pos_max = B, H, D, Lq, Lk, pos_max
         d.scale = float(D) ** -0.5
-        self.add(L_.OP_ATTENTION, d, tag)
+        if self_attn and Lq in self.valid:
+            v = L_.AttentionVar()
+            v.attn, v.valid = d, self.valid[Lq]
+            self.add(L_.OP_ATTENTION_VAR, v, tag)
+        else:
+            self.add(L_.OP_ATTENTION, d, tag)
 
     def s4conv(self, u: View, Kt: int, Dp: int, y: View, B: int, Lrows: int, tag: int = 0):
         d = L_.S4Conv()
@@ -242,17 +263,25 @@ class UNetCompiler:
     def w(self, name: str) -> int:
         return self.wbase + 4 * self.blob.offset(name)
 
-    def compile(self, arena: Arena, Beff: int, Lz: int, ext: Dict[str, int], per_sample_t: bool, fold_ln: Optional[bool] = None) -> dict:
+    def compile(self, arena: Arena, Beff: int, Lz: int, ext: Dict[str, int], per_sample_t: bool, fold_ln: Optional[bool] = None,
+                valid: Optional[Sequence[int]] = None) -> dict:
         """fold_ln: every LayerNorm of the transformer blocks is folded into the Linear behind it (the producer of its input delivers
         the row moments, the Linear corrects in its epilogue; no LayerNorm kernel, the normalised tensor is never written).  It gains
         at small batches and loses slightly at large ones, so None = fold below 8192 token rows.
-        False = stand-alone LayerNorm kernels (the referee path, and what the exact-fp32 FFMA GEMM uses)."""
+        False = stand-alone LayerNorm kernels (the referee path, and what the exact-fp32 FFMA GEMM uses).
+        valid: a ragged plan, whose Beff samples are padded to Lz rows but valid only in their first L_b: valid[l] is the device
+        address of an int32 [Beff] array holding L_b >> l, level l's valid rows.  Every GroupNorm and self-attention then takes its
+        _VAR op, and every k = 3 conv whose input is not a GroupNorm output (conv_in on x and the audio slots, Downsample, Upsample,
+        the S4 block's out_layer) finds its padded rows zeroed by a ROW_MASK op.  None = today's op list, op for op."""
         cfg = self.cfg
-        ops = OpList(self.tc_map)
         nlev = cfg.levels
         assert Lz % (1 << (nlev - 1)) == 0 and (Lz >> (nlev - 1)) % 4 == 0, "z_length must be a multiple of 32"
         rows = [Beff * (Lz >> l) for l in range(nlev)]
         lens = [Lz >> l for l in range(nlev)]
+        if valid is not None:
+            assert len(valid) == nlev, (len(valid), nlev)
+        ops = OpList(self.tc_map, None if valid is None else {lens[l]: int(valid[l]) for l in range(nlev)})
+        ragged = valid is not None
         mc = cfg.model_channels
         G = cfg.gn_groups
         if fold_ln is None:
@@ -332,6 +361,11 @@ class UNetCompiler:
         def copy(src: View, dst: View, tag: int):
             ops.copy2d(src, dst, tag)
 
+        def mask(x: View, lvl: int, tag: int):
+            """a ragged plan zeroes the padded rows of a k = 3 conv's input that no GroupNorm wrote"""
+            if ragged:
+                ops.row_mask(x, Beff, lens[lvl], tag)
+
         def groupnorm(x: View, y: View, gamma: int, beta: int, Lr: int, silu: bool, tag: int):
             ops.groupnorm(x, y, gamma, beta, Beff, Lr, G, silu, tag)
 
@@ -371,7 +405,7 @@ class UNetCompiler:
             ao = arena.alloc(x.rows, Cc)
             ops.attention(qkv.c(0, Cc), qkv.c(Cc, 2 * Cc), qkv.c(2 * Cc, 3 * Cc), ao,
                           self.w(t + "attn1.relative_position_embedding"), self.w(t + "attn1.C_embedding"),
-                          Beff, H, Lr, Lr, cfg.pos_max, TAG_ATTN)
+                          Beff, H, Lr, Lr, cfg.pos_max, TAG_ATTN, self_attn=True)
             h1 = arena.alloc(x.rows, Cc)
             i_h1 = gemm(ao, self.w(t + "attn1.to_out.0.weight"), Cc, Cc, h1, bias=self.w(t + "attn1.to_out.0.bias"),
                         residual=h0, Lout=Lr, tag=TAG_ATTN)
@@ -402,6 +436,7 @@ class UNetCompiler:
             z = g
             gemm(y, self.w(s_ + "output_linear.0.weight"), 2 * Hc, Hc, z, bias=self.w(s_ + "output_linear.0.bias"),
                  gate=L_.GATE_GLU, Lout=Lr, tag=TAG_S4)
+            mask(z, lvl, TAG_S4)                      # the causal conv carries valid rows into padded ones, the k = 3 conv back
             gemm(z, self.w(p + "out_layer.weight"), Hc, Hc, out, bias=self.w(p + "out_layer.bias"), taps=3,
                  mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, residual=x, tag=TAG_S4)
             arena.release(m)
@@ -414,6 +449,7 @@ class UNetCompiler:
                 if b.kind == "up":
                     tgt_rows = rows[lvl - 1]
                     out = final_out if (last and final_out is not None) else arena.alloc(tgt_rows, b.cout)
+                    mask(cur, lvl, TAG_UPDOWN)
                     emit_upsample_conv(ops, self.blob, self.w, b.prefix, cur, out, lens[lvl], b.cin, b.cout, TAG_UPDOWN)
                     lvl -= 1
                     cur = out
@@ -429,6 +465,12 @@ class UNetCompiler:
                     raise ValueError(b.kind)
                 cur = out
             return cur, lvl
+
+        # ---- a ragged plan starts with x and the audio slots zeroed past each sample's length (conv_in reads them) -------
+        if ragged:
+            mask(xin, 0, TAG_IO)
+            for l, view in audio_slots:
+                mask(view, l, TAG_IO)
 
         # ---- input blocks --------------------------------------------------------------------
         k = 0            # skip push counter
@@ -448,6 +490,7 @@ class UNetCompiler:
                 h = dst
             elif b0.kind == "down":
                 dst = down_cat[lvl + 1].c(0, b0.cout)
+                mask(h, lvl, TAG_UPDOWN)
                 gemm(h, self.w(b0.prefix + "conv.weight"), b0.cout, b0.cin, dst, bias=self.w(b0.prefix + "conv.bias"),
                      taps=3, mode=L_.CONV_DOWN, Lin=lens[lvl], Lout=lens[lvl + 1], tag=TAG_UPDOWN)
                 copy(dst, skip_home[k], TAG_UPDOWN)
@@ -504,11 +547,15 @@ class DecoderCompiler:
     def w(self, name: str) -> int:
         return self.wbase + 4 * self.blob.offset(name)
 
-    def compile(self, arena: Arena, B: int, Lz: int) -> dict:
+    def compile(self, arena: Arena, B: int, Lz: int, valid: Optional[Dict[int, int]] = None) -> dict:
         """ops for B samples; a block of length multiplier ``mul`` runs on Lz * mul rows per sample.  Returns the input rows
-        (``inp``: [B * Lz * mul_first, cin_first]), the output rows (``out``) and their length per sample (``Lout``)."""
+        (``inp``: [B * Lz * mul_first, cin_first]), the output rows (``out``) and their length per sample (``Lout``).
+        valid: a ragged plan (see UNetCompiler.compile): {mul: device address of an int32 [B] array holding mul * L_b} for every
+        multiplier the blocks use.  GroupNorms take their _VAR op, the input and every Upsample / Downsample input are masked, and
+        so is the output, which is then 0 past each sample's length.  None = today's op list."""
         cfg = self.cfg
-        ops = OpList(self.tc_map)
+        ops = OpList(self.tc_map, None if valid is None else {Lz * m: int(p) for m, p in valid.items()})
+        ragged = valid is not None
         G = cfg.num_groups
         first = self.seq[0]
         inp = arena.alloc(B * Lz * first.mul, first.cin)
@@ -517,6 +564,8 @@ class DecoderCompiler:
         for b in self.seq:
             Lr = Lz * b.mul
             p = b.prefix
+            if ragged and b.kind in ("dec_conv_in", "up", "down"):
+                ops.row_mask(cur, B, Lr, TAG_IO if b.kind == "dec_conv_in" else TAG_UPDOWN)
             if b.kind == "dec_conv_in":
                 o = arena.alloc(B * Lr, b.cout)
                 ops.gemm(cur, self.w(p + "weight"), b.cout, b.cin, o, bias=self.w(p + "bias"), taps=3, mode=L_.CONV_SAME,
@@ -542,6 +591,8 @@ class DecoderCompiler:
                 out_view = arena.alloc(B * Lr, b.cout)
                 ops.gemm(t, self.w(p + "conv_out.weight"), b.cout, b.cin, out_view, bias=self.w(p + "conv_out.bias"), taps=3,
                          mode=L_.CONV_SAME, Lin=Lr, Lout=Lr, tag=TAG_IO)
+                if ragged:
+                    ops.row_mask(out_view, B, Lr, TAG_IO)
             else:
                 raise ValueError(b.kind)
         return dict(ops=ops, inp=inp, out=out_view, Lout=Lz * self.seq[-1].mul)

@@ -268,9 +268,13 @@ class MugEngine:
             cache.move_to_end(key)
         return s
 
-    def session(self, Beff: int, Lz: int, per_sample_t: bool = False) -> "Session":
+    def session(self, Beff: int, Lz: int, per_sample_t: bool = False, ragged: bool = False) -> "Session":
+        """the compiled U-Net of (Beff, Lz).  ``ragged``: the plan for samples padded to Lz whose valid lengths are set per request
+        (Session.set_lengths); a separate session, so requests without lengths keep today's plan."""
         check_z_length(Lz)
-        return self._lru_get(self.sessions, (Beff, Lz, per_sample_t), lambda: Session(self, Beff, Lz, per_sample_t))
+        if not ragged:
+            return self._lru_get(self.sessions, (Beff, Lz, per_sample_t), lambda: Session(self, Beff, Lz, per_sample_t))
+        return self._lru_get(self.sessions, (Beff, Lz, per_sample_t, "ragged"), lambda: Session(self, Beff, Lz, per_sample_t, ragged=True))
 
     def wave_session(self, B: int, T: int):
         """Audio encoder plan for B mel-spectrograms of T frames (SURVEY §8f N1); needs wave weights in the blob."""
@@ -279,9 +283,11 @@ class MugEngine:
         from .wave import WaveSession
         return self._lru_get(self.dec_sessions, ("wave", B, T), lambda: WaveSession(self, B, T))
 
-    def decoder_session(self, B: int, Lz: int) -> "DecoderSession":
+    def decoder_session(self, B: int, Lz: int, ragged: bool = False) -> "DecoderSession":
         check_z_length(Lz)
-        return self._lru_get(self.dec_sessions, (B, Lz), lambda: DecoderSession(self, B, Lz))
+        if not ragged:
+            return self._lru_get(self.dec_sessions, (B, Lz), lambda: DecoderSession(self, B, Lz))
+        return self._lru_get(self.dec_sessions, (B, Lz, "ragged"), lambda: DecoderSession(self, B, Lz, ragged=True))
 
     @property
     def encoder_cfg(self) -> EncoderConfig:
@@ -307,10 +313,13 @@ class MugEngine:
 class Session:
     """Compiled U-Net evaluation for Beff samples of length Lz (Beff = 2B under classifier-free guidance)."""
 
-    def __init__(self, engine: MugEngine, Beff: int, Lz: int, per_sample_t: bool):
+    def __init__(self, engine: MugEngine, Beff: int, Lz: int, per_sample_t: bool, ragged: bool = False):
         self.engine, self.Beff, self.Lz, self.per_sample_t = engine, Beff, Lz, per_sample_t
         cfg = engine.cfg.unet
         dev = engine.device
+        # ragged: valid rows of each sample at every level ([levels, Beff] int32, row l = L_b >> l), data of the captured graph
+        self.valid = torch.tensor([[Lz >> l] * Beff for l in range(cfg.levels)], dtype=torch.int32, device=dev) if ragged else None
+        self.lens: Optional[List[int]] = None
         self.comp = UNetCompiler(cfg, engine.blob, engine.wbase, engine.tc_map)
         emb_total = engine.blob.meta["emb_total"]
         attn_blocks = [b for b in self.comp.lay.blocks() if b.kind == "attn"]
@@ -379,8 +388,9 @@ class Session:
         # the LayerNorm fold lives in the tensor-core GEMM epilogues; the exact-fp32 FFMA path keeps the stand-alone LayerNorm
         # kernels and doubles as the referee of the folded plan.  engine.fold_ln: None = by size, True / False = forced (A/B, tests)
         fold = False if self.engine.gemm_impl == "simt" else self.engine.fold_ln
+        valid = None if self.valid is None else [_ptr(self.valid[l]) for l in range(self.valid.shape[0])]
         self.arena_t, res, self.plan = compile_sized(self.engine, lambda arena: self.comp.compile(
-            arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold))
+            arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold, valid))
         self.xin: View = res["xin"]
         self.eps: View = res["eps"]
         self.audio_slots = res["audio_slots"]
@@ -393,6 +403,16 @@ class Session:
             self._build()
 
     # ---- per-request preparation ---------------------------------------------------------------
+    def set_lengths(self, lens: Sequence[int]):
+        """a ragged session's valid length of each of its Beff samples (multiples of 32 in [32, Lz]; under classifier-free guidance
+        both halves): written into the device arrays the plan reads, so the captured graph serves any mix"""
+        assert self.valid is not None, "set_lengths needs a ragged session"
+        lens = [int(v) for v in lens]
+        assert len(lens) == self.Beff and all(32 <= v <= self.Lz and v % 32 == 0 for v in lens), lens
+        t = torch.tensor([[v >> l for v in lens] for l in range(self.valid.shape[0])], dtype=torch.int32)
+        self.valid.copy_(t.to(self.engine.device))
+        self.lens = lens
+
     def set_timestep_table(self, timesteps: Sequence[int]):
         """Time-embedding MLP + all ResBlock emb projections for the given timesteps, one row each
         (unet.py:335-339, 166-172; model/util.py:156-176).  The sinusoid is evaluated on the host exactly
@@ -667,10 +687,14 @@ class Session:
 
 
 class DecoderSession:
-    def __init__(self, engine: MugEngine, B: int, Lz: int):
+    def __init__(self, engine: MugEngine, B: int, Lz: int, ragged: bool = False):
         self.engine, self.B, self.Lz = engine, B, Lz
         comp = DecoderCompiler(engine.cfg.decoder, engine.blob, engine.wbase, engine.tc_map)
-        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz))
+        # ragged: valid rows per sample at every length multiplier of the blocks ([n_mul, B] int32, row k = muls[k] * L_b)
+        self.muls = sorted({b.mul for b in comp.seq} | {b.mul * 2 for b in comp.seq if b.kind == "up"}) if ragged else []
+        self.valid = torch.zeros(len(self.muls), B, dtype=torch.int32, device=engine.device) if ragged else None
+        valid = {m: _ptr(self.valid[k]) for k, m in enumerate(self.muls)} if ragged else None
+        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz, valid))
         self.zin, self.logits, self.Lout = res["inp"], res["out"], res["Lout"]
 
     def notes(self, frame_ms: float, key_count: int = 4):
@@ -693,9 +717,19 @@ class DecoderSession:
         nmax = int(cnt_c.max()) if cnt_c.numel() else 0
         return cnt_c, st[:, :, :max(nmax, 1)].cpu(), en[:, :, :max(nmax, 1)].cpu()
 
-    def decode(self, z: torch.Tensor) -> torch.Tensor:
+    def set_lengths(self, lens: Sequence[int]):
+        """a ragged session's latent length of each chart (its logits are valid for mul * L_b rows at multiplier mul)"""
+        assert self.valid is not None and len(lens) == self.B and all(32 <= int(v) <= self.Lz for v in lens), lens
+        t = torch.tensor([[m * int(v) for v in lens] for m in self.muls], dtype=torch.int32)
+        self.valid.copy_(t.to(self.engine.device))
+
+    def decode(self, z: torch.Tensor, lens: Optional[Sequence[int]] = None) -> torch.Tensor:
+        """logits [B, x_channels, Lout] of the latents z [B, z_channels, Lz]; a ragged session takes each chart's length ``lens`` and
+        returns logits that are 0 past Lout / Lz * lens[b]"""
         eng = self.engine
         cfg = eng.cfg.decoder
+        if self.valid is not None:
+            self.set_lengths(lens)
         z = z.to(eng.device, torch.float32)
         if cfg.scale != 1.0:
             z = z / cfg.scale                 # autoencoder.py:76

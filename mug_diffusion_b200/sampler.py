@@ -190,11 +190,16 @@ class _Wrapper:
     __call__ = forward
 
     @torch.no_grad()
-    def decode(self, z: torch.Tensor) -> torch.Tensor:
+    def decode(self, z: torch.Tensor, z_lengths=None) -> torch.Tensor:
+        """the decoder's logits [B, 16, 8L] of z [B, C, L].  ``z_lengths`` (one multiple of 32 in [32, L] per chart): charts of
+        different lengths padded to L, run on the ragged decoder plan; chart b's logits are 0 past 8 * z_lengths[b]."""
         o = self._o
+        B, _, Lz = z.shape
+        lens = ragged_lengths(z_lengths, B, Lz)
         with o.engine.lock:
-            B, _, Lz = z.shape
-            return o.engine.decoder_session(B, Lz).decode(z)
+            if lens is None:
+                return o.engine.decoder_session(B, Lz).decode(z)
+            return o.engine.decoder_session(B, Lz, ragged=True).decode(z, lens)
 
 
     @torch.no_grad()
@@ -287,15 +292,17 @@ class _Wrapper:
             return chartpost.postprocess_charts(o.grid_scanner, o.chart_post, charts, auto_snap, jack_interval)
 
     @torch.no_grad()
-    def decode_to_hit_objects(self, z: torch.Tensor, frame_ms: float, key_count: int = 4):
+    def decode_to_hit_objects(self, z: torch.Tensor, frame_ms: float, key_count: int = 4, z_lengths=None):
         """decode(z) followed by OsuManiaConvertor.array_to_objects (convertor.py:232-264) on the GPU: the [B,16,8L] logits
-        never leave the device, only the compact note lists do.  Returns one list of .osu hit-object lines per chart."""
+        never leave the device, only the compact note lists do.  Returns one list of .osu hit-object lines per chart.
+        ``z_lengths``: as for ``decode``; the zero logits past a chart's length hold no note (a note needs a logit > 0)."""
         from .runtime import hit_object_lines
         o = self._o
+        B, _, Lz = z.shape
+        lens = ragged_lengths(z_lengths, B, Lz)
         with o.engine.lock:
-            B, _, Lz = z.shape
-            ds = o.engine.decoder_session(B, Lz)
-            ds.decode(z)
+            ds = o.engine.decoder_session(B, Lz, ragged=lens is not None)
+            ds.decode(z, lens)
             cnt, st, en = ds.notes(frame_ms, key_count)
             return hit_object_lines(cnt, st, en, key_count)
 
@@ -473,24 +480,28 @@ class _DeviceLoopSampler:
         """the request's start latent: x_T on the device, or drawn from its generator when not given"""
         return torch.randn(shape, device=self.device) if x_T is None else x_T.to(self.device, torch.float32)
 
-    def _seeded(self, seeds, shape) -> Optional[seeding.ChartNoise]:
-        """the request's ChartNoise (its seeds on the device), None when it is not seeded"""
-        return None if seeds is None else seeding.ChartNoise(seeding.chart_seeds(seeds, shape[0]), shape, self.device)
+    def _seeded(self, seeds, shape, lens=None) -> Optional[seeding.ChartNoise]:
+        """the request's ChartNoise (its seeds on the device; ``lens``: a ragged request's chart lengths), None when it is not
+        seeded"""
+        return None if seeds is None else seeding.ChartNoise(seeding.chart_seeds(seeds, shape[0]), shape, self.device, lens)
 
-    def _seeded_start(self, seeds, shape, x_T):
+    def _seeded_start(self, seeds, shape, x_T, lens=None):
         """(ChartNoise or None, x_T): a seeded request without x_T starts from its charts' seeding.X_T draw"""
-        seeded = self._seeded(seeds, shape)
+        seeded = self._seeded(seeds, shape, lens)
         return seeded, (seeded.draw(seeding.X_T, 0) if seeded is not None and x_T is None else x_T)
 
-    def _load_session(self, w, c, shape, x_T, scale, uc, time_range):
+    def _load_session(self, w, c, shape, x_T, scale, uc, time_range, lens=None):
         """x_T (drawn when not given), whether classifier-free guidance is on, and the session of this shape with the timestep table
-        (row i = time_range[i], the i-th loop iteration), context, audio and x loaded, its step counter at 0."""
+        (row i = time_range[i], the i-th loop iteration), context, audio and x loaded, its step counter at 0.  ``lens``: a ragged
+        request (ragged_lengths), run on the ragged session of this shape with the charts' lengths set."""
         model = self.model
         B, Cz, Lz = shape
         x = self._x_T(shape, x_T)
         cfg_on = not (uc is None or scale == 1.)
         Beff = 2 * B if cfg_on else B
-        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False)
+        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False, ragged=lens is not None)
+        if lens is not None:
+            sess.set_lengths(list(lens) * 2 if cfg_on else lens)
         sess.set_timestep_table(time_range.copy())
         # ddim.py:170-174 concatenates [uc, c] and [w, w]; here the two halves are written straight into their rows
         sess.set_context([uc, c] if cfg_on else c)
@@ -505,13 +516,21 @@ class _DeviceLoopSampler:
         cls = (tqdm_class if tqdm_class is not None else _tqdm) if progress else None
         return iterable if cls is None else cls(iterable, desc=desc, total=total)
 
+    @staticmethod
+    def _zero_tails(x: torch.Tensor, sess: Session) -> torch.Tensor:
+        """a ragged session's [B, C, L] result with every chart's positions past its length set to 0 (in place)"""
+        for b, Lb in enumerate((getattr(sess, "lens", None) or [])[:x.shape[0]]):
+            x[b, :, Lb:] = 0.
+        return x
+
     def _read_x(self, sess: Session, shape) -> torch.Tensor:
         B, Cz, Lz = shape
-        return sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz)
+        return self._zero_tails(sess.read_rows(sess.xin.r(0, B * Lz), B, Cz, Lz), sess)
 
-    def _read_pred(self, pred: torch.Tensor, shape) -> torch.Tensor:
+    def _read_pred(self, pred: torch.Tensor, shape, sess: Optional[Session] = None) -> torch.Tensor:
         B, Cz, Lz = shape
-        return self.model.engine.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
+        x = self.model.engine.rows_to_ncl(View(_ptr(pred), Cz, B * Lz, Cz), B, Cz, Lz)
+        return x if sess is None else self._zero_tails(x, sess)
 
     def _run_request(self, sess: Session, x, shape, pred, time_range, total, log_every_t, desc, tqdm_class, progress, callback,
                      img_callback, device_loop, launch, step, tail_launches, chunk=None):
@@ -523,11 +542,13 @@ class _DeviceLoopSampler:
         Otherwise ``step(i, t)`` runs step i at time_range[i], followed by ``callback(i)`` and ``img_callback(pred, i)``.
         ``tail_launches``: the launches each step adds to the U-Net plan's (``last_launches_per_step``)."""
         iterator = self._progress(time_range, desc, total, tqdm_class, progress)
+        if getattr(sess, "lens", None) is not None:
+            x = self._zero_tails(x.clone(), sess)
         intermediates = {'x_inter': [x], 'pred_x0': [x]}
 
         def record():
             intermediates['x_inter'].append(self._read_x(sess, shape))
-            intermediates['pred_x0'].append(self._read_pred(pred, shape))
+            intermediates['pred_x0'].append(self._read_pred(pred, shape, sess))
 
         def logged(i):
             index = total - i - 1
@@ -557,7 +578,7 @@ class _DeviceLoopSampler:
                 if callback:
                     callback(i)
                 if img_callback:
-                    img_callback(self._read_pred(pred, shape), i)
+                    img_callback(self._read_pred(pred, shape, sess), i)
                 if logged(i):
                     record()
         self.last_launches_per_step = sess.plan.launches + tail_launches
@@ -727,6 +748,54 @@ def _request_seeds(seeds, B: int, noise_dropout=0., match_reference_rng=False) -
     return seeding.chart_seeds(seeds, B)
 
 
+def ragged_lengths(z_lengths, B: int, Lz: int) -> Optional[list]:
+    """the checked per-chart latent lengths of a ragged request of B charts padded to Lz (``z_lengths``: one multiple of 32 in
+    [32, Lz] per chart), None when there are none or every chart is Lz long (today's path: same session, plan and bits).
+    MugdError for malformed lengths."""
+    if z_lengths is None:
+        return None
+    if isinstance(z_lengths, (np.ndarray, torch.Tensor)):
+        z_lengths = z_lengths.tolist()
+    if not isinstance(z_lengths, (list, tuple)):
+        raise L_.MugdError(f"z_lengths={z_lengths!r} must hold one length per chart")
+    if len(z_lengths) != B:
+        raise L_.MugdError(f"z_lengths has {len(z_lengths)} entries for {B} charts")
+    out = []
+    for v in z_lengths:
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or int(v) % 32 or not 32 <= int(v) <= Lz:
+            raise L_.MugdError(f"z_lengths={list(z_lengths)!r}: every length must be a multiple of 32 in [32, {Lz}] "
+                               f"(the request's padded length)")
+        out.append(int(v))
+    return None if all(v == Lz for v in out) else out
+
+
+def _ragged_request(z_lengths, shape, mask=None, x0=None, noise_dropout=0., match_reference_rng=False, seeds=None) -> Optional[list]:
+    """ragged_lengths of a sampling request, with the flows a ragged request cannot take refused (MugdError) before any GPU work:
+    inpainting (its chart encoder and blend are not ragged), noise dropout and the reference's generator order (a ragged request
+    draws each chart at its own length, which neither reproduces)"""
+    lens = ragged_lengths(z_lengths, shape[0], shape[2])
+    if z_lengths is None:
+        return lens
+    if mask is not None or x0 is not None:
+        raise L_.MugdError("z_lengths: inpainting (mask / x0) is not supported for charts of different lengths")
+    if noise_dropout > 0.:
+        raise L_.MugdError(f"z_lengths: noise_dropout={noise_dropout!r} is not supported for charts of different lengths")
+    if match_reference_rng and seeds is None:
+        raise L_.MugdError("z_lengths: match_reference_rng=True is not supported for charts of different lengths")
+    return lens
+
+
+def _ragged_kw(lens) -> dict:
+    """the lens= keyword of _load_session / _load_request for a ragged request; none for a plain one, whose calls stay as they were"""
+    return {} if lens is None else dict(lens=lens)
+
+
+def _refuse_ragged(z_lengths, what: str):
+    """MugdError for z_lengths on a flow that starts from an existing chart (it would need a ragged chart encoder)"""
+    if z_lengths is not None:
+        raise L_.MugdError(f"z_lengths: {what} is not supported for charts of different lengths; group the charts by length")
+
+
 def _conditioning(c, conditioning):
     """``c``, which may also be given as the reference's ``conditioning``"""
     if conditioning is None:
@@ -779,7 +848,7 @@ class DDIMSampler(_DeviceLoopSampler):
     @torch.no_grad()
     def sample(self, S, c, w, batch_size, shape=None, callback=None, img_callback=None, eta=0., mask=None, x0=None,
                temperature=1., noise_dropout=0., verbose=True, x_T=None, log_every_t=100,
-               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, seeds=None, **kwargs):
+               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, seeds=None, z_lengths=None, **kwargs):
         if c is not None and not isinstance(c, dict) and c.shape[0] != batch_size:
             print(f"Warning: Got {c.shape[0]} conditionings but batch-size is {batch_size}")
         self.make_schedule(ddim_num_steps=S, ddim_eta=eta, verbose=verbose)
@@ -793,7 +862,8 @@ class DDIMSampler(_DeviceLoopSampler):
                                   noise_dropout=noise_dropout, temperature=temperature, x_T=x_T, log_every_t=log_every_t,
                                   unconditional_guidance_scale=unconditional_guidance_scale,
                                   unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class,
-                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)), seeds=seeds)
+                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)), seeds=seeds,
+                                  z_lengths=z_lengths)
 
     def _schedule_subset(self, timesteps, ddim_use_original_steps) -> np.ndarray:
         """the DDIM timesteps a request runs: all of make_schedule's, or ddim_timesteps[:ddim_subset_end(k, n)] for timesteps=k
@@ -808,46 +878,56 @@ class DDIMSampler(_DeviceLoopSampler):
             raise ValueError(f"timesteps={timesteps!r} must be a finite number")
         return self.ddim_timesteps[:ddim_subset_end(timesteps, self.ddim_timesteps.shape[0])]
 
-    def _load_request(self, w, c, shape, x_T, scale, uc, timesteps=None):
+    def _load_request(self, w, c, shape, x_T, scale, uc, timesteps=None, lens=None):
         """Once per request, all DDIM-schedule samplers: _load_session over the DDIM timesteps (or the prefix ``timesteps`` of them),
         with the coefficient rows of make_schedule (a request of n steps reads rows n - 1 .. 0, the prefix's).
         Returns (x, cfg_on, session, time_range)."""
         ts = self.ddim_timesteps if timesteps is None else timesteps
-        x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, uc, np.flip(ts))
+        x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, uc, np.flip(ts), **_ragged_kw(lens))
         sess.set_ddim_schedule(self.ddim_alphas, self.ddim_alphas_prev, self.ddim_sigmas, self.ddim_sqrt_one_minus_alphas)
         return x, cfg_on, sess, time_range
 
-    def _empty_request(self, shape, x_T):
-        """the result of a request whose timestep subset is empty: x_T (drawn when not given), which is also both intermediate lists"""
+    def _empty_request(self, shape, x_T, lens=None):
+        """the result of a request whose timestep subset is empty: x_T (drawn when not given), which is also both intermediate lists
+        (0 past each chart's length for a ragged request)"""
         x = self._x_T(shape, x_T)
+        if lens is not None:
+            x = x.clone()
+            for b, Lb in enumerate(lens):
+                x[b, :, Lb:] = 0.
         return x, {'x_inter': [x], 'pred_x0': [x]}
 
     @torch.no_grad()
     def ddim_sampling(self, w, c, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None, mask=None, x0=None,
                       img_callback=None, log_every_t=100, temperature=1., noise_dropout=0., unconditional_guidance_scale=1.,
-                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False, seeds=None):
+                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False, seeds=None,
+                      z_lengths=None):
         """ddim.py:110-159 on the GPU.  ``timesteps=k`` runs the reference's truncated schedule, the last, low-noise
         ddim_timesteps[:ddim_subset_end(k, n)] from x_T; when that is empty, x_T comes back with both intermediate lists [x_T].
         ``ddim_use_original_steps=True`` raises ValueError before any GPU work (see ORIGINAL_STEPS).
         ``seeds`` (seeding.chart_seeds: an int s for charts s, s + 1, ..., or one per chart): every random number comes from the
         charts' seeds, x_T (unless given), the step noise and the inpainting noise of schedule row r from draw r, and torch's
-        generator is left untouched; noise_dropout and match_reference_rng are refused with it."""
+        generator is left untouched; noise_dropout and match_reference_rng are refused with it.
+        ``z_lengths`` (one multiple of 32 in [32, L] per chart): charts of different lengths padded to L = shape[2], chart b equal to
+        the chart requested alone at z_length z_lengths[b] (with seeds, the same seed), its result 0 past that length; inpainting,
+        noise_dropout and match_reference_rng without seeds are refused with it (MugdError)."""
         B, Cz, Lz = shape
         seeds = _request_seeds(seeds, B, noise_dropout, match_reference_rng)
+        lens = _ragged_request(z_lengths, shape, mask, x0, noise_dropout, match_reference_rng, seeds)
         model = self.model
         eng = model.engine
         dev = self.device
         ts = self._schedule_subset(timesteps, ddim_use_original_steps)
         if ts.shape[0] == 0:
-            return self._empty_request(shape, self._seeded_start(seeds, shape, x_T)[1])
+            return self._empty_request(shape, self._seeded_start(seeds, shape, x_T, lens)[1], lens)
         # the reference draws (and, with noise_dropout, masks) noise every step even when sigma == 0 (ddim.py:192-194); the
         # draw is skipped here unless it can change the result or the caller asks for the same global-RNG consumption
         has_noise = bool(np.any(np.asarray(self.ddim_sigmas) != 0))
         blend, draw = mask is not None, has_noise or bool(match_reference_rng)
         with eng.lock:
-            seeded, x_T = self._seeded_start(seeds, shape, x_T)
+            seeded, x_T = self._seeded_start(seeds, shape, x_T, lens)
             x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, unconditional_guidance_scale, unconditional_conditioning,
-                                                             ts)
+                                                             ts, **_ragged_kw(lens))
             total = time_range.shape[0]
             # pred_x0 and the noise of a step: channels-last rows [B*Lz, Cz]
             pred = torch.empty(B * Lz, Cz, device=dev)
@@ -917,14 +997,15 @@ class DDIMSampler(_DeviceLoopSampler):
             raise ValueError(f"{what} needs the DDIM schedule: call make_schedule(S) first")
 
     @torch.no_grad()
-    def stochastic_encode(self, x0, t, use_original_steps=False, noise=None, seeds=None):
+    def stochastic_encode(self, x0, t, use_original_steps=False, noise=None, seeds=None, z_lengths=None):
         """Noise the latent ``x0`` [B, C, L] to DDIM index ``t[b]`` per chart: sqrt(ddim_alphas)[t] * x0 + ddim_sqrt_one_minus_alphas[t]
         * noise (Stable Diffusion's formulation), with noise = torch.randn_like(x0) when not given (the generator ends where randn_like
         leaves it), or chart b's seeding.ENCODE draw with ``seeds`` (one int for charts s, s + 1, ..., or one per chart).  ``t``: a [B]
         integer tensor (or sequence) of indices into make_schedule's tables; ``use_original_steps=True``
         indexes the model's sqrt_alphas_cumprod / sqrt_one_minus_alphas_cumprod instead.  One kernel, bit-identical to those torch
         expressions on CUDA (the square root is torch's).  ValueError, before any GPU work, for malformed arguments and indices
-        outside the table."""
+        outside the table; MugdError for ``z_lengths`` (not supported here)."""
+        _refuse_ragged(z_lengths, "stochastic_encode")
         model = self.model
         dev = self.device
         if not use_original_steps:
@@ -954,7 +1035,7 @@ class DDIMSampler(_DeviceLoopSampler):
 
     @torch.no_grad()
     def decode(self, x_latent, c, w, t_start, unconditional_guidance_scale=1., unconditional_conditioning=None,
-               use_original_steps=False, tqdm_class=None):
+               use_original_steps=False, tqdm_class=None, z_lengths=None):
         """Stable Diffusion's DDIMSampler.decode with Mug's (c, w) conditioning: denoise ``x_latent`` [B, C, L] (e.g. from
         stochastic_encode) over ddim_timesteps[:t_start] flipped, at index = t_start - i - 1 and eta = 0, and return the final latent.
         With a scalar t_start = s it equals ddim_sampling(w, c, shape, x_T=x_latent, timesteps=s + 1) wherever that subset has s steps;
@@ -962,7 +1043,9 @@ class DDIMSampler(_DeviceLoopSampler):
         iterations in which chart b joins at iteration m - t_start[b] from x_latent[b] (a join kernel holds its rows until then) and
         then follows the coefficient rows of its own scalar run; a chart with t_start[b] = 0 comes back as x_latent[b].  Charts with a
         smaller start still occupy their batch rows for all m iterations: group charts by strength into separate calls to avoid the
-        idle rows.  Every argument is checked before any GPU work (ValueError): the schedule must be make_schedule's at eta = 0."""
+        idle rows.  Every argument is checked before any GPU work (ValueError): the schedule must be make_schedule's at eta = 0.
+        ``z_lengths`` is refused (MugdError)."""
+        _refuse_ragged(z_lengths, "decode(x_latent, ...)")
         model = self.model
         eng = model.engine
         dev = self.device
@@ -1005,7 +1088,7 @@ class DDIMSampler(_DeviceLoopSampler):
     # ---- inverting an existing chart to its noise (DDIM inversion) -------------------------------------------------------------------
     @torch.no_grad()
     def invert(self, x0, c, w, t_enc, unconditional_guidance_scale=1., unconditional_conditioning=None, callback=None, img_callback=None,
-               log_every_t=100, tqdm_class=None, verbose=True, **kwargs):
+               log_every_t=100, tqdm_class=None, verbose=True, z_lengths=None, **kwargs):
         """DDIM inversion: run the latent ``x0`` [B, C, z_length] of a chart backwards along DDIM's deterministic (eta = 0) update,
         t_enc[b] steps for chart b (``t_enc``: an integer in [0, n], n = len(ddim_timesteps), or one per chart), so that chart b ends
         at timestep ddim_timesteps[t_enc[b] - 1], where ``decode(z, c, w, t_start=t_enc)`` starts it.  Decoding with the same (c, w)
@@ -1013,7 +1096,9 @@ class DDIMSampler(_DeviceLoopSampler):
         It is DPMSolverSampler.invert of order 1 on DDIM's grid (``dpm_solver.ddim_grid``), the same kernels and bits; step j
         evaluates the U-Net at timestep 0 (j = 0) or ddim_timesteps[j - 1].  Draws no random numbers.  Returns z;
         ``last_intermediates`` holds {'x_inter', 'pred_x0'} logged as by ``sample``.  Every argument is checked before any GPU work
-        (ValueError): the schedule must be make_schedule's at eta = 0; mask, eta, temperature and noise dropout are refused."""
+        (ValueError): the schedule must be make_schedule's at eta = 0; mask, eta, temperature and noise dropout are refused, and
+        z_lengths (MugdError)."""
+        _refuse_ragged(z_lengths, "invert")
         self._require_schedule("invert")
         if np.any(np.asarray(self.ddim_sigmas) != 0):
             raise ValueError("invert runs at eta = 0: call make_schedule(S, ddim_eta=0.)")
@@ -1073,7 +1158,7 @@ class PLMSSampler(DDIMSampler):
     @torch.no_grad()
     def sample(self, S, c=None, w=None, batch_size=None, shape=None, callback=None, img_callback=None, eta=0., mask=None, x0=None,
                temperature=1., noise_dropout=0., verbose=True, x_T=None, log_every_t=100, unconditional_guidance_scale=1.,
-               unconditional_conditioning=None, tqdm_class=None, conditioning=None, seeds=None, **kwargs):
+               unconditional_conditioning=None, tqdm_class=None, conditioning=None, seeds=None, z_lengths=None, **kwargs):
         """The call scripts/mapping.py:476-483 makes (``c`` may also be given as the reference's ``conditioning``).  Returns
         ``(samples, {'x_inter', 'pred_x0'})`` with plms.py:134,166-168's logging rule.  Every argument is checked before any GPU
         work.  Requests without callback / img_callback / mask run from mugd_sample_plms calls, one per stretch between two recorded
@@ -1093,7 +1178,8 @@ class PLMSSampler(DDIMSampler):
                                   log_every_t=log_every_t, noise_dropout=noise_dropout,
                                   unconditional_guidance_scale=unconditional_guidance_scale,
                                   unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class,
-                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)), seeds=seeds)
+                                  match_reference_rng=bool(kwargs.get("match_reference_rng", False)), seeds=seeds,
+                                  z_lengths=z_lengths)
 
     def _check_request(self, S, c, w, batch_size, shape, x_T, mask, x0, scale, uc, log_every_t):
         """the request's [B, C, L] shape; ValueError / TypeError for what the device path cannot take"""
@@ -1110,17 +1196,19 @@ class PLMSSampler(DDIMSampler):
     @torch.no_grad()
     def plms_sampling(self, w, c, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None, mask=None, x0=None,
                       img_callback=None, log_every_t=100, noise_dropout=0., unconditional_guidance_scale=1.,
-                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False, seeds=None):
+                      unconditional_conditioning=None, tqdm_class=None, progress=True, match_reference_rng=False, seeds=None,
+                      z_lengths=None):
         """plms.py:115-170 (and p_sample_plms, :172-236) on the GPU.  ``timesteps=k`` runs the truncated schedule of plms.py:128-136
-        (t_next and the warm-up follow it); ``ddim_use_original_steps=True`` raises as in ddim_sampling."""
+        (t_next and the warm-up follow it); ``ddim_use_original_steps=True`` raises as in ddim_sampling; ``z_lengths`` as there."""
         B, Cz, Lz = shape
         seeds = _request_seeds(seeds, B, noise_dropout, match_reference_rng)
+        lens = _ragged_request(z_lengths, shape, mask, x0, noise_dropout, match_reference_rng, seeds)
         model = self.model
         eng = model.engine
         dev = self.device
         ts = self._schedule_subset(timesteps, ddim_use_original_steps)
         if ts.shape[0] == 0:
-            return self._empty_request(shape, self._seeded_start(seeds, shape, x_T)[1])
+            return self._empty_request(shape, self._seeded_start(seeds, shape, x_T, lens)[1], lens)
         match_rng = bool(match_reference_rng)
         scale = unconditional_guidance_scale
 
@@ -1130,8 +1218,8 @@ class PLMSSampler(DDIMSampler):
                 draw_step_noise(k, shape, None, None, True, None, noise_dropout, dev)
 
         with eng.lock:
-            seeded, x_T = self._seeded_start(seeds, shape, x_T)
-            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, scale, unconditional_conditioning, ts)
+            seeded, x_T = self._seeded_start(seeds, shape, x_T, lens)
+            x, cfg_on, sess, time_range = self._load_request(w, c, shape, x_T, scale, unconditional_conditioning, ts, **_ragged_kw(lens))
             total = time_range.shape[0]
             pred = torch.empty(B * Lz, Cz, device=dev)
             work = torch.empty(5, B * Lz * Cz, device=dev)                    # e', the e_t ring [3], the x stash
@@ -1188,7 +1276,8 @@ class DDPMSampler(_DeviceLoopSampler):
 
     @torch.no_grad()
     def sample(self, c, w, batch_size, shape=None, x_T=None, callback=None, img_callback=None, log_every_t=100, clip_denoised=None,
-               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True, seeds=None, **kwargs):
+               unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True, seeds=None, z_lengths=None,
+               **kwargs):
         """``T = model.num_timesteps`` ancestral steps for ``batch_size`` latents of ``shape`` = (channels, length) (default the
         model's).  ``clip_denoised=None`` takes the model's.  Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then the x and
         x_recon of every step whose timestep i has ``i % log_every_t == 0 or i == T - 1`` (diffusion.py:279).  Every argument is
@@ -1210,25 +1299,31 @@ class DDPMSampler(_DeviceLoopSampler):
         scale = _finite_scale(unconditional_guidance_scale)
         size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
         seeds = _request_seeds(seeds, size[0])
+        _ragged_request(z_lengths, size)
         if verbose:
             print(f'Data shape for DDPM sampling is {size}, {T} steps')
         return self.ddpm_sampling(w, c, size, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
                                   clip_denoised=bool(clip), unconditional_guidance_scale=scale,
-                                  unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class, seeds=seeds)
+                                  unconditional_conditioning=unconditional_conditioning, tqdm_class=tqdm_class, seeds=seeds,
+                                  z_lengths=z_lengths)
 
     @torch.no_grad()
     def ddpm_sampling(self, w, c, shape, x_T=None, callback=None, img_callback=None, log_every_t=100, clip_denoised=True,
-                      unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, seeds=None):
-        """diffusion.py:234-282 on the GPU; ``seeds``: checked per-chart seeds (step i draws timestep T - 1 - i)."""
+                      unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, seeds=None,
+                      z_lengths=None):
+        """diffusion.py:234-282 on the GPU; ``seeds``: checked per-chart seeds (step i draws timestep T - 1 - i); ``z_lengths`` as in
+        DDIMSampler.ddim_sampling."""
         model = self.model
         eng = model.engine
         dev = self.device
         B, Cz, Lz = shape
+        lens = _ragged_request(z_lengths, shape)
         T = self.ddpm_num_timesteps
         scale = unconditional_guidance_scale
         with eng.lock:
-            seeded, x_T = self._seeded_start(seeds, shape, x_T)
-            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, np.arange(T)[::-1])
+            seeded, x_T = self._seeded_start(seeds, shape, x_T, lens)
+            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, np.arange(T)[::-1],
+                                                             **_ragged_kw(lens))
             coef = model.ddpm_coef_table()
             pred = torch.empty(B * Lz, Cz, device=dev)
             per_call = max(1, STAGE_TABLE_BYTES // (4 * B * Cz * Lz))
@@ -1303,7 +1398,7 @@ class DPMSolverSampler(_DeviceLoopSampler):
     def sample(self, S, c=None, w=None, batch_size=None, shape=None, x_T=None, order=2, skip_type="time_uniform",
                solver_type="dpmsolver", lower_order_final=True, callback=None, img_callback=None, log_every_t=100,
                unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True, conditioning=None,
-               seeds=None, **kwargs):
+               seeds=None, z_lengths=None, **kwargs):
         """S steps of DPM-Solver++ multistep of ``order`` from x_T (drawn when not given) to t = 1/N; ``c`` may also be given as
         ``conditioning``.  Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then x and the data prediction m of every step i with
         ``(S - i - 1) % log_every_t == 0`` or i = 0 (DDIM's rule).  Every argument is checked before any GPU work (ValueError; TypeError
@@ -1315,11 +1410,12 @@ class DPMSolverSampler(_DeviceLoopSampler):
         scale, sched, size = self._check_request(S, c, w, batch_size, shape, x_T, None, None, order, skip_type, solver_type,
                                                  lower_order_final, log_every_t, unconditional_guidance_scale, unconditional_conditioning)
         seeds = _request_seeds(seeds, size[0])
+        _ragged_request(z_lengths, size)
         if verbose:
             print(f'Data shape for DPM-Solver++ sampling is {size}, {S} steps of order {order} ({skip_type}, {solver_type})')
         return self.dpm_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
                                  unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
-                                 tqdm_class=tqdm_class, seeds=seeds)
+                                 tqdm_class=tqdm_class, seeds=seeds, z_lengths=z_lengths)
 
     @torch.no_grad()
     def inpaint(self, S, c=None, w=None, batch_size=None, mask=None, x0=None, shape=None, x_T=None, order=2, skip_type="time_uniform", solver_type="dpmsolver",
@@ -1349,9 +1445,10 @@ class DPMSolverSampler(_DeviceLoopSampler):
     @torch.no_grad()
     def dpm_sampling(self, w, c, shape, sched: dpm_solver.DPMSchedule, x_T=None, callback=None, img_callback=None, log_every_t=100,
                      unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, mask=None, x0=None,
-                     seeds=None):
+                     seeds=None, z_lengths=None):
         """the request of ``sched`` (make_dpm_schedule) on the GPU; with ``mask`` / ``x0`` the inpainting of ``inpaint``; ``seeds``:
-        checked per-chart seeds"""
+        checked per-chart seeds; ``z_lengths`` as in DDIMSampler.ddim_sampling"""
+        lens = _ragged_request(z_lengths, shape, mask, x0)
         model = self.model
         eng = model.engine
         dev = self.device
@@ -1361,8 +1458,9 @@ class DPMSolverSampler(_DeviceLoopSampler):
         blend = mask is not None
         self.last_schedule = sched
         with eng.lock:
-            seeded, x_T = self._seeded_start(seeds, shape, x_T)
-            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times)
+            seeded, x_T = self._seeded_start(seeds, shape, x_T, lens)
+            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times,
+                                                             **_ragged_kw(lens))
             coef = torch.from_numpy(sched.rows_f32()).to(dev)
             ring = torch.empty(3, B * Lz * Cz, device=dev)                     # the data predictions of the last three steps
             pred = torch.empty(B * Lz, Cz, device=dev)
@@ -1416,13 +1514,14 @@ class DPMSolverSampler(_DeviceLoopSampler):
             raise ValueError("sched must be a DPMSchedule from make_dpm_schedule")
 
     @torch.no_grad()
-    def stochastic_encode(self, x0, t_enc, sched: dpm_solver.DPMSchedule, noise=None, seeds=None):
+    def stochastic_encode(self, x0, t_enc, sched: dpm_solver.DPMSchedule, noise=None, seeds=None, z_lengths=None):
         """Noise the latent ``x0`` [B, C, L] for a remix over the last ``t_enc[b]`` steps of ``sched`` (an integer in [0, S], or one per
         chart): alpha(t_S-s) * x0 + sigma(t_S-s) * noise with s = t_enc[b], the marginal at the time where ``decode`` with t_start = s
         starts (no off-by-one, unlike DDIM's stochastic_encode / decode pair); s = 0 returns x0 exactly.  noise = torch.randn_like(x0)
         when not given, chart b's seeding.ENCODE draw with ``seeds``.  One kernel (mugd_stochastic_encode over the schedule's float32
         tables of S + 1 rows).  ValueError, before any
-        GPU work, for malformed arguments."""
+        GPU work, for malformed arguments; MugdError for ``z_lengths``."""
+        _refuse_ragged(z_lengths, "stochastic_encode")
         self._require_schedule(sched)
         return self._stochastic_encode(x0, noise, lambda B: per_chart_steps(B, t_enc, sched.S, "t_enc", " (S = sched.S)"),
                                        lambda: [torch.from_numpy(v).to(self.device) for v in sched.encode_tables_f32()], sched.S + 1,
@@ -1430,7 +1529,7 @@ class DPMSolverSampler(_DeviceLoopSampler):
 
     @torch.no_grad()
     def invert(self, x0, c, w, t_enc, sched: dpm_solver.DPMSchedule, unconditional_guidance_scale=1., unconditional_conditioning=None,
-               callback=None, img_callback=None, log_every_t=100, tqdm_class=None, verbose=True, **kwargs):
+               callback=None, img_callback=None, log_every_t=100, tqdm_class=None, verbose=True, z_lengths=None, **kwargs):
         """Deterministic inversion: run the latent ``x0`` [B, C, z_length] of a chart backwards along the probability-flow ODE of
         ``sched`` (make_dpm_schedule), with the U-Net in the loop, t_enc[b] steps for chart b (``t_enc``: an integer in [0, S], or
         one per chart).  Step j goes from t_S-j to t_S-j-1 at order min(j + 1, order) (``dpm_solver.inversion_schedule``), so chart b
@@ -1441,14 +1540,15 @@ class DPMSolverSampler(_DeviceLoopSampler):
         Draws no random numbers.  Returns z; ``last_intermediates`` holds {'x_inter', 'pred_x0'} logged as by ``sample`` (a stopped
         chart's prediction rows keep its last prediction).  Without callbacks the steps run from mugd_sample_dpm_stop calls, with them
         one by one through mugd_dpm_stop_update.  Every argument is checked before any GPU work (ValueError); mask, eta, temperature
-        and noise dropout are refused."""
+        and noise dropout are refused, and z_lengths (MugdError)."""
+        _refuse_ragged(z_lengths, "invert")
         self._require_schedule(sched)
         return self._invert("DPMSolverSampler", x0, c, w, t_enc, dpm_solver.inversion_schedule(sched), unconditional_guidance_scale,
                             unconditional_conditioning, callback, img_callback, log_every_t, tqdm_class, verbose, kwargs)
 
     @torch.no_grad()
     def decode(self, x_latent, c, w, t_start, sched: dpm_solver.DPMSchedule, unconditional_guidance_scale=1.,
-               unconditional_conditioning=None, tqdm_class=None):
+               unconditional_conditioning=None, tqdm_class=None, z_lengths=None):
         """Denoise ``x_latent`` [B, C, L] (e.g. from ``stochastic_encode``) under (c, w) over the last ``t_start`` steps of ``sched``:
         chart b runs steps S - t_start[b] .. S - 1 from x_latent[b] (``t_start``: an integer in [0, S], or one per chart) and returns
         the final latent.  A chart's first step is order 1 and its order at step i is min(sched.orders[i], i - (S - t_start[b]) + 1)
@@ -1456,7 +1556,9 @@ class DPMSolverSampler(_DeviceLoopSampler):
         of m = max(t_start) iterations from step S - m (mugd_sample_dpm_ex, the launches per step of mugd_sample_dpm); a chart is left
         untouched until its start, and one with t_start[b] = 0 comes back as x_latent[b].  With every t_start = S this is
         dpm_sampling(x_T=x_latent) bit for bit.  Charts with a smaller start still occupy their batch rows for all m iterations: group
-        charts by strength into separate calls to avoid the idle rows.  Every argument is checked before any GPU work (ValueError)."""
+        charts by strength into separate calls to avoid the idle rows.  Every argument is checked before any GPU work (ValueError;
+        MugdError for z_lengths)."""
+        _refuse_ragged(z_lengths, "decode(x_latent, ...)")
         model = self.model
         self._require_schedule(sched)
         self._check_latent(x_latent)
@@ -1530,7 +1632,7 @@ class UniPCSampler(_DeviceLoopSampler):
     def sample(self, S, c=None, w=None, batch_size=None, shape=None, x_T=None, order=2, skip_type="time_uniform", variant="bh2",
                lower_order_final=True, use_corrector=True, disable_corrector=(), t_grid=None, callback=None, img_callback=None,
                log_every_t=100, unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, verbose=True,
-               conditioning=None, seeds=None, **kwargs):
+               conditioning=None, seeds=None, z_lengths=None, **kwargs):
         """S steps of UniPC of ``order`` from x_T (drawn when not given) to t = 1/N; ``c`` may also be given as ``conditioning``.
         Returns ``(z, {'x_inter', 'pred_x0'})``: x_T first, then, after every iteration i with ``(S - i - 1) % log_every_t == 0`` or
         i = 0 (DDIM's rule), the latent the next evaluation sees (the predicted x~_i+1; the last one is z) and the data prediction m_i.
@@ -1545,11 +1647,12 @@ class UniPCSampler(_DeviceLoopSampler):
         sched = self.make_unipc_schedule(S, order, skip_type, variant, lower_order_final, use_corrector, disable_corrector, t_grid)
         size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
         seeds = _request_seeds(seeds, size[0])
+        _ragged_request(z_lengths, size)
         if verbose:
             print(f'Data shape for UniPC sampling is {size}, {S} steps of order {order} ({skip_type}, {variant})')
         return self.unipc_sampling(w, c, size, sched, x_T=x_T, callback=callback, img_callback=img_callback, log_every_t=log_every_t,
                                    unconditional_guidance_scale=scale, unconditional_conditioning=unconditional_conditioning,
-                                   tqdm_class=tqdm_class, seeds=seeds)
+                                   tqdm_class=tqdm_class, seeds=seeds, z_lengths=z_lengths)
 
     @torch.no_grad()
     def inpaint(self, S, c=None, w=None, batch_size=None, mask=None, x0=None, shape=None, x_T=None, order=2, skip_type="time_uniform",
@@ -1584,9 +1687,10 @@ class UniPCSampler(_DeviceLoopSampler):
     @torch.no_grad()
     def unipc_sampling(self, w, c, shape, sched: unipc.UniPCSchedule, x_T=None, callback=None, img_callback=None, log_every_t=100,
                        unconditional_guidance_scale=1., unconditional_conditioning=None, tqdm_class=None, progress=True, mask=None,
-                       x0=None, seeds=None):
+                       x0=None, seeds=None, z_lengths=None):
         """the request of ``sched`` (make_unipc_schedule) on the GPU, from checked arguments (``seeds``: per-chart seeds); with
-        ``mask`` / ``x0`` the inpainting of ``inpaint``"""
+        ``mask`` / ``x0`` the inpainting of ``inpaint``; ``z_lengths`` as in DDIMSampler.ddim_sampling"""
+        lens = _ragged_request(z_lengths, shape, mask, x0)
         model = self.model
         eng = model.engine
         dev = self.device
@@ -1596,8 +1700,9 @@ class UniPCSampler(_DeviceLoopSampler):
         blend = mask is not None
         self.last_schedule = sched
         with eng.lock:
-            seeded, x_T = self._seeded_start(seeds, shape, x_T)
-            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times)
+            seeded, x_T = self._seeded_start(seeds, shape, x_T, lens)
+            x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, sched.model_times,
+                                                             **_ragged_kw(lens))
             coef = torch.from_numpy(sched.rows_f32()).to(dev)
             corr = torch.from_numpy(sched.corr_rows_f32()).to(dev)
             ring = torch.empty(3, B * Lz * Cz, device=dev)                     # the data predictions of the last three steps
@@ -1653,12 +1758,13 @@ class UniPCSampler(_DeviceLoopSampler):
             raise ValueError("sched must be a UniPCSchedule from make_unipc_schedule")
 
     @torch.no_grad()
-    def stochastic_encode(self, x0, t_enc, sched: unipc.UniPCSchedule, noise=None, seeds=None):
+    def stochastic_encode(self, x0, t_enc, sched: unipc.UniPCSchedule, noise=None, seeds=None, z_lengths=None):
         """Noise the latent ``x0`` [B, C, L] for a remix over the last ``t_enc[b]`` steps of ``sched`` (an integer in [0, S], or one per
         chart): alpha(t_S-s) * x0 + sigma(t_S-s) * noise with s = t_enc[b], the marginal at the time where ``decode`` with t_start = s
         starts; s = 0 returns x0 exactly.  noise = torch.randn_like(x0) when not given, chart b's seeding.ENCODE draw with ``seeds``.
         DPMSolverSampler.stochastic_encode's kernel
-        and contract.  ValueError, before any GPU work, for malformed arguments."""
+        and contract.  ValueError, before any GPU work, for malformed arguments; MugdError for ``z_lengths``."""
+        _refuse_ragged(z_lengths, "stochastic_encode")
         self._require_schedule(sched)
         return self._stochastic_encode(x0, noise, lambda B: per_chart_steps(B, t_enc, sched.S, "t_enc", " (S = sched.S)"),
                                        lambda: [torch.from_numpy(v).to(self.device) for v in sched.encode_tables_f32()], sched.S + 1,
@@ -1666,7 +1772,7 @@ class UniPCSampler(_DeviceLoopSampler):
 
     @torch.no_grad()
     def decode(self, x_latent, c, w, t_start, sched: unipc.UniPCSchedule, unconditional_guidance_scale=1.,
-               unconditional_conditioning=None, tqdm_class=None):
+               unconditional_conditioning=None, tqdm_class=None, z_lengths=None):
         """Denoise ``x_latent`` [B, C, L] (e.g. from ``stochastic_encode``) under (c, w) over the last ``t_start`` steps of ``sched``:
         chart b runs iterations f_b = S - t_start[b] .. S - 1 from x_latent[b] (``t_start``: an integer in [0, S], or one per chart)
         and returns the final latent.  It warms up like a fresh request (``unipc.chart_orders``): its predictor at iteration i has
@@ -1674,7 +1780,9 @@ class UniPCSampler(_DeviceLoopSampler):
         no earlier evaluation at f_b), at order min(sched.orders[i - 1], i - f_b).  All charts run in one device loop of
         m = max(t_start) iterations from iteration S - m (mugd_sample_unipc_ex, the launches per step of mugd_sample_unipc); a chart
         is left untouched until its start, and one with t_start[b] = 0 comes back as x_latent[b].  With every t_start = S this is
-        unipc_sampling(x_T=x_latent) bit for bit.  Every argument is checked before any GPU work (ValueError)."""
+        unipc_sampling(x_T=x_latent) bit for bit.  Every argument is checked before any GPU work (ValueError; MugdError for
+        z_lengths)."""
+        _refuse_ragged(z_lengths, "decode(x_latent, ...)")
         model = self.model
         self._require_schedule(sched)
         self._check_latent(x_latent)
@@ -1730,7 +1838,7 @@ class UniPCSampler(_DeviceLoopSampler):
 
     @torch.no_grad()
     def invert(self, x0, c, w, t_enc, sched: unipc.UniPCSchedule, unconditional_guidance_scale=1., unconditional_conditioning=None,
-               callback=None, img_callback=None, log_every_t=100, tqdm_class=None, verbose=True, **kwargs):
+               callback=None, img_callback=None, log_every_t=100, tqdm_class=None, verbose=True, z_lengths=None, **kwargs):
         """Deterministic inversion: run the latent ``x0`` [B, C, z_length] of a chart backwards along UniPC's ODE solution of ``sched``
         (make_unipc_schedule), with the U-Net in the loop, t_enc[b] iterations for chart b (an integer in [0, S], or one per chart),
         on ``unipc.inversion_schedule(sched)``: the reversed grid, predictor orders min(j + 1, order), and the corrector on every
@@ -1739,7 +1847,8 @@ class UniPCSampler(_DeviceLoopSampler):
         charts run in one loop of max(t_enc) iterations; a chart is left untouched once it has run its steps.  Draws no random
         numbers.  Returns z; ``last_intermediates`` holds {'x_inter', 'pred_x0'} logged as by ``sample``.  Without callbacks the steps
         run from mugd_sample_unipc_stop calls, with them one by one through mugd_unipc_stop_update.  Every argument is checked before
-        any GPU work (ValueError); mask, eta, temperature and noise dropout are refused."""
+        any GPU work (ValueError); mask, eta, temperature and noise dropout are refused, and z_lengths (MugdError)."""
+        _refuse_ragged(z_lengths, "invert")
         self._require_schedule(sched)
         inv = unipc.inversion_schedule(sched)
         return self._invert("UniPCSampler", x0, c, w, t_enc, inv, unconditional_guidance_scale, unconditional_conditioning, callback,

@@ -18,7 +18,7 @@ filled with draw_stride = -1.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Sequence
+from typing import Optional, Sequence
 
 import numpy as np
 import torch
@@ -71,21 +71,37 @@ def randn(out: torch.Tensor, seeds_dev: torch.Tensor, purpose: int, first_draw: 
 
 
 class ChartNoise:
-    """The random numbers of one seeded request of ``shape`` = (B, C, L): its seeds on the device and the two ways to draw."""
+    """The random numbers of one seeded request of ``shape`` = (B, C, L): its seeds on the device and the two ways to draw.
+    ``lens`` (a ragged request: chart b valid for its first lens[b] of the L positions): chart b is drawn at its own length, as a
+    [C, lens[b]] chart requested alone, and placed into the padded [C, L] slot with zeros behind it.  An element's counter is
+    c * L + l, so one launch over the padded table would give a shorter chart other values."""
 
-    def __init__(self, seeds: Sequence[int], shape, device):
+    def __init__(self, seeds: Sequence[int], shape, device, lens: Optional[Sequence[int]] = None):
         self.shape = tuple(int(v) for v in shape)
         if len(seeds) != self.shape[0]:
             raise ValueError(f"{len(seeds)} seeds for {self.shape[0]} charts")
         self.seeds_dev = torch.from_numpy(seed_array(seeds).view(np.int64)).to(device)
         self.device = device
+        self.lens = None if lens is None else [int(v) for v in lens]
 
     def fill(self, table: torch.Tensor, purpose: int, first_draw: int, n_draws: int, draw_stride: int = 1):
-        """rows 0 .. n_draws - 1 of a [>= n_draws, B, C, L] table: draws first_draw + draw_stride * k, one launch"""
-        randn(table[:n_draws], self.seeds_dev, purpose, first_draw, n_draws, draw_stride)
+        """rows 0 .. n_draws - 1 of a [>= n_draws, B, C, L] table: draws first_draw + draw_stride * k, one launch (one per chart when
+        ragged)"""
+        if self.lens is None:
+            randn(table[:n_draws], self.seeds_dev, purpose, first_draw, n_draws, draw_stride)
+            return
+        _, C_, L = self.shape
+        for b, Lb in enumerate(self.lens):
+            part = torch.empty(n_draws, 1, C_, Lb, device=self.device)
+            randn(part, self.seeds_dev[b:b + 1], purpose, first_draw, n_draws, draw_stride)
+            table[:n_draws, b, :, :Lb].copy_(part[:, 0])
+            table[:n_draws, b, :, Lb:].zero_()
 
     def draw(self, purpose: int, draw: int) -> torch.Tensor:
         """a fresh [B, C, L] tensor of one draw"""
         out = torch.empty(self.shape, device=self.device)
-        randn(out, self.seeds_dev, purpose, draw, 1)
+        if self.lens is None:
+            randn(out, self.seeds_dev, purpose, draw, 1)
+        else:
+            self.fill(out[None], purpose, draw, 1)
         return out
