@@ -261,10 +261,6 @@ s4conv_stream_kernel(const mugd_s4conv s, int nsplit) {
 static int launch_s4conv_stream(const DeviceInfo& dev, const mugd_s4conv& s, cudaStream_t st) {
     MUGD_REQUIRE((int)S4S_SMEM <= dev.max_smem_optin, "s4conv: the streamed kernel needs %zu B of shared memory (max %d)", S4S_SMEM,
                  dev.max_smem_optin);
-    // windows read u rows other CTAs have already written outputs for: y must not overlap u
-    const char *u0 = (const char*)s.u, *u1 = (const char*)(s.u + ((int64_t)s.B * s.L - 1) * s.ldu + s.H);
-    const char *y0 = (const char*)s.y, *y1 = (const char*)(s.y + ((int64_t)s.B * s.L - 1) * s.ldy + s.H);
-    MUGD_REQUIRE(y1 <= u0 || u1 <= y0, "s4conv: y overlaps u (the streamed kernel cannot run in place)");
     const int base = (s.H / S4_CH) * s.B;
     const int nwin = (s.L + S4S_W - 1) / S4S_W, npairs = (nwin + 1) / 2;
     // every pair of windows costs nwin + 1 tiles: split the pairs over more CTAs until the grid covers the SMs, two CTAs each
@@ -278,6 +274,12 @@ static int launch_s4conv_stream(const DeviceInfo& dev, const mugd_s4conv& s, cud
 int launch_s4conv(const DeviceInfo& dev, const mugd_s4conv& s, cudaStream_t st, int* launches) {
     MUGD_REQUIRE(s.B > 0 && s.L > 0 && s.H > 0 && s.H % S4_CH == 0, "s4conv: H=%d must be a positive multiple of %d", s.H, S4_CH);
     MUGD_REQUIRE(s.ldu >= s.H && s.ldy >= s.H, "s4conv: ld < H");
+    // neither kernel runs in place: the streamed one reads u rows other CTAs have already written outputs for, and with nsplit > 1
+    // the resident one stages the same u rows in every CTA of a split, so one CTA's outputs could replace rows a sibling has not
+    // loaded yet.  nsplit depends on the SM count, so y must not overlap u on any device.
+    const char *u0 = (const char*)s.u, *u1 = (const char*)(s.u + ((int64_t)s.B * s.L - 1) * s.ldu + s.H);
+    const char *y0 = (const char*)s.y, *y1 = (const char*)(s.y + ((int64_t)s.B * s.L - 1) * s.ldy + s.H);
+    MUGD_REQUIRE(y1 <= u0 || u1 <= y0, "s4conv: y overlaps u (the convolution cannot run in place)");
     const int Lpad = (s.L + 2 * S4_R - 1) / (2 * S4_R) * (2 * S4_R);
     const size_t smem = ((size_t)(S4_PAD + Lpad) + (size_t)(Lpad + 3 * S4_R)) * S4_PITCH * sizeof(float);
     // automatic: the resident kernel wherever its u and K fit in shared memory, the streamed one beyond
