@@ -59,7 +59,12 @@ enum mugd_op_kind {
      * int32 `valid[B]` of rows per sample at the op's resolution, clamped to [0, L] by the kernel.  Rows l >= valid[b] are padding. */
     MUGD_OP_GROUPNORM_VAR = 14,/* GroupNorm(+SiLU) over the valid rows only; padded rows are never read and are written as 0   */
     MUGD_OP_ATTENTION_VAR = 15,/* self-attention with keys j < valid[b] only (rows past it never read); padded queries -> 0    */
-    MUGD_OP_ROW_MASK = 16      /* x[b*L + l][0..cols) = 0 for l >= valid[b] (a store, never a multiply)                        */
+    MUGD_OP_ROW_MASK = 16,     /* x[b*L + l][0..cols) = 0 for l >= valid[b] (a store, never a multiply)                        */
+    /* MUGD_OP_GEMM with its K split finished inside each CTA (the `gemm` union member, tensor-core path only): split_k >= 1 K-ranges of
+     * every output tile run one after another in one CTA, summed in the split-K reduce's order, then the fused epilogue.  The result
+     * equals MUGD_OP_GEMM with the same split_k bit for bit, without the workspace and the reduce launch.  Batch-invariant plans use
+     * it where a one-chart K split would put too many partial tiles on a large batch. */
+    MUGD_OP_GEMM_SERIAL = 17
 };
 
 /* A-operand row addressing of MUGD_OP_GEMM (rows are tokens of B samples, Lout output rows each) */

@@ -59,6 +59,7 @@ static int dispatch(mugd_handle* h, const mugd_op& op, cudaStream_t st, int* lau
         case MUGD_OP_GROUPNORM_VAR: return launch_groupnorm_var(h->dev, op.u.gnv, st, launches);
         case MUGD_OP_ATTENTION_VAR: return launch_attention_var(h->dev, op.u.attnv, st, launches);
         case MUGD_OP_ROW_MASK: return launch_row_mask(h->dev, op.u.mask, st, launches);
+        case MUGD_OP_GEMM_SERIAL: return launch_gemm_serial(h->dev, op.u.gemm, h->default_gemm_impl, next_tc, st, launches);
         default:
             set_error("unknown op kind %d", op.kind);
             return MUGD_ERR_INVALID;
@@ -223,7 +224,8 @@ int mugd_plan_run(mugd_plan* p, void* stream) {
     std::vector<const mugd_gemm*> next_tc(n, nullptr);
     for (size_t i = n; i-- > 1;) {
         const mugd_op& o = p->ops[i];
-        next_tc[i - 1] = o.kind == MUGD_OP_GEMM && gemm_runs_tc(o.u.gemm, p->h->default_gemm_impl) ? &o.u.gemm : next_tc[i];
+        const bool tc = (o.kind == MUGD_OP_GEMM && gemm_runs_tc(o.u.gemm, p->h->default_gemm_impl)) || o.kind == MUGD_OP_GEMM_SERIAL;
+        next_tc[i - 1] = tc ? &o.u.gemm : next_tc[i];
     }
     for (size_t i = 0; i < n; ++i) {
         int rc = dispatch(p->h, p->ops[i], (cudaStream_t)stream, &launches, next_tc[i]);

@@ -102,6 +102,11 @@ int launch_unipc_stop_update(const mugd_unipc_stop& e, cudaStream_t st);
 int check_join(const mugd_join& j);
 int launch_join(const mugd_join& j, const int32_t* step, cudaStream_t st);
 int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, cudaStream_t st, int* launches);
+// MUGD_OP_GEMM_SERIAL: the forced K split (g.split_k) of a tensor-core GEMM finished inside each CTA.  validate_gemm_serial runs every
+// check of the op on the host; launch_gemm_serial runs them before its launch.
+int validate_gemm(const mugd_gemm& g);
+int validate_gemm_serial(const mugd_gemm& g, int default_impl);
+int launch_gemm_serial(const DeviceInfo& dev, const mugd_gemm& g, int default_impl, const mugd_gemm* next, cudaStream_t st, int* launches);
 bool gemm_tc_supported(const mugd_gemm& g);
 
 // Descriptor checks shared by the sampler kernels; `who` prefixes the message ("ddpm", "dpm", ...).

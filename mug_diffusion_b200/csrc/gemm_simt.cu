@@ -214,7 +214,7 @@ gemm_simt_kernel(const GemmParams p) {
     }
 }
 
-static int validate_gemm(const mugd_gemm& g) {
+int validate_gemm(const mugd_gemm& g) {
     MUGD_REQUIRE(g.M > 0 && g.N > 0 && g.K > 0, "gemm: empty shape M=%d N=%d K=%d", g.M, g.N, g.K);
     MUGD_REQUIRE(g.K % 16 == 0, "gemm: K=%d must be a multiple of 16", g.K);
     MUGD_REQUIRE(g.N % 4 == 0, "gemm: N=%d must be a multiple of 4", g.N);

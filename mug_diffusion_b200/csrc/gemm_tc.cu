@@ -6,27 +6,47 @@
 
 namespace mugd {
 
+// one-time CTA setup of the wgmma kernels: arm the barriers and warm the TMA descriptor cache; nothing here touches memory written by
+// the previous kernel.  Returns the 1024-byte aligned shared-memory base of the tile pool.
+template <int BN>
+__device__ __forceinline__ uint32_t tc_cta_setup(uint8_t* smem_raw, const CUtensorMap* tmA, const CUtensorMap* tmA1, const CUtensorMap* tmA2,
+                                                 const CUtensorMap* tmB, const CUtensorMap* tmWhi, const CUtensorMap* tmWlo, const TcParams& p) {
+    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;       // SWIZZLE_128B needs 1024-B alignment
+    const TcBars<BN> B(base);
+    TC_STAMP(p, 0, blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0);
+    if (threadIdx.x < 32) {
+        B.init_parallel((int)threadIdx.x);
+    } else if (threadIdx.x < 38) {
+        // warm the TMA descriptor cache while the barriers are set up
+        const CUtensorMap* m = threadIdx.x == 32 ? tmA : threadIdx.x == 33 ? tmA1 : threadIdx.x == 34 ? tmA2
+                             : threadIdx.x == 35 ? tmB : threadIdx.x == 36 ? tmWhi : tmWlo;
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
+    }
+    __syncthreads();
+    TC_STAMP(p, 1, blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0);
+    return base;
+}
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA1,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmWhi,
                const __grid_constant__ CUtensorMap tmWlo, const __grid_constant__ TcParams p) {
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;       // SWIZZLE_128B needs 1024-B alignment
-    const TcBars<BN> B(base);
-    TC_STAMP(p, 0, blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0);
-    // ---- one-time setup: barriers; nothing here touches memory written by the previous kernel ----
-    if (threadIdx.x < 32) {
-        B.init_parallel((int)threadIdx.x);
-    } else if (threadIdx.x < 38) {
-        // warm the TMA descriptor cache while the barriers are set up
-        const CUtensorMap* m = threadIdx.x == 32 ? &tmA : threadIdx.x == 33 ? &tmA1 : threadIdx.x == 34 ? &tmA2
-                             : threadIdx.x == 35 ? &tmB : threadIdx.x == 36 ? &tmWhi : &tmWlo;
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
-    }
-    __syncthreads();
-    TC_STAMP(p, 1, blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0);
+    const uint32_t base = tc_cta_setup<BN>(smem_raw, &tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p);
     gemm_tc_tile<BN, EPI>(&tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p, blockIdx.x, blockIdx.y, blockIdx.z, base);
+}
+
+// split-K finished inside the CTA (MUGD_OP_GEMM_SERIAL): grid gx x gy, each CTA runs the h.splits K-ranges of its tile in turn and
+// sums them in the reduce kernel's order before the fused epilogue (gemm_tc_tile, SERIAL).
+template <int BN, int EPI>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_serial_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA1,
+                      const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB,
+                      const __grid_constant__ CUtensorMap tmWhi, const __grid_constant__ CUtensorMap tmWlo, const __grid_constant__ TcParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t base = tc_cta_setup<BN>(smem_raw, &tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p);
+    gemm_tc_tile<BN, EPI, true>(&tmA, &tmA1, &tmA2, &tmB, &tmWhi, &tmWlo, p, blockIdx.x, blockIdx.y, 0, base);
 }
 
 // split-K second pass: fully parallel over the GPU and L2-resident (see tc_reduce).
@@ -133,13 +153,13 @@ TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split) {
     return t;
 }
 
-int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, TcPlanned* out) {
+int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, TcPlanned* out, bool serial) {
     MUGD_REQUIRE(gemm_tc_supported(g), "gemm_tc: unsupported shape/operands");
     int rc = tc_validate_fusions(g);
     if (rc != MUGD_OK) return rc;
     const TcGeometry t = tc_geometry(g, dev.sm_count, g.split_k);
     const TcParams::Hot& h = t.hot;
-    if (h.splits > 1) {
+    if (h.splits > 1 && !serial) {
         MUGD_REQUIRE(g.workspace, "gemm_tc: split-K needs a workspace");
         MUGD_REQUIRE(g.workspace_bytes >= t.ws_floats * 4, "gemm_tc: workspace too small (%lld < %lld)", (long long)g.workspace_bytes,
                      (long long)t.ws_floats * 4);
@@ -212,37 +232,72 @@ static int tc_launch(const TcPlanned& pl, cudaStream_t st) {
     return MUGD_OK;
 }
 
+template <int BN, int EPI>
+static int tc_launch_serial(const TcPlanned& pl, cudaStream_t st) {
+    const TcParams& p = pl.p;
+    MUGD_CHECK_CUDA(launch_k(gemm_tc_serial_kernel<BN, EPI>, dim3(p.hot.gx, p.gy, 1), dim3(TC_THREADS), TcSmem<BN>::TOTAL, st, pl.maps[0],
+                             pl.maps[1], pl.maps[2], pl.maps[3], pl.maps[4], pl.maps[5], p));
+    return MUGD_OK;
+}
+
 template <int BN, int... EPI>
 static cudaError_t allow_smem_bn(int bytes, std::integer_sequence<int, EPI...>) {
-    return allow_dynamic_smem(bytes, gemm_tc_kernel<BN, EPI>...);
+    const cudaError_t e = allow_dynamic_smem(bytes, gemm_tc_kernel<BN, EPI>...);
+    return e != cudaSuccess ? e : allow_dynamic_smem(bytes, gemm_tc_serial_kernel<BN, EPI>...);
 }
 cudaError_t gemm_tc_allow_smem(int bytes) {
     const cudaError_t e = allow_smem_bn<64>(bytes, std::make_integer_sequence<int, TC_E_COUNT>{});
     return e != cudaSuccess ? e : allow_smem_bn<128>(bytes, std::make_integer_sequence<int, TC_E_COUNT>{});
 }
 
-template <int BN>
+template <int BN, template <int, int> class Launch>
 static int tc_launch_bn(const TcPlanned& pl, cudaStream_t st) {
     switch (tc_epi_of(pl.p.g)) {
-        case TC_E_GEGLU: return tc_launch<BN, TC_E_GEGLU>(pl, st);
-        case TC_E_GLU: return tc_launch<BN, TC_E_GLU>(pl, st);
-        case TC_E_SILU: return tc_launch<BN, TC_E_SILU>(pl, st);
-        case TC_E_GELU: return tc_launch<BN, TC_E_GELU>(pl, st);
-        case TC_E_SINK: return tc_launch<BN, TC_E_SINK>(pl, st);
-        case TC_E_LN: return tc_launch<BN, TC_E_LN>(pl, st);
-        case TC_E_LN_GEGLU: return tc_launch<BN, TC_E_LN_GEGLU>(pl, st);
-        default: return tc_launch<BN, TC_E_NONE>(pl, st);
+        case TC_E_GEGLU: return Launch<BN, TC_E_GEGLU>::run(pl, st);
+        case TC_E_GLU: return Launch<BN, TC_E_GLU>::run(pl, st);
+        case TC_E_SILU: return Launch<BN, TC_E_SILU>::run(pl, st);
+        case TC_E_GELU: return Launch<BN, TC_E_GELU>::run(pl, st);
+        case TC_E_SINK: return Launch<BN, TC_E_SINK>::run(pl, st);
+        case TC_E_LN: return Launch<BN, TC_E_LN>::run(pl, st);
+        case TC_E_LN_GEGLU: return Launch<BN, TC_E_LN_GEGLU>::run(pl, st);
+        default: return Launch<BN, TC_E_NONE>::run(pl, st);
     }
 }
+template <int BN, int EPI> struct TcSplitLaunch { static int run(const TcPlanned& pl, cudaStream_t st) { return tc_launch<BN, EPI>(pl, st); } };
+template <int BN, int EPI> struct TcSerialLaunch { static int run(const TcPlanned& pl, cudaStream_t st) { return tc_launch_serial<BN, EPI>(pl, st); } };
 
 int launch_gemm_tc(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, cudaStream_t st, int* launches) {
     TcPlanned pl;
     int rc = tc_plan(dev, g, next, &pl);
     if (rc != MUGD_OK) return rc;
-    if (pl.BN == 128) rc = tc_launch_bn<128>(pl, st);
-    else rc = tc_launch_bn<64>(pl, st);
+    if (pl.BN == 128) rc = tc_launch_bn<128, TcSplitLaunch>(pl, st);
+    else rc = tc_launch_bn<64, TcSplitLaunch>(pl, st);
     if (rc != MUGD_OK) return rc;
     if (launches) *launches += pl.p.hot.splits > 1 ? 2 : 1;
+    return MUGD_OK;
+}
+
+int validate_gemm_serial(const mugd_gemm& g, int default_impl) {
+    const int impl = g.impl == MUGD_GEMM_AUTO ? default_impl : g.impl;
+    MUGD_REQUIRE(impl == MUGD_GEMM_TC, "gemm_serial: runs on the tensor-core path only (impl %d)", impl);
+    MUGD_REQUIRE(g.split_k >= 1, "gemm_serial: needs a forced K split (split_k = %d)", g.split_k);
+    MUGD_REQUIRE(tc_shape_ok(g) && g.split_k <= (g.taps * g.K + g.K2) / TC_BK,
+                 "gemm_serial: shape the tensor-core kernel does not take, or more splits than k-steps (M=%d N=%d K=%d taps=%d K2=%d split_k=%d)",
+                 g.M, g.N, g.K, g.taps, g.K2, g.split_k);
+    MUGD_REQUIRE(gemm_tc_supported(g), "gemm_serial: needs TF32 hi / lo weights and 16-byte aligned operands (M=%d N=%d K=%d)", g.M, g.N, g.K);
+    return MUGD_OK;
+}
+
+int launch_gemm_serial(const DeviceInfo& dev, const mugd_gemm& g, int default_impl, const mugd_gemm* next, cudaStream_t st, int* launches) {
+    int rc = validate_gemm(g);
+    if (rc != MUGD_OK) return rc;
+    if ((rc = validate_gemm_serial(g, default_impl)) != MUGD_OK) return rc;
+    TcPlanned pl;
+    if ((rc = tc_plan(dev, g, next, &pl, true)) != MUGD_OK) return rc;
+    if (pl.BN == 128) rc = tc_launch_bn<128, TcSerialLaunch>(pl, st);
+    else rc = tc_launch_bn<64, TcSerialLaunch>(pl, st);
+    if (rc != MUGD_OK) return rc;
+    if (launches) *launches += 1;
     return MUGD_OK;
 }
 

@@ -316,7 +316,11 @@ __device__ __forceinline__ void tc_load_split(uint32_t a_tile, int r0, int t, Tc
 // threads call it: warpgroup w computes rows 64w..64w+63 with wgmma (A = the split activation rows from registers, B = the weight
 // tiles from shared memory); one elected lane of warp 0 also drives the TMA ring.  On return every TMA has landed, every MMA has
 // retired, and the tile (or its split-K partial) is on its way to global memory.
-template <int BN, int EPI>
+// SERIAL (gemm_tc_serial_kernel): the CTA runs all h.splits K-ranges of its tile one after another (bz = 0) and keeps a running fp32
+// sum: after each range the accumulator is added to it and restarted from zero, the same adds in the same order as tc_reduce's sum
+// of the partial tiles, and the sum goes through the tile epilogue.  The result equals split kernel + reduce bit for bit, without
+// the workspace round trip and the second launch.
+template <int BN, int EPI, bool SERIAL = false>
 __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUtensorMap* tmA1, const CUtensorMap* tmA2, const CUtensorMap* tmB,
                                              const CUtensorMap* tmWhi, const CUtensorMap* tmWlo, const TcParams& p, int bx, int by, int bz,
                                              uint32_t base) {
@@ -335,8 +339,8 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     int b_base, l_base, rows_valid;
     tc_tile_rows(p, by, b_base, l_base, rows_valid);
     const int m_base = b_base * h.Lrows + l_base;
-    const int it_begin = bz * h.it_base + min(bz, h.it_rem);
-    const int nit = h.it_base + (bz < h.it_rem ? 1 : 0);
+    const int it_begin = SERIAL ? 0 : bz * h.it_base + min(bz, h.it_rem);
+    const int nit = SERIAL ? h.total_it : h.it_base + (bz < h.it_rem ? 1 : 0);
     const uint32_t a_tx = (uint32_t)(h.box_l * h.box_b) * TC_BK * 4;
     const uint32_t w_tx = (h.single_pass ? 1u : 2u) * S::B_BYTES;
 
@@ -371,7 +375,7 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
             pdl_wait();                          // activations written by the previous kernel are touched from here on
             for (int i = 0; i < pro; ++i) issue_a(i);
             if (p.pf_bytes > 0) {                // after this CTA's own loads: CTA c prefetches slice c of the next GEMM's weights
-                const int64_t ncta = (int64_t)h.gx * p.gy * h.splits;
+                const int64_t ncta = (int64_t)h.gx * p.gy * (SERIAL ? 1 : h.splits);
                 const int64_t per = (p.pf_bytes / ncta + 15) & ~(int64_t)15;
                 const int64_t off = (((int64_t)bz * p.gy + by) * h.gx + bx) * per;
                 const int64_t n = min(per, p.pf_bytes - off);
@@ -392,7 +396,7 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     double ln_s = 0.0, ln_ss = 0.0;
     {
         pdl_wait();                                          // the step counter / LayerNorm moments are written by the previous kernels
-        if (h.splits == 1) {
+        if (SERIAL || h.splits == 1) {
             const int nn = n0 + ((int)threadIdx.x % (BN / 4)) * 4;
             if (g.step) epi_step = *g.step;
             if (g.bias && nn < g.N) epi_bias = ld_f4(g.bias + nn);
@@ -419,6 +423,13 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     float acc[NACC];
 #pragma unroll
     for (int j = 0; j < NACC; ++j) acc[j] = 0.f;
+    float run[SERIAL ? NACC : 1];                                  // SERIAL: sum of the finished K-ranges
+    int seg = 0, seg_end = 0;                                      // SERIAL: current K-range and its end (k-steps)
+    if constexpr (SERIAL) {
+#pragma unroll
+        for (int j = 0; j < NACC; ++j) run[j] = 0.f;
+        seg_end = h.it_base + (0 < h.it_rem ? 1 : 0);
+    }
     TcAFrag f0, f1;
     if (nit > 0) {
         mbar_wait(B.full(0), 0u);
@@ -458,6 +469,15 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
                 mbar_wait(B.full((i + 1) % STAGES), (uint32_t)((i + 1) / STAGES) & 1u);
                 tc_load_split(a_raw((i + 1) % STAGES), r0, t4, nxt);
             }
+            if constexpr (SERIAL) {
+                if (i + 1 == seg_end) {                           // last k-step of a K-range: run += its accumulator, restart it
+                    wgmma_wait<0>();
+#pragma unroll
+                    for (int j = 0; j < NACC; ++j) { run[j] = __fadd_rn(run[j], acc[j]); acc[j] = 0.f; }
+                    ++seg;
+                    seg_end += h.it_base + (seg < h.it_rem ? 1 : 0);
+                }
+            }
         };
         for (int i = 0; i < nit; i += 2) {
             kstep(i, f0, f1);
@@ -478,8 +498,9 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
         const int c = j * 8 + 2 * t4;
-        sts_f2(base + (uint32_t)(r0 * SP + c) * 4u, acc[4 * j], acc[4 * j + 1]);
-        sts_f2(base + (uint32_t)((r0 + 8) * SP + c) * 4u, acc[4 * j + 2], acc[4 * j + 3]);
+        const float* fin = SERIAL ? run : acc;
+        sts_f2(base + (uint32_t)(r0 * SP + c) * 4u, fin[4 * j], fin[4 * j + 1]);
+        sts_f2(base + (uint32_t)((r0 + 8) * SP + c) * 4u, fin[4 * j + 2], fin[4 * j + 3]);
     }
     if constexpr (TcEpiTraits<EPI>::MODE == TC_EPI_LN) {     // (mean, rstd) of tile row r for phase 2, in the last KB of the pipeline buffers
         if (threadIdx.x < TC_BM) sts_f2(base + S::TILE_BYTES - 1024u + (uint32_t)threadIdx.x * 8u, lnrow.x, lnrow.y);
@@ -489,7 +510,7 @@ __device__ __forceinline__ void gemm_tc_tile(const CUtensorMap* tmA, const CUten
     TC_STAMP(p, 3, bx == 0 && by == 0 && bz == 0);
     {
         const float* rowvec = g.rowvec ? g.rowvec + (int64_t)epi_step * g.rowvec_step_stride : nullptr;
-        if (h.splits > 1) {
+        if (!SERIAL && h.splits > 1) {
             const int tile_lin = by * h.gx + bx;
             float* wsp = p.ws + ((int64_t)tile_lin * h.splits + bz) * (TC_BM * BN);
             constexpr int C4 = BN / 4;
@@ -593,7 +614,8 @@ struct alignas(64) TcPlanned {
     int BN;
 };
 TcGeometry tc_geometry(const mugd_gemm& g, int sm_count, int forced_split);
-// validates, picks the geometry, encodes the maps; `next` (or NULL): the tensor-core GEMM whose weights this one prefetches into L2
-int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, TcPlanned* out);
+// validates, picks the geometry, encodes the maps; `next` (or NULL): the tensor-core GEMM whose weights this one prefetches into L2;
+// `serial`: the K splits run inside one CTA (gemm_tc_serial_kernel), no workspace
+int tc_plan(const DeviceInfo& dev, const mugd_gemm& g, const mugd_gemm* next, TcPlanned* out, bool serial = false);
 
 }  // namespace mugd

@@ -45,6 +45,12 @@ static const PtrField k_ptr_fields[] = {
     PF(MUGD_OP_ATTENTION_VAR, attnv.attn.o), PF(MUGD_OP_ATTENTION_VAR, attnv.attn.relpos), PF(MUGD_OP_ATTENTION_VAR, attnv.attn.cgain),
     PF(MUGD_OP_ATTENTION_VAR, attnv.valid),
     PF(MUGD_OP_ROW_MASK, mask.x), PF(MUGD_OP_ROW_MASK, mask.valid),
+    // the serial-split GEMM shares the GEMM descriptor: the same pointer fields
+    PF(MUGD_OP_GEMM_SERIAL, gemm.A), PF(MUGD_OP_GEMM_SERIAL, gemm.W), PF(MUGD_OP_GEMM_SERIAL, gemm.W_hi), PF(MUGD_OP_GEMM_SERIAL, gemm.W_lo),
+    PF(MUGD_OP_GEMM_SERIAL, gemm.bias), PF(MUGD_OP_GEMM_SERIAL, gemm.rowvec), PF(MUGD_OP_GEMM_SERIAL, gemm.step),
+    PF(MUGD_OP_GEMM_SERIAL, gemm.residual), PF(MUGD_OP_GEMM_SERIAL, gemm.C), PF(MUGD_OP_GEMM_SERIAL, gemm.workspace),
+    PF(MUGD_OP_GEMM_SERIAL, gemm.counters), PF(MUGD_OP_GEMM_SERIAL, gemm.A2), PF(MUGD_OP_GEMM_SERIAL, gemm.row_moments),
+    PF(MUGD_OP_GEMM_SERIAL, gemm.ln_stats), PF(MUGD_OP_GEMM_SERIAL, gemm.ln_colsum),
 };
 #undef PF
 

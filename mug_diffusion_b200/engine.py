@@ -199,6 +199,59 @@ class OpList:
         self.add(L_.OP_COPY2D, d, tag)
 
 
+def tc_plan_of(g: L_.Gemm, sm_count: int) -> Tuple[int, int, int]:
+    """(supported, K splits, output tiles) the tensor-core planner picks for ``g`` at ``sm_count`` SMs (mugd_gemm_tc_query)"""
+    sup, sp, tiles, ws = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int64()
+    L_.check(L_.load().mugd_gemm_tc_query(None, C.byref(g), sm_count, C.byref(sup), C.byref(sp), C.byref(ws), C.byref(tiles)),
+             "gemm_tc_query")
+    return sup.value, sp.value, tiles.value
+
+
+def gemm_runs_tc(g: L_.Gemm, sm_count: int) -> bool:
+    """whether ``g`` runs on the tensor-core kernel (gemm_simt.cu gemm_runs_tc with a tensor-core handle): a shape the kernel takes
+    (mugd_gemm_tc_query), TF32 hi / lo weights, row strides in whole 16-byte units and 16-byte aligned operands.  Anything else runs
+    on the FFMA kernel."""
+    if not (g.A and g.W_hi and g.W_lo) or g.lda % 4 or g.A % 16 or g.W_hi % 16 or g.W_lo % 16:
+        return False
+    if g.K2 > 0 and (not g.A2 or g.lda2 % 4 or g.A2 % 16):
+        return False
+    return bool(tc_plan_of(g, sm_count)[0])
+
+
+def unit_batch_splits(ops: OpList, B: int, unit: int, sm_count: int) -> OpList:
+    """Batch-invariant plans (DESIGN §6b N18): every tensor-core GEMM of ``ops``, compiled for B samples, sums its K range in the
+    order the planner picks for the same op at ``unit`` samples (one chart: 2 under classifier-free guidance, else 1).  A row's bits
+    then do not depend on the batch it runs in.  Only the K split depends on the batch (the tile width follows N), so the op keeps
+    split_k = 0 where the planner's own choice at B already equals the unit one, and takes the unit split otherwise.  A forced split
+    whose partial tiles would exceed what the split-K kernel launches (tiles * splits > 2 * SMs, the planner's workspace bound)
+    becomes MUGD_OP_GEMM_SERIAL: the same sums finished inside each CTA, without the workspace and the reduce launch.  GEMMs
+    that run on the FFMA kernel (gemm_runs_tc false: no TF32 hi / lo weights, an unaligned operand) have no K split and are left
+    alone.  Rewrites
+    ``ops`` in place and returns it; B == unit leaves it as it is."""
+    if B == unit:
+        return ops
+    if unit <= 0 or B % unit:
+        raise ValueError(f"batch {B} is not a multiple of the one-chart batch {unit}")
+    for op in ops.ops:
+        if op.kind != L_.OP_GEMM:
+            continue
+        g = op.u.gemm
+        if g.split_k or not gemm_runs_tc(g, sm_count):
+            continue
+        if g.M % B:
+            raise ValueError(f"GEMM of {g.M} rows in a plan of {B} samples")
+        one = L_.Gemm.from_buffer_copy(g)
+        one.M = g.M // B * unit
+        _, s_unit, _ = tc_plan_of(one, sm_count)
+        _, s_here, tiles = tc_plan_of(g, sm_count)
+        if s_here == s_unit:
+            continue
+        g.split_k = s_unit
+        if s_unit > 1 and tiles * s_unit > 2 * sm_count:
+            op.kind = L_.OP_GEMM_SERIAL
+    return ops
+
+
 def emit_upsample_conv(ops: "OpList", blob: WeightBlob, wfn, prefix: str, x: View, out: View, Lin: int, cin: int, cout: int, tag: int):
     """Upsample (nearest x2) + conv3 (models.py:66-70).  With the parity-split weights of the packer this is two 2-tap
     GEMMs over the Lin input rows writing the even / odd output rows (row stride 2*ld) -- 2/3 of the FLOPs of the

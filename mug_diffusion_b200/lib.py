@@ -16,6 +16,7 @@ LIB_PATH = os.environ.get("MUGD_LIB") or os.path.join(HERE, "libmugd.so")      #
 (OP_GEMM, OP_GROUPNORM, OP_LAYERNORM, OP_ATTENTION, OP_S4CONV, OP_DDIM_UPDATE, OP_TRANSPOSE, OP_COPY2D, OP_STEP_ADVANCE, OP_NOTES, OP_EMBED,
  OP_TF32_SPLIT, OP_POSTERIOR) = range(1, 14)
 OP_GROUPNORM_VAR, OP_ATTENTION_VAR, OP_ROW_MASK = 14, 15, 16           # ragged batches: the base descriptor + valid[B]
+OP_GEMM_SERIAL = 17                    # the GEMM descriptor, its forced K split finished inside each CTA (batch-invariant plans)
 CONV_NONE, CONV_SAME, CONV_DOWN, CONV_UP, CONV_TAPS = range(5)
 ACT_NONE, ACT_SILU, ACT_GELU = range(3)
 GATE_NONE, GATE_GEGLU, GATE_GLU = range(3)
@@ -182,7 +183,7 @@ class Op(C.Structure):
 
 _KIND_FIELD = {OP_GEMM: "gemm", OP_GROUPNORM: "gn", OP_LAYERNORM: "ln", OP_ATTENTION: "attn", OP_S4CONV: "s4",
                OP_DDIM_UPDATE: "ddim", OP_TRANSPOSE: "tr", OP_COPY2D: "cp", OP_STEP_ADVANCE: "adv", OP_NOTES: "notes", OP_EMBED: "embed", OP_TF32_SPLIT: "split",
-               OP_POSTERIOR: "post", OP_GROUPNORM_VAR: "gnv", OP_ATTENTION_VAR: "attnv", OP_ROW_MASK: "mask"}
+               OP_POSTERIOR: "post", OP_GROUPNORM_VAR: "gnv", OP_ATTENTION_VAR: "attnv", OP_ROW_MASK: "mask", OP_GEMM_SERIAL: "gemm"}
 
 
 def make_op(kind: int, desc, tag: int = 0) -> Op:

@@ -13,7 +13,8 @@ from torch.utils.weak import WeakIdKeyDictionary
 from . import lib as L_
 from .audio import check_z_length
 from .config import EncoderConfig, ModelConfig
-from .engine import (Arena, CTX_TOKENS_MAX, DecoderCompiler, EncoderCompiler, MAX_STEPS, OpList, UNetCompiler, View, tc_weight_map)
+from .engine import (Arena, CTX_TOKENS_MAX, DecoderCompiler, EncoderCompiler, MAX_STEPS, OpList, UNetCompiler, View, tc_weight_map,
+                     unit_batch_splits)
 from .packer import WeightBlob, pack_model
 
 
@@ -129,15 +130,18 @@ class Plan:
             pass
 
 
-def compile_sized(engine: "MugEngine", compile_fn: Callable[[Arena], dict]):
+def compile_sized(engine: "MugEngine", compile_fn: Callable[[Arena], dict], batch: Optional[Tuple[int, int]] = None):
     """Compile into a zeroed device arena of exactly the size the plan needs: a dry compile measures it, the real one runs at a
-    256-byte aligned base.  compile_fn(arena) returns the compiler's result dict.  Returns (arena tensor, result, Plan)."""
+    256-byte aligned base.  compile_fn(arena) returns the compiler's result dict.  ``batch`` = (samples of the plan, samples of one
+    chart): the plan takes the engine's batch policy (MugEngine.batch_ops).  Returns (arena tensor, result, Plan)."""
     dry = Arena(0)
     compile_fn(dry)
     nbytes = dry.high + 1024
     arena_t = torch.zeros(nbytes // 4 + 64, device=engine.device)
     base = (arena_t.data_ptr() + 255) // 256 * 256
     res = compile_fn(Arena(base, nbytes))
+    if batch is not None:
+        engine.batch_ops(res["ops"], *batch)
     return arena_t, res, Plan(engine, res["ops"])
 
 
@@ -153,7 +157,7 @@ class MugEngine:
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], cfg: Optional[ModelConfig] = None,
                  device: Optional[torch.device] = None, gemm_impl: str = "auto", blob: Optional[WeightBlob] = None,
-                 max_sessions: int = 4, fold_ln: Optional[bool] = None):
+                 max_sessions: int = 4, fold_ln: Optional[bool] = None, batch_invariant: bool = False):
         if not torch.cuda.is_available():
             raise L_.MugdError("mug_diffusion_b200 needs an sm_90 (H100) GPU; there is no CPU fallback")
         self.cfg = cfg or ModelConfig()
@@ -162,6 +166,12 @@ class MugEngine:
         self.lib = L_.load()
         self.handle = C.c_void_p()
         L_.check(self.lib.mugd_create(self.device.index or 0, C.byref(self.handle)), "mugd_create")
+        sms, cc_major, cc_minor = C.c_int32(), C.c_int32(), C.c_int32()
+        L_.check(self.lib.mugd_device_info(self.handle, C.byref(sms), C.byref(cc_major), C.byref(cc_minor)), "device_info")
+        self.sm_count = sms.value
+        # batch_invariant: every plan sums each GEMM's K range as the plan of one chart does, so a chart's bits do not depend on the
+        # batch it is generated in (DESIGN §6b N18).  Off: today's plans, op for op.
+        self.batch_invariant = bool(batch_invariant)
         self.blob = blob if blob is not None else pack_model(state_dict, self.cfg.unet, self.cfg.decoder, encoder_cfg=self.cfg.encoder)
         self.weights = self.blob.data.to(self.device)          # every weight once, fp32 (0.56 GB); tensor-core weights become hi in place
         self.wbase = self.weights.data_ptr()
@@ -228,10 +238,17 @@ class MugEngine:
 
     def attach_workspace(self, ops: OpList):
         for op in ops.ops:
-            if op.kind == L_.OP_GEMM:
+            if op.kind in (L_.OP_GEMM, L_.OP_GEMM_SERIAL):
                 g = op.u.gemm
                 g.workspace, g.workspace_bytes = self.tc_ws.data_ptr(), self.tc_ws.numel() * 4
                 g.counters, g.n_counters = self.tc_counters.data_ptr(), self.tc_counters.numel()
+
+    def batch_ops(self, ops: OpList, B: int, unit: int) -> OpList:
+        """``ops`` compiled for B samples, of which ``unit`` make one chart, under this engine's batch policy: unchanged by default;
+        with batch_invariant, every tensor-core GEMM takes the K split of the one-chart plan (engine.unit_batch_splits)"""
+        if not self.batch_invariant or self.gemm_impl == "simt":
+            return ops
+        return unit_batch_splits(ops, B, unit, self.sm_count)
 
     def run_ops(self, ops: OpList):
         self.attach_workspace(ops)
@@ -268,13 +285,14 @@ class MugEngine:
             cache.move_to_end(key)
         return s
 
-    def session(self, Beff: int, Lz: int, per_sample_t: bool = False, ragged: bool = False) -> "Session":
+    def session(self, Beff: int, Lz: int, per_sample_t: bool = False, ragged: bool = False, unit: int = 1) -> "Session":
         """the compiled U-Net of (Beff, Lz).  ``ragged``: the plan for samples padded to Lz whose valid lengths are set per request
-        (Session.set_lengths); a separate session, so requests without lengths keep today's plan."""
+        (Session.set_lengths); a separate session, so requests without lengths keep today's plan.  ``unit``: samples per chart (2 under
+        classifier-free guidance); with batch_invariant the plan sums as the plan of ``unit`` samples does, else it is ignored."""
         check_z_length(Lz)
-        if not ragged:
-            return self._lru_get(self.sessions, (Beff, Lz, per_sample_t), lambda: Session(self, Beff, Lz, per_sample_t))
-        return self._lru_get(self.sessions, (Beff, Lz, per_sample_t, "ragged"), lambda: Session(self, Beff, Lz, per_sample_t, ragged=True))
+        unit = unit if self.batch_invariant else 1
+        key = (Beff, Lz, per_sample_t) + (("ragged",) if ragged else ()) + ((("unit", unit),) if self.batch_invariant else ())
+        return self._lru_get(self.sessions, key, lambda: Session(self, Beff, Lz, per_sample_t, ragged=ragged, unit=unit))
 
     def wave_session(self, B: int, T: int):
         """Audio encoder plan for B mel-spectrograms of T frames (SURVEY §8f N1); needs wave weights in the blob."""
@@ -313,8 +331,9 @@ class MugEngine:
 class Session:
     """Compiled U-Net evaluation for Beff samples of length Lz (Beff = 2B under classifier-free guidance)."""
 
-    def __init__(self, engine: MugEngine, Beff: int, Lz: int, per_sample_t: bool, ragged: bool = False):
+    def __init__(self, engine: MugEngine, Beff: int, Lz: int, per_sample_t: bool, ragged: bool = False, unit: int = 1):
         self.engine, self.Beff, self.Lz, self.per_sample_t = engine, Beff, Lz, per_sample_t
+        self.unit = unit                      # samples of one chart: the batch the batch-invariant policy plans for
         cfg = engine.cfg.unet
         dev = engine.device
         # ragged: valid rows of each sample at every level ([levels, Beff] int32, row l = L_b >> l), data of the captured graph
@@ -388,9 +407,11 @@ class Session:
         # the LayerNorm fold lives in the tensor-core GEMM epilogues; the exact-fp32 FFMA path keeps the stand-alone LayerNorm
         # kernels and doubles as the referee of the folded plan.  engine.fold_ln: None = by size, True / False = forced (A/B, tests)
         fold = False if self.engine.gemm_impl == "simt" else self.engine.fold_ln
+        if fold is None and self.engine.batch_invariant:
+            fold = self.unit * self.Lz < 8192      # the compiler's size rule (UNetCompiler.compile), taken at one chart's rows
         valid = None if self.valid is None else [_ptr(self.valid[l]) for l in range(self.valid.shape[0])]
         self.arena_t, res, self.plan = compile_sized(self.engine, lambda arena: self.comp.compile(
-            arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold, valid))
+            arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold, valid), batch=(self.Beff, self.unit))
         self.xin: View = res["xin"]
         self.eps: View = res["eps"]
         self.audio_slots = res["audio_slots"]
@@ -452,7 +473,8 @@ class Session:
         ops.gemm(h1, w(up + "time_embed.2.weight"), cfg.time_embed_dim, cfg.time_embed_dim, h2, bias=w(up + "time_embed.2.bias"),
                  act=L_.ACT_SILU)
         ops.gemm(h2, w(up + "emb_all.weight"), self.emb_table.shape[1], cfg.time_embed_dim, et, bias=w(up + "emb_all.bias"))
-        return ops
+        # per-sample timesteps: one row per sample; otherwise one row per schedule step, the same rows at any batch
+        return eng.batch_ops(ops, self.Beff, self.unit) if self.per_sample_t else ops
 
     def set_context(self, context):
         """context [Beff, ctx_dim, T] (reference layout; or a list of such tensors that follow each other along the batch, e.g.
@@ -485,7 +507,7 @@ class Session:
         for b, kv in zip(blocks, self.ctx_kv):
             o = View(_ptr(kv), kv.shape[1], Bc * T, kv.shape[1])
             ops.gemm(cv, self.comp.w(b.prefix + "transformer_blocks.0.attn2.kv.weight"), 2 * b.cin, Cd, o, Lout=T)
-        return ops
+        return eng.batch_ops(ops, Bc, self.unit)
 
     def set_audio(self, audios: Sequence[torch.Tensor], dup: bool = False):
         """The last ``levels`` entries of the wave-encoder output list (unet.py:527-543), NCL layout, written
@@ -694,7 +716,7 @@ class DecoderSession:
         self.muls = sorted({b.mul for b in comp.seq} | {b.mul * 2 for b in comp.seq if b.kind == "up"}) if ragged else []
         self.valid = torch.zeros(len(self.muls), B, dtype=torch.int32, device=engine.device) if ragged else None
         valid = {m: _ptr(self.valid[k]) for k, m in enumerate(self.muls)} if ragged else None
-        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz, valid))
+        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz, valid), batch=(B, 1))
         self.zin, self.logits, self.Lout = res["inp"], res["out"], res["Lout"]
 
     def notes(self, frame_ms: float, key_count: int = 4):
@@ -746,7 +768,7 @@ class EncoderSession:
         self.cfg = engine.encoder_cfg
         comp = EncoderCompiler(self.cfg, engine.blob, engine.wbase, engine.tc_map)
         self.frames = Lz * comp.seq[0].mul
-        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz))
+        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, Lz), batch=(B, 1))
         self.notes_rows, self.moments = res["inp"], res["out"]
 
     def encode(self, notes: torch.Tensor) -> "DiagonalGaussianDistribution":

@@ -311,11 +311,14 @@ class MugDiffusionB200:
     """Drop-in for the reference ``DDPM`` object on the sampler path (attributes of SURVEY §8b)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], cfg: Optional[ModelConfig] = None, z_length: int = 512,
-                 device=None, gemm_impl: str = "auto", blob=None, fold_ln: Optional[bool] = None):
+                 device=None, gemm_impl: str = "auto", blob=None, fold_ln: Optional[bool] = None, batch_invariant: bool = False):
+        """``batch_invariant``: every chart of a batch is bit-identical to the same chart requested alone (same seeds, prompt, audio,
+        z_length and sampler arguments, same GPU model): each plan sums its GEMMs as the one-chart plan does (DESIGN §6b N18).
+        Off (the default): today's plans, whose charts match the alone ones to GEMM rounding."""
         self.cfg = cfg or ModelConfig()
         if self.cfg.parameterization != "eps":
             raise MugdError(f'parameterization "{self.cfg.parameterization}" is not supported: the samplers run "eps" models only')
-        self.engine = MugEngine(state_dict, self.cfg, device, gemm_impl=gemm_impl, blob=blob, fold_ln=fold_ln)
+        self.engine = MugEngine(state_dict, self.cfg, device, gemm_impl=gemm_impl, blob=blob, fold_ln=fold_ln, batch_invariant=batch_invariant)
         self.device = self.engine.device
         self.z_channels = self.cfg.z_channels
         self.z_length = z_length
@@ -361,8 +364,8 @@ class MugDiffusionB200:
         self.prompt_embedder = PromptEmbedder(self.engine, weight)
 
     @classmethod
-    def from_state_dict(cls, sd, cfg=None, z_length=512, device=None, gemm_impl="auto"):
-        return cls(sd, cfg, z_length, device, gemm_impl)
+    def from_state_dict(cls, sd, cfg=None, z_length=512, device=None, gemm_impl="auto", batch_invariant: bool = False):
+        return cls(sd, cfg, z_length, device, gemm_impl, batch_invariant=batch_invariant)
 
     @classmethod
     def from_reference(cls, ddpm, device=None, gemm_impl: str = "auto") -> "MugDiffusionB200":
@@ -499,7 +502,7 @@ class _DeviceLoopSampler:
         x = self._x_T(shape, x_T)
         cfg_on = not (uc is None or scale == 1.)
         Beff = 2 * B if cfg_on else B
-        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False, ragged=lens is not None)
+        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False, ragged=lens is not None, unit=2 if cfg_on else 1)
         if lens is not None:
             sess.set_lengths(list(lens) * 2 if cfg_on else lens)
         sess.set_timestep_table(time_range.copy())

@@ -278,7 +278,7 @@ class WaveSession:
         self.engine, self.B, self.T = engine, B, T
         cfg = engine.blob.meta["wave_cfg"]
         comp = WaveCompiler(cfg, engine.blob, engine.wbase, engine.tc_map)
-        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, T))
+        self.arena_t, res, self.plan = compile_sized(engine, lambda arena: comp.compile(arena, B, T), batch=(B, 1))
         self.mel, self.outs = res["mel"], res["outs"]
         self.cfg = cfg
 
