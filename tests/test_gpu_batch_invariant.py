@@ -11,6 +11,7 @@ pytestmark = pytest.mark.gpu
 from mug_diffusion_b200 import lib as L_  # noqa: E402
 from mug_diffusion_b200 import packer, synth  # noqa: E402
 from mug_diffusion_b200.config import ModelConfig  # noqa: E402
+from mug_diffusion_b200.engine import OpList, View, unit_batch_splits  # noqa: E402
 from mug_diffusion_b200.sampler import (DDIMSampler, DDPMSampler, DPMSolverSampler, MugDiffusionB200, PLMSSampler,  # noqa: E402
                                         UniPCSampler)
 
@@ -101,6 +102,93 @@ def test_serial_split_equals_split_kernel_and_reduce(L):
             assert torch.equal(a[1], b[1]), key
         seen.add(key)
     assert len(seen) >= 3
+
+
+# one op in isolation: the policy picks kind and split for B charts of L rows; each chart's rows equal the one-chart op's.  L = 48:
+# several samples share a 128-row tile and the last tile is part-filled; L = 200: a sample spans two tiles.
+ONE_OP_EPIS = {
+    "none_rowvec_res": dict(taps=3, mode=L_.CONV_SAME, rowvec=True, residual=True),
+    "sink": dict(sink=True),
+    "ln": dict(ln=True),
+    "glu": dict(gate=L_.GATE_GLU),
+}
+
+
+def _one_op(eng, epi, Beff, L, x, keep):
+    """the GEMM of ``epi`` over Beff samples of L rows whose operands are the one-chart operands ``x`` repeated; returns (op, out,
+    row moments or None)"""
+    e = ONE_OP_EPIS[epi]
+    reps = Beff // x["unit"]
+    K, N = x["A"].shape[1], x["W"].shape[0]
+    a = x["A"].repeat(reps, 1).cuda()
+    nout = N // 2 if e.get("gate") else N
+    out = torch.full((Beff * L, nout), float("nan"), device="cuda")
+    keep += [a, out]
+    kw = dict(bias=x["bias"].data_ptr(), W_hi=x["hi"].data_ptr(), W_lo=x["lo"].data_ptr(), impl=L_.GEMM_TC, gate=e.get("gate", 0),
+              taps=e.get("taps", 1), mode=e.get("mode", L_.CONV_NONE), Lin=L, Lout=L)
+    if e.get("rowvec"):
+        t = x["table"].repeat(reps, 1).cuda()
+        kw.update(rowvec=t.data_ptr(), rowvec_b_stride=N)
+        keep.append(t)
+    if e.get("residual"):
+        r = x["res"].repeat(reps, 1).cuda()
+        kw["residual"] = View(r.data_ptr(), N, Beff * L, N)
+        keep.append(r)
+    if e.get("ln"):
+        st = x["stats"].repeat(reps, 1).cuda()
+        kw["ln"] = (st.data_ptr(), x["colsum"].data_ptr(), 1e-5)
+        keep.append(st)
+    ops = OpList()
+    ops.gemm(View(a.data_ptr(), K, Beff * L, K), x["W"].data_ptr(), N, K, View(out.data_ptr(), nout, Beff * L, nout), **kw)
+    mom = None
+    if e.get("sink"):
+        mom = torch.zeros(Beff * L, 2, dtype=torch.float64, device="cuda")
+        ops.ops[0].u.gemm.row_moments = mom.data_ptr()
+        keep.append(mom)
+    ops = unit_batch_splits(ops, Beff, x["unit"], eng.sm_count)
+    op = ops.ops[0]
+    d = op.u.gemm
+    ws = C.c_int64()
+    L_.check(eng.lib.mugd_gemm_tc_query(None, C.byref(d), eng.sm_count, None, None, C.byref(ws), None), "query")
+    wsp = torch.empty(max(ws.value // 4, 4), device="cuda")
+    keep.append(wsp)
+    d.workspace, d.workspace_bytes = wsp.data_ptr(), wsp.numel() * 4
+    L_.check(eng.lib.mugd_op_run(eng.handle, C.byref(op), torch.cuda.current_stream().cuda_stream), f"{epi} Beff={Beff} L={L}")
+    return op, out, mom
+
+
+@pytest.mark.parametrize("epi", list(ONE_OP_EPIS))
+def test_one_op_every_chart_equals_the_chart_alone(epi):
+    """for L in {48, 200, 512}, B in {3, 8, 32} charts and a one-chart unit of 1 and 2 samples: each sample's rows (and row moments)
+    of the B-chart op, kind and split chosen by engine.unit_batch_splits, equal the one-chart op's; the serial kind is taken at least
+    once"""
+    eng = model_for(96).engine
+    e = ONE_OP_EPIS[epi]
+    K, N = 256, 192
+    kinds = set()
+    for L in (48, 200, 512):
+        for unit in (1, 2):
+            name = f"{epi}.{L}.{unit}"
+            kt = e.get("taps", 1) * K
+            W = synth._gauss(synth._rng(5, name + ".W"), (N, kt)) / kt ** 0.5
+            hi, lo = packer.tf32_split(W)
+            A = synth._gauss(synth._rng(5, name + ".A"), (unit * L, K))
+            a64 = A.double()
+            x = dict(unit=unit, A=A, W=W.cuda(), hi=hi.cuda(), lo=lo.cuda(), bias=(0.1 * synth._gauss(synth._rng(5, name + ".b"), (N,))).cuda(),
+                     table=synth._gauss(synth._rng(5, name + ".t"), (unit, N)), res=synth._gauss(synth._rng(5, name + ".r"), (unit * L, N)),
+                     stats=torch.stack([a64.sum(1), (a64 * a64).sum(1)], dim=1), colsum=W.double().sum(1).float().cuda())
+            keep = []
+            _, one, mom1 = _one_op(eng, epi, unit, L, x, keep)
+            for B in (3, 8, 32):
+                op, many, mom = _one_op(eng, epi, B * unit, L, x, keep)
+                kinds.add(op.kind)
+                torch.cuda.synchronize()
+                what = (epi, L, unit, B, op.kind, op.u.gemm.split_k)
+                assert not torch.isnan(many).any(), what
+                assert torch.equal(many.view(B, unit * L, -1), one.view(1, unit * L, -1).expand(B, -1, -1)), what
+                if mom is not None:
+                    assert torch.equal(mom.view(B, unit * L, 2), mom1.view(1, unit * L, 2).expand(B, -1, -1)), what
+    assert L_.OP_GEMM_SERIAL in kinds, epi
 
 
 # ---- 2. op by op: every output row of a plan for B charts is the one-chart plan's --------------------------------------------------
