@@ -64,7 +64,10 @@ enum mugd_op_kind {
      * every output tile run one after another in one CTA, summed in the split-K reduce's order, then the fused epilogue.  The result
      * equals MUGD_OP_GEMM with the same split_k bit for bit, without the workspace and the reduce launch.  Batch-invariant plans use
      * it where a one-chart K split would put too many partial tiles on a large batch. */
-    MUGD_OP_GEMM_SERIAL = 17
+    MUGD_OP_GEMM_SERIAL = 17,
+    /* classifier-free guidance at one scale per chart (mugd_cfg_scales): the guided noise prediction of B charts from the 2B eps rows of
+     * an evaluation, for a sampler update that then runs unguided (cfg = 0) on the output rows */
+    MUGD_OP_CFG_SCALES = 18
 };
 
 /* A-operand row addressing of MUGD_OP_GEMM (rows are tokens of B samples, Lout output rows each) */
@@ -235,6 +238,18 @@ typedef struct mugd_row_mask {
     int32_t B, L, cols, reserved_;
 } mugd_row_mask;
 
+/* Classifier-free guidance with one scale per chart (MUGD_OP_CFG_SCALES).  For chart b = row / L of the B*L output rows:
+ *   out[row][c] = e_u + s_b * (e_c - e_u)   (the update kernels' guidance expression: __fsub_rn, __fmul_rn, __fadd_rn, no contraction)
+ *   out[row][c] = e_c                        when s_b == 1 (no guidance: the uncond row is not read)
+ * with e_u = eps[row][c] (the uncond half, rows 0 .. B*L - 1) and e_c = eps[B*L + row][c] (the cond half).  The scales are device
+ * data, so one captured plan serves any mix.  out must not overlap the eps rows. */
+typedef struct mugd_cfg_scales {
+    const float* eps; int64_t ld;          /* [2B*L, ld] columns 0 .. C - 1: uncond rows first              */
+    float* out;                            /* [B*L, C] dense                                                */
+    const float* scales;                   /* [B] device: the guidance scale of each chart (finite)         */
+    int32_t B, L, C, reserved_;
+} mugd_cfg_scales;
+
 typedef struct mugd_op {
     int32_t kind;
     int32_t tag;                           /* free for the host (profiling labels)                          */
@@ -243,6 +258,7 @@ typedef struct mugd_op {
         mugd_ddim_update ddim; mugd_transpose tr; mugd_copy2d cp; mugd_step_advance adv; mugd_notes notes;
         mugd_embed embed; mugd_tf32_split split; mugd_posterior post;
         mugd_groupnorm_var gnv; mugd_attention_var attnv; mugd_row_mask mask;   /* ragged batches (same union size) */
+        mugd_cfg_scales cfgs;                                                   /* per-chart guidance scales        */
     } u;
 } mugd_op;
 
@@ -685,7 +701,8 @@ int  mugd_debug_set_tc_timing(long long* device_buf);
 int  mugd_fill_i32(int32_t* dst, int32_t value, void* stream);
 /* sizeof() of {mugd_op, mugd_gemm, mugd_groupnorm, mugd_layernorm, mugd_attention, mugd_s4conv, mugd_ddim_update, mugd_transpose,
  * mugd_copy2d, mugd_notes, mugd_embed, mugd_tf32_split, mugd_posterior} so a foreign-language mirror can verify its layout; with
- * n >= 16 also {mugd_groupnorm_var, mugd_attention_var, mugd_row_mask} in entries 13..15 (n >= 13 is enough for the first 13) */
+ * n >= 16 also {mugd_groupnorm_var, mugd_attention_var, mugd_row_mask} in entries 13..15, with n >= 17 also mugd_cfg_scales in entry 16
+ * (n >= 13 is enough for the first 13) */
 int  mugd_abi_sizes(int32_t* out, int32_t n);
 
 #ifdef __cplusplus

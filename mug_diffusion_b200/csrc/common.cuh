@@ -67,6 +67,8 @@ int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_
 int launch_groupnorm_var(const DeviceInfo& dev, const mugd_groupnorm_var& g, cudaStream_t st, int* launches);
 int launch_attention_var(const DeviceInfo& dev, const mugd_attention_var& a, cudaStream_t st, int* launches);
 int launch_row_mask(const DeviceInfo& dev, const mugd_row_mask& m, cudaStream_t st, int* launches);
+// per-chart guidance scales (elementwise.cu)
+int launch_cfg_scales(const DeviceInfo& dev, const mugd_cfg_scales& g, cudaStream_t st, int* launches);
 // mugd_sample_staged: check_stage validates a stage for n_steps (host arrays included); launch_stage runs step i of it
 int check_stage(const mugd_stage& s, int32_t n_steps);
 int launch_stage(const mugd_stage& s, int32_t i, cudaStream_t st);
@@ -173,13 +175,17 @@ inline cudaError_t allow_dynamic_smem(int bytes, Kernels... kernels) {
 // (at entry, in the short kernels only, after the GEMM main loop) were tried and not kept.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// The noise prediction of element i of the sampler's eps rows: with cfg, the guidance combine e_u + scale * (e_c - e_u) of the
-// uncond half [0, n) and the cond half [n, 2n) (ddim.py:175), each operation one IEEE round-to-nearest in torch's eager order, no
-// contraction.  Every update kernel forms e here, so all of them match torch bit for bit.
+// The guidance combine e_u + scale * (e_c - e_u) (ddim.py:175), each operation one IEEE round-to-nearest in torch's eager order, no
+// contraction.  cfg_eps and the per-chart-scale kernel (MUGD_OP_CFG_SCALES) both form it here, so they agree bit for bit.
+__device__ __forceinline__ float cfg_guide(float eu, float ec, float scale) {
+    return __fadd_rn(eu, __fmul_rn(scale, __fsub_rn(ec, eu)));
+}
+
+// The noise prediction of element i of the sampler's eps rows: with cfg, cfg_guide of the uncond half [0, n) and the cond half
+// [n, 2n).  Every update kernel forms e here, so all of them match torch bit for bit.
 __device__ __forceinline__ float cfg_eps(const float* eps, int64_t i, int64_t n, int cfg, float scale) {
     if (!cfg) return eps[i];
-    const float eu = eps[i], ec = eps[n + i];
-    return __fadd_rn(eu, __fmul_rn(scale, __fsub_rn(ec, eu)));
+    return cfg_guide(eps[i], eps[n + i], scale);
 }
 
 // Loads the 32x32 tile at (c0, l0) of one sample's NCL rows `in` [C, L] into tile[c - c0][l - l0], coalesced along L by a CTA of

@@ -4,6 +4,7 @@
 //   transpose   : [B,C,L] <-> channels-last [B*L, ld] at the Python boundary (reference tensors are NCL)
 //   copy2d      : strided row copy (the 4 per-level tensors that live in two concat buffers)
 //   step_advance: device-side step counter so one CUDA graph serves every DDIM step
+//   cfg_scales  : classifier-free guidance at one scale per chart, in front of an unguided update
 //   posterior   : first-stage encoder moments -> mean / logvar / std / z   mug/firststage/autoencoder.py:356-387
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -204,6 +205,56 @@ int launch_row_mask(const DeviceInfo& dev, const mugd_row_mask& m, cudaStream_t 
     int blocks = (int)((per_sample + 255) / 256);
     if (blocks > 64) blocks = 64;
     MUGD_CHECK_CUDA(launch_k(row_mask_kernel, dim3(blocks, m.B), dim3(256), 0, st, m));
+    if (launches) *launches += 1;
+    return MUGD_OK;
+}
+
+// Per-chart guidance scales (MUGD_OP_CFG_SCALES): output row r belongs to chart r / L and gets cfg_guide(e_u, e_c, s_b), or e_c itself
+// where s_b == 1 (the uncond row is then not read).  VEC: four columns per thread through 16-byte loads and stores (C and ld multiples
+// of 4, eps and out 16-byte aligned); otherwise one element per thread.
+template <bool VEC>
+__global__ void __launch_bounds__(256)
+cfg_scales_kernel(const mugd_cfg_scales g) {
+    pdl_wait();
+    constexpr int W = VEC ? 4 : 1;
+    const int cw = g.C / W;
+    const int rows = g.B * g.L;                           // the launcher keeps B * L * C within int32
+    const int total = rows * cw;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+        const int r = i / cw;
+        const int c = (i - r * cw) * W;
+        const float s = g.scales[r / g.L];
+        const float* pu = g.eps + (int64_t)r * g.ld + c;
+        const float* pc = pu + (int64_t)rows * g.ld;
+        float* po = g.out + (int64_t)r * g.C + c;
+        if constexpr (VEC) {
+            const float4 ec = ld_f4(pc);
+            if (s == 1.0f) {
+                st_f4(po, ec);
+            } else {
+                const float4 eu = ld_f4(pu);
+                st_f4(po, make_float4(cfg_guide(eu.x, ec.x, s), cfg_guide(eu.y, ec.y, s), cfg_guide(eu.z, ec.z, s),
+                                      cfg_guide(eu.w, ec.w, s)));
+            }
+        } else {
+            *po = s == 1.0f ? *pc : cfg_guide(*pu, *pc, s);
+        }
+    }
+}
+
+int launch_cfg_scales(const DeviceInfo& dev, const mugd_cfg_scales& g, cudaStream_t st, int* launches) {
+    MUGD_REQUIRE(g.eps && g.out && g.scales, "cfg_scales: eps, out and scales must be given");
+    MUGD_REQUIRE(g.B > 0 && g.L > 0 && g.C > 0 && g.ld >= g.C && (int64_t)g.B * g.L * g.C <= INT32_MAX,
+                 "cfg_scales: bad shape B=%d L=%d C=%d ld=%lld", g.B, g.L, g.C, (long long)g.ld);
+    const int64_t rows = (int64_t)g.B * g.L;
+    const uintptr_t e0 = reinterpret_cast<uintptr_t>(g.eps), e1 = e0 + 4 * ((2 * rows - 1) * g.ld + g.C);
+    const uintptr_t o0 = reinterpret_cast<uintptr_t>(g.out), o1 = o0 + 4 * rows * g.C;
+    MUGD_REQUIRE(o1 <= e0 || e1 <= o0, "cfg_scales: out overlaps the eps rows");
+    const bool vec = g.C % 4 == 0 && g.ld % 4 == 0 && aligned16(g.eps) && aligned16(g.out);
+    const int64_t total = rows * (vec ? g.C / 4 : g.C);
+    int blocks = (int)((total + 255) / 256 < (int64_t)dev.sm_count * 8 ? (total + 255) / 256 : (int64_t)dev.sm_count * 8);
+    if (vec) MUGD_CHECK_CUDA(launch_k(cfg_scales_kernel<true>, dim3(blocks), dim3(256), 0, st, g));
+    else MUGD_CHECK_CUDA(launch_k(cfg_scales_kernel<false>, dim3(blocks), dim3(256), 0, st, g));
     if (launches) *launches += 1;
     return MUGD_OK;
 }

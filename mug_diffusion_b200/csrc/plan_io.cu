@@ -51,6 +51,7 @@ static const PtrField k_ptr_fields[] = {
     PF(MUGD_OP_GEMM_SERIAL, gemm.residual), PF(MUGD_OP_GEMM_SERIAL, gemm.C), PF(MUGD_OP_GEMM_SERIAL, gemm.workspace),
     PF(MUGD_OP_GEMM_SERIAL, gemm.counters), PF(MUGD_OP_GEMM_SERIAL, gemm.A2), PF(MUGD_OP_GEMM_SERIAL, gemm.row_moments),
     PF(MUGD_OP_GEMM_SERIAL, gemm.ln_stats), PF(MUGD_OP_GEMM_SERIAL, gemm.ln_colsum),
+    PF(MUGD_OP_CFG_SCALES, cfgs.eps), PF(MUGD_OP_CFG_SCALES, cfgs.out), PF(MUGD_OP_CFG_SCALES, cfgs.scales),
 };
 #undef PF
 

@@ -252,6 +252,23 @@ def unit_batch_splits(ops: OpList, B: int, unit: int, sm_count: int) -> OpList:
     return ops
 
 
+def guided_scales_ops(ops: OpList, xin: View, eps: View, B: int, Lz: int, out: int, scales: int) -> OpList:
+    """The U-Net plan of a request with one guidance scale per chart (DESIGN §6b N19), around ``ops``, the plan of its 2B samples
+    (uncond half first, input rows ``xin``, output rows ``eps``): a copy of the B charts' x rows into the second half (the sampler's
+    update writes the first half only), ``ops`` op for op, then MUGD_OP_CFG_SCALES from the eps rows into ``out`` ([B*Lz, C] dense,
+    the guided noise prediction the update reads unguided) at the device scales ``scales`` [B]."""
+    half = B * Lz
+    assert xin.rows == eps.rows == 2 * half, (xin.rows, eps.rows, half)
+    g = OpList(ops.tc_map, ops.valid)
+    g.copy2d(xin.r(0, half), xin.r(half, 2 * half), TAG_IO)
+    g.ops.extend(ops.ops)
+    d = L_.CfgScales()
+    d.eps, d.ld, d.out, d.scales = eps.ptr, eps.ld, out, scales
+    d.B, d.L, d.C = B, Lz, eps.cols
+    g.add(L_.OP_CFG_SCALES, d, TAG_IO)
+    return g
+
+
 def emit_upsample_conv(ops: "OpList", blob: WeightBlob, wfn, prefix: str, x: View, out: View, Lin: int, cin: int, cout: int, tag: int):
     """Upsample (nearest x2) + conv3 (models.py:66-70).  With the parity-split weights of the packer this is two 2-tap
     GEMMs over the Lin input rows writing the even / odd output rows (row stride 2*ld) -- 2/3 of the FLOPs of the

@@ -13,8 +13,8 @@ from torch.utils.weak import WeakIdKeyDictionary
 from . import lib as L_
 from .audio import check_z_length
 from .config import EncoderConfig, ModelConfig
-from .engine import (Arena, CTX_TOKENS_MAX, DecoderCompiler, EncoderCompiler, MAX_STEPS, OpList, UNetCompiler, View, tc_weight_map,
-                     unit_batch_splits)
+from .engine import (Arena, CTX_TOKENS_MAX, DecoderCompiler, EncoderCompiler, MAX_STEPS, OpList, UNetCompiler, View,
+                     guided_scales_ops, tc_weight_map, unit_batch_splits)
 from .packer import WeightBlob, pack_model
 
 
@@ -285,14 +285,18 @@ class MugEngine:
             cache.move_to_end(key)
         return s
 
-    def session(self, Beff: int, Lz: int, per_sample_t: bool = False, ragged: bool = False, unit: int = 1) -> "Session":
+    def session(self, Beff: int, Lz: int, per_sample_t: bool = False, ragged: bool = False, unit: int = 1,
+                guided: bool = False) -> "Session":
         """the compiled U-Net of (Beff, Lz).  ``ragged``: the plan for samples padded to Lz whose valid lengths are set per request
         (Session.set_lengths); a separate session, so requests without lengths keep today's plan.  ``unit``: samples per chart (2 under
-        classifier-free guidance); with batch_invariant the plan sums as the plan of ``unit`` samples does, else it is ignored."""
+        classifier-free guidance); with batch_invariant the plan sums as the plan of ``unit`` samples does, else it is ignored.
+        ``guided``: Beff = 2B samples of B charts under classifier-free guidance with one scale per chart, set per request
+        (Session.set_scales); a separate session, so requests with one scale keep today's plan."""
         check_z_length(Lz)
         unit = unit if self.batch_invariant else 1
-        key = (Beff, Lz, per_sample_t) + (("ragged",) if ragged else ()) + ((("unit", unit),) if self.batch_invariant else ())
-        return self._lru_get(self.sessions, key, lambda: Session(self, Beff, Lz, per_sample_t, ragged=ragged, unit=unit))
+        key = ((Beff, Lz, per_sample_t) + (("ragged",) if ragged else ()) + ((("unit", unit),) if self.batch_invariant else ())
+               + (("guided",) if guided else ()))
+        return self._lru_get(self.sessions, key, lambda: Session(self, Beff, Lz, per_sample_t, ragged=ragged, unit=unit, guided=guided))
 
     def wave_session(self, B: int, T: int):
         """Audio encoder plan for B mel-spectrograms of T frames (SURVEY §8f N1); needs wave weights in the blob."""
@@ -331,7 +335,11 @@ class MugEngine:
 class Session:
     """Compiled U-Net evaluation for Beff samples of length Lz (Beff = 2B under classifier-free guidance)."""
 
-    def __init__(self, engine: MugEngine, Beff: int, Lz: int, per_sample_t: bool, ragged: bool = False, unit: int = 1):
+    scales: Optional[torch.Tensor] = None     # a guided session's per-chart scales (None: not a guided session)
+    e_guided: Optional[torch.Tensor] = None   # and the guided noise prediction its plan writes
+
+    def __init__(self, engine: MugEngine, Beff: int, Lz: int, per_sample_t: bool, ragged: bool = False, unit: int = 1,
+                 guided: bool = False):
         self.engine, self.Beff, self.Lz, self.per_sample_t = engine, Beff, Lz, per_sample_t
         self.unit = unit                      # samples of one chart: the batch the batch-invariant policy plans for
         cfg = engine.cfg.unet
@@ -339,6 +347,11 @@ class Session:
         # ragged: valid rows of each sample at every level ([levels, Beff] int32, row l = L_b >> l), data of the captured graph
         self.valid = torch.tensor([[Lz >> l] * Beff for l in range(cfg.levels)], dtype=torch.int32, device=dev) if ragged else None
         self.lens: Optional[List[int]] = None
+        # guided: one guidance scale per chart of the Beff / 2 charts ([B] float32, data of the captured graph) and the guided noise
+        # prediction [B*Lz, C] the plan's last op writes; every update descriptor of the session reads it unguided
+        assert not guided or (Beff % 2 == 0 and not per_sample_t), (Beff, per_sample_t)
+        self.scales = torch.ones(Beff // 2, device=dev) if guided else None
+        self.e_guided = torch.zeros(Beff // 2 * Lz, cfg.out_channels, device=dev) if guided else None
         self.comp = UNetCompiler(cfg, engine.blob, engine.wbase, engine.tc_map)
         emb_total = engine.blob.meta["emb_total"]
         attn_blocks = [b for b in self.comp.lay.blocks() if b.kind == "attn"]
@@ -410,8 +423,15 @@ class Session:
         if fold is None and self.engine.batch_invariant:
             fold = self.unit * self.Lz < 8192      # the compiler's size rule (UNetCompiler.compile), taken at one chart's rows
         valid = None if self.valid is None else [_ptr(self.valid[l]) for l in range(self.valid.shape[0])]
-        self.arena_t, res, self.plan = compile_sized(self.engine, lambda arena: self.comp.compile(
-            arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold, valid), batch=(self.Beff, self.unit))
+
+        def compile_fn(arena):
+            res = self.comp.compile(arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold, valid)
+            if self.scales is not None:
+                res["ops"] = guided_scales_ops(res["ops"], res["xin"], res["eps"], self.Beff // 2, self.Lz, _ptr(self.e_guided),
+                                               _ptr(self.scales))
+            return res
+
+        self.arena_t, res, self.plan = compile_sized(self.engine, compile_fn, batch=(self.Beff, self.unit))
         self.xin: View = res["xin"]
         self.eps: View = res["eps"]
         self.audio_slots = res["audio_slots"]
@@ -433,6 +453,13 @@ class Session:
         t = torch.tensor([[v >> l for v in lens] for l in range(self.valid.shape[0])], dtype=torch.int32)
         self.valid.copy_(t.to(self.engine.device))
         self.lens = lens
+
+    def set_scales(self, scales: Sequence[float]):
+        """a guided session's guidance scale of each of its Beff / 2 charts (finite; 1 = no guidance for that chart): written into
+        the device array the plan reads, so the captured graph serves any mix"""
+        assert self.scales is not None, "set_scales needs a guided session"
+        assert len(scales) == self.scales.numel(), (len(scales), self.scales.numel())
+        self.scales.copy_(torch.tensor([float(v) for v in scales], dtype=torch.float32).to(self.engine.device))
 
     def set_timestep_table(self, timesteps: Sequence[int]):
         """Time-embedding MLP + all ResBlock emb projections for the given timesteps, one row each
@@ -565,17 +592,25 @@ class Session:
 
     def _x_rows(self, B: int, cfg_on: bool):
         """the device addresses of the x rows a step updates: the first B samples' xin rows, and under classifier-free guidance
-        their copy in the second half (else None)"""
-        return self.xin.ptr, (self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on else None)
+        their copy in the second half (else None; also on a guided session, whose plan copies them itself)"""
+        return self.xin.ptr, (self.xin.r(B * self.Lz, 2 * B * self.Lz).ptr if cfg_on and self.scales is None else None)
+
+    def _guidance(self, cfg_on: bool, scale) -> Tuple[int, int, float]:
+        """(eps rows, cfg, scale) of an update: the plan's eps rows with the request's guidance, or on a guided session the guided
+        rows the plan's last op wrote, read unguided"""
+        if self.scales is not None:
+            return _ptr(self.e_guided), 0, 1.0
+        return self.eps.ptr, int(cfg_on), 1.0 if isinstance(scale, list) else float(scale)
 
     def ddim_update(self, B: int, S: int, cfg_on: bool, scale: float, temperature: float, pred_x0: int, noise: int = 0) -> L_.DdimUpdate:
         """the DDIM update of ddim_tail"""
         n = B * self.Lz * self.engine.cfg.unet.in_channels
         upd = L_.DdimUpdate()
         upd.x, upd.x_dup = self._x_rows(B, cfg_on)
-        upd.eps, upd.noise, upd.pred_x0 = self.eps.ptr, noise or None, pred_x0
+        upd.eps, upd.cfg, upd.scale = self._guidance(cfg_on, scale)
+        upd.noise, upd.pred_x0 = noise or None, pred_x0
         upd.coef, upd.step = _ptr(self.coef), _ptr(self.step)
-        upd.S, upd.n, upd.cfg, upd.scale, upd.temperature = S, n, int(cfg_on), float(scale), float(temperature)
+        upd.S, upd.n, upd.temperature = S, n, float(temperature)
         return upd
 
     def plms(self, B: int, S: int, cfg_on: bool, scale: float, pred_x0: int, work: torch.Tensor) -> L_.Plms:
@@ -587,8 +622,8 @@ class Session:
         p = L_.Plms()
         p.update = self.ddim_update(B, S, cfg_on, 1.0, 1.0, pred_x0)
         p.update.cfg, p.update.eps = 0, _ptr(work[0])
-        p.eps, p.e_prime, p.hist, p.x_stash = self.eps.ptr, _ptr(work[0]), _ptr(work[1]), _ptr(work[4])
-        p.cfg, p.scale = int(cfg_on), float(scale)
+        p.eps, p.cfg, p.scale = self._guidance(cfg_on, scale)
+        p.e_prime, p.hist, p.x_stash = _ptr(work[0]), _ptr(work[1]), _ptr(work[4])
         return p
 
     def ddpm(self, B: int, T: int, cfg_on: bool, scale: float, clip: bool, pred_x0: int, noise: int, coef: torch.Tensor) -> L_.Ddpm:
@@ -598,9 +633,10 @@ class Session:
         assert coef.shape == (T, 5) and coef.dtype == torch.float32 and coef.is_contiguous()
         d = L_.Ddpm()
         d.x, d.x_dup = self._x_rows(B, cfg_on)
-        d.eps, d.pred_x0, d.noise, d.coef, d.step = self.eps.ptr, pred_x0 or None, noise, _ptr(coef), _ptr(self.step)
+        d.eps, d.cfg, d.scale = self._guidance(cfg_on, scale)
+        d.pred_x0, d.noise, d.coef, d.step = pred_x0 or None, noise, _ptr(coef), _ptr(self.step)
         d.T, d.B, d.C, d.L = T, B, self.engine.cfg.unet.in_channels, self.Lz
-        d.cfg, d.scale, d.clip = int(cfg_on), float(scale), int(bool(clip))
+        d.clip = int(bool(clip))
         return d
 
     def dpm(self, B: int, S: int, cfg_on: bool, scale: float, pred_x0: int, ring: torch.Tensor, coef: torch.Tensor) -> L_.Dpm:
@@ -612,8 +648,9 @@ class Session:
         assert ring.shape == (3, n) and ring.dtype == torch.float32 and ring.is_contiguous()
         d = L_.Dpm()
         d.x, d.x_dup = self._x_rows(B, cfg_on)
-        d.eps, d.pred_x0, d.ring, d.coef, d.step = self.eps.ptr, pred_x0 or None, _ptr(ring), _ptr(coef), _ptr(self.step)
-        d.n, d.S, d.cfg, d.scale = n, S, int(cfg_on), float(scale)
+        d.eps, d.cfg, d.scale = self._guidance(cfg_on, scale)
+        d.pred_x0, d.ring, d.coef, d.step = pred_x0 or None, _ptr(ring), _ptr(coef), _ptr(self.step)
+        d.n, d.S = n, S
         return d
 
     def dpm_ex(self, dpm: L_.Dpm, stage: Optional[L_.Stage] = None, B: int = 0, start: Optional[torch.Tensor] = None,

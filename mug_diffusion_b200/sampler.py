@@ -470,6 +470,10 @@ class _DeviceLoopSampler:
     """The constructor, the per-request session load and the request loop (``_run_request``) of every sampler here, and the
     encode launch and latent check of the samplers that remix a chart."""
 
+    # True: every guided request runs on the per-chart-scale session (DESIGN §6b N19), one shared scale included, so tests and
+    # tools/bench_guidance.py can hold that path against today's.  False (the default): only a mix of scales takes it.
+    force_per_chart_scales = False
+
     def __init__(self, model, schedule="linear", **kwargs):
         if not isinstance(model, MugDiffusionB200):
             model = MugDiffusionB200.from_reference(model)
@@ -496,13 +500,20 @@ class _DeviceLoopSampler:
     def _load_session(self, w, c, shape, x_T, scale, uc, time_range, lens=None):
         """x_T (drawn when not given), whether classifier-free guidance is on, and the session of this shape with the timestep table
         (row i = time_range[i], the i-th loop iteration), context, audio and x loaded, its step counter at 0.  ``lens``: a ragged
-        request (ragged_lengths), run on the ragged session of this shape with the charts' lengths set."""
+        request (ragged_lengths), run on the ragged session of this shape with the charts' lengths set.  ``scale``: a number, or a
+        mix of per-chart scales (guidance_scales' list), run on the guided session of this shape with the charts' scales set; its
+        update descriptors read the guided noise prediction unguided."""
         model = self.model
         B, Cz, Lz = shape
         x = self._x_T(shape, x_T)
         cfg_on = not (uc is None or scale == 1.)
         Beff = 2 * B if cfg_on else B
-        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False, ragged=lens is not None, unit=2 if cfg_on else 1)
+        scales = scale if isinstance(scale, list) else [float(scale)] * B if self.force_per_chart_scales else None
+        guided = cfg_on and scales is not None
+        sess: Session = model.engine.session(Beff, Lz, per_sample_t=False, ragged=lens is not None, unit=2 if cfg_on else 1,
+                                             **({"guided": True} if guided else {}))
+        if guided:
+            sess.set_scales(scales)
         if lens is not None:
             sess.set_lengths(list(lens) * 2 if cfg_on else lens)
         sess.set_timestep_table(time_range.copy())
@@ -634,7 +645,7 @@ class _DeviceLoopSampler:
                              + (f", got {x0.dtype} {tuple(x0.shape)} on {x0.device}" if isinstance(x0, torch.Tensor) else ""))
         B = int(x0.shape[0])
         stops = per_chart_steps(B, t_enc, inv.S, "t_enc", f" (S = {inv.S})")
-        scale = _finite_scale(scale)
+        scale = guidance_scales(_finite_scale(scale), B)
         request_size(model, c, B, z_shape, None, None, None, scale, uc, log_every_t)
         if c is None or w is None:
             raise ValueError("invert needs the conditioning c and the audio features w")
@@ -808,10 +819,36 @@ def _conditioning(c, conditioning):
     return conditioning
 
 
+def _per_chart(scale) -> bool:
+    """whether ``unconditional_guidance_scale`` gives one scale per chart (a sequence) rather than one number"""
+    return isinstance(scale, (list, tuple)) or isinstance(scale, (np.ndarray, torch.Tensor)) and scale.ndim > 0
+
+
 def _finite_scale(scale):
+    """a one-number scale checked; one scale per chart passes through to guidance_scales, which checks it against the batch"""
+    if _per_chart(scale):
+        return scale
     if isinstance(scale, bool) or not isinstance(scale, (int, float, np.floating)) or not np.isfinite(scale):
         raise ValueError(f"unconditional_guidance_scale={scale!r} must be a finite number")
     return scale
+
+
+def guidance_scales(scale, B: int):
+    """``unconditional_guidance_scale`` of a request of B charts: one number, returned as given (today's path), or one finite number
+    per chart (a list, tuple, numpy array or torch tensor of B), returned as their shared float when all are equal (today's path:
+    same session, plan and bits; all 1 is the unguided request) and as a list of B floats for a mix (DESIGN §6b N19: chart b guided
+    at scale s_b, exactly e_c where s_b == 1).  ValueError for a wrong count, a bool, a non-number or a non-finite entry."""
+    if not _per_chart(scale):
+        return scale
+    vals = scale.tolist() if isinstance(scale, (np.ndarray, torch.Tensor)) else list(scale)
+    if len(vals) != B:
+        raise ValueError(f"unconditional_guidance_scale has {len(vals)} entries for {B} charts")
+    for v in vals:
+        if (isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating))
+                or not np.isfinite(float(v))):
+            raise ValueError(f"unconditional_guidance_scale={vals!r}: every entry must be a finite number")
+    vals = [float(v) for v in vals]
+    return vals[0] if all(v == vals[0] for v in vals) else vals
 
 
 def per_chart_steps(B: int, value, n: int, name: str, where: str = "") -> list:
@@ -915,6 +952,7 @@ class DDIMSampler(_DeviceLoopSampler):
         the chart requested alone at z_length z_lengths[b] (with seeds, the same seed), its result 0 past that length; inpainting,
         noise_dropout and match_reference_rng without seeds are refused with it (MugdError)."""
         B, Cz, Lz = shape
+        unconditional_guidance_scale = guidance_scales(unconditional_guidance_scale, B)
         seeds = _request_seeds(seeds, B, noise_dropout, match_reference_rng)
         lens = _ragged_request(z_lengths, shape, mask, x0, noise_dropout, match_reference_rng, seeds)
         model = self.model
@@ -1059,8 +1097,8 @@ class DDIMSampler(_DeviceLoopSampler):
             raise ValueError("decode runs at eta = 0: call make_schedule(S, ddim_eta=0.)")
         self._check_latent(x_latent)
         starts = self._decode_starts(x_latent, t_start)
-        scale, uc = unconditional_guidance_scale, unconditional_conditioning
         B, Cz, Lz = (int(v) for v in x_latent.shape)
+        scale, uc = guidance_scales(unconditional_guidance_scale, B), unconditional_conditioning
         shape = (B, Cz, Lz)
         request_size(model, c, B, (Cz, Lz), x_latent, None, None, scale, uc, 1)
         if w is None:
@@ -1128,6 +1166,7 @@ def request_size(model, c, batch_size, shape, x_T, mask, x0, scale, uc, log_ever
         size = (int(batch_size), int(shape[0]), int(shape[1]))
     if size[1] != model.z_channels:
         raise ValueError(f"shape {size}: the model's latents have {model.z_channels} channels")
+    scale = guidance_scales(scale, size[0])
     cfg_on = not (uc is None or scale == 1.)
     for name, t in (("c", c), ("unconditional_conditioning", uc if cfg_on else None)):
         if t is not None and (not isinstance(t, torch.Tensor) or t.dim() != 3 or t.shape[0] != size[0]):
@@ -1204,6 +1243,7 @@ class PLMSSampler(DDIMSampler):
         """plms.py:115-170 (and p_sample_plms, :172-236) on the GPU.  ``timesteps=k`` runs the truncated schedule of plms.py:128-136
         (t_next and the warm-up follow it); ``ddim_use_original_steps=True`` raises as in ddim_sampling; ``z_lengths`` as there."""
         B, Cz, Lz = shape
+        scale = guidance_scales(unconditional_guidance_scale, B)
         seeds = _request_seeds(seeds, B, noise_dropout, match_reference_rng)
         lens = _ragged_request(z_lengths, shape, mask, x0, noise_dropout, match_reference_rng, seeds)
         model = self.model
@@ -1213,7 +1253,6 @@ class PLMSSampler(DDIMSampler):
         if ts.shape[0] == 0:
             return self._empty_request(shape, self._seeded_start(seeds, shape, x_T, lens)[1], lens)
         match_rng = bool(match_reference_rng)
-        scale = unconditional_guidance_scale
 
         def draw(k):
             # the reference's step noise at sigma = 0 (plms.py:212-214): values discarded, generator advanced
@@ -1301,6 +1340,7 @@ class DDPMSampler(_DeviceLoopSampler):
             raise ValueError(f"clip_denoised={clip_denoised!r} must be True, False or None")
         scale = _finite_scale(unconditional_guidance_scale)
         size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
+        scale = guidance_scales(scale, size[0])
         seeds = _request_seeds(seeds, size[0])
         _ragged_request(z_lengths, size)
         if verbose:
@@ -1322,7 +1362,7 @@ class DDPMSampler(_DeviceLoopSampler):
         B, Cz, Lz = shape
         lens = _ragged_request(z_lengths, shape)
         T = self.ddpm_num_timesteps
-        scale = unconditional_guidance_scale
+        scale = guidance_scales(unconditional_guidance_scale, B)
         with eng.lock:
             seeded, x_T = self._seeded_start(seeds, shape, x_T, lens)
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_T, scale, unconditional_conditioning, np.arange(T)[::-1],
@@ -1395,7 +1435,7 @@ class DPMSolverSampler(_DeviceLoopSampler):
         scale = _finite_scale(scale)
         sched = self.make_dpm_schedule(S, order, skip_type, solver_type, lower_order_final)
         size = request_size(self.model, c, batch_size, shape, x_T, mask, x0, scale, uc, log_every_t)
-        return scale, sched, size
+        return guidance_scales(scale, size[0]), sched, size
 
     @torch.no_grad()
     def sample(self, S, c=None, w=None, batch_size=None, shape=None, x_T=None, order=2, skip_type="time_uniform",
@@ -1457,7 +1497,7 @@ class DPMSolverSampler(_DeviceLoopSampler):
         dev = self.device
         B, Cz, Lz = shape
         total = sched.S
-        scale = unconditional_guidance_scale
+        scale = guidance_scales(unconditional_guidance_scale, B)
         blend = mask is not None
         self.last_schedule = sched
         with eng.lock:
@@ -1566,8 +1606,8 @@ class DPMSolverSampler(_DeviceLoopSampler):
         self._require_schedule(sched)
         self._check_latent(x_latent)
         starts = per_chart_steps(x_latent.shape[0], t_start, sched.S, "t_start", " (S = sched.S)")
-        scale = _finite_scale(unconditional_guidance_scale)
         B, Cz, Lz = (int(v) for v in x_latent.shape)
+        scale = guidance_scales(_finite_scale(unconditional_guidance_scale), B)
         request_size(model, c, B, (Cz, Lz), x_latent, None, None, scale, unconditional_conditioning, 1)
         if c is None or w is None:
             raise ValueError("decode needs the conditioning c and the audio features w")
@@ -1586,6 +1626,7 @@ class DPMSolverSampler(_DeviceLoopSampler):
         B, Cz, Lz = (int(v) for v in x_latent.shape)
         shape = (B, Cz, Lz)
         S, m = sched.S, max(starts)
+        unconditional_guidance_scale = guidance_scales(unconditional_guidance_scale, B)
         with eng.lock:
             # the timestep table holds all S model times and the counter starts at S - m, so step i reads row i of every table
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_latent, unconditional_guidance_scale,
@@ -1649,6 +1690,7 @@ class UniPCSampler(_DeviceLoopSampler):
         scale = _finite_scale(unconditional_guidance_scale)
         sched = self.make_unipc_schedule(S, order, skip_type, variant, lower_order_final, use_corrector, disable_corrector, t_grid)
         size = request_size(self.model, c, batch_size, shape, x_T, None, None, scale, unconditional_conditioning, log_every_t)
+        scale = guidance_scales(scale, size[0])
         seeds = _request_seeds(seeds, size[0])
         _ragged_request(z_lengths, size)
         if verbose:
@@ -1680,6 +1722,7 @@ class UniPCSampler(_DeviceLoopSampler):
         scale = _finite_scale(unconditional_guidance_scale)
         sched = self.make_unipc_schedule(S, order, skip_type, variant, lower_order_final, use_corrector, disable_corrector, t_grid)
         size = request_size(self.model, c, batch_size, shape, x_T, mask, x0, scale, unconditional_conditioning, log_every_t)
+        scale = guidance_scales(scale, size[0])
         seeds = _request_seeds(seeds, size[0])
         if verbose:
             print(f'Data shape for UniPC inpainting is {size}, {S} steps of order {order} ({skip_type}, {variant})')
@@ -1699,7 +1742,7 @@ class UniPCSampler(_DeviceLoopSampler):
         dev = self.device
         B, Cz, Lz = shape
         total = sched.S
-        scale = unconditional_guidance_scale
+        scale = guidance_scales(unconditional_guidance_scale, B)
         blend = mask is not None
         self.last_schedule = sched
         with eng.lock:
@@ -1790,8 +1833,8 @@ class UniPCSampler(_DeviceLoopSampler):
         self._require_schedule(sched)
         self._check_latent(x_latent)
         starts = per_chart_steps(x_latent.shape[0], t_start, sched.S, "t_start", " (S = sched.S)")
-        scale = _finite_scale(unconditional_guidance_scale)
         B, Cz, Lz = (int(v) for v in x_latent.shape)
+        scale = guidance_scales(_finite_scale(unconditional_guidance_scale), B)
         request_size(model, c, B, (Cz, Lz), x_latent, None, None, scale, unconditional_conditioning, 1)
         if c is None or w is None:
             raise ValueError("decode needs the conditioning c and the audio features w")
@@ -1810,6 +1853,7 @@ class UniPCSampler(_DeviceLoopSampler):
         B, Cz, Lz = (int(v) for v in x_latent.shape)
         shape = (B, Cz, Lz)
         S, m = sched.S, max(starts)
+        unconditional_guidance_scale = guidance_scales(unconditional_guidance_scale, B)
         with eng.lock:
             # the timestep table holds all S model times and the counter starts at S - m, so step i reads row i of every table
             x, cfg_on, sess, time_range = self._load_session(w, c, shape, x_latent, unconditional_guidance_scale,
