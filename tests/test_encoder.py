@@ -240,24 +240,35 @@ def test_library_abi_has_posterior():
 _model = {}
 
 
-def _encoder_model(L=96):
+def _encoder_model(L=96, impl="auto"):
     from mug_diffusion_b200.sampler import MugDiffusionB200
 
-    if L not in _model:
+    if (L, impl) not in _model:
         _model.clear()
         sd = {**synth.synthetic_state_dict(L), **synth.synthetic_encoder_state_dict(seed=ec.ENCODER_SEED)}
-        _model[L] = MugDiffusionB200.from_state_dict(sd, z_length=L)
-    return _model[L]
+        _model[L, impl] = MugDiffusionB200.from_state_dict(sd, z_length=L, gemm_impl=impl)
+    return _model[L, impl]
 
 
 @pytest.mark.gpu
 def test_encode_matches_reference_golden(golden_dir):
+    _encode_vs_golden(golden_dir, "auto")
+
+
+@pytest.mark.gpu
+def test_encode_simt_matches_reference_golden(golden_dir):
+    """the chart encoder with every GEMM on the exact-fp32 FFMA kernel: same tolerance"""
+    _encode_vs_golden(golden_dir, "simt")
+
+
+def _encode_vs_golden(golden_dir, impl):
     g = _golden(golden_dir)
-    m = _encoder_model()
+    m = _encoder_model(impl=impl)
     post = m.model.encode({"note": _golden_notes().cuda()})
     for k in ("parameters", "mean", "logvar", "std"):
         got = getattr(post, k)
         assert got.is_cuda and got.shape == g[k].shape, k
+        print(f"encode {impl} {k} rel_err={_rel(got, g[k]):.2e}")
         assert _rel(got, g[k]) <= 1e-4, (k, _rel(got, g[k]))
     assert torch.equal(post.mode(), post.mean * 1.0)
     assert torch.equal(post.var, torch.exp(post.logvar))

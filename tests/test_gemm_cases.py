@@ -1,7 +1,9 @@
 """The GEMM tests' fp64 statement and cases, without a GPU: ref_gemm (gemm_cases.py) against independent float64 torch statements of
 every addressing mode and epilogue operand -- were it wrong in the same way as a kernel, the GPU tests would pass both -- and the
 serial-split cases against the planner and the batch-invariant plans: every class of serial op the plans contain has a GPU case,
-every case runs the K split and K-range remainder it claims, and the GPU cases launch all 16 serial instantiations."""
+every case runs the K split and K-range remainder it claims, and the GPU cases launch all 16 serial instantiations.  For the FFMA
+kernel: the bound admits a float32 computation of every case and rejects wrong kernels on each case's own operands, every class of
+FFMA op in the plans has a GPU case, every case takes the tile it claims at 132 and 114 SMs, and bad descriptors are refused."""
 import ctypes as C
 
 import pytest
@@ -12,9 +14,11 @@ from mug_diffusion_b200 import lib as L_
 from mug_diffusion_b200 import packer, synth
 from mug_diffusion_b200.config import ModelConfig
 from mug_diffusion_b200.engine import OpList
+from mug_diffusion_b200.packer import tf32_split
 
-from gemm_cases import (EPIS, EXTRA, LAYOUT_BASES, LAYOUTS, LN_EPS, MATRIX, SERIAL, SPLIT, Case, case_gemm, epilogue_of, layout_split,
-                        matrix_case, plan_serial_classes, ref_gemm, serial_class)
+from gemm_cases import (EPIS, EXTRA, FFMA_C, FFMA_SMS, LAYOUT_BASES, LAYOUTS, LN_EPS, MATRIX, SERIAL, SPLIT, STEP, Case, Operands,
+                        case_gemm, epilogue_of, ffma_bound, ffma_class, ffma_gpu_cases, ffma_tile, layout_split, matrix_case,
+                        plan_ffma_classes, plan_serial_classes, ref_finish, ref_gemm, rowvec_rows, serial_class, src_rows)
 
 SMS = 132
 
@@ -224,3 +228,188 @@ def test_epilogue_of_matches_the_op_fields():
     for e, kw in EPIS.items():
         c = Case(2, 100, 100, 128, 192, rowvec="", residual=False, **kw)
         assert epilogue_of(_gemm(c, 2)) == e
+
+
+# ---- the FFMA kernel: the generic Upsample, the error bound, the plan classes and the host refusals ---------------------------
+def test_generic_upsample_conv_up():
+    """CONV_UP: nearest x2 then conv3, output row l tap t reads source (l+t-1) >> 1 where 0 <= l+t-1 < Lout"""
+    for L in (1, 2, 9):
+        B, K, N = 2, 16, 24
+        x, w, b = rnd("x", B, K, L), rnd("w", N, K, 3), rnd("b", N)
+        want = F.conv1d(x.repeat_interleave(2, dim=-1), w, b, padding=1)
+        got = ref_gemm(rows(x), packer._conv3(w), B=B, Lin=L, Lout=2 * L, K=K, taps=3, mode=L_.CONV_UP, bias=b)
+        close(got, rows(want))
+
+
+def ffma32(o: Operands):
+    """the case in float32 on the CPU, one rounding per tap sum, bias, time-embedding row and epilogue step"""
+    c = o.c
+    kw = o.kwargs()
+    a = o.A.float().reshape(c.B, c.Lin, c.K)
+    lo = torch.arange(c.Lout)
+    y = torch.zeros(c.B, c.Lout, c.N)
+    for t in range(c.taps):
+        src = src_rows(c.mode, t, lo, c.Lin, c.Lout, c.shift, c.dilation)
+        xs = torch.zeros(c.B, c.Lout, c.K)
+        xs[:, src >= 0] = a[:, src[src >= 0]]
+        y += xs @ o.W[:, t * c.K:(t + 1) * c.K].T
+    if c.K2:
+        y += o.A2.reshape(c.B, c.Lout, -1) @ o.W[:, c.taps * c.K:].T
+    y = y.reshape(c.M, c.N)
+    if o.bias is not None:
+        y = y + o.bias
+    if o.table is not None:
+        y = y + rowvec_rows(o.table, c.B, c.Lout, c.N, *c.rowvec_strides, STEP).float()
+    y = {L_.ACT_SILU: F.silu, L_.ACT_GELU: F.gelu}.get(c.act, lambda v: v)(y)
+    if c.gate:
+        y = y[:, 0::2] * (F.gelu(y[:, 1::2]) if c.gate == L_.GATE_GEGLU else torch.sigmoid(y[:, 1::2]))
+    if kw["residual"] is not None:
+        y = y + kw["residual"]
+    return y
+
+
+@pytest.fixture(scope="module")
+def ffma_operands():
+    return {name: (c, Operands(c, name)) for name, (c, _) in ffma_gpu_cases().items()}
+
+
+@pytest.fixture(scope="module")
+def ffma_refs(ffma_operands):
+    return {name: (o.ref(), ffma_bound(o)) for name, (c, o) in ffma_operands.items()}
+
+
+def test_ffma_bound_passes_a_float32_computation_of_every_case(ffma_operands, ffma_refs):
+    worst = 0.0
+    for name, (c, o) in ffma_operands.items():
+        ref, E = ffma_refs[name]
+        r = float(((ffma32(o).double() - ref).abs() / E).max())
+        worst = max(worst, r)
+        assert r <= FFMA_C, (name, r)
+        if r == worst:
+            at = name
+    print(f"at {at}: worst |y32 - y64| / E over {len(ffma_operands)} cases: {worst:.3f} (c = {FFMA_C})")
+
+
+def _clamped(mode, t, lo, Lin, Lout, *_):                       # the SAME halo clamped to the sample's edge rows
+    return (lo + t - 1).clamp(0, Lin - 1)
+
+
+def _left_padded(mode, t, lo, Lin, Lout, *_):                   # DOWN padded on the left instead of the right
+    src = 2 * lo + t - 1
+    return torch.where((src >= 0) & (src < Lin), src, torch.full_like(src, -1))
+
+
+def mutations(o: Operands) -> dict:
+    """fp64 results of wrong kernels on the case's own operands: name -> output"""
+    c, out = o.c, {}
+    for t in range(c.taps):                                     # the last k-step of a tap, and of the second source, dropped
+        W = o.W.clone()
+        W[:, (t + 1) * c.K - 16:(t + 1) * c.K] = 0
+        out[f"drop_last_kstep_of_tap{t}"] = o.ref(W=W)
+    if c.K2:
+        W = o.W.clone()
+        W[:, -16:] = 0
+        out["drop_last_k2_kstep"] = o.ref(W=W)
+    if c.mode == L_.CONV_SAME:
+        out["same_halo_clamped"] = o.ref(rows=_clamped)
+    if c.mode == L_.CONV_DOWN:
+        out["down_left_padded"] = o.ref(rows=_left_padded)
+    if c.mode == L_.CONV_TAPS:
+        out["tap_shift_off_by_one"] = o.ref(tap_shift=c.shift + 1)
+    if c.dilation > 1:
+        out["dilation_1"] = o.ref(dilation=1)
+    if c.rowvec in ("both", "batch") and c.B > 1:
+        out["rowvec_of_sample_0"] = o.ref(rowvec_b_stride=0)
+    if c.gate:
+        z = o.ref(pre=True)
+        z = torch.stack([z[:, 1::2], z[:, 0::2]], dim=2).reshape(z.shape)
+        out["gate_halves_swapped"] = ref_finish(z, c.act, c.gate, o.residual)
+    if c.residual:
+        out["residual_one_column_off"] = o.ref(residual=o.res[:, 17:17 + c.nout])
+    out["a_rounded_to_tf32"] = o.ref(A=tf32_split(o.A)[0])
+    return out
+
+
+def test_ffma_bound_rejects_wrong_kernels(ffma_operands, ffma_refs):
+    """every mutation that changes a case's fp64 result at all (a dropped k-step of a tap that only reads the zero padding, as at
+    L = 1, does not) exceeds the bound somewhere"""
+    kinds = set()
+    for name, (c, o) in ffma_operands.items():
+        ref, E = ffma_refs[name]
+        for what, y in mutations(o).items():
+            if torch.equal(y, ref):
+                continue
+            kinds.add(what.split("_of_tap")[0])
+            assert bool(((y - ref).abs() > FFMA_C * E).any()), (name, what)
+    assert {"drop_last_kstep", "drop_last_k2_kstep", "same_halo_clamped", "down_left_padded", "tap_shift_off_by_one",
+            "dilation_1", "rowvec_of_sample_0", "gate_halves_swapped", "residual_one_column_off", "a_rounded_to_tf32"} <= kinds
+
+
+def _ffma_gemm(c: Case):
+    """the FFMA descriptor test_gpu_gemm_epilogue.Device builds for ``c``, at fake 256-byte aligned addresses"""
+    names = ("a", "w", "out", "a2", "res", "bias", "table", "step")
+    ops = OpList()
+    i = case_gemm(ops, c, 0, w_hi=0, w_lo=0, impl=L_.GEMM_SIMT, **{n: (1 << 40) + (k << 32) for k, n in enumerate(names)})
+    return ops.ops[i].u.gemm
+
+
+@pytest.mark.parametrize("sms", FFMA_SMS)
+def test_every_ffma_case_takes_the_tile_it_claims(sms):
+    for name, (c, tile) in ffma_gpu_cases().items():
+        assert ffma_tile(c.M, c.N, sms) == tile, name
+        assert ffma_class(_ffma_gemm(c), sms)[-1] == tile, name
+    tiles = {t for _, t in ffma_gpu_cases().values()}
+    assert tiles == {64, 128}
+
+
+def test_every_plan_ffma_class_has_a_gpu_case():
+    """every class of GEMM the plans run on the FFMA kernel (plan_ffma_classes: default and empty TF32 map) is the class of an FFMA
+    GPU case: a plan change that makes a new class fails here, naming it"""
+    covered = {}
+    for name, (c, _) in ffma_gpu_cases().items():
+        covered.setdefault(ffma_class(_ffma_gemm(c), SMS), name)
+    plans = plan_ffma_classes()
+    print(f"{len(plans)} classes of FFMA op in the plans (mode, taps, dilated, shift, K2, act, gate, bias, rowvec, residual, strided, "
+          "K % 32, N < 64, tile):")
+    for cls, where in sorted(plans.items(), key=str):
+        print(f"  {cls}  first in {where}  <- {covered.get(cls, 'NOT COVERED')}")
+    missing = [(cls, where) for cls, where in plans.items() if cls not in covered]
+    assert not missing, missing
+    assert len(plans) >= 45
+    # the default engine's own FFMA GEMMs: the K = 16 convs (U-Net input conv into its concat window, decoder and encoder inputs)
+    assert {cls[11] for cls, where in plans.items() if where.startswith("auto")} == {True}
+
+
+def _simt_gemm(**kw):
+    """a valid FFMA descriptor at fake, aligned device addresses"""
+    g = L_.Gemm()
+    g.A, g.lda, g.W = 1 << 40, 64, 1 << 41
+    g.C, g.ldc = 1 << 43, 64
+    g.M, g.N, g.K, g.taps, g.conv_mode, g.Lin, g.Lout = 128, 64, 48, 3, L_.CONV_SAME, 64, 64
+    g.impl = L_.GEMM_SIMT
+    for k, v in kw.items():
+        setattr(g, k, v)
+    return g
+
+
+@pytest.mark.parametrize("kw,msg", [
+    (dict(W_hi=1 << 41), "split into TF32 hi/lo in place"),
+    (dict(row_moments=1 << 44), "tensor-core path only"),
+    (dict(ln_stats=1 << 44, ln_colsum=1 << 45), "tensor-core path only"),
+    (dict(K=24, lda=24), "multiple of 16"),
+    (dict(N=66), "multiple of 4"),
+    (dict(conv_mode=L_.CONV_DOWN, Lin=64, Lout=32, M=64, A2=1 << 44, lda2=16, K2=16), "second source"),
+    (dict(conv_mode=L_.CONV_UP, Lin=32, Lout=64, A2=1 << 44, lda2=16, K2=16), "second source"),
+    (dict(A=(1 << 40) + 4), "A/W alignment"),
+    (dict(C=(1 << 43) + 4), "C alignment"),
+    (dict(residual=(1 << 44) + 4, ldr=64), "residual alignment"),
+    (dict(residual=(1 << 44) + 4, ldr=64, gate=L_.GATE_GLU, ldc=32), "residual alignment"),
+], ids=["w_split_in_place", "row_moments", "folded_ln", "k24", "n66", "k2_down", "k2_up", "a_misaligned", "c_misaligned",
+        "residual_misaligned", "gated_residual_misaligned"])
+def test_ffma_refuses_bad_descriptors_before_any_device_call(kw, msg):
+    """mugd_op_run on a zeroed handle (no device behind it): every refusal comes from the host checks"""
+    lib = L_.load()
+    handle = (C.c_char * 4096)()
+    op = L_.make_op(L_.OP_GEMM, _simt_gemm(**kw))
+    assert lib.mugd_op_run(C.cast(handle, C.c_void_p), C.byref(op), None) == 1
+    assert msg in lib.mugd_last_error().decode()

@@ -1,6 +1,7 @@
 """Batch-invariant plans on the GPU (torch.equal throughout): the serial-split GEMM equals split kernel + reduce at every op the
 invariant plans launch it for; every chart of a seeded batch equals the chart requested alone, for the samplers, inpainting, remix,
-inversion, the encoder and the decoder; at one chart the invariant engine is today's engine."""
+inversion, the encoder and the decoder; at one chart the invariant engine is today's engine.  A `simt` engine keeps its plans (no serial
+split, no TF32 operand) and is batch-invariant through the FFMA kernel alone, also where a batch moves its GEMMs to 128 x 128 tiles."""
 import ctypes as C
 
 import pytest
@@ -18,15 +19,15 @@ from mug_diffusion_b200.sampler import (DDIMSampler, DDPMSampler, DPMSolverSampl
 _models = {}
 
 
-def model_for(L, invariant=True, T=1000):
-    key = (L, invariant, T)
+def model_for(L, invariant=True, T=1000, impl="auto"):
+    key = (L, invariant, T, impl)
     if key not in _models:
         if len(_models) > 1:
             _models.clear()
         cfg = ModelConfig(timesteps=T)
         sd = {**synth.synthetic_state_dict(L), **synth.synthetic_encoder_state_dict()}
         blob = packer.pack_model(sd, cfg.unet, cfg.decoder, encoder_cfg=cfg.encoder)
-        _models[key] = MugDiffusionB200(sd, cfg, z_length=L, blob=blob, batch_invariant=invariant)
+        _models[key] = MugDiffusionB200(sd, cfg, z_length=L, blob=blob, batch_invariant=invariant, gemm_impl=impl)
     return _models[key]
 
 
@@ -348,6 +349,52 @@ def test_every_chart_of_a_batch_is_the_chart_alone(L, B):
             assert torch.equal(zb[0], z[b]), (name, b)
             assert torch.equal(m.model.decode(zb)[0], logits[b]), (name, b)
             assert _notes(m, zb)[0] == notes[b], (name, b)
+
+
+def _simt_plans_are_plain(eng):
+    """every op of the `simt` engine's plans: no serial split, no K split, no TF32 hi / lo operand"""
+    plans = [s.plan._arr for s in list(eng.sessions.values()) + list(eng.dec_sessions.values())]
+    assert plans
+    for arr in plans:
+        for o in arr:
+            assert o.kind != L_.OP_GEMM_SERIAL
+            if o.kind == L_.OP_GEMM:
+                assert not o.u.gemm.W_hi and not o.u.gemm.W_lo and not o.u.gemm.split_k
+
+
+def test_simt_engine_every_chart_of_a_batch_is_the_chart_alone():
+    """gemm_impl="simt" with batch_invariant: batch_ops leaves the plans alone, and a seeded chart's z, logits and notes are still
+    the chart requested alone"""
+    L, B = 96, 4
+    m = model_for(L, impl="simt")
+    kw = request(B, L)
+    run = RUNS["ddim_eta0"]
+    z = run(m, seeds=500, **kw)
+    logits = m.model.decode(z)
+    notes = _notes(m, z)
+    for b in range(B):
+        zb = run(m, seeds=[500 + b], **one_chart(kw, b))
+        assert torch.equal(zb[0], z[b]), b
+        assert torch.equal(m.model.decode(zb)[0], logits[b]), b
+        assert _notes(m, zb)[0] == notes[b], b
+    _simt_plans_are_plain(m.engine)
+
+
+def test_simt_engine_decode_where_the_ffma_tile_flips():
+    """32 charts at L = 512: the decoder's plan puts GEMMs on the FFMA kernel's 128 x 128 tiles that one chart runs on 64 x 64
+    tiles; every chart's logits are its own decode's, bit for bit"""
+    from gemm_cases import ffma_tile
+    L, B = 512, 32
+    m = model_for(L, impl="simt")
+    eng = m.engine
+    tiles = lambda n: [ffma_tile(o.u.gemm.M, o.u.gemm.N, eng.sm_count) for o in eng.decoder_session(n, L).plan._arr  # noqa: E731
+                       if o.kind == L_.OP_GEMM]
+    assert 128 in tiles(B) and 128 not in tiles(1)
+    z = torch.randn(B, 16, L, device="cuda", generator=torch.Generator("cuda").manual_seed(11))
+    logits = m.model.decode(z)
+    for b in range(B):
+        assert torch.equal(m.model.decode(z[b:b + 1])[0], logits[b]), b
+    _simt_plans_are_plain(eng)
 
 
 def test_every_chart_of_a_long_batch_is_the_chart_alone():

@@ -7,6 +7,8 @@ Stated fp32 tolerances (max-abs error relative to the tensor's max magnitude):
   10-step DDIM latent / decoder logits<= 1e-3
   50-step CFG-5 trajectory (L=512)    <= 5e-3   (random-weight CFG trajectory amplifies rounding noise)
   note on/off masks: identical except where the REFERENCE logit magnitude is below the logit tolerance.
+The U-Net goldens, the small and ragged lengths and the two L=96 DDIM trajectories also run on a `simt` engine (every GEMM on the
+exact-fp32 FFMA kernel) at the same tolerances.
 """
 import os
 
@@ -24,17 +26,23 @@ from oracle import mug_oracle as orc  # noqa: E402
 _models = {}
 
 
-def model_for(L):
-    if L not in _models:
+def model_for(L, impl="auto"):
+    if (L, impl) not in _models:
         _models.clear()                      # one resident model at a time
-        _models[L] = MugDiffusionB200.from_state_dict(synth.synthetic_state_dict(L), z_length=L)
-    return _models[L]
+        _models[L, impl] = MugDiffusionB200.from_state_dict(synth.synthetic_state_dict(L), z_length=L, gemm_impl=impl)
+    return _models[L, impl]
 
 
-@pytest.mark.parametrize("name", list(gc.UNET_CASES))
-def test_unet_forward_vs_reference_golden(name, golden_dir):
+def with_simt(cases, ids):
+    """each case on the default engine (its id unchanged) and on a `simt` engine (id + "-simt"); cases: tuples of arguments"""
+    return [pytest.param(*c, "auto", id=i) for c, i in zip(cases, ids)] + [pytest.param(*c, "simt", id=f"{i}-simt")
+                                                                           for c, i in zip(cases, ids)]
+
+
+@pytest.mark.parametrize("name,impl", with_simt([(n,) for n in gc.UNET_CASES], list(gc.UNET_CASES)))
+def test_unet_forward_vs_reference_golden(name, impl, golden_dir):
     case = gc.UNET_CASES[name]
-    m = model_for(case["L"])
+    m = model_for(case["L"], impl)
     inp = synth.synthetic_inputs(case["B"], case["L"])
     eps = m.model.forward(inp["x_T"].cuda(), torch.tensor(case["t"]).cuda(), inp["c"].cuda(), synth.wave_list([w.cuda() for w in inp["w"]]))
     gold = gc.load_golden(os.path.join(golden_dir, name + ".npz"))["eps"]
@@ -73,12 +81,12 @@ def test_unet_forward_vs_oracle_other_batch():
     assert rel_err(eps, ref) < 1e-4
 
 
-@pytest.mark.parametrize("L,B", [(32, 3), (224, 2), (64, 5)])
-def test_unet_forward_small_and_ragged_lengths(L, B):
+@pytest.mark.parametrize("L,B,impl", with_simt([(32, 3), (224, 2), (64, 5)], ["32-3", "224-2", "64-5"]))
+def test_unet_forward_small_and_ragged_lengths(L, B, impl):
     """shortest legal chart (L=32 -> level lengths 32/16/8/4), lengths that are not multiples of the 128-row GEMM tile
     (224 -> 224/112/56/28: partial tiles and several samples per tile), odd batch: live oracle"""
     sd = synth.synthetic_state_dict(L)
-    m = model_for(L)
+    m = model_for(L, impl)
     inp = synth.synthetic_inputs(B, L, seed=7 + L)
     t = torch.arange(B) * 211 + 3
     with torch.no_grad():
@@ -96,10 +104,14 @@ def _notes_match(logits, ref_logits, tol_abs):
     return int(flips.sum()), bool((ref8[flips].abs() <= tol_abs).all())
 
 
-@pytest.mark.parametrize("name,tol", [("ddim_L96_B1_S10_nocfg", 1e-3), ("ddim_L96_B2_S10_cfg5", 1e-3), ("ddim_L512_B1_S50_cfg5", 5e-3)])
-def test_ddim_sample_and_decode_vs_reference_golden(name, tol, golden_dir):
+_DDIM = [("ddim_L96_B1_S10_nocfg", 1e-3), ("ddim_L96_B2_S10_cfg5", 1e-3), ("ddim_L512_B1_S50_cfg5", 5e-3)]
+
+
+# the 50-step L=512 trajectory on the default engine only
+@pytest.mark.parametrize("name,tol,impl", with_simt(_DDIM, [f"{n}-{t}" for n, t in _DDIM])[:-1])
+def test_ddim_sample_and_decode_vs_reference_golden(name, tol, impl, golden_dir):
     case = gc.DDIM_CASES[name]
-    m = model_for(case["L"])
+    m = model_for(case["L"], impl)
     m.z_length = case["L"]
     inp = synth.synthetic_inputs(case["B"], case["L"])
     sampler = DDIMSampler(m)

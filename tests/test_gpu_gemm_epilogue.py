@@ -8,7 +8,13 @@ split is also bit-equal to split kernel + reduce at the same split (the batch-in
 tile width, addressing mode, class of serial op the invariant plans contain and K-range layout.  Also the step counter under
 CUDA-graph replay and the opt-in single-pass TF32 mode.
 
-Tolerances are those of test_gpu_gemm_tc.py / test_gpu_fusion.py: 1e-5 of max |ref| (2e-5 with the folded LayerNorm)."""
+The exact-fp32 FFMA kernel (gemm_simt.cu) is one more path of the same matrix, addressing modes and graph replay, held element by
+element to the bound gemm_cases.ffma_bound (|y - y64| <= FFMA_C E) at its factor cases and one case of every class of FFMA op the
+plans contain; the row-moment sink and the folded LayerNorm are refused on it.  A sample's rows from a launch on 128 x 128 tiles
+are bit-equal to the same sample launched alone on 64 x 64 tiles: what lets a `simt` engine keep its plans under batch_invariant.
+
+Tolerances of the tensor-core paths are those of test_gpu_gemm_tc.py / test_gpu_fusion.py: 1e-5 of max |ref| (2e-5 with the folded
+LayerNorm)."""
 import ctypes as C
 
 import pytest
@@ -20,20 +26,21 @@ from mug_diffusion_b200 import lib as L_  # noqa: E402
 from mug_diffusion_b200.engine import OpList  # noqa: E402
 from mug_diffusion_b200.packer import tf32_split  # noqa: E402
 
-from gemm_cases import (EXTRA, LAYOUT_BASES, LAYOUTS, MATRIX, SENT, SERIAL, SPLIT, STEP, STEPS, TOL, TOL_LN, Case,  # noqa: E402
-                        Operands, case_gemm, layout_split, matrix_case, ref_gemm)
+from gemm_cases import (EXTRA, FFMA, FFMA_C, LAYOUT_BASES, LAYOUTS, MATRIX, SENT, SERIAL, SPLIT, STEP, STEPS, TOL,  # noqa: E402
+                        TOL_LN, Case, Operands, case_gemm, ffma_bound, ffma_gpu_cases, ffma_tile, layout_split, matrix_case,
+                        ref_gemm)
 from gpu_util import OpRunner, ptr, rel_err  # noqa: E402
 
 
 class Device:
     """the operands of a case on the GPU, an output buffer pre-filled with SENT and the op list of the GEMM (serial: the
-    MUGD_OP_GEMM_SERIAL op at the same forced split)"""
+    MUGD_OP_GEMM_SERIAL op at the same forced split; ffma: forced to the FFMA kernel, plain fp32 weight only)"""
 
-    def __init__(self, o: Operands, split: int, serial: bool = False):
+    def __init__(self, o: Operands, split: int, serial: bool = False, ffma: bool = False, a_off: int = 32):
         c = o.c
         self.c = c
-        a = torch.zeros(c.B * c.Lin, c.K + 64)                       # A is columns 32 .. 32+K of a wider buffer
-        a[:, 32:32 + c.K] = o.A
+        a = torch.zeros(c.B * c.Lin, c.K + 64)                       # A is columns a_off .. a_off+K of a wider buffer
+        a[:, a_off:a_off + c.K] = o.A
         self.a = a.cuda()
         kw = {}
         if c.K2:
@@ -41,8 +48,10 @@ class Device:
             a2[:, 32:32 + c.K2] = o.A2
             self.a2 = a2.cuda()
             kw["a2"] = ptr(self.a2)
-        hi, lo = tf32_split(o.W)
-        self.w, self.w_hi, self.w_lo = o.W.cuda(), hi.cuda(), lo.cuda()
+        self.w = o.W.cuda()
+        if not ffma:
+            hi, lo = tf32_split(o.W)
+            self.w_hi, self.w_lo = hi.cuda(), lo.cuda()
         self.step = torch.tensor([STEP], dtype=torch.int32).cuda()
         if c.bias:
             self.bias = o.bias.cuda()
@@ -55,6 +64,8 @@ class Device:
             kw["res"] = ptr(self.res)
         if c.parity >= 0:
             self.out = torch.full((2 * c.M, c.nout), SENT).cuda()
+        elif c.dense:
+            self.out = torch.full((c.M + 2, c.nout), SENT).cuda()     # the output is rows 1 .. M+1
         else:
             self.out = torch.full((c.M, c.nout + 64), SENT).cuda()   # the output is columns 32 .. 32+nout
         if c.ln:
@@ -65,8 +76,12 @@ class Device:
             self.moments = torch.zeros(c.M, 2, dtype=torch.float64).cuda()
             kw["moments"] = self.moments.data_ptr()
         self.ops = OpList()
-        self.i = case_gemm(self.ops, c, split, a=ptr(self.a), w=ptr(self.w), w_hi=ptr(self.w_hi), w_lo=ptr(self.w_lo),
-                           out=ptr(self.out), **kw)
+        out = ptr(self.out) + (4 * c.nout if c.dense else 0)
+        if ffma:
+            kw.update(w_hi=0, w_lo=0, impl=L_.GEMM_SIMT)
+        else:
+            kw.update(w_hi=ptr(self.w_hi), w_lo=ptr(self.w_lo))
+        self.i = case_gemm(self.ops, c, split, a=ptr(self.a), w=ptr(self.w), out=out, a_off=a_off, **kw)
         if serial:
             self.ops.ops[self.i].kind = L_.OP_GEMM_SERIAL
 
@@ -79,6 +94,8 @@ class Device:
         c, o = self.c, self.out.cpu()
         if c.parity >= 0:
             win, rest = o[c.parity::2], o[1 - c.parity::2]
+        elif c.dense:
+            win, rest = o[1:-1], torch.cat([o[:1], o[-1:]])
         else:
             win, rest = o[:, 32:32 + c.nout], torch.cat([o[:, :32], o[:, 32 + c.nout:]], dim=1)
         return win.clone(), bool((rest == SENT).all())
@@ -158,25 +175,89 @@ def check_case(R, c: Case, name: str, split: int, bn: int, tol: float, serial: b
         assert float((d.moments.cpu() - exp).abs().max() / exp.abs().max()) < 1e-6
 
 
+def check_ffma(R, c: Case, name: str, tile: int, o: Operands = None):
+    """the GEMM of ``c`` forced to the FFMA kernel on ``tile`` x ``tile`` tiles against fp64, element by element within FFMA_C times
+    ffma_bound; the output window's surroundings untouched, two runs equal.  The row-moment sink and the folded LayerNorm are
+    refused.  Returns |y - y64| / E at its worst and the output."""
+    o = o or Operands(c, name)
+    if c.sink or c.ln:
+        with pytest.raises(L_.MugdError, match="tensor-core path only"):
+            R.run(Device(o, 0, ffma=True).ops)
+        return 0.0, None
+    assert ffma_tile(c.M, c.N, sm_count(R)) == tile                 # the variant under test is the one that runs
+    d = Device(o, 0, ffma=True)
+    R.run(d.ops)
+    out, kept = d.output()
+    d2 = Device(o, 0, ffma=True)
+    R.run(d2.ops)
+    ratio = float(((out.double() - o.ref()).abs() / ffma_bound(o)).max())
+    print(f"{name} ffma tile={tile} |y - y64| / E = {ratio:.3f}")
+    assert ratio <= FFMA_C, ratio
+    assert kept, "a store left the output window"
+    assert torch.equal(out, d2.output()[0]), "two runs differ"
+    return ratio, out
+
+
 PATHS = ["direct", "reduce", "serial"]
+MATRIX_PATHS = [(p, bn) for p in PATHS for bn in (128, 64)] + [("ffma", 64)]      # FFMA: these shapes take its 64-tile variant
 
 
-@pytest.mark.parametrize("bn", [128, 64])
-@pytest.mark.parametrize("path", PATHS)
+@pytest.mark.parametrize("path,bn", MATRIX_PATHS, ids=[f"{p}-{bn}" for p, bn in MATRIX_PATHS])
 @pytest.mark.parametrize("epi,conv,shape", MATRIX, ids=["-".join(m) for m in MATRIX])
 def test_epilogue_matrix(R, epi, conv, shape, path, bn):
-    """every epilogue at both tile widths on every path: with the serial path, all 16 serial instantiations (8 epilogues x BN)"""
+    """every epilogue at both tile widths on every path: with the serial path, all 16 serial instantiations (8 epilogues x BN); on
+    the FFMA kernel the sink and the folded LayerNorm are refused"""
     c = matrix_case(epi, conv, shape)
     assert c.ksteps % SPLIT != 0                                   # the last split owns fewer k-steps (it_rem != 0)
+    if path == "ffma":
+        check_ffma(R, c, f"{epi}-{conv}-{shape}", bn)
+        return
     check_case(R, c, f"{epi}-{conv}-{shape}", 1 if path == "direct" else SPLIT, bn, TOL_LN if c.ln else TOL, serial=path == "serial")
 
 
-@pytest.mark.parametrize("path", PATHS)
+@pytest.mark.parametrize("path", PATHS + ["ffma"])
 @pytest.mark.parametrize("name", list(EXTRA))
 def test_addressing_modes(R, name, path):
     c, split, bn = EXTRA[name]
     assert c.ksteps % split != 0
+    if path == "ffma":
+        check_ffma(R, c, name, ffma_tile(c.M, c.N, sm_count(R)))
+        return
     check_case(R, c, name, 1 if path == "direct" else split, bn, TOL, serial=path == "serial")
+
+
+# ---- the FFMA kernel ------------------------------------------------------------------------------------------------------------
+def test_ffma_cases_within_the_bound(R):
+    """the FFMA factor cases and one case of every class of FFMA op the plans contain (test_gemm_cases.py checks both lists):
+    within the bound, sentinels intact, two runs bit-equal; the worst ratio per tile variant is what DESIGN §2 records"""
+    worst = {}
+    for name, (c, tile) in ffma_gpu_cases().items():
+        r, _ = check_ffma(R, c, name, tile)
+        worst[tile] = max(worst.get(tile, (0.0, "")), (r, name))
+    print("worst |y - y64| / E per tile variant:", worst)
+    assert set(worst) == {64, 128}
+
+
+ROW_INVARIANCE = ["big_none", "big_same", "big_down", "big_up", "big_taps_d2", "big_k2", "big_glu", "big_l1"]
+
+
+@pytest.mark.parametrize("name", ROW_INVARIANCE)
+def test_ffma_rows_do_not_depend_on_the_batch(R, name):
+    """each sample's rows of a B-sample launch on 128 x 128 tiles are bit-equal to the same sample launched alone on 64 x 64 tiles
+    with A at another column offset: the FFMA kernel sums every element in the same order whatever its tile and batch, the claim
+    MugEngine.batch_ops relies on when it leaves a `simt` engine's plans alone under batch_invariant"""
+    c, tile = FFMA[name]
+    assert tile == 128
+    o = Operands(c, name)
+    _, out = check_ffma(R, c, name, tile, o)
+    for b in sorted({0, 1, c.B // 2, c.B - 1}):
+        one = o.sample(b)
+        assert ffma_tile(one.c.M, one.c.N, sm_count(R)) == 64
+        d = Device(one, 0, ffma=True, a_off=4)
+        R.run(d.ops)
+        alone, kept = d.output()
+        assert kept
+        assert torch.equal(alone, out[b * c.Lout:(b + 1) * c.Lout]), (name, b)
 
 
 @pytest.mark.parametrize("name", list(SERIAL))
@@ -213,18 +294,21 @@ def make_plan(R, ops: OpList):
     return plan
 
 
-@pytest.mark.parametrize("path", PATHS)
+@pytest.mark.parametrize("path", PATHS + ["ffma"])
 def test_step_counter_under_graph_replay(R, path):
     """[ResBlock conv3 + time-embedding row of the current step ; STEP_ADVANCE] captured once, replayed once per step: replay i
     adds table row i (mugd.h: step-dependent rows are selected on the device, so one graph serves all steps).  The reduce reads the
-    counter in its second pass, the direct path and the serial split in the tile's epilogue-operand preload."""
+    counter in its second pass, the direct path and the serial split in the tile's epilogue-operand preload, the FFMA kernel in its
+    epilogue."""
     split = 1 if path == "direct" else 4
     c = Case(2, 200, 200, 64, 192, taps=3, mode=L_.CONV_SAME, rowvec="step", residual=False)
     assert c.ksteps % 4 != 0
     o = Operands(c, "graph")
-    d = Device(o, split, serial=path == "serial")
+    ffma = path == "ffma"
+    d = Device(o, 0 if ffma else split, serial=path == "serial", ffma=ffma)
     d.step.zero_()
-    assert planned(R, d.gemm)[0] == split
+    if not ffma:
+        assert planned(R, d.gemm)[0] == split
     adv = L_.StepAdvance()
     adv.step = ptr(d.step)
     d.ops.add(L_.OP_STEP_ADVANCE, adv)
@@ -240,7 +324,10 @@ def test_step_counter_under_graph_replay(R, path):
             L_.check(R.lib.mugd_plan_replay(plan, 1, C.c_void_p(st.cuda_stream)), "replay")
             st.synchronize()
             out, kept = d.output()
-            assert rel_err(out, o.ref(step=i)) < TOL, i
+            if ffma:
+                assert bool(((out.double() - o.ref(step=i)).abs() <= FFMA_C * ffma_bound(o, step=i)).all()), i
+            else:
+                assert rel_err(out, o.ref(step=i)) < TOL, i
             assert kept
         assert int(d.step.item()) == STEPS
     finally:

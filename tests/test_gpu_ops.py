@@ -81,58 +81,7 @@ def test_gemm_rowvec_step_indexing(R):
     assert rel_err(ncl(out.cpu(), B), ref) < 2e-5
 
 
-@pytest.mark.parametrize("B,L,C", [(2, 48, 128), (1, 24, 384)])
-def test_gemm_downsample(R, B, L, C):
-    x, w, b = g("dx", (B, C, L)), g("dw", (C, C, 3)) / math.sqrt(3 * C), 0.1 * g("db", (C,))
-    ref = F.conv1d(F.pad(x, (0, 1)), w, b, stride=2)
-    wp, bc = w.permute(0, 2, 1).contiguous().reshape(C, 3 * C).cuda(), b.cuda()
-    out = run_gemm(R, nlc(x).cuda(), wp, C, C, B * L // 2, C, bias=ptr(bc), taps=3, mode=L_.CONV_DOWN, Lin=L, Lout=L // 2)
-    assert rel_err(ncl(out.cpu(), B), ref) < 2e-5
-
-
-@pytest.mark.parametrize("B,L,C", [(2, 24, 256), (1, 12, 512)])
-def test_gemm_upsample(R, B, L, C):
-    x, w, b = g("ux", (B, C, L)), g("uw", (C, C, 3)) / math.sqrt(3 * C), 0.1 * g("ub", (C,))
-    ref = F.conv1d(x.repeat_interleave(2, dim=-1), w, b, padding=1)
-    wp, bc = w.permute(0, 2, 1).contiguous().reshape(C, 3 * C).cuda(), b.cuda()
-    out = run_gemm(R, nlc(x).cuda(), wp, C, C, B * L * 2, C, bias=ptr(bc), taps=3, mode=L_.CONV_UP, Lin=L, Lout=2 * L)
-    assert rel_err(ncl(out.cpu(), B), ref) < 2e-5
-
-
-@pytest.mark.parametrize("gate", [L_.GATE_GEGLU, L_.GATE_GLU])
-def test_gemm_gated(R, gate):
-    from mug_diffusion_b200.packer import _interleave_halves
-    M, K, Hh = 130, 256, 512
-    x, w, b, res = g("gx", (M, K)), g("gw", (2 * Hh, K)) / math.sqrt(K), 0.1 * g("gb", (2 * Hh,)), g("gr", (M, Hh))
-    proj = F.linear(x, w, b)
-    a, gt = proj.chunk(2, dim=-1)
-    ref = (a * F.gelu(gt) if gate == L_.GATE_GEGLU else a * torch.sigmoid(gt)) + res
-    wi, bi, rc = _interleave_halves(w).cuda(), _interleave_halves(b).cuda(), res.cuda()
-    out = run_gemm(R, x.cuda(), wi, 2 * Hh, K, M, Hh, bias=ptr(bi), gate=gate, residual=view(rc))
-    assert rel_err(out, ref) < 2e-5
-
-
-def test_gemm_strided_views(R):
-    """A read from, and C written into, column windows of wider (concat) buffers"""
-    M, K, N = 96, 128, 256
-    x, w = g("vx", (M, K)), g("vw", (N, K)) / math.sqrt(K)
-    wide_in = torch.zeros(M, K + 64).cuda()
-    wide_in[:, 32:32 + K] = x.cuda()
-    wide_out = torch.full((M, N + 128), 7.0).cuda()
-    wc = w.cuda()
-    ops = OpList()
-    ops.gemm(view(wide_in, 32, 32 + K), ptr(wc), N, K, view(wide_out, 64, 64 + N))
-    R.run(ops)
-    assert rel_err(wide_out[:, 64:64 + N], F.linear(x, w)) < 2e-5
-    assert float((wide_out[:, :64] - 7).abs().max()) == 0 and float((wide_out[:, 64 + N:] - 7).abs().max()) == 0
-
-
-def test_gemm_rejects_bad_shapes(R):
-    x, w = torch.zeros(8, 24).cuda(), torch.zeros(16, 24).cuda()
-    ops = OpList()
-    ops.gemm(view(x), ptr(w), 16, 24, view(torch.zeros(8, 16).cuda()))
-    with pytest.raises(L_.MugdError):
-        R.run(ops)
+# the FFMA GEMM's addressing modes, gates, column windows and refusals: test_gpu_gemm_epilogue.py (ffma path) and test_gemm_cases.py
 
 
 # ---------------------------------------------------------------------------------------------------

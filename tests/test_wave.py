@@ -58,15 +58,27 @@ def test_wave_plan_compiles():
     assert dil == [1, 2, 4, 8]
 
 
-@pytest.mark.gpu
-def test_gpu_wave_encoder_vs_reference(gold):
+def _wave_vs_reference(gold, impl):
     from mug_diffusion_b200.sampler import MugDiffusionB200
     sd = {**synth.synthetic_state_dict(96), **wave.synthetic_wave_state_dict()}
-    m = MugDiffusionB200.from_state_dict(sd, z_length=96)
+    m = MugDiffusionB200.from_state_dict(sd, z_length=96, gemm_impl=impl)
     hs = m.model.wave_model(wave.synthetic_mel(2, 64 * 96).cuda())
     assert len(hs) == 10 and all(h is None for h in hs[:6])
     for i in range(6, 10):
-        assert rel(hs[i], gold[f"h{i}"]) < 1e-4
+        e = rel(hs[i], gold[f"h{i}"])
+        print(f"audio encoder {impl} h{i} rel_err={e:.2e}")
+        assert e < 1e-4
+
+
+@pytest.mark.gpu
+def test_gpu_wave_encoder_vs_reference(gold):
+    _wave_vs_reference(gold, "auto")
+
+
+@pytest.mark.gpu
+def test_gpu_wave_encoder_simt_vs_reference(gold):
+    """every GEMM of the audio encoder on the exact-fp32 FFMA kernel (dilated taps, Downsample, residuals): same tolerance"""
+    _wave_vs_reference(gold, "simt")
 
 
 @pytest.mark.gpu
