@@ -67,7 +67,10 @@ enum mugd_op_kind {
     MUGD_OP_GEMM_SERIAL = 17,
     /* classifier-free guidance at one scale per chart (mugd_cfg_scales): the guided noise prediction of B charts from the 2B eps rows of
      * an evaluation, for a sampler update that then runs unguided (cfg = 0) on the output rows */
-    MUGD_OP_CFG_SCALES = 18
+    MUGD_OP_CFG_SCALES = 18,
+    /* cross-attention with a prompt per section of each sample (mugd_attention_sec): query row i attends to the Lk tokens of the
+     * section that holds it, with the same bias, gain and formula as MUGD_OP_ATTENTION at its own row index i */
+    MUGD_OP_ATTENTION_SEC = 19
 };
 
 /* A-operand row addressing of MUGD_OP_GEMM (rows are tokens of B samples, Lout output rows each) */
@@ -250,6 +253,17 @@ typedef struct mugd_cfg_scales {
     int32_t B, L, C, reserved_;
 } mugd_cfg_scales;
 
+/* Section prompts (MUGD_OP_ATTENTION_SEC).  Sample b has MUGD_SECTIONS section slots; slot s holds Lk keys at rows
+ * (MUGD_SECTIONS * b + s) * sec_stride of k and v (sec_stride >= Lk).  starts[b][s] is the first query row of slot s at the op's
+ * resolution: starts[b][0] = 0, used slots strictly increasing below Lq, unused slots = Lq.  Query row i of sample b takes slot
+ * s = #{t >= 1 : starts[b][t] <= i}.  The starts are device data, so one captured plan serves any layout. */
+#define MUGD_SECTIONS 8
+typedef struct mugd_attention_sec {
+    mugd_attention attn;                   /* cross-attention: k / v hold B * MUGD_SECTIONS * sec_stride rows     */
+    const int32_t* starts;                 /* [B][MUGD_SECTIONS] device                                          */
+    int32_t sec_stride, reserved_;         /* rows of k / v from one section slot to the next                   */
+} mugd_attention_sec;
+
 typedef struct mugd_op {
     int32_t kind;
     int32_t tag;                           /* free for the host (profiling labels)                          */
@@ -259,6 +273,7 @@ typedef struct mugd_op {
         mugd_embed embed; mugd_tf32_split split; mugd_posterior post;
         mugd_groupnorm_var gnv; mugd_attention_var attnv; mugd_row_mask mask;   /* ragged batches (same union size) */
         mugd_cfg_scales cfgs;                                                   /* per-chart guidance scales        */
+        mugd_attention_sec attns;                                               /* section prompts                  */
     } u;
 } mugd_op;
 
@@ -701,8 +716,8 @@ int  mugd_debug_set_tc_timing(long long* device_buf);
 int  mugd_fill_i32(int32_t* dst, int32_t value, void* stream);
 /* sizeof() of {mugd_op, mugd_gemm, mugd_groupnorm, mugd_layernorm, mugd_attention, mugd_s4conv, mugd_ddim_update, mugd_transpose,
  * mugd_copy2d, mugd_notes, mugd_embed, mugd_tf32_split, mugd_posterior} so a foreign-language mirror can verify its layout; with
- * n >= 16 also {mugd_groupnorm_var, mugd_attention_var, mugd_row_mask} in entries 13..15, with n >= 17 also mugd_cfg_scales in entry 16
- * (n >= 13 is enough for the first 13) */
+ * n >= 16 also {mugd_groupnorm_var, mugd_attention_var, mugd_row_mask} in entries 13..15, with n >= 17 also mugd_cfg_scales in entry 16,
+ * with n >= 18 also mugd_attention_sec in entry 17 (n >= 13 is enough for the first 13; entries past those are left untouched) */
 int  mugd_abi_sizes(int32_t* out, int32_t n);
 
 #ifdef __cplusplus

@@ -61,6 +61,7 @@ static int dispatch(mugd_handle* h, const mugd_op& op, cudaStream_t st, int* lau
         case MUGD_OP_ROW_MASK: return launch_row_mask(h->dev, op.u.mask, st, launches);
         case MUGD_OP_GEMM_SERIAL: return launch_gemm_serial(h->dev, op.u.gemm, h->default_gemm_impl, next_tc, st, launches);
         case MUGD_OP_CFG_SCALES: return launch_cfg_scales(h->dev, op.u.cfgs, st, launches);
+        case MUGD_OP_ATTENTION_SEC: return launch_attention_sec(h->dev, op.u.attns, st, launches);
         default:
             set_error("unknown op kind %d", op.kind);
             return MUGD_ERR_INVALID;
@@ -436,6 +437,7 @@ int mugd_abi_sizes(int32_t* out, int32_t n) {
     out[12] = sizeof(mugd_posterior);
     if (n >= 16) { out[13] = sizeof(mugd_groupnorm_var); out[14] = sizeof(mugd_attention_var); out[15] = sizeof(mugd_row_mask); }
     if (n >= 17) out[16] = sizeof(mugd_cfg_scales);
+    if (n >= 18) out[17] = sizeof(mugd_attention_sec);
     return MUGD_OK;
 }
 

@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <string>
+#include <type_traits>
 #include <utility>
 
 #include "../../include/mugd.h"
@@ -67,6 +68,8 @@ int launch_posterior(const DeviceInfo& dev, const mugd_posterior& p, cudaStream_
 int launch_groupnorm_var(const DeviceInfo& dev, const mugd_groupnorm_var& g, cudaStream_t st, int* launches);
 int launch_attention_var(const DeviceInfo& dev, const mugd_attention_var& a, cudaStream_t st, int* launches);
 int launch_row_mask(const DeviceInfo& dev, const mugd_row_mask& m, cudaStream_t st, int* launches);
+// section prompts: a cross-attention whose keys / values change along the rows (attention.cu)
+int launch_attention_sec(const DeviceInfo& dev, const mugd_attention_sec& a, cudaStream_t st, int* launches);
 // per-chart guidance scales (elementwise.cu)
 int launch_cfg_scales(const DeviceInfo& dev, const mugd_cfg_scales& g, cudaStream_t st, int* launches);
 // mugd_sample_staged: check_stage validates a stage for n_steps (host arrays included); launch_stage runs step i of it
@@ -206,14 +209,17 @@ __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf
 // exact-erf GELU (nn.GELU() default; attention.py:45, s4.py:187-188)
 __device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
-// Attention kernels are instantiated for both descriptors: mugd_attention (every row valid) and mugd_attention_var (ragged batches,
-// sample b's first clamp(valid[b], 0, n) rows valid).  With the plain descriptor attn_rows() is n, so those instances compile to the
-// code they had before ragged batches existed.
+// Attention kernels are instantiated for the descriptors: mugd_attention (every row valid), mugd_attention_var (ragged batches,
+// sample b's first clamp(valid[b], 0, n) rows valid) and, in attention.cu, mugd_attention_sec (section prompts, every row valid).
+// With the plain descriptor attn_rows() is n, so those instances compile to the code they had before ragged batches existed.
 __host__ __device__ __forceinline__ const mugd_attention& attn_desc(const mugd_attention& a) { return a; }
 __host__ __device__ __forceinline__ const mugd_attention& attn_desc(const mugd_attention_var& a) { return a.attn; }
+__host__ __device__ __forceinline__ const mugd_attention& attn_desc(const mugd_attention_sec& a) { return a.attn; }
 __device__ __forceinline__ int attn_rows(const mugd_attention&, int, int n) { return n; }
 __device__ __forceinline__ int attn_rows(const mugd_attention_var& a, int b, int n) { return min(max(a.valid[b], 0), n); }
-template <typename Desc> constexpr bool attn_is_var = sizeof(Desc) != sizeof(mugd_attention);
+__device__ __forceinline__ int attn_rows(const mugd_attention_sec&, int, int n) { return n; }
+template <typename Desc> constexpr bool attn_is_var = std::is_same<Desc, mugd_attention_var>::value;
+template <typename Desc> constexpr bool attn_is_sec = std::is_same<Desc, mugd_attention_sec>::value;
 
 __device__ __forceinline__ float4 ld_f4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ void st_f4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }

@@ -52,6 +52,9 @@ static const PtrField k_ptr_fields[] = {
     PF(MUGD_OP_GEMM_SERIAL, gemm.counters), PF(MUGD_OP_GEMM_SERIAL, gemm.A2), PF(MUGD_OP_GEMM_SERIAL, gemm.row_moments),
     PF(MUGD_OP_GEMM_SERIAL, gemm.ln_stats), PF(MUGD_OP_GEMM_SERIAL, gemm.ln_colsum),
     PF(MUGD_OP_CFG_SCALES, cfgs.eps), PF(MUGD_OP_CFG_SCALES, cfgs.out), PF(MUGD_OP_CFG_SCALES, cfgs.scales),
+    PF(MUGD_OP_ATTENTION_SEC, attns.attn.q), PF(MUGD_OP_ATTENTION_SEC, attns.attn.k), PF(MUGD_OP_ATTENTION_SEC, attns.attn.v),
+    PF(MUGD_OP_ATTENTION_SEC, attns.attn.o), PF(MUGD_OP_ATTENTION_SEC, attns.attn.relpos), PF(MUGD_OP_ATTENTION_SEC, attns.attn.cgain),
+    PF(MUGD_OP_ATTENTION_SEC, attns.starts),
 };
 #undef PF
 

@@ -166,14 +166,20 @@ class OpList:
         return len(self.ops) - 1
 
     def attention(self, q: View, k: View, v: View, o: View, relpos: int, cgain: int, B: int, H: int, Lq: int,
-                  Lk: int, pos_max: int, tag: int = 0, self_attn: bool = False):
+                  Lk: int, pos_max: int, tag: int = 0, self_attn: bool = False, starts: int = 0, sec_stride: int = 0):
+        """``starts``: a cross-attention with section prompts (MUGD_OP_ATTENTION_SEC): the device address of its [B, 8] int32 section
+        starts at Lq rows per sample, k / v holding B * 8 * sec_stride rows (sample b's section s from row (8b + s) * sec_stride)"""
         d = L_.Attention()
         D = q.cols // H
         d.q, d.ldq, d.k, d.ldk, d.v, d.ldv, d.o, d.ldo = q.ptr, q.ld, k.ptr, k.ld, v.ptr, v.ld, o.ptr, o.ld
         d.relpos, d.cgain = relpos, cgain
         d.B, d.H, d.D, d.Lq, d.Lk, d.pos_max = B, H, D, Lq, Lk, pos_max
         d.scale = float(D) ** -0.5
-        if self_attn and Lq in self.valid:
+        if starts:
+            sec = L_.AttentionSec()
+            sec.attn, sec.starts, sec.sec_stride = d, starts, sec_stride
+            self.add(L_.OP_ATTENTION_SEC, sec, tag)
+        elif self_attn and Lq in self.valid:
             v = L_.AttentionVar()
             v.attn, v.valid = d, self.valid[Lq]
             self.add(L_.OP_ATTENTION_VAR, v, tag)
@@ -334,7 +340,7 @@ class UNetCompiler:
         return self.wbase + 4 * self.blob.offset(name)
 
     def compile(self, arena: Arena, Beff: int, Lz: int, ext: Dict[str, int], per_sample_t: bool, fold_ln: Optional[bool] = None,
-                valid: Optional[Sequence[int]] = None) -> dict:
+                valid: Optional[Sequence[int]] = None, sections: Optional[int] = None) -> dict:
         """fold_ln: every LayerNorm of the transformer blocks is folded into the Linear behind it (the producer of its input delivers
         the row moments, the Linear corrects in its epilogue; no LayerNorm kernel, the normalised tensor is never written).  It gains
         at small batches and loses slightly at large ones, so None = fold below 8192 token rows.
@@ -342,7 +348,10 @@ class UNetCompiler:
         valid: a ragged plan, whose Beff samples are padded to Lz rows but valid only in their first L_b: valid[l] is the device
         address of an int32 [Beff] array holding L_b >> l, level l's valid rows.  Every GroupNorm and self-attention then takes its
         _VAR op, and every k = 3 conv whose input is not a GroupNorm output (conv_in on x and the audio slots, Downsample, Upsample,
-        the S4 block's out_layer) finds its padded rows zeroed by a ROW_MASK op.  None = today's op list, op for op."""
+        the S4 block's out_layer) finds its padded rows zeroed by a ROW_MASK op.  None = today's op list, op for op.
+        sections: a plan with section prompts (DESIGN §6b N20): the device address of an int32 [levels, Beff, 8] table of section
+        starts in rows of each level, and ext["ctx_kv"] holding Beff * 8 sections of ctx_tokens rows.  Every cross-attention then
+        takes MUGD_OP_ATTENTION_SEC; nothing else changes.  None = today's op list, op for op."""
         cfg = self.cfg
         nlev = cfg.levels
         assert Lz % (1 << (nlev - 1)) == 0 and (Lz >> (nlev - 1)) % 4 == 0, "z_length must be a multiple of 32"
@@ -481,9 +490,10 @@ class UNetCompiler:
                         residual=h0, Lout=Lr, tag=TAG_ATTN)
             q2 = arena.alloc(x.rows, Cc)
             normed_linear(h1, i_h1, "norm2", "attn2.to_q", Cc, q2)
+            sec = {} if sections is None else dict(starts=sections + 4 * lvl * Beff * L_.SECTIONS, sec_stride=ctx_tokens)
             ops.attention(q2, kv.c(0, Cc), kv.c(Cc, 2 * Cc), ao,
                           self.w(t + "attn2.relative_position_embedding"), self.w(t + "attn2.C_embedding"),
-                          Beff, H, Lr, ctx_tokens, cfg.pos_max, TAG_ATTN)
+                          Beff, H, Lr, ctx_tokens, cfg.pos_max, TAG_ATTN, **sec)
             h2 = h0                                    # h0 is dead after the first residual add
             i_h2 = gemm(ao, self.w(t + "attn2.to_out.0.weight"), Cc, Cc, h2, bias=self.w(t + "attn2.to_out.0.bias"),
                         residual=h1, Lout=Lr, tag=TAG_ATTN)

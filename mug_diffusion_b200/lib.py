@@ -18,6 +18,8 @@ LIB_PATH = os.environ.get("MUGD_LIB") or os.path.join(HERE, "libmugd.so")      #
 OP_GROUPNORM_VAR, OP_ATTENTION_VAR, OP_ROW_MASK = 14, 15, 16           # ragged batches: the base descriptor + valid[B]
 OP_GEMM_SERIAL = 17                    # the GEMM descriptor, its forced K split finished inside each CTA (batch-invariant plans)
 OP_CFG_SCALES = 18                     # classifier-free guidance at one scale per chart
+OP_ATTENTION_SEC = 19                  # cross-attention with a prompt per section of each sample
+SECTIONS = 8                           # MUGD_SECTIONS: section slots per sample
 CONV_NONE, CONV_SAME, CONV_DOWN, CONV_UP, CONV_TAPS = range(5)
 ACT_NONE, ACT_SILU, ACT_GELU = range(3)
 GATE_NONE, GATE_GEGLU, GATE_GLU = range(3)
@@ -177,11 +179,15 @@ class CfgScales(C.Structure):
                 ("reserved_", C.c_int32)]
 
 
+class AttentionSec(C.Structure):
+    _fields_ = [("attn", Attention), ("starts", _f), ("sec_stride", C.c_int32), ("reserved_", C.c_int32)]
+
+
 class _OpU(C.Union):
     _fields_ = [("gemm", Gemm), ("gn", GroupNorm), ("ln", LayerNorm), ("attn", Attention), ("s4", S4Conv),
                 ("ddim", DdimUpdate), ("tr", Transpose), ("cp", Copy2D), ("adv", StepAdvance), ("notes", Notes), ("embed", Embed),
                 ("split", Tf32Split), ("post", Posterior), ("gnv", GroupNormVar), ("attnv", AttentionVar), ("mask", RowMask),
-                ("cfgs", CfgScales)]
+                ("cfgs", CfgScales), ("attns", AttentionSec)]
 
 
 class Op(C.Structure):
@@ -191,7 +197,7 @@ class Op(C.Structure):
 _KIND_FIELD = {OP_GEMM: "gemm", OP_GROUPNORM: "gn", OP_LAYERNORM: "ln", OP_ATTENTION: "attn", OP_S4CONV: "s4",
                OP_DDIM_UPDATE: "ddim", OP_TRANSPOSE: "tr", OP_COPY2D: "cp", OP_STEP_ADVANCE: "adv", OP_NOTES: "notes", OP_EMBED: "embed", OP_TF32_SPLIT: "split",
                OP_POSTERIOR: "post", OP_GROUPNORM_VAR: "gnv", OP_ATTENTION_VAR: "attnv", OP_ROW_MASK: "mask", OP_GEMM_SERIAL: "gemm",
-               OP_CFG_SCALES: "cfgs"}
+               OP_CFG_SCALES: "cfgs", OP_ATTENTION_SEC: "attns"}
 
 
 def make_op(kind: int, desc, tag: int = 0) -> Op:
@@ -253,10 +259,10 @@ def load() -> C.CDLL:
     lib.mugd_abi_sizes.argtypes = [C.POINTER(C.c_int32), C.c_int32]
     if lib.mugd_abi_version() != ABI_VERSION:
         raise MugdError(f"libmugd ABI {lib.mugd_abi_version()} != binding {ABI_VERSION}: rebuild the library")
-    sizes = (C.c_int32 * 17)()
-    lib.mugd_abi_sizes(sizes, 17)
+    sizes = (C.c_int32 * 18)()
+    lib.mugd_abi_sizes(sizes, 18)
     mine = [C.sizeof(t) for t in (Op, Gemm, GroupNorm, LayerNorm, Attention, S4Conv, DdimUpdate, Transpose, Copy2D, Notes, Embed, Tf32Split,
-                                  Posterior, GroupNormVar, AttentionVar, RowMask, CfgScales)]
+                                  Posterior, GroupNormVar, AttentionVar, RowMask, CfgScales, AttentionSec)]
     if list(sizes) != mine:
         raise MugdError(f"struct layout mismatch: C {list(sizes)} vs ctypes {mine}")
     lib.mugd_sample.argtypes = [C.c_void_p, C.POINTER(Op), C.c_int32, C.c_int32, C.c_void_p]

@@ -286,17 +286,20 @@ class MugEngine:
         return s
 
     def session(self, Beff: int, Lz: int, per_sample_t: bool = False, ragged: bool = False, unit: int = 1,
-                guided: bool = False) -> "Session":
+                guided: bool = False, sectioned: bool = False) -> "Session":
         """the compiled U-Net of (Beff, Lz).  ``ragged``: the plan for samples padded to Lz whose valid lengths are set per request
         (Session.set_lengths); a separate session, so requests without lengths keep today's plan.  ``unit``: samples per chart (2 under
         classifier-free guidance); with batch_invariant the plan sums as the plan of ``unit`` samples does, else it is ignored.
         ``guided``: Beff = 2B samples of B charts under classifier-free guidance with one scale per chart, set per request
-        (Session.set_scales); a separate session, so requests with one scale keep today's plan."""
+        (Session.set_scales); a separate session, so requests with one scale keep today's plan.
+        ``sectioned``: the plan whose samples change prompt along the song (DESIGN §6b N20), its section starts set per request
+        (Session.set_sections); a separate session, so requests without sections keep today's plan."""
         check_z_length(Lz)
         unit = unit if self.batch_invariant else 1
         key = ((Beff, Lz, per_sample_t) + (("ragged",) if ragged else ()) + ((("unit", unit),) if self.batch_invariant else ())
-               + (("guided",) if guided else ()))
-        return self._lru_get(self.sessions, key, lambda: Session(self, Beff, Lz, per_sample_t, ragged=ragged, unit=unit, guided=guided))
+               + (("guided",) if guided else ()) + (("sectioned",) if sectioned else ()))
+        return self._lru_get(self.sessions, key, lambda: Session(self, Beff, Lz, per_sample_t, ragged=ragged, unit=unit, guided=guided,
+                                                                 sectioned=sectioned))
 
     def wave_session(self, B: int, T: int):
         """Audio encoder plan for B mel-spectrograms of T frames (SURVEY §8f N1); needs wave weights in the blob."""
@@ -337,9 +340,11 @@ class Session:
 
     scales: Optional[torch.Tensor] = None     # a guided session's per-chart scales (None: not a guided session)
     e_guided: Optional[torch.Tensor] = None   # and the guided noise prediction its plan writes
+    starts: Optional[torch.Tensor] = None     # a sectioned session's section starts (None: not a sectioned session)
+    n_sec = 1                                 # context slots per sample (8 on a sectioned session)
 
     def __init__(self, engine: MugEngine, Beff: int, Lz: int, per_sample_t: bool, ragged: bool = False, unit: int = 1,
-                 guided: bool = False):
+                 guided: bool = False, sectioned: bool = False):
         self.engine, self.Beff, self.Lz, self.per_sample_t = engine, Beff, Lz, per_sample_t
         self.unit = unit                      # samples of one chart: the batch the batch-invariant policy plans for
         cfg = engine.cfg.unet
@@ -352,6 +357,11 @@ class Session:
         assert not guided or (Beff % 2 == 0 and not per_sample_t), (Beff, per_sample_t)
         self.scales = torch.ones(Beff // 2, device=dev) if guided else None
         self.e_guided = torch.zeros(Beff // 2 * Lz, cfg.out_channels, device=dev) if guided else None
+        # sectioned: each sample's section starts in rows of every level ([levels, Beff, 8] int32, data of the captured graph; slot 0
+        # at row 0, unused slots at the level's length) and 8 context slots per sample, sample b's slot s at context row (8b + s) * T
+        self.starts = (torch.tensor([[[0] + [Lz >> l] * (L_.SECTIONS - 1)] * Beff for l in range(cfg.levels)], dtype=torch.int32,
+                                    device=dev) if sectioned else None)
+        self.n_sec = L_.SECTIONS if sectioned else 1
         self.comp = UNetCompiler(cfg, engine.blob, engine.wbase, engine.tc_map)
         emb_total = engine.blob.meta["emb_total"]
         attn_blocks = [b for b in self.comp.lay.blocks() if b.kind == "attn"]
@@ -365,8 +375,8 @@ class Session:
         self.emb_h2 = torch.zeros(emb_rows, cfg.time_embed_dim, device=dev)
         self.step = torch.zeros(1, dtype=torch.int32, device=dev)
         self.coef = torch.zeros(MAX_STEPS, 4, device=dev)
-        self.ctx = torch.zeros(Beff * CTX_TOKENS_MAX, cfg.context_dim, device=dev)
-        self.ctx_kv = [torch.zeros(Beff * CTX_TOKENS_MAX, 2 * b.cin, device=dev) for b in attn_blocks]
+        self.ctx = torch.zeros(Beff * self.n_sec * CTX_TOKENS_MAX, cfg.context_dim, device=dev)
+        self.ctx_kv = [torch.zeros(Beff * self.n_sec * CTX_TOKENS_MAX, 2 * b.cin, device=dev) for b in attn_blocks]
         self.ctx_tokens = 21
         self.s4_kt = {b.prefix: torch.zeros(Lz // b.ds, b.cin, device=dev) for b in s4b}
         self._gen_s4_kernels(s4b)
@@ -412,7 +422,7 @@ class Session:
     def _ext(self, base_ctx_tokens: int) -> dict:
         return dict(
             emb_table=_ptr(self.emb_table), step=_ptr(self.step), ctx_tokens=base_ctx_tokens,
-            ctx_kv=[View(_ptr(t), t.shape[1], self.Beff * base_ctx_tokens, t.shape[1]) for t in self.ctx_kv],
+            ctx_kv=[View(_ptr(t), t.shape[1], self.Beff * self.n_sec * base_ctx_tokens, t.shape[1]) for t in self.ctx_kv],
             s4_kt={p: View(_ptr(t), t.shape[1], t.shape[0], t.shape[1]) for p, t in self.s4_kt.items()},
         )
 
@@ -425,7 +435,8 @@ class Session:
         valid = None if self.valid is None else [_ptr(self.valid[l]) for l in range(self.valid.shape[0])]
 
         def compile_fn(arena):
-            res = self.comp.compile(arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold, valid)
+            res = self.comp.compile(arena, self.Beff, self.Lz, self._ext(self.ctx_tokens), self.per_sample_t, fold, valid,
+                                    **({} if self.starts is None else dict(sections=_ptr(self.starts))))
             if self.scales is not None:
                 res["ops"] = guided_scales_ops(res["ops"], res["xin"], res["eps"], self.Beff // 2, self.Lz, _ptr(self.e_guided),
                                                _ptr(self.scales))
@@ -453,6 +464,24 @@ class Session:
         t = torch.tensor([[v >> l for v in lens] for l in range(self.valid.shape[0])], dtype=torch.int32)
         self.valid.copy_(t.to(self.engine.device))
         self.lens = lens
+
+    def set_sections(self, starts: Sequence[Sequence[int]]):
+        """a sectioned session's section starts: starts[b] lists the latent frames at which sample b changes prompt (multiples of 8,
+        strictly increasing in (0, Lz), at most 7; empty = one prompt), written into the device table the plan reads, so the
+        captured graph serves any layout"""
+        assert self.starts is not None, "set_sections needs a sectioned session"
+        assert len(starts) == self.Beff, (len(starts), self.Beff)
+        levels = self.starts.shape[0]
+        rows = []
+        for l in range(levels):
+            lev = []
+            for st in starts:
+                st = [int(v) for v in st]
+                assert len(st) < L_.SECTIONS and all(v % 8 == 0 and 0 < v < self.Lz for v in st), st
+                assert all(a < b for a, b in zip(st, st[1:])), st
+                lev.append([0] + [v >> l for v in st] + [self.Lz >> l] * (L_.SECTIONS - 1 - len(st)))
+            rows.append(lev)
+        self.starts.copy_(torch.tensor(rows, dtype=torch.int32).to(self.engine.device))
 
     def set_scales(self, scales: Sequence[float]):
         """a guided session's guidance scale of each of its Beff / 2 charts (finite; 1 = no guidance for that chart): written into
@@ -506,14 +535,14 @@ class Session:
     def set_context(self, context):
         """context [Beff, ctx_dim, T] (reference layout; or a list of such tensors that follow each other along the batch, e.g.
         [uc, c] under classifier-free guidance, ddim.py:173) -> per-layer cross-attention K|V projections (attention.py:97-98),
-        constant over the DDIM steps."""
+        constant over the DDIM steps.  A sectioned session takes Beff * 8 contexts: sample b's section slot s at index 8b + s."""
         eng = self.engine
         cfg = eng.cfg.unet
         parts = list(context) if isinstance(context, (list, tuple)) else [context]
         parts = [c.to(eng.device, torch.float32).contiguous() for c in parts]
         Bc = sum(int(c.shape[0]) for c in parts)
         _, Cd, T = parts[0].shape
-        assert Bc == self.Beff and Cd == cfg.context_dim and T <= CTX_TOKENS_MAX and all(c.shape[1:] == parts[0].shape[1:] for c in parts)
+        assert Bc == self.Beff * self.n_sec and Cd == cfg.context_dim and T <= CTX_TOKENS_MAX and all(c.shape[1:] == parts[0].shape[1:] for c in parts)
         self.set_ctx_tokens(T)
         eng.run_ops(self.context_ops([(_ptr(c), int(c.shape[0])) for c in parts], T))
         self._keep = parts
@@ -534,7 +563,7 @@ class Session:
         for b, kv in zip(blocks, self.ctx_kv):
             o = View(_ptr(kv), kv.shape[1], Bc * T, kv.shape[1])
             ops.gemm(cv, self.comp.w(b.prefix + "transformer_blocks.0.attn2.kv.weight"), 2 * b.cin, Cd, o, Lout=T)
-        return eng.batch_ops(ops, Bc, self.unit)
+        return eng.batch_ops(ops, Bc, self.unit * (Bc // self.Beff))      # a chart's contexts: 8 per sample on a sectioned session
 
     def set_audio(self, audios: Sequence[torch.Tensor], dup: bool = False):
         """The last ``levels`` entries of the wave-encoder output list (unet.py:527-543), NCL layout, written
